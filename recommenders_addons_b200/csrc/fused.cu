@@ -563,7 +563,10 @@ segment_sum_staged_kernel(TableView t, const long long* __restrict__ slots, cons
   cp_async_wait<0>();
 }
 
-// K6 phase B, wide rows (several vectors per lane): one lane-group per output row
+// K6 phase B, wide rows (several vectors per lane): one lane-group per output row.  A lane holds at most
+// kMaxVecPerLane vectors, so a row wider than kMaxVecPerLane * lpr vectors is swept in column chunks of that width;
+// every chunk re-walks the segment's ids in order (same per-column summation order, same wsum / wsq), so the result
+// does not depend on the chunking.  Rows of up to one chunk run the loop body once.
 template <int VF>
 __global__ void __launch_bounds__(kThreadsF)
 segment_sum_wide_kernel(TableView t, const long long* __restrict__ slots, const long long* __restrict__ seg_start,
@@ -575,6 +578,7 @@ segment_sum_wide_kernel(TableView t, const long long* __restrict__ slots, const 
   const unsigned gpw = 32u >> lpr_shift;
   const unsigned gidx = (unsigned)lane >> lpr_shift;
   const unsigned dim = t.dim;
+  const unsigned chunk = (unsigned)kMaxVecPerLane * lpr;   // vectors per column chunk
   const size_t warp0 = ((size_t)blockIdx.x * kThreadsF + threadIdx.x) >> 5;
   const size_t nwarps = ((size_t)gridDim.x * kThreadsF) >> 5;
   const float* table = (const float*)t.planes[0];
@@ -583,40 +587,42 @@ segment_sum_wide_kernel(TableView t, const long long* __restrict__ slots, const 
     const bool act_seg = b < batch;
     const long long start = act_seg ? seg_start[b] : 0;
     const long long end = act_seg ? seg_start[b + 1] : 0;
-    FVec<VF> acc[kMaxVecPerLane];
+    for (unsigned c0 = 0; c0 < vpr; c0 += chunk) {
+      FVec<VF> acc[kMaxVecPerLane];
 #pragma unroll
-    for (int v = 0; v < kMaxVecPerLane; ++v) acc[v].zero();
-    float wsum = 0.f, wsq = 0.f;
-    for (long long i = start; i < end; ++i) {
-      const long long slot = __ldg(slots + i);
-      const float w = weights ? __ldg(weights + i) : 1.f;
-      const float* src = slot >= 0 ? table + (size_t)slot * dim : default_row;
+      for (int v = 0; v < kMaxVecPerLane; ++v) acc[v].zero();
+      float wsum = 0.f, wsq = 0.f;
+      for (long long i = start; i < end; ++i) {
+        const long long slot = __ldg(slots + i);
+        const float w = weights ? __ldg(weights + i) : 1.f;
+        const float* src = slot >= 0 ? table + (size_t)slot * dim : default_row;
 #pragma unroll
-      for (int v = 0; v < kMaxVecPerLane; ++v) {
-        const unsigned c = (unsigned)gl + (unsigned)v * lpr;
-        if (c < vpr) {
-          FVec<VF> x;
-          x.load(src + (size_t)c * VF);
-          acc[v].zip(x, [w](float& a, float xv) { a = a + xv * w; });
+        for (int v = 0; v < kMaxVecPerLane; ++v) {
+          const unsigned c = c0 + (unsigned)gl + (unsigned)v * lpr;
+          if (c < vpr) {
+            FVec<VF> x;
+            x.load(src + (size_t)c * VF);
+            acc[v].zip(x, [w](float& a, float xv) { a = a + xv * w; });
+          }
         }
+        wsum = wsum + w;
+        wsq = wsq + w * w;
       }
-      wsum = wsum + w;
-      wsq = wsq + w * w;
-    }
-    if (act_seg) {
-      float div = 1.f;
-      bool do_div = false;
-      if (end > start) {
-        if (combiner == DET_COMBINER_MEAN) { div = wsum; do_div = true; }
-        else if (combiner == DET_COMBINER_SQRTN) { div = sqrtf(wsq); do_div = true; }
-      }
-      float* dst = out + b * dim;
+      if (act_seg) {
+        float div = 1.f;
+        bool do_div = false;
+        if (end > start) {
+          if (combiner == DET_COMBINER_MEAN) { div = wsum; do_div = true; }
+          else if (combiner == DET_COMBINER_SQRTN) { div = sqrtf(wsq); do_div = true; }
+        }
+        float* dst = out + b * dim;
 #pragma unroll
-      for (int v = 0; v < kMaxVecPerLane; ++v) {
-        const unsigned c = (unsigned)gl + (unsigned)v * lpr;
-        if (c < vpr) {
-          if (do_div) acc[v].apply([div](float& a) { a = a / div; });
-          acc[v].store(dst + (size_t)c * VF);
+        for (int v = 0; v < kMaxVecPerLane; ++v) {
+          const unsigned c = c0 + (unsigned)gl + (unsigned)v * lpr;
+          if (c < vpr) {
+            if (do_div) acc[v].apply([div](float& a) { a = a / div; });
+            acc[v].store(dst + (size_t)c * VF);
+          }
         }
       }
     }
@@ -1578,14 +1584,13 @@ static det_status lookup_sparse_impl(det_table* t, const int64_t* ids, const int
       DET_LAUNCH(segment_sum_kernel<4>, grid, kThreadsF, 0, s, t->view, slots, seg_start, weights, batch, combiner, default_row, out, vpr, lpr, sh, noclip, gate, epoch);
     else
       DET_LAUNCH(segment_sum_kernel<1>, grid, kThreadsF, 0, s, t->view, slots, seg_start, weights, batch, combiner, default_row, out, vpr, lpr, sh, noclip, gate, epoch);
-  } else if ((vpr + lpr - 1) / lpr <= (unsigned)kMaxVecPerLane) {
+  } else {
+    // rows wider than kMaxVecPerLane vectors per lane are swept in column chunks by the same kernel
     const int grid = grid_for(batch, (int)(gpw * (kThreadsF / 32)), t->sm_count, 8);
     if (vec4)
       DET_LAUNCH(segment_sum_wide_kernel<4>, grid, kThreadsF, 0, s, t->view, slots, seg_start, weights, batch, combiner, default_row, out, vpr, lpr, sh);
     else
       DET_LAUNCH(segment_sum_wide_kernel<1>, grid, kThreadsF, 0, s, t->view, slots, seg_start, weights, batch, combiner, default_row, out, vpr, lpr, sh);
-  } else {
-    rc = fail(DET_UNIMPLEMENTED, "det_lookup_sparse: dim too large for the fused kernel");
   }
   if (rc == DET_OK && cudaGetLastError() != cudaSuccess) rc = fail(DET_CUDA_ERROR, "det_lookup_sparse: launch failed");
   return rc;
