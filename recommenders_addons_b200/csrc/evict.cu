@@ -311,7 +311,7 @@ det_status evict_room(det_table* t, const long long* keys, size_t n, cudaStream_
 // det_insert / det_insert_scored on a table with an eviction strategy
 det_status evict_insert(det_table* t, const int64_t* keys, const void* values, const uint64_t* scores, size_t n,
                         cudaStream_t s) {
-  std::lock_guard<std::mutex> _lk(t->mu);
+  det::MutLock _lk(t);
   if (n == 0) return DET_OK;
   if (!keys || !values) return fail(DET_INVALID_ARGUMENT, "det_insert: null keys/values");
   EvictState* ev = t->ev;
@@ -387,7 +387,7 @@ det_status det_find_scores(det_table* t, const int64_t* keys, size_t n, uint64_t
 det_status det_set_global_epoch(det_table* t, uint64_t epoch) {
   if (!t) return fail(DET_INVALID_ARGUMENT, "det_set_global_epoch: null table");
   if (!t->ev) return fail(DET_INVALID_ARGUMENT, "det_set_global_epoch: the table was created without an eviction strategy");
-  std::lock_guard<std::mutex> _lk(t->mu);
+  det::MutLock _lk(t);
   t->ev->epoch = epoch;
   return DET_OK;
 }
@@ -395,7 +395,7 @@ det_status det_set_global_epoch(det_table* t, uint64_t epoch) {
 det_status det_evict(det_table* t, uint64_t n_evict, int64_t* n_evicted_out_host, det_stream_t stream) {
   if (!t) return fail(DET_INVALID_ARGUMENT, "det_evict: null table");
   if (!t->ev) return fail(DET_INVALID_ARGUMENT, "det_evict: the table was created without an eviction strategy");
-  std::lock_guard<std::mutex> _lk(t->mu);
+  det::MutLock _lk(t);
   det::DevGuard _dg(t->cfg.device);
   cudaStream_t s = (cudaStream_t)stream;
   const uint64_t before = t->ev->n_evicted;

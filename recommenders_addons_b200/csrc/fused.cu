@@ -1488,7 +1488,7 @@ static det_status lookup_sparse_impl(det_table* t, const int64_t* ids, const int
                                      float* out, det_stream_t stream) {
   if (!t) return fail(DET_INVALID_ARGUMENT, "det_lookup_sparse: null table");
   if (!(max_norm >= 0.f)) return fail(DET_INVALID_ARGUMENT, "det_lookup_sparse: max_norm must be >= 0 (0 = no clipping)");
-  std::lock_guard<std::mutex> _lk(t->mu);
+  det::MutLock _lk(t);
   if (t->cfg.value_dtype != DET_FLOAT32) return fail(DET_UNIMPLEMENTED, "det_lookup_sparse: float32 tables only");
   if (combiner < DET_COMBINER_SUM || combiner > DET_COMBINER_SQRTN)
     return fail(DET_INVALID_ARGUMENT, "combiner must be one of 'mean', 'sqrtn' or 'sum'");
@@ -1614,7 +1614,7 @@ static det_status apply_common(det_table* t, const int64_t* keys, const float* g
                                const float* init_param, int full_init, int opt, cudaStream_t s,
                                const long long* n_dev = nullptr) {
   if (!t) return fail(DET_INVALID_ARGUMENT, "det_apply: null table");
-  std::lock_guard<std::mutex> _lk(t->mu);
+  det::MutLock _lk(t);
   if (t->cfg.value_dtype != DET_FLOAT32) return fail(DET_UNIMPLEMENTED, "det_apply: float32 tables only");
   if (t->cfg.num_slot_planes < (opt == 0 ? 1 : 2))
     return fail(DET_INVALID_ARGUMENT, "det_apply: table was created with too few optimizer slot planes");

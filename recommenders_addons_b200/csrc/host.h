@@ -8,6 +8,7 @@
 #include <stdint.h>
 #include <stdlib.h>
 
+#include <atomic>
 #include <mutex>
 #include <shared_mutex>
 #include <string>
@@ -133,7 +134,40 @@ struct det_table {
   uint64_t last_used_snap = 0;       // last exact value of DevState::used the host has seen (snapshot or sync read)
   void* sparse_flag = nullptr;       // det_lookup_sparse: where the one-id-per-row flag word lives (scratch may move)
   unsigned sparse_epoch = 0;         // ... and the call counter it is compared with
+  // Slot hints (table.cu "slot hints").  `gen` advances whenever an entry point that took `mu` returns (det::MutLock),
+  // i.e. after every mutation has been enqueued; a hint written by a find at generation g is used only while gen == g.
+  std::atomic<uint64_t> gen{0};
+  std::mutex hint_mu;                 // the fields below (det_find only try_locks it: a find never waits for it)
+  long long* hint_keys = nullptr;     // device [hint_cap]: key i of the last hint-writing find
+  unsigned* hint_slots = nullptr;     // device [hint_cap]: the slot it resolved to (kNoHint: absent)
+  size_t hint_cap = 0;
+  struct {
+    const void* keys = nullptr;
+    size_t n = 0;
+    cudaStream_t stream = nullptr;
+    uint64_t gen = 0;
+    bool wrote = false;               // the find wrote hints for these keys
+    bool consumed = true;             // an insert has already matched this find
+  } last_find;
+  bool hints_armed = false;           // finds on hint_stream write hints
+  cudaStream_t hint_stream = nullptr;
+  int hint_unused = 0;                // hint-writing finds since an insert last used hints
+  cudaEvent_t hint_ev = nullptr;      // recorded after every hint-writing find
 };
+
+namespace det {
+// Lock of the mutating (and scratch-using) entry points.  Releasing it advances the table generation, which retires
+// every slot hint written before: the bump comes after the call has enqueued its kernels, so a find that read the old
+// generation may have run before them, and one that reads the new one runs after them (same stream).
+struct MutLock {
+  det_table* t;
+  std::lock_guard<std::mutex> lk;
+  explicit MutLock(det_table* t_) : t(t_), lk(t_->mu) {}
+  ~MutLock() { t->gen.fetch_add(1, std::memory_order_release); }
+  MutLock(const MutLock&) = delete;
+  MutLock& operator=(const MutLock&) = delete;
+};
+}  // namespace det
 
 namespace det {
 struct RegionLayout {

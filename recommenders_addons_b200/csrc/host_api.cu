@@ -235,7 +235,7 @@ static det_status insert_host_impl(det_table* t, const int64_t* keys, const void
   }
   // growth (if any) must happen before the chunks are in flight on several streams
   {
-    std::lock_guard<std::mutex> _lk(t->mu);
+    det::MutLock _lk(t);
     st = ensure_room(t, nullptr, n, p->streams[0]);
     if (st != DET_OK) return st;
     if (t->snap_inflight) t->n_since_snap += n;  // these keys are not covered by a snapshot already in flight

@@ -1240,7 +1240,7 @@ det_status det_peer_xchg_insert(det_peer_group* g, const int64_t* keys, const vo
   det::DevGuard _dg(g->device);
   det_status rs = peer_room(g, "det_peer_xchg_insert");
   if (rs != DET_OK) return rs;
-  std::lock_guard<std::mutex> _lk(g->local->mu);
+  det::MutLock _lk(g->local);
   xchg_time_collect(g, 1, 1);
   xchg_mark(g, 1, 0, s);
   const XchgView& xv = g->xv;

@@ -79,15 +79,28 @@ constexpr int kThreads = 256;
 #endif
 constexpr int kWarpsPerBlock = kThreads / 32;
 
+// Slot hints (host side: "slot hints" below): a find may leave {key, slot} of its key i at index i of these two arrays,
+// and the insert of the same keys that follows it then skips the probe of every key whose hint still matches.
+// keys == nullptr: no hints.
+struct SlotHints {
+  long long* keys;
+  unsigned* slots;  // kNoHint: the key was absent
+};
+constexpr unsigned kNoHint = 0xffffffffu;
+
 // K1: Find / FindWithExists with the default-row fill folded in (replaces HKV find +
 // gpu_fill_default_values, lookup_table_op_hkv.h:317-327, 719-732).  One warp-step = 32 keys.
 template <int VEC>
 __device__ __forceinline__ void find_step(const TableView& t, long long key, size_t i, bool valid,
                                           const unsigned char* __restrict__ defaults, int full_default,
                                           unsigned char* __restrict__ out, unsigned char* __restrict__ exists,
-                                          const RowGeom& g, int lane) {
+                                          const RowGeom& g, int lane, const SlotHints& h) {
   const long long slot = warp_find_slots<false>(t, key, valid, lane);
   if (exists != nullptr && valid) exists[i] = slot >= 0 ? 1 : 0;
+  if (h.keys != nullptr && valid) {
+    h.keys[i] = key;
+    h.slots[i] = slot >= 0 ? (unsigned)slot : kNoHint;
+  }
   const unsigned char* src = nullptr;
   unsigned char* dst = nullptr;
   if (valid) {
@@ -103,7 +116,7 @@ template <int VEC>
 __global__ void DET_FIND_BOUNDS
 find_kernel(TableView t, const long long* __restrict__ keys, size_t n,
             const unsigned char* __restrict__ defaults, int full_default,
-            unsigned char* __restrict__ out, unsigned char* __restrict__ exists, RowGeom g) {
+            unsigned char* __restrict__ out, unsigned char* __restrict__ exists, RowGeom g, SlotHints h) {
   const int lane = threadIdx.x & 31;
   const size_t warp0 = ((size_t)blockIdx.x * kThreads + threadIdx.x) >> 5;
   const size_t nwarps = ((size_t)gridDim.x * kThreads) >> 5;
@@ -111,7 +124,7 @@ find_kernel(TableView t, const long long* __restrict__ keys, size_t n,
     const size_t i = base + lane;
     const bool valid = i < n;
     const long long key = valid ? __ldg(keys + i) : 0;
-    find_step<VEC>(t, key, i, valid, defaults, full_default, out, exists, g, lane);
+    find_step<VEC>(t, key, i, valid, defaults, full_default, out, exists, g, lane, h);
   }
 }
 
@@ -121,7 +134,7 @@ template <int VEC>
 __global__ void DET_FIND_BOUNDS
 find_kernel_tma(TableView t, const long long* __restrict__ keys, size_t n,
                 const unsigned char* __restrict__ defaults, int full_default,
-                unsigned char* __restrict__ out, unsigned char* __restrict__ exists, RowGeom g) {
+                unsigned char* __restrict__ out, unsigned char* __restrict__ exists, RowGeom g, SlotHints h) {
   __shared__ __align__(128) long long s_keys[kStages][kTileKeys];
   __shared__ __align__(8) unsigned long long s_bar[kStages];
   const int lane = threadIdx.x & 31;
@@ -131,7 +144,7 @@ find_kernel_tma(TableView t, const long long* __restrict__ keys, size_t n,
     size_t i;
     bool valid;
     const long long key = kt.key(i, valid);
-    find_step<VEC>(t, key, i, valid, defaults, full_default, out, exists, g, lane);
+    find_step<VEC>(t, key, i, valid, defaults, full_default, out, exists, g, lane, h);
   }
 }
 
@@ -140,13 +153,25 @@ struct SlotInit {
   int n_planes;  // number of slot planes (excluding values)
 };
 
-// K2: Insert (insert_or_assign).
-template <int VEC, bool BATCH>
+// K2: Insert (insert_or_assign).  HINTED: the host has checked that no mutation was enqueued since the find that wrote
+// `h`, so a hint whose key is this lane's key gives the slot the probe would find; the other lanes probe as usual.
+template <int VEC, bool BATCH, bool HINTED>
 __device__ __forceinline__ void insert_step(const TableView& t, long long key, size_t i, bool valid,
                                             const unsigned char* __restrict__ values, const RowGeom& g,
-                                            const SlotInit& si, int lane, unsigned* s_new, unsigned* s_used) {
+                                            const SlotInit& si, int lane, unsigned* s_new, unsigned* s_used,
+                                            const SlotHints& h) {
+  bool hinted = false;
+  unsigned hslot = kNoHint;
+  if (HINTED && valid) {
+    hslot = h.slots[i];
+    hinted = hslot != kNoHint && h.keys[i] == key;
+  }
+#ifdef DET_EMU
+  if (hinted) __atomic_fetch_add(&g_det_emu_stat[3], 1ull, __ATOMIC_RELAXED);
+#endif
   bool is_new, from_empty;
-  const long long slot = warp_find_or_claim_v<BATCH>(t, key, valid, valid, lane, is_new, from_empty);
+  long long slot = warp_find_or_claim_v<BATCH>(t, key, valid && !hinted, valid && !hinted, lane, is_new, from_empty);
+  if (hinted) slot = (long long)hslot;
   const unsigned bn = __ballot_sync(kFull, is_new), bu = __ballot_sync(kFull, from_empty);
   if (lane == 0 && bn) {
     atomicAdd(s_new, __popc(bn));
@@ -167,10 +192,10 @@ __device__ __forceinline__ void insert_step(const TableView& t, long long key, s
       *reinterpret_cast<unsigned*>(t.planes[p] + (size_t)slot * t.dim * 4u) = kSlotUninit;
 }
 
-template <int VEC, bool BATCH = false>
+template <int VEC, bool BATCH = false, bool HINTED = false>
 __global__ void DET_INSERT_BOUNDS
 insert_kernel(TableView t, const long long* __restrict__ keys, const unsigned char* __restrict__ values,
-              size_t n, RowGeom g, SlotInit si) {
+              size_t n, RowGeom g, SlotInit si, SlotHints h) {
   __shared__ unsigned s_new, s_used;
   if (threadIdx.x == 0) {
     s_new = 0;
@@ -184,7 +209,7 @@ insert_kernel(TableView t, const long long* __restrict__ keys, const unsigned ch
     const size_t i = base + lane;
     const bool valid = i < n;
     const long long key = valid ? __ldg(keys + i) : 0;
-    insert_step<VEC, BATCH>(t, key, i, valid, values, g, si, lane, &s_new, &s_used);
+    insert_step<VEC, BATCH, HINTED>(t, key, i, valid, values, g, si, lane, &s_new, &s_used, h);
   }
   __syncthreads();
   if (threadIdx.x == 0 && s_new) {
@@ -193,10 +218,10 @@ insert_kernel(TableView t, const long long* __restrict__ keys, const unsigned ch
   }
 }
 
-template <int VEC, bool BATCH = false>
+template <int VEC, bool BATCH = false, bool HINTED = false>
 __global__ void DET_INSERT_BOUNDS
 insert_kernel_tma(TableView t, const long long* __restrict__ keys, const unsigned char* __restrict__ values,
-                  size_t n, RowGeom g, SlotInit si) {
+                  size_t n, RowGeom g, SlotInit si, SlotHints h) {
   __shared__ __align__(128) long long s_keys[kStages][kTileKeys];
   __shared__ __align__(8) unsigned long long s_bar[kStages];
   __shared__ unsigned s_new, s_used;
@@ -211,7 +236,7 @@ insert_kernel_tma(TableView t, const long long* __restrict__ keys, const unsigne
     size_t i;
     bool valid;
     const long long key = kt.key(i, valid);
-    insert_step<VEC, BATCH>(t, key, i, valid, values, g, si, lane, &s_new, &s_used);
+    insert_step<VEC, BATCH, HINTED>(t, key, i, valid, values, g, si, lane, &s_new, &s_used, h);
   }
   __syncthreads();
   if (threadIdx.x == 0 && s_new) {
@@ -844,6 +869,9 @@ det_status rehash_to(det_table* t, uint64_t new_nb, cudaStream_t s) {
   for (int i = 0; i < 1 + kMaxPlanes; ++i) t->raw[i] = raw[i];
   t->view = nv;
   t->rehash_count++;
+  // every slot has moved: retire the slot hints now, not only when the caller's MutLock is released (an insert that
+  // grew the table in its ensure_room checks them next)
+  t->gen.fetch_add(1, std::memory_order_release);
   return DET_OK;
 }
 
@@ -1000,6 +1028,104 @@ SlotInit slot_init_of(const det_table* t) {
   return si;
 }
 
+// ---- slot hints -------------------------------------------------------------------------------------------------
+// The training step of every optimizer that is not fused is find(ids) -> dense rule -> insert(ids): the insert probes
+// for the same keys the find has just probed, and by then the buckets have long left L2.  Once an insert has followed
+// a find of the same (keys pointer, n, stream), the finds of the table on that stream record {key, slot} per key; an
+// insert that matches the last find, with no mutation of the table in between (generation unchanged), uses them and
+// probes only the keys whose hint is absent or no longer names its key (the key buffer was rewritten in place).
+// Finds stop recording after kHintIdleFinds finds that no insert used (a training step uses its find's hints at once;
+// lookups that follow training, e.g. evaluation, stop paying the ~2 % of hint writes after two finds).  DET_SLOT_HINTS=0
+// turns hints off.
+constexpr int kHintIdleFinds = 2;
+
+// Tables whose key plane other processes or GPUs write (peer shards), whose inserts go through the eviction path, and
+// slot indices that do not fit the 32-bit hint take no hints.
+static bool hints_allowed(const det_table* t) {
+  return t->ev == nullptr && t->peer_bar == nullptr && t->view.capacity() + 2 < (unsigned long long)kNoHint;
+}
+
+static bool stream_capturing(cudaStream_t s) {
+#ifdef DET_EMU
+  (void)s;
+  return false;
+#else
+  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+  if (cudaStreamIsCapturing(s, &cs) != cudaSuccess) {
+    cudaGetLastError();
+    return true;  // e.g. the legacy stream while another stream captures: leave it alone
+  }
+  return cs != cudaStreamCaptureStatusNone;
+#endif
+}
+
+// det_find, with hint_mu held: record this find and return where it writes hints (none unless armed for this stream)
+static SlotHints find_hints(det_table* t, const void* keys, size_t n, cudaStream_t s) {
+  bool write = t->hints_armed && s == t->hint_stream && n <= t->hint_cap;
+  if (write && t->hint_unused >= kHintIdleFinds) {
+    t->hints_armed = false;
+    write = false;
+  }
+  if (write) ++t->hint_unused;
+  auto& r = t->last_find;
+  r.keys = keys;
+  r.n = n;
+  r.stream = s;
+  r.gen = t->gen.load(std::memory_order_acquire);
+  r.wrote = write;
+  r.consumed = false;
+  return write ? SlotHints{t->hint_keys, t->hint_slots} : SlotHints{nullptr, nullptr};
+}
+
+// insert_impl, with t->mu held: the hints of the last find if this insert may use them.  An insert of the keys of a
+// find that wrote none arms the hints for this stream (and grows the buffer: the only allocation of the scheme).
+static SlotHints insert_hints(det_table* t, const void* keys, size_t n, cudaStream_t s) {
+  std::lock_guard<std::mutex> hl(t->hint_mu);
+  auto& r = t->last_find;
+  if (r.consumed || r.keys != keys || r.n != n || r.stream != s) return SlotHints{nullptr, nullptr};
+  r.consumed = true;  // one find gives at most one hinted insert
+  if (env_int("DET_SLOT_HINTS", 1) == 0 || !hints_allowed(t) || stream_capturing(s)) {
+    t->hints_armed = false;
+    return SlotHints{nullptr, nullptr};
+  }
+  if (r.wrote) {
+    if (r.gen != t->gen.load(std::memory_order_acquire)) return SlotHints{nullptr, nullptr};
+    t->hint_unused = 0;
+    return SlotHints{t->hint_keys, t->hint_slots};
+  }
+  // arm.  Hint writers stay on one stream at a time: a switch waits until the last hint-writing find has completed.
+  if (s != t->hint_stream && cudaEventQuery(t->hint_ev) != cudaSuccess) {
+    cudaGetLastError();
+    return SlotHints{nullptr, nullptr};
+  }
+  if (n > t->hint_cap) {
+    if (t->hint_keys) {
+      if (cudaDeviceSynchronize() != cudaSuccess) {
+        cudaGetLastError();
+        return SlotHints{nullptr, nullptr};
+      }
+      cudaFree(t->hint_keys);
+      t->hint_keys = nullptr;
+      t->hint_slots = nullptr;
+      t->hint_cap = 0;
+    }
+    const size_t want = n + (n >> 2) + 1024;
+    void* p = nullptr;
+    if (cudaMalloc(&p, want * (sizeof(long long) + sizeof(unsigned))) != cudaSuccess) {
+      cudaGetLastError();  // no room for hints: the table works without them
+      t->hints_armed = false;
+      return SlotHints{nullptr, nullptr};
+    }
+    t->hint_keys = (long long*)p;
+    t->hint_slots = (unsigned*)(t->hint_keys + want);
+    t->hint_cap = want;
+  }
+  t->hints_armed = true;
+  t->hint_stream = s;
+  t->hint_unused = 0;
+  return SlotHints{nullptr, nullptr};
+}
+
 }  // namespace det
 
 using namespace det;
@@ -1083,6 +1209,7 @@ static det_status create_common(det_table** out, const det_config* cfg, void* re
   cudaError_t e = cudaMallocHost((void**)&t->h_state, sizeof(DevState));
   if (e == cudaSuccess) e = cudaMallocHost((void**)&t->h_used_snap, sizeof(unsigned long long));
   if (e == cudaSuccess) e = cudaEventCreateWithFlags(&t->snap_ev, cudaEventDisableTiming);
+  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&t->hint_ev, cudaEventDisableTiming);
   if (e == cudaSuccess && region == nullptr) e = cudaMalloc((void**)&t->view.st, sizeof(DevState));
   if (e != cudaSuccess) {
     cudaGetLastError();
@@ -1163,6 +1290,8 @@ det_status det_table_destroy(det_table* t) {
   if (t->h_state) cudaFreeHost(t->h_state);
   if (t->h_used_snap) cudaFreeHost(t->h_used_snap);
   if (t->snap_ev) cudaEventDestroy(t->snap_ev);
+  if (t->hint_ev) cudaEventDestroy(t->hint_ev);
+  if (t->hint_keys) cudaFree(t->hint_keys);
   if (t->scratch) cudaFree(t->scratch);
   host_pipe_free(t);
   evict_free(t);
@@ -1181,6 +1310,11 @@ det_status det_find(det_table* t, const int64_t* keys, size_t n, const void* def
   const RowGeom g = make_geom((unsigned)t->row_bytes, vec);
   std::shared_lock<std::shared_mutex> _vl(t->view_mu);   // vs a concurrent growth on another host thread (host.h)
   const TableView v = t->view;
+  // slot hints: bookkeeping only when the hint lock is free right now (a find never waits) and the stream is not
+  // being captured into a graph
+  std::unique_lock<std::mutex> hl(t->hint_mu, std::try_to_lock);
+  const bool track = hl.owns_lock() && hints_allowed(t) && !stream_capturing(s);
+  const SlotHints h = track ? find_hints(t, keys, n, s) : SlotHints{nullptr, nullptr};
   // variant 1 (default): persistent CTAs + TMA-staged key tiles; needs 16 B aligned keys.  DET_FIND_VARIANT=0
   // selects the plain grid-stride kernel.
   static const int variant = env_int("DET_FIND_VARIANT", 1);
@@ -1190,13 +1324,14 @@ det_status det_find(det_table* t, const int64_t* keys, size_t n, const void* def
     if (tma) {
       const int grid = grid_for(n, kTileKeys, t->sm_count, occupancy_of(find_kernel_tma<VV>, kThreads));
       DET_LAUNCH(find_kernel_tma<VV>, grid, kThreads, 0, s, v, (const long long*)keys, n, (const unsigned char*)defaults,
-                                                    full_size_default, (unsigned char*)values_out, exists, g);
+                                                    full_size_default, (unsigned char*)values_out, exists, g, h);
     } else {
       const int grid = grid_for(n, kThreads, t->sm_count, occupancy_of(find_kernel<VV>, kThreads));
       DET_LAUNCH(find_kernel<VV>, grid, kThreads, 0, s, v, (const long long*)keys, n, (const unsigned char*)defaults,
-                                                full_size_default, (unsigned char*)values_out, exists, g);
+                                                full_size_default, (unsigned char*)values_out, exists, g, h);
     }
     CUDA_TRY(cudaGetLastError());
+    if (h.keys != nullptr) CUDA_TRY(cudaEventRecord(t->hint_ev, s));
     return DET_OK;
   });
 }
@@ -1212,7 +1347,7 @@ namespace det {
 det_status insert_impl(det_table* t, const int64_t* keys, const void* values, size_t n, cudaStream_t s,
                        bool check_room) {
   if (!t) return fail(DET_INVALID_ARGUMENT, "det_insert: null table");
-  std::lock_guard<std::mutex> _lk(t->mu);
+  det::MutLock _lk(t);
   if (n == 0) return DET_OK;
   if (!keys || !values) return fail(DET_INVALID_ARGUMENT, "det_insert: null keys/values");
   det::DevGuard _dg(t->cfg.device);
@@ -1224,6 +1359,9 @@ det_status insert_impl(det_table* t, const int64_t* keys, const void* values, si
   const RowGeom g = make_geom((unsigned)t->row_bytes, vec);
   const TableView v = t->view;
   const SlotInit si = slot_init_of(t);
+  // after ensure_room: a growth it triggered has advanced the generation.  The chunks of det_insert_host run on
+  // several streams of their own and take no hints.
+  const SlotHints h = check_room ? insert_hints(t, keys, n, s) : SlotHints{nullptr, nullptr};
   static const int variant = env_int("DET_INSERT_VARIANT", 1);
   const bool tma = variant == 1 && (((uintptr_t)keys & 15u) == 0);
   return dispatch_vec(vec, [&](auto V) -> det_status {
@@ -1231,11 +1369,13 @@ det_status insert_impl(det_table* t, const int64_t* keys, const void* values, si
     // DET_CLAIM_BATCH=1: the batched-claim probe (common.cuh), a round-2 candidate for inserts of NEW keys; the
     // default is the validated serial claim
     const bool batch = env_int("DET_CLAIM_BATCH", 0) != 0;
-    using KernelFn = void (*)(TableView, const long long*, const unsigned char*, size_t, RowGeom, SlotInit);
-    const KernelFn kfn = tma ? (batch ? (KernelFn)insert_kernel_tma<VV, true> : (KernelFn)insert_kernel_tma<VV, false>)
-                             : (batch ? (KernelFn)insert_kernel<VV, true> : (KernelFn)insert_kernel<VV, false>);
+    using KernelFn = void (*)(TableView, const long long*, const unsigned char*, size_t, RowGeom, SlotInit, SlotHints);
+    KernelFn kfn = tma ? (batch ? (KernelFn)insert_kernel_tma<VV, true> : (KernelFn)insert_kernel_tma<VV, false>)
+                       : (batch ? (KernelFn)insert_kernel<VV, true> : (KernelFn)insert_kernel<VV, false>);
+    if (h.keys != nullptr && !batch)
+      kfn =tma ? (KernelFn)insert_kernel_tma<VV, false, true> : (KernelFn)insert_kernel<VV, false, true>;
     const int grid = grid_for(n, tma ? kTileKeys : kThreads, t->sm_count, occupancy_of(kfn, kThreads));
-    DET_LAUNCH(kfn, grid, kThreads, 0, s, v, (const long long*)keys, (const unsigned char*)values, n, g, si);
+    DET_LAUNCH(kfn, grid, kThreads, 0, s, v, (const long long*)keys, (const unsigned char*)values, n, g, si, h);
     CUDA_TRY(cudaGetLastError());
     if (check_room) note_mutation(t, n, s);
     return DET_OK;
@@ -1249,7 +1389,7 @@ static det_status accum_impl(det_table* t, const int64_t* keys, const void* vod,
                              const uint64_t* scores, size_t n, det_stream_t stream) {
   if (!t) return fail(DET_INVALID_ARGUMENT, "det_accum: null table");
   if (scores && !t->ev) return fail(DET_INVALID_ARGUMENT, "det_accum_scored: the table was created without an eviction strategy");
-  std::lock_guard<std::mutex> _lk(t->mu);
+  det::MutLock _lk(t);
   if (n == 0) return DET_OK;
   if (!keys || !vod || !exists) return fail(DET_INVALID_ARGUMENT, "det_accum: null keys/values_or_deltas/exists");
   cudaStream_t s = (cudaStream_t)stream;
@@ -1292,7 +1432,7 @@ det_status det_accum_scored(det_table* t, const int64_t* keys, const void* vod, 
 
 det_status det_remove(det_table* t, const int64_t* keys, size_t n, det_stream_t stream) {
   if (!t) return fail(DET_INVALID_ARGUMENT, "det_remove: null table");
-  std::lock_guard<std::mutex> _lk(t->mu);
+  det::MutLock _lk(t);
   if (n == 0) return DET_OK;
   if (!keys) return fail(DET_INVALID_ARGUMENT, "det_remove: null keys");
   cudaStream_t s = (cudaStream_t)stream;
@@ -1308,7 +1448,7 @@ det_status det_remove(det_table* t, const int64_t* keys, size_t n, det_stream_t 
 
 det_status det_clear(det_table* t, det_stream_t stream) {
   if (!t) return fail(DET_INVALID_ARGUMENT, "det_clear: null table");
-  std::lock_guard<std::mutex> _lk(t->mu);
+  det::MutLock _lk(t);
   det::DevGuard _dg(t->cfg.device);
   return table_clear_async(t, (cudaStream_t)stream);
 }
@@ -1332,7 +1472,7 @@ det_status det_capacity(det_table* t, uint64_t* out) {
 
 det_status det_reserve(det_table* t, uint64_t total_keys, det_stream_t stream) {
   if (!t) return fail(DET_INVALID_ARGUMENT, "det_reserve: null table");
-  std::lock_guard<std::mutex> _lk(t->mu);
+  det::MutLock _lk(t);
   det::DevGuard _dg(t->cfg.device);
   const uint64_t limit = (uint64_t)((double)t->view.capacity() * t->max_lf);
   if (total_keys <= limit) return DET_OK;
@@ -1353,7 +1493,7 @@ det_status det_reserve(det_table* t, uint64_t total_keys, det_stream_t stream) {
 det_status det_export_window(det_table* t, int plane, uint64_t first, int64_t* keys_out, void* values_out,
                              size_t max_n, int64_t* n_out_host, det_stream_t stream) {
   if (!t || !n_out_host) return fail(DET_INVALID_ARGUMENT, "det_export: null argument");
-  std::lock_guard<std::mutex> _lk(t->mu);
+  det::MutLock _lk(t);
   if (plane < 0 || plane > t->cfg.num_slot_planes) return fail(DET_INVALID_ARGUMENT, "det_export: bad plane");
   cudaStream_t s = (cudaStream_t)stream;
   det::DevGuard _dg(t->cfg.device);
@@ -1401,7 +1541,7 @@ det_status det_export(det_table* t, int plane, int64_t* keys_out, void* values_o
 det_status det_import_plane(det_table* t, int plane, const int64_t* keys, const float* rows, size_t n,
                             det_stream_t stream) {
   if (!t) return fail(DET_INVALID_ARGUMENT, "det_import_plane: null table");
-  std::lock_guard<std::mutex> _lk(t->mu);
+  det::MutLock _lk(t);
   if (plane < 1 || plane > t->cfg.num_slot_planes)
     return fail(DET_INVALID_ARGUMENT, "det_import_plane: plane must be one of the table's optimizer slot planes (1.." +
                                           std::to_string(t->cfg.num_slot_planes) + ")");
