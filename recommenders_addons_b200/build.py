@@ -38,7 +38,7 @@ def needs_build():
 
 
 def _extra_flags():
-  """DET_NVCC_EXTRA="-DDET_FIND_MINB=5 ...": extra nvcc flags for measurement builds"""
+  """DET_NVCC_EXTRA="-Xptxas -v ...": extra nvcc flags for measurement builds"""
   return os.environ.get("DET_NVCC_EXTRA", "").split()
 
 

@@ -68,22 +68,13 @@ __device__ __forceinline__ bool is_special(long long key) { return key == kEmpty
 
 // ---- memory access flavours -----------------------------------------------------------------
 // L2-coherent 16 B load of two keys (mutating kernels: L1 may hold lines older than a peer's CAS)
-// Measurement builds may put an L2 prefetch-size qualifier on the bucket loads (-DDET_KEY_L2=64 -> ".L2::64B"): the L2
-// may fill whole 128 B lines for these 64 B bucket probes.  Undefined = the validated default (no qualifier).
-#define DET_STR2(x) #x
-#define DET_STR(x) DET_STR2(x)
-#ifdef DET_KEY_L2
-#define DET_KEY_L2_QUAL ".L2::" DET_STR(DET_KEY_L2) "B"
-#else
-#define DET_KEY_L2_QUAL ""
-#endif
 __device__ __forceinline__ longlong2 ld_keys_cg(const long long* p) {
   longlong2 r;
 #ifdef DET_EMU
   r.x = __atomic_load_n(p, __ATOMIC_RELAXED);
   r.y = __atomic_load_n(p + 1, __ATOMIC_RELAXED);
 #else
-  asm volatile("ld.global.cg" DET_KEY_L2_QUAL ".v2.s64 {%0, %1}, [%2];" : "=l"(r.x), "=l"(r.y) : "l"(p));
+  asm volatile("ld.global.cg.v2.s64 {%0, %1}, [%2];" : "=l"(r.x), "=l"(r.y) : "l"(p));
 #endif
   return r;
 }
@@ -94,7 +85,7 @@ __device__ __forceinline__ longlong2 ld_keys_nc(const long long* p) {
   r.x = p[0];
   r.y = p[1];
 #else
-  asm volatile("ld.global.nc" DET_KEY_L2_QUAL ".v2.s64 {%0, %1}, [%2];" : "=l"(r.x), "=l"(r.y) : "l"(p));
+  asm volatile("ld.global.nc.v2.s64 {%0, %1}, [%2];" : "=l"(r.x), "=l"(r.y) : "l"(p));
 #endif
   return r;
 }
@@ -411,190 +402,11 @@ __device__ __forceinline__ long long warp_find_or_claim_t(const TabRef& my, long
   return result;
 }
 
-// Batched-claim variant (candidate for round 2, selected by DET_CLAIM_BATCH=1 in the insert kernels; the default
-// stays the validated primitive above).  Insert of NEW keys is latency-bound: the
-// primitive above resolves its 4 rounds one after the other and every round that creates a key waits for its own
-// CAS round trip.  Here the 4 rounds are probed first WITHOUT claiming (phase A: found slot, or the first free slot
-// of the chain), then lane r of every subgroup issues the CAS of round r, so up to 4 claims per subgroup are in
-// flight together (phase B: one atomic round trip instead of four).  A claim that lost its slot to another key
-// (another warp, or another round of this warp that chose the same free slot) is simply left PENDING and resolved by
-// the serial primitive, which re-probes with fresh L2-coherent loads -- rare, and exactly the validated protocol.
 #ifdef DET_EMU
-// emulator-only counters (tests/test_detable_emu.py checks that the candidate path and its fallback really ran)
-extern "C" unsigned long long g_det_emu_stat[4];   // [0] warp-steps through the batched claim, [1] ... with a pending key, [2] staged segment-sum launches
+// emulator-only counter (tests/test_slot_hints_emu.py reads it as det_emu_stat(3)): lanes of insert kernels that
+// took a slot hint
+extern "C" unsigned long long g_det_emu_hint_lanes;
 #endif
-
-template <bool MULTI>
-__device__ __forceinline__ long long warp_find_or_claim_batched_t(const TabRef& my, long long mykey, bool valid,
-                                                                  bool claim, int lane, bool& is_new,
-                                                                  bool& from_empty) {
-  const int sg = lane >> 2, sl = lane & 3;
-  const bool special = is_special(mykey);
-  const unsigned long long myb = bucket_of(mykey, my.nb);
-  const bool probe_me = valid && !special;
-
-  longlong2 first[4];
-  long long* kbr[4];
-  unsigned long long nbr[4];
-#pragma unroll
-  for (int r = 0; r < 4; ++r) {
-    const int src = r * 8 + sg;
-    const unsigned long long b0 = (unsigned long long)shfl_ll((long long)myb, src);
-    const bool act = __shfl_sync(kFull, (int)probe_me, src) != 0;
-    if (MULTI) {
-      kbr[r] = (long long*)shfl_ll((long long)my.keys, src);
-      nbr[r] = (unsigned long long)shfl_ll((long long)my.nb, src);
-    } else {
-      kbr[r] = my.keys;
-      nbr[r] = my.nb;
-    }
-    first[r] = make_longlong2(0, 0);
-    if (act) first[r] = ld_keys_cg(kbr[r] + b0 * kBucket + sl * 2);
-  }
-  // phase A: probe, no claims.  Per round (identical in the 4 lanes of a subgroup): found slot, or free slot to claim
-  long long foundr[4], freer[4];
-  bool tombr[4], casr[4];
-#pragma unroll
-  for (int r = 0; r < 4; ++r) {
-    const int src = r * 8 + sg;
-    const long long key = shfl_ll(mykey, src);
-    bool active = __shfl_sync(kFull, (int)probe_me, src) != 0;
-    const bool may_claim = __shfl_sync(kFull, (int)claim, src) != 0;
-    long long* const kb = kbr[r];
-    const unsigned long long nb = nbr[r];
-    unsigned long long b = (unsigned long long)shfl_ll((long long)myb, src);
-    long long found = -1, first_free = -1;
-    bool ff_tomb = false, want = false;
-    unsigned long long probes = 0;
-    bool use_first = true;
-    while (__any_sync(kFull, active)) {
-      longlong2 kk = first[r];
-      if (active && !use_first) kk = ld_keys_cg(kb + b * kBucket + sl * 2);
-      use_first = false;
-      const unsigned bh0 = __ballot_sync(kFull, active && kk.x == key);
-      const unsigned bh1 = __ballot_sync(kFull, active && kk.y == key);
-      const unsigned be0 = __ballot_sync(kFull, active && kk.x == kEmptyKey);
-      const unsigned be1 = __ballot_sync(kFull, active && kk.y == kEmptyKey);
-      const unsigned bt0 = __ballot_sync(kFull, active && kk.x == kTombKey);
-      const unsigned bt1 = __ballot_sync(kFull, active && kk.y == kTombKey);
-      if (active) {
-        const unsigned H = mask8(bh0, bh1, sg);
-        const unsigned E = mask8(be0, be1, sg);
-        const unsigned T = mask8(bt0, bt1, sg);
-        if (H) {
-          found = (long long)(b * kBucket) + (__ffs(H) - 1);
-          active = false;
-        } else {
-          const unsigned F = E | T;
-          if (first_free < 0 && F) {
-            const int f = __ffs(F) - 1;
-            first_free = (long long)(b * kBucket) + f;
-            ff_tomb = ((T >> f) & 1u) != 0;
-          }
-          ++probes;
-          if (E || probes >= nb) {   // end of the chain: the key is absent
-            if (may_claim) {
-              if (first_free < 0) {
-                if (MULTI) atomicOr_system(&my.st->error, kErrTableFull); else atomicOr(&my.st->error, kErrTableFull);
-              } else {
-                want = true;
-              }
-            }
-            active = false;
-          } else {
-            b = (b + 1 == nb) ? 0 : b + 1;
-          }
-        }
-      }
-    }
-    foundr[r] = found;
-    freer[r] = first_free;
-    tombr[r] = ff_tomb;
-    casr[r] = want;
-  }
-  // phase B: lane r of the subgroup claims for round r -- the (up to) 4 atomics of a subgroup overlap
-  long long my_old = 0;
-  long long keyr[4];   // shuffles are executed by every lane: fetch the 4 keys first, then branch
-#pragma unroll
-  for (int r = 0; r < 4; ++r) keyr[r] = shfl_ll(mykey, r * 8 + sg);
-#pragma unroll
-  for (int r = 0; r < 4; ++r) {
-    if (sl == r && casr[r]) {
-      const long long expect = tombr[r] ? kTombKey : kEmptyKey;
-      unsigned long long* addr = (unsigned long long*)(kbr[r] + freer[r]);
-      my_old = MULTI ? (long long)atomicCAS_system(addr, (unsigned long long)expect, (unsigned long long)keyr[r])
-                     : (long long)atomicCAS(addr, (unsigned long long)expect, (unsigned long long)keyr[r]);
-    }
-  }
-  // phase C: outcome per round, handed to the lane that owns the key (lane r*8 + sg <- lane sg*4)
-  long long result = -1;
-  bool res_new = false, res_empty = false, pending = false;
-#pragma unroll
-  for (int r = 0; r < 4; ++r) {
-    const long long old = shfl_ll(my_old, sg * 4 + r);
-    long long found = foundr[r];
-    bool fnew = false, fempty = false, pend = false;
-    if (casr[r]) {
-      const long long expect = tombr[r] ? kTombKey : kEmptyKey;
-      if (old == expect) {
-        found = freer[r];
-        fnew = true;
-        fempty = !tombr[r];
-      } else if (old == keyr[r]) {
-        found = freer[r];  // a duplicate of this key won the race
-      } else {
-        pend = true;       // the slot went to another key: re-probe with the serial primitive
-      }
-    }
-    const long long v = shfl_ll(found, (lane & 7) * 4);
-    const int vn = __shfl_sync(kFull, (int)fnew | ((int)fempty << 1) | ((int)pend << 2), (lane & 7) * 4);
-    if ((lane >> 3) == r) {
-      result = v;
-      res_new = (vn & 1) != 0;
-      res_empty = (vn & 2) != 0;
-      pending = (vn & 4) != 0;
-    }
-  }
-#ifdef DET_EMU
-  if (lane == 0) __atomic_fetch_add(&g_det_emu_stat[0], 1ull, __ATOMIC_RELAXED);
-#endif
-  if (__any_sync(kFull, pending)) {
-#ifdef DET_EMU
-    if (lane == 0) __atomic_fetch_add(&g_det_emu_stat[1], 1ull, __ATOMIC_RELAXED);
-#endif
-    bool n2 = false, e2 = false;
-    const long long s2 = warp_find_or_claim_t<MULTI>(my, mykey, pending, pending, lane, n2, e2);
-    if (pending) {
-      result = s2;
-      res_new = n2;
-      res_empty = e2;
-    }
-  }
-  if (valid && special) {
-    const int idx = (mykey == kTombKey) ? 1 : 0;
-    const long long s = (long long)(my.nb * kBucket + idx);
-    if (claim) {
-      const unsigned old = MULTI ? atomicExch_system(&my.st->special[idx], 1u) : atomicExch(&my.st->special[idx], 1u);
-      result = s;
-      res_new = (old == 0);
-      res_empty = false;
-    } else {
-      const unsigned present = *((volatile unsigned*)&my.st->special[idx]);
-      result = present ? s : -1;
-    }
-  }
-  is_new = res_new;
-  from_empty = res_empty;
-  return result;
-}
-
-template <bool BATCH>
-__device__ __forceinline__ long long warp_find_or_claim_v(const TableView& t, long long mykey, bool valid, bool claim,
-                                                          int lane, bool& is_new, bool& from_empty) {
-  const TabRef my = {t.keys, t.nb, t.st};
-  if (BATCH) return warp_find_or_claim_batched_t<false>(my, mykey, valid, claim, lane, is_new, from_empty);
-  return warp_find_or_claim_t<false>(my, mykey, valid, claim, lane, is_new, from_empty);
-}
 
 __device__ __forceinline__ long long warp_find_or_claim(const TableView& t, long long mykey, bool valid,
                                                         bool claim, int lane, bool& is_new,

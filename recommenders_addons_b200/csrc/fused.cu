@@ -302,14 +302,9 @@ template <> struct FVec<1> {
 
 constexpr int kMaxVecPerLane = 8;
 // segments a lane-group works on concurrently (independent load chains) and the resident CTAs per SM the register
-// budget is capped for; measurement builds override them (-DDET_SEG_U=8 -DDET_SEG_MINB=2)
-#ifndef DET_SEG_U
-#define DET_SEG_U 4
-#endif
-#ifndef DET_SEG_MINB
-#define DET_SEG_MINB 3
-#endif
-constexpr int kSegPerGroup = DET_SEG_U;
+// budget is capped for
+constexpr int kSegPerGroup = 4;
+constexpr int kSegMinBlocks = 3;
 
 // K6 phase B, common case (one vector per lane covers the row): each lane-group owns kSegPerGroup
 // consecutive output rows and walks their ids in lock step, so up to 4 independent row loads are in flight
@@ -323,7 +318,7 @@ template <bool CLIP> __device__ __forceinline__ float clip_norm_of(const ClipArg
 template <> __device__ __forceinline__ float clip_norm_of<true>(const ClipArg<true>& c) { return c.max_norm; }
 
 template <int VF, bool CLIP = false>
-__global__ void __launch_bounds__(kThreadsF, DET_SEG_MINB)
+__global__ void __launch_bounds__(kThreadsF, kSegMinBlocks)
 segment_sum_kernel(TableView t, const long long* __restrict__ slots, const long long* __restrict__ seg_start,
                    const float* __restrict__ weights, size_t batch, int combiner,
                    const float* __restrict__ default_row, float* __restrict__ out, unsigned vpr, unsigned lpr,
@@ -411,158 +406,6 @@ segment_sum_kernel(TableView t, const long long* __restrict__ slots, const long 
   }
 }
 
-// K6 phase B, staged variant (DET_SEGSUM_STAGED=1; a round-2 candidate, default off): the register-held kernel above
-// keeps kSegPerGroup 16 B loads in flight per lane and cannot go further (8 segments spill or drop to one CTA per
-// SM).  Here every warp owns a CONTIGUOUS range
-// of output rows, so the ids it needs are one contiguous stretch of `slots`: the warp streams that stretch through a
-// 3-stage ring of shared memory in windows of kWinSteps row-steps with cp.async (LDGSTS: up to two windows = 4 KB per
-// warp in flight, no registers held), and sums window k while k+1 and k+2 are loading.  A segment always belongs to the
-// same lane-group (segment index mod groups per warp), which adds its rows strictly in id order and carries the partial
-// sum across windows -- the arithmetic, its order and the results are those of segment_sum_kernel.
-// Requires VF == 4 rows of one vector per lane (dim % 4 == 0, dim <= 128).
-constexpr int kWinSteps = 4;   // row-steps per window: 4 x 32 lanes x 16 B = 2 KB
-constexpr int kWinStages = 3;
-constexpr int kWinFloat4 = kWinSteps * 32;                       // float4 per stage
-constexpr int kWinStageBytes = kWinFloat4 * 16 + 32 * 4;         // rows + one weight per staged row
-constexpr int kWinWarpBytes = kWinStages * kWinStageBytes;
-
-__global__ void __launch_bounds__(kThreadsF)
-segment_sum_staged_kernel(TableView t, const long long* __restrict__ slots, const long long* __restrict__ seg_start,
-                          const float* __restrict__ weights, size_t batch, int combiner,
-                          const float* __restrict__ default_row, float* __restrict__ out, unsigned vpr, unsigned lpr,
-                          unsigned lpr_shift) {
-  DET_DYN_SHARED(dyn_smem);
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const unsigned gl = (unsigned)lane & (lpr - 1u);
-  const unsigned gpw = 32u >> lpr_shift;          // lane-groups per warp = rows per row-step
-  const unsigned gidx = (unsigned)lane >> lpr_shift;
-  const unsigned gsh = 5u - lpr_shift;            // log2(gpw)
-  const unsigned wsteps = gpw * (unsigned)kWinSteps > 32u ? 32u / gpw : (unsigned)kWinSteps;
-  const unsigned W = wsteps * gpw;                // rows per window (<= 32: lane r holds the slot of row r)
-  const unsigned dim = t.dim;
-  const bool lane_on = gl < vpr;
-  const float* table = (const float*)t.planes[0];
-  unsigned char* wbase = dyn_smem + (size_t)warp * kWinWarpBytes;
-  auto s_row = [&](int stage) -> float4* { return reinterpret_cast<float4*>(wbase + (size_t)stage * kWinStageBytes); };
-  auto s_wt = [&](int stage) -> float* { return reinterpret_cast<float*>(wbase + (size_t)stage * kWinStageBytes + kWinFloat4 * 16); };
-  // this warp's contiguous range of segments [S0, S1)
-  const size_t nwarps = ((size_t)gridDim.x * kThreadsF) >> 5;
-  const size_t spw = (batch + nwarps - 1) / nwarps;
-  const size_t S0 = ((((size_t)blockIdx.x * kThreadsF) >> 5) + (size_t)warp) * spw;
-  if (S0 >= batch) return;
-  const size_t S1 = S0 + spw < batch ? S0 + spw : batch;
-  const unsigned nseg = (unsigned)(S1 - S0);
-  const long long p_begin = seg_start[S0], p_end = seg_start[S1];
-  const unsigned npos = (unsigned)(p_end - p_begin);
-  const unsigned nwin = npos ? (npos + W - 1) / W : 1u;   // an empty range still flushes its (empty) segments
-  // segment boundaries relative to p_begin, 64 at a time: lane i of b_lo holds boundary c*32 + i, b_hi the next 32
-  auto load_bounds = [&](unsigned first) -> unsigned {
-    const unsigned i = first + (unsigned)lane;
-    return (unsigned)(seg_start[S0 + (i < nseg ? i : nseg)] - p_begin);
-  };
-  unsigned chunk = 0;
-  unsigned b_lo = load_bounds(0), b_hi = load_bounds(32);
-  auto bound = [&](unsigned i) -> unsigned {    // boundary i, chunk*32 <= i < chunk*32 + 64; warp-uniform call
-    const unsigned o = i - chunk * 32u;
-    const unsigned lo = __shfl_sync(kFull, b_lo, (int)(o & 31u)), hi = __shfl_sync(kFull, b_hi, (int)(o & 31u));
-    return o < 32u ? lo : hi;
-  };
-  // producer: the slot of row `lane` of a window, then the cp.async copies of the window
-  auto load_slot = [&](unsigned k) -> long long {
-    const unsigned r = k * W + (unsigned)lane;
-    return (k < nwin && (unsigned)lane < W && r < npos) ? __ldg(slots + p_begin + r) : -1;
-  };
-  auto issue = [&](unsigned k, long long sl_of_lane) {
-    const int stage = (int)(k % (unsigned)kWinStages);
-    const unsigned w0 = k * W;
-#pragma unroll
-    for (int stp = 0; stp < kWinSteps; ++stp) {
-      const unsigned r = (unsigned)stp * gpw + gidx;
-      const long long sl = shfl_ll(sl_of_lane, (int)r);
-      if ((unsigned)stp < wsteps && k < nwin && w0 + r < npos && lane_on)
-        cp_async16(s_row(stage) + stp * 32 + lane,
-                   sl >= 0 ? table + (size_t)sl * dim + (size_t)gl * 4 : default_row + (size_t)gl * 4);
-    }
-    if (weights && k < nwin && (unsigned)lane < W && w0 + (unsigned)lane < npos)
-      cp_async4(s_wt(stage) + lane, weights + p_begin + w0 + lane);
-    cp_async_commit();
-  };
-  long long sl_next = load_slot(0);
-  issue(0, sl_next);
-  sl_next = load_slot(1);
-  issue(1, sl_next);
-  sl_next = load_slot(2);
-  // consumer state: cs = first segment (relative) that is not finished; my group's running sums
-  unsigned cs = 0;
-  FVec<4> acc;
-  acc.zero();
-  float wsum = 0.f, wsq = 0.f;
-  for (unsigned k = 0; k < nwin; ++k) {
-    const long long sl_issue = sl_next;
-    sl_next = load_slot(k + 3);                   // in flight while this window is summed
-    issue(k + 2, sl_issue);
-    cp_async_wait<2>();
-    __syncwarp();
-    const int stage = (int)(k % (unsigned)kWinStages);
-    const unsigned w0 = k * W;
-    const unsigned w1 = w0 + W < npos ? w0 + W : npos;
-    const float4* rows = s_row(stage);
-    const float* wts = s_wt(stage);
-    unsigned done = cs;                           // segments [cs, done) are finished after this window
-    if ((cs & ~(gpw - 1u)) < chunk * 32u) {       // the unfinished segment lies before the boundaries held: step back
-      chunk = (cs & ~(gpw - 1u)) >> 5;
-      b_lo = load_bounds(chunk * 32u);
-      b_hi = load_bounds(chunk * 32u + 32u);
-    }
-    for (unsigned base = cs & ~(gpw - 1u); base < nseg; base += gpw) {
-      while (base + gpw > chunk * 32u + 63u) {    // keep boundaries base .. base + gpw inside the 64 held
-        ++chunk;
-        b_lo = b_hi;
-        b_hi = load_bounds(chunk * 32u + 32u);
-      }
-      const unsigned first_st = bound(base < cs ? cs : base);
-      if (first_st > w1) break;                   // every later segment starts after this window (uniform)
-      const unsigned seg = base + gidx;
-      const unsigned st = bound(seg < nseg ? seg : nseg), en = bound(seg + 1u < nseg ? seg + 1u : nseg);
-      if (seg >= cs && seg < nseg && st <= w1) {
-        const unsigned a = st > w0 ? st : w0, b = en < w1 ? en : w1;
-        for (unsigned p = a; p < b; ++p) {
-          const unsigned r = p - w0;
-          const float wu = weights ? wts[r] : 1.f;
-          if (lane_on) {
-            FVec<4> x;
-            x.v = rows[(r >> gsh) * 32u + ((r & (gpw - 1u)) << lpr_shift) + gl];
-            acc.zip(x, [wu](float& av, float xv) { av = av + xv * wu; });
-          }
-          wsum = wsum + wu;
-          wsq = wsq + wu * wu;
-        }
-        if (en <= w1) {                           // the segment ends inside this window: normalise, store, reset
-          if (lane_on) {
-            if (en > st && combiner != DET_COMBINER_SUM) {
-              const float div = combiner == DET_COMBINER_MEAN ? wsum : sqrtf(wsq);
-              acc.apply([div](float& av) { av = av / div; });
-            }
-            acc.store(out + (S0 + seg) * dim + (size_t)gl * 4);
-          }
-          acc.zero();
-          wsum = 0.f;
-          wsq = 0.f;
-          done = seg + 1u;
-        }
-      }
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const unsigned other = __shfl_xor_sync(kFull, done, o);
-      done = other > done ? other : done;
-    }
-    cs = done;
-    __syncwarp();   // every lane is done with this stage before the next issue overwrites it
-  }
-  cp_async_wait<0>();
-}
-
 // K6 phase B, wide rows (several vectors per lane): one lane-group per output row.  A lane holds at most
 // kMaxVecPerLane vectors, so a row wider than kMaxVecPerLane * lpr vectors is swept in column chunks of that width;
 // every chunk re-walks the segment's ids in order (same per-column summation order, same wsum / wsq), so the result
@@ -639,7 +482,7 @@ struct OptHyper {
   float init_slot;  // adagrad initial accumulator
 };
 
-template <int VF, int OPT, int RU>
+template <int VF, int OPT>
 __global__ void __launch_bounds__(kThreadsF)
 apply_kernel(TableView t, const long long* __restrict__ keys, const float* __restrict__ grads, size_t n,
              OptHyper h, const float* __restrict__ init_param, int full_init, unsigned vpr, unsigned lpr,
@@ -675,7 +518,9 @@ apply_kernel(TableView t, const long long* __restrict__ keys, const float* __res
       atomicAdd(&s_new, __popc(bn));
       atomicAdd(&s_used, __popc(bu));
     }
-    // two row-steps per iteration: all loads of both rows are issued before the first update/store
+    // one row-step per iteration: fewer registers, more resident CTAs.  The loop keeps its per-step arrays (of one
+    // entry) because that form compiles to the instructions this kernel was validated with.
+    constexpr int RU = 1;
     for (unsigned j0 = 0; j0 < 32u; j0 += rows_per_step * RU) {
       bool ok[RU], nwv[RU], fresh[RU];
       size_t ro[RU], gi[RU];
@@ -1033,12 +878,9 @@ static void fgeom(unsigned dim, bool vec4, unsigned min_lpr, unsigned* vpr, unsi
 //      the whole CTA stages a tile of rows in shared memory with every load in flight, then thread c adds column c
 //      in order), all other CTAs give each lane-group two short groups at a time, 4 row loads in flight per group.
 // Indices outside [0, n_groups) are dropped like unsorted_segment_sum drops negative ids.
-// 8-bit digits by default: 11-bit digits (-DDET_RADIX_BITS=11) save a pass over 19 significant bits, but the 2048-bin
-// scatter pays for its shared-memory counters.  The kernels below are written for any width <= 11.
-#ifndef DET_RADIX_BITS
-#define DET_RADIX_BITS 8
-#endif
-constexpr int kRadixBits = DET_RADIX_BITS;
+// 8-bit digits: 11-bit digits save a pass over 19 significant bits, but the 2048-bin scatter pays for its shared-memory
+// counters.  The kernels below are written for any width <= 11.
+constexpr int kRadixBits = 8;
 constexpr int kRadixBins = 1 << kRadixBits;
 constexpr int kRadixThreads = 256;
 constexpr int kRadixBpt = kRadixBins / kRadixThreads;   // bins per thread: thread t owns bins [t * kRadixBpt, (t + 1) * kRadixBpt)
@@ -1516,8 +1358,7 @@ static det_status lookup_sparse_impl(det_table* t, const int64_t* ids, const int
   // dense output.  Whether the segment ids really are 0..nnz-1 is only known on the DEVICE (segment_offsets_kernel
   // computes it): the find-shaped kernel and the general pair are both launched, the flag lets exactly one of them work.
   const int ivec = pick_vec(t->row_bytes, default_row, out, nullptr);
-  const bool try_identity = nnz == batch && nnz > 0 && weights == nullptr && !(max_norm > 0.f) && vpr <= lpr && ivec >= 4 &&
-                            env_int("DET_SEGSUM_STAGED", 0) == 0 && env_int("DET_SPARSE_IDENTITY", 1) != 0;
+  const bool try_identity = nnz == batch && nnz > 0 && weights == nullptr && !(max_norm > 0.f) && vpr <= lpr && ivec >= 4;
   const unsigned* gate = try_identity ? not_identity : nullptr;
   // the flag word is compared with a per-table call counter instead of being reset by a memset launch per call
   unsigned epoch = 0;
@@ -1565,17 +1406,6 @@ static det_status lookup_sparse_impl(det_table* t, const int64_t* ids, const int
   } else if (max_norm > 0.f) {
     rc = fail(DET_UNIMPLEMENTED, "det_lookup_sparse_clip: max_norm is fused for rows of at most 32 vectors (dim <= 128 when "
                                  "dim % 4 == 0, else dim <= 32); use the composed path for wider rows");
-  } else if (vpr <= lpr && vec4 && env_int("DET_SEGSUM_STAGED", 0) != 0) {
-    // round-2 candidate (default off): rows staged through shared memory with cp.async, see segment_sum_staged_kernel
-    const size_t smem = (size_t)(kThreadsF / 32) * kWinWarpBytes;
-    int occ = 1;
-    CUDA_TRY(cudaFuncSetAttribute(segment_sum_staged_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, segment_sum_staged_kernel, kThreadsF, smem) != cudaSuccess || occ < 1) occ = 1;
-    const int grid = grid_for(batch, kThreadsF / 32, t->sm_count, occ);
-#ifdef DET_EMU
-    __atomic_fetch_add(&g_det_emu_stat[2], 1ull, __ATOMIC_RELAXED);
-#endif
-    DET_LAUNCH(segment_sum_staged_kernel, grid, kThreadsF, smem, s, t->view, slots, seg_start, weights, batch, combiner, default_row, out, vpr, lpr, sh);
   } else if (vpr <= lpr) {
     const ClipArg<false> noclip;
     const int occ = vec4 ? occupancy_of(segment_sum_kernel<4>, kThreadsF) : occupancy_of(segment_sum_kernel<1>, kThreadsF);
@@ -1629,11 +1459,9 @@ static det_status apply_common(det_table* t, const int64_t* keys, const float* g
     return fail(DET_UNIMPLEMENTED, "det_apply_*_dup: rows of up to 32 aligned 16-byte vectors only (use unique + segment_reduce + apply)");
   det_status st = ensure_room(t, n_dev ? nullptr : (const long long*)keys, n, s);
   if (st != DET_OK) return st;
-  static const int ru = env_int("DET_APPLY_RU", 1);  // one row-step per iteration: fewer registers, more resident CTAs
-  static const int staged = env_int("DET_APPLY_STAGED", 1);  // rows staged through shared memory (DET_APPLY_STAGED=0: register-held)
   const TableView v = t->view;
   const long long* k = (const long long*)keys;
-  if ((staged || n_dev) && vec4 && vpr <= lpr) {
+  if (vec4 && vpr <= lpr) {
     // cp.async-staged variant: 2 stages x kStageSteps x streams x 512 B per warp of dynamic shared memory
     const int ns = opt == 0 ? 3 : 4;
     const size_t smem = (size_t)(kThreadsF / 32) * 2 * kStageSteps * ns * 32 * 16;
@@ -1662,19 +1490,19 @@ static det_status apply_common(det_table* t, const int64_t* keys, const float* g
     note_mutation(t, n, s);
     return DET_OK;   // scores of a table with an eviction strategy were written by the kernel itself
   }
-#define DET_LAUNCH_APPLY(VF_, OPT_, RU_)                                                                      \
+#define DET_LAUNCH_APPLY(VF_, OPT_)                                                                           \
   {                                                                                                           \
-    const int grid = grid_for(n, kTileKeys, t->sm_count, occupancy_of(apply_kernel<VF_, OPT_, RU_>, kThreadsF)); \
-    const auto kern = apply_kernel<VF_, OPT_, RU_>;                                                           \
+    const int grid = grid_for(n, kTileKeys, t->sm_count, occupancy_of(apply_kernel<VF_, OPT_>, kThreadsF));   \
+    const auto kern = apply_kernel<VF_, OPT_>;                                                                \
     DET_LAUNCH(kern, grid, kThreadsF, 0, s, v, k, grads, n, h, init_param, full_init, vpr, lpr, sh,                   \
                                     (((uintptr_t)keys & 15u) == 0) ? 1 : 0);                                  \
   }
   if (opt == 0) {
-    if (vec4) { if (ru == 2) DET_LAUNCH_APPLY(4, 0, 2) else DET_LAUNCH_APPLY(4, 0, 1) }
-    else DET_LAUNCH_APPLY(1, 0, 1)
+    if (vec4) DET_LAUNCH_APPLY(4, 0)
+    else DET_LAUNCH_APPLY(1, 0)
   } else {
-    if (vec4) { if (ru == 2) DET_LAUNCH_APPLY(4, 1, 2) else DET_LAUNCH_APPLY(4, 1, 1) }
-    else DET_LAUNCH_APPLY(1, 1, 1)
+    if (vec4) DET_LAUNCH_APPLY(4, 1)
+    else DET_LAUNCH_APPLY(1, 1)
   }
 #undef DET_LAUNCH_APPLY
   CUDA_TRY(cudaGetLastError());
@@ -1772,7 +1600,7 @@ det_status det_gather_rows(const void* rows_in, const int32_t* perm, size_t n, s
 // TRAINING, where the unique rows live in the TrainableWrapper's scratch (python/ops/dynamic_embedding_ops.py:247-289:
 // gather(embeddings, idx) * weights -> segment_sum -> / sum(w) | / sqrt(sum(w^2))).  The gather, its weighted copy and
 // the segment reduction are ONE pass of the kernels det_lookup_sparse uses for its phase B (segment_sum_kernel /
-// segment_sum_wide_kernel, or the staged variant under DET_SEGSUM_STAGED=1) over a view whose "table" is the matrix.
+// segment_sum_wide_kernel) over a view whose "table" is the matrix.
 size_t det_sparse_segment_sum_workspace_bytes(size_t batch) {
   return align256((batch + 1) * sizeof(long long)) + align256(sizeof(DevState));
 }
@@ -1805,17 +1633,7 @@ det_status det_sparse_segment_sum(const float* rows, size_t dim, const int64_t* 
   unsigned vpr, lpr, sh;
   fgeom((unsigned)dim, vec4, 1, &vpr, &lpr, &sh);
   const unsigned gpw = 32u >> sh;
-  if (vpr <= lpr && vec4 && env_int("DET_SEGSUM_STAGED", 0) != 0) {
-    const size_t smem = (size_t)(kThreadsF / 32) * kWinWarpBytes;
-    int occ = 1;
-    CUDA_TRY(cudaFuncSetAttribute(segment_sum_staged_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, segment_sum_staged_kernel, kThreadsF, smem) != cudaSuccess || occ < 1) occ = 1;
-    const int grid = grid_for(batch, kThreadsF / 32, sms, occ);
-#ifdef DET_EMU
-    __atomic_fetch_add(&g_det_emu_stat[2], 1ull, __ATOMIC_RELAXED);
-#endif
-    DET_LAUNCH(segment_sum_staged_kernel, grid, kThreadsF, smem, s, v, slots, seg_start, weights, batch, combiner, default_row, out, vpr, lpr, sh);
-  } else if (vpr <= lpr) {
+  if (vpr <= lpr) {
     const ClipArg<false> noclip;
     const int occ = vec4 ? occupancy_of(segment_sum_kernel<4>, kThreadsF) : occupancy_of(segment_sum_kernel<1>, kThreadsF);
     const int grid = grid_for(batch, (int)(gpw * kSegPerGroup * (kThreadsF / 32)), sms, occ);
@@ -1885,10 +1703,8 @@ static det_status seg_reduce_run(const float* rows, const int32_t* idx, size_t n
   unsigned vpr, lpr, sh;
   fgeom((unsigned)dim, vec4, 1, &vpr, &lpr, &sh);
   const unsigned gpw = 32u >> sh;
-  // CTAs of the launch reserved for the long groups (default one per SM); a tuning knob until the kernel has been timed
-  int n_long_ctas = env_int("DET_SEGRED_LONG_CTAS", 2 * sms);
-  if (n_long_ctas < 1) n_long_ctas = 1;
-  if (n_long_ctas > 4 * sms) n_long_ctas = 4 * sms;
+  // CTAs of the launch reserved for the long groups
+  const int n_long_ctas = 2 * sms;
   const auto k4 = segment_reduce_kernel<4>;
   const auto k1 = segment_reduce_kernel<1>;
   const int occ = vec4 ? occupancy_of(k4, kThreadsF) : occupancy_of(k1, kThreadsF);

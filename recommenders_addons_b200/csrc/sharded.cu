@@ -83,8 +83,8 @@ peer_find_kernel(PeerViews pv, const long long* __restrict__ keys, size_t n,
 }
 
 // K8b: sharded Insert -- find-or-claim in the owner's key plane (system-scope CAS), row stored to the owner's HBM
-// MINB: resident CTAs per SM the register budget is capped for (1 = uncapped: 83 registers, 3 CTAs/SM; 4 = the default:
-// 64 registers -- more remote probes in flight per SM; DET_PEER_MINB selects)
+// MINB: resident CTAs per SM the register budget is capped for (1 = uncapped: 83 registers, 3 CTAs/SM; 4, used for
+// 16 B rows: 64 registers -- more remote probes in flight per SM)
 template <int VEC, int MINB = 1>
 __global__ void __launch_bounds__(kThreadsP, MINB)
 peer_insert_kernel(PeerViews pv, const long long* __restrict__ keys, const unsigned char* __restrict__ values,
@@ -627,25 +627,13 @@ struct det_peer_group {
   XchgView xv{};
   bool xchg = false;
   unsigned long long* xcursor = nullptr;     // owned: [kMaxPeers] cursors + 2 ticket words (senders / owner-side kernels)
-  cudaStream_t s_route = nullptr, s_apply = nullptr;   // chunk pipeline of det_peer_xchg_insert
-  cudaEvent_t ev_in = nullptr, ev_route = nullptr, ev_apply = nullptr;
-  int chunks = 1;
   unsigned long long ep_find = 0, ep_ins = 0;
   unsigned char* ins_ws = nullptr;           // owned: compacted inbound (keys, rows) of det_peer_xchg_insert on shards that evict
   long long* h_ins_n = nullptr;              // pinned: their count
   DevState* h_snap = nullptr;                // pinned: async snapshot of the local shard's DevState
   cudaEvent_t snap_ev = nullptr;
   bool snap_inflight = false;
-  // DET_XCHG_TIMING=1: CUDA events between the kernels of a call, accumulated and printed when the group is destroyed
-  bool timing = false;
-  cudaEvent_t tev[2][6] = {};                // [find | insert][boundary]
-  bool tev_pending[2] = {false, false};
-  double tacc[2][5] = {};
-  unsigned long long tcalls[2] = {0, 0};
 };
-extern "C" {
-static void xchg_time_collect(det_peer_group* g, int which, int n_iv);
-}
 
 
 // A shard with an eviction strategy is read and written by its OWNER's kernels only: a remote claim would bypass the
@@ -700,24 +688,7 @@ det_status det_peer_group_destroy(det_peer_group* g) {
       if (g->opened[p][q]) cudaIpcCloseMemHandle(g->opened[p][q]);
   if (g->cursor) cudaFree(g->cursor);
   if (g->h_counts) cudaFreeHost(g->h_counts);
-  if (g->timing) {
-    xchg_time_collect(g, 0, 4);
-    xchg_time_collect(g, 1, 1);
-    const double cf = g->tcalls[0] ? (double)g->tcalls[0] : 1.0, ci = g->tcalls[1] ? (double)g->tcalls[1] : 1.0;
-    fprintf(stderr, "[det xchg timing rank %d] find x%llu: route %.1f us, wait_req %.1f, serve %.1f, wait_done %.1f | "
-                    "insert x%llu (%d chunks, pipelined): %.1f us\n", g->pv.rank,
-            g->tcalls[0], g->tacc[0][0] / cf * 1e3, g->tacc[0][1] / cf * 1e3, g->tacc[0][2] / cf * 1e3, g->tacc[0][3] / cf * 1e3,
-            g->tcalls[1], g->chunks, g->tacc[1][0] / ci * 1e3);
-    for (int a = 0; a < 2; ++a)
-      for (int b = 0; b < 6; ++b)
-        if (g->tev[a][b]) cudaEventDestroy(g->tev[a][b]);
-  }
   if (g->xcursor) cudaFree(g->xcursor);
-  if (g->s_route) cudaStreamDestroy(g->s_route);
-  if (g->s_apply) cudaStreamDestroy(g->s_apply);
-  if (g->ev_in) cudaEventDestroy(g->ev_in);
-  if (g->ev_route) cudaEventDestroy(g->ev_route);
-  if (g->ev_apply) cudaEventDestroy(g->ev_apply);
   if (g->h_snap) cudaFreeHost(g->h_snap);
   if (g->snap_ev) cudaEventDestroy(g->snap_ev);
   if (g->ins_ws) cudaFree(g->ins_ws);
@@ -997,21 +968,9 @@ det_status det_peer_xchg_attach(det_peer_group* g, const void* const* mailbox_pt
   if (!g->xcursor) {
     CUDA_TRY(cudaMalloc((void**)&g->xcursor, (kMaxPeers + 2) * sizeof(unsigned long long)));
     CUDA_TRY(cudaMemset(g->xcursor, 0, (kMaxPeers + 2) * sizeof(unsigned long long)));
-    CUDA_TRY(cudaStreamCreateWithFlags(&g->s_route, cudaStreamNonBlocking));
-    CUDA_TRY(cudaStreamCreateWithFlags(&g->s_apply, cudaStreamNonBlocking));
-    CUDA_TRY(cudaEventCreateWithFlags(&g->ev_in, cudaEventDisableTiming));
-    CUDA_TRY(cudaEventCreateWithFlags(&g->ev_route, cudaEventDisableTiming));
-    CUDA_TRY(cudaEventCreateWithFlags(&g->ev_apply, cudaEventDisableTiming));
   }
-  // chunks of one det_peer_xchg_insert call (every chunk is a collective epoch: the SAME value on every rank)
-  // (every extra chunk adds a round of flag waits that can cost more than the overlap returns, so the default is ONE
-  // chunk; the pipeline stays selectable)
-  g->chunks = env_int("DET_XCHG_CHUNKS", 1);
-  if (g->chunks < 1) g->chunks = 1;
-  if (g->chunks > 16) g->chunks = 16;
   g->ep_find = g->ep_ins = 0;
   g->xchg = true;
-  g->timing = env_int("DET_XCHG_TIMING", 0) != 0;
   return DET_OK;
 }
 
@@ -1064,22 +1023,6 @@ static void peer_snapshot(det_peer_group* g, cudaStream_t s) {
     cudaGetLastError();
 }
 
-static void xchg_time_collect(det_peer_group* g, int which, int n_iv) {
-  if (!g->timing || !g->tev_pending[which]) return;
-  if (cudaEventSynchronize(g->tev[which][n_iv]) != cudaSuccess) { cudaGetLastError(); return; }
-  for (int i = 0; i < n_iv; ++i) {
-    float ms = 0.f;
-    if (cudaEventElapsedTime(&ms, g->tev[which][i], g->tev[which][i + 1]) == cudaSuccess) g->tacc[which][i] += ms;
-  }
-  g->tcalls[which]++;
-  g->tev_pending[which] = false;
-}
-static void xchg_mark(det_peer_group* g, int which, int i, cudaStream_t s) {
-  if (!g->timing) return;
-  if (!g->tev[which][i]) cudaEventCreate(&g->tev[which][i]);
-  cudaEventRecord(g->tev[which][i], s);
-}
-
 // Sharded Find through the owners.  COLLECTIVE: every rank of the group calls it (n may differ, 0 allowed), in the same
 // order as its peers.  Rows land in this rank's output ring (2 entries): *rows_view (if non-null) receives the device
 // pointer of the n rows, valid until the next-but-one det_peer_xchg_find; values_out (if non-null) additionally gets a
@@ -1094,7 +1037,6 @@ det_status det_peer_xchg_find(det_peer_group* g, const int64_t* keys, size_t n, 
   det::DevGuard _dg(g->device);
   det_status rs = peer_room(g, "det_peer_xchg_find");
   if (rs != DET_OK && rs != DET_TABLE_FULL) return rs;
-  xchg_time_collect(g, 0, 4);
   const unsigned long long ep = ++g->ep_find;
   const int parity = (int)(ep & 1ull);
   const XchgView& xv = g->xv;
@@ -1107,14 +1049,11 @@ det_status det_peer_xchg_find(det_peer_group* g, const int64_t* keys, size_t n, 
   unsigned* ticket = reinterpret_cast<unsigned*>(g->xcursor + kMaxPeers);
   DevState* st = g->local->view.st;
   const long long* k = (const long long*)keys;
-  xchg_mark(g, 0, 0, s);
   {
     const int grid = grid_for(n, kThreadsP * kRouteKpt, g->sm_count, 4);
     DET_LAUNCH((xchg_route_kernel<false, 16>), grid, kThreadsP, 0, s, xv, k, (const unsigned char*)nullptr, n, geo, g->xcursor, ticket, ep, st);
   }
-  xchg_mark(g, 0, 1, s);
   xchg_wait(g, kFlagReq, ep, s);
-  xchg_mark(g, 0, 2, s);
   {
     const unsigned char* d = (const unsigned char*)defaults;
     const TableView tv = g->local->view;
@@ -1132,10 +1071,7 @@ det_status det_peer_xchg_find(det_peer_group* g, const int64_t* keys, size_t n, 
 #undef DET_XSERVE
     }
   }
-  xchg_mark(g, 0, 3, s);
   xchg_wait(g, kFlagDone, ep, s);
-  xchg_mark(g, 0, 4, s);
-  g->tev_pending[0] = g->timing;
   if (full_size_default && n) {
     const int grid = grid_for(n, kThreadsP, g->sm_count, 4);
     const unsigned char* d = (const unsigned char*)defaults;
@@ -1224,12 +1160,11 @@ static det_status xchg_insert_evicting(det_peer_group* g, const int64_t* keys, c
 }
 
 
-// Sharded Insert (insert_or_assign) through the owners.  COLLECTIVE like det_peer_xchg_find.
-// The batch can be cut into `chunks` pieces (DET_XCHG_CHUNKS, default 1 = off, the same on every rank) and PIPELINED over two
-// internal streams: while the owner-side kernel applies the pairs of chunk c to the local shard (HBM-bound, no NVLink
-// traffic), the sender kernel already routes chunk c+1 to its owners (NVLink-bound, little SM time).  Every chunk is an
-// epoch of the flag protocol; epochs alternate between two sets of inbox segments, so a sender only ever waits for
-// the owners to have consumed the epoch before the previous one.  The caller's stream is fenced on both sides by events.
+// Sharded Insert (insert_or_assign) through the owners.  COLLECTIVE like det_peer_xchg_find.  One epoch of the flag
+// protocol per call: the sender kernel routes the pairs to their owners, and the owner-side kernel applies what arrived
+// to the local shard, both on the caller's stream.  Epochs alternate between two sets of inbox segments, so a sender
+// only ever waits for the owners to have consumed the epoch before the previous one.  (Cutting the batch into chunks
+// pipelined over two streams was measured slower at N = 2: every chunk adds a round of flag waits; DESIGN.md section 5.)
 det_status det_peer_xchg_insert(det_peer_group* g, const int64_t* keys, const void* values, size_t n,
                                 det_stream_t stream) {
   if (!g || !g->xchg) return fail(DET_INVALID_ARGUMENT, "det_peer_xchg_insert: no exchange mailbox attached");
@@ -1241,8 +1176,6 @@ det_status det_peer_xchg_insert(det_peer_group* g, const int64_t* keys, const vo
   det_status rs = peer_room(g, "det_peer_xchg_insert");
   if (rs != DET_OK) return rs;
   det::MutLock _lk(g->local);
-  xchg_time_collect(g, 1, 1);
-  xchg_mark(g, 1, 0, s);
   const XchgView& xv = g->xv;
   const int vec = pick_vec(g->row_bytes, values, nullptr, nullptr);
   const RowGeom geo = make_geom((unsigned)g->row_bytes, vec);
@@ -1253,69 +1186,43 @@ det_status det_peer_xchg_insert(det_peer_group* g, const int64_t* keys, const vo
   DevState* st = g->local->view.st;
   const TableView tv = g->local->view;
   const int np = g->n_slot_planes;
-  const int C = g->chunks;
-  const bool piped = C > 1;
-  cudaStream_t sr = piped ? g->s_route : s, sa = piped ? g->s_apply : s;
-  if (piped) {
-    CUDA_TRY(cudaEventRecord(g->ev_in, s));
-    CUDA_TRY(cudaStreamWaitEvent(sr, g->ev_in, 0));
-    CUDA_TRY(cudaStreamWaitEvent(sa, g->ev_in, 0));
+  const long long* k = (const long long*)keys;
+  const unsigned char* r = (const unsigned char*)values;
+  const unsigned long long ep = ++g->ep_ins;
+  // sender side: the owners have consumed the segment set this epoch is about to overwrite (epoch ep - 2)
+  if (ep > 2) {
+    const unsigned long long* flags = reinterpret_cast<const unsigned long long*>(xv.base[xv.rank] + kFlagAck * 64);
+    DET_LAUNCH_SPIN(xchg_wait_kernel, 1, 32, 0, s, flags, xv.world, ep - 2, st, kXchgTimeoutCycles);
   }
-  // per-chunk key ranges: multiples of 256 keys so that every chunk's rows stay 16 B aligned like the batch
-  const size_t per = ((n + (size_t)C - 1) / (size_t)C + 255) & ~(size_t)255;
-  // two kernels share the SMs: neither grid may take every resident slot (registers) of an SM
-  const int route_cap = piped ? 2 : 4;
-  for (int c = 0; c < C; ++c) {
-    const size_t b = (size_t)c * per < n ? (size_t)c * per : n;
-    const size_t e = b + per < n ? b + per : n;
-    const size_t m = e - b;
-    const long long* k = (const long long*)keys + b;
-    const unsigned char* r = (const unsigned char*)values + b * g->row_bytes;
-    const unsigned long long ep = ++g->ep_ins;
-    // sender side: the owners have consumed the segment set this epoch is about to overwrite (epoch ep - 2)
-    if (ep > 2) {
-      const unsigned long long* flags = reinterpret_cast<const unsigned long long*>(xv.base[xv.rank] + kFlagAck * 64);
-      DET_LAUNCH_SPIN(xchg_wait_kernel, 1, 32, 0, sr, flags, xv.world, ep - 2, st, kXchgTimeoutCycles);
+  {
+    const int grid = grid_for(n, kThreadsP * kRouteKpt, g->sm_count, 4);
+    switch (vec) {
+      case 16: DET_LAUNCH((xchg_route_kernel<true, 16>), grid, kThreadsP, 0, s, xv, k, r, n, geo, g->xcursor, ticket_r, ep, st); break;
+      case 8: DET_LAUNCH((xchg_route_kernel<true, 8>), grid, kThreadsP, 0, s, xv, k, r, n, geo, g->xcursor, ticket_r, ep, st); break;
+      case 4: DET_LAUNCH((xchg_route_kernel<true, 4>), grid, kThreadsP, 0, s, xv, k, r, n, geo, g->xcursor, ticket_r, ep, st); break;
+      case 2: DET_LAUNCH((xchg_route_kernel<true, 2>), grid, kThreadsP, 0, s, xv, k, r, n, geo, g->xcursor, ticket_r, ep, st); break;
+      default: DET_LAUNCH((xchg_route_kernel<true, 1>), grid, kThreadsP, 0, s, xv, k, r, n, geo, g->xcursor, ticket_r, ep, st); break;
     }
-    {
-      const int grid = grid_for(m, kThreadsP * kRouteKpt, g->sm_count, route_cap);
-      switch (vec) {
-        case 16: DET_LAUNCH((xchg_route_kernel<true, 16>), grid, kThreadsP, 0, sr, xv, k, r, m, geo, g->xcursor, ticket_r, ep, st); break;
-        case 8: DET_LAUNCH((xchg_route_kernel<true, 8>), grid, kThreadsP, 0, sr, xv, k, r, m, geo, g->xcursor, ticket_r, ep, st); break;
-        case 4: DET_LAUNCH((xchg_route_kernel<true, 4>), grid, kThreadsP, 0, sr, xv, k, r, m, geo, g->xcursor, ticket_r, ep, st); break;
-        case 2: DET_LAUNCH((xchg_route_kernel<true, 2>), grid, kThreadsP, 0, sr, xv, k, r, m, geo, g->xcursor, ticket_r, ep, st); break;
-        default: DET_LAUNCH((xchg_route_kernel<true, 1>), grid, kThreadsP, 0, sr, xv, k, r, m, geo, g->xcursor, ticket_r, ep, st); break;
-      }
-    }
-    // owner side: every source has published its count of this epoch
-    {
-      const unsigned long long* flags = reinterpret_cast<const unsigned long long*>(xv.base[xv.rank] + ((ep & 1ull) ? kFlagIns1 : kFlagIns) * 64);
-      DET_LAUNCH_SPIN(xchg_wait_kernel, 1, 32, 0, sa, flags, xv.world, ep, st, kXchgTimeoutCycles);
-    }
-    switch (avec) {
+  }
+  // owner side: every source has published its count of this epoch
+  {
+    const unsigned long long* flags = reinterpret_cast<const unsigned long long*>(xv.base[xv.rank] + ((ep & 1ull) ? kFlagIns1 : kFlagIns) * 64);
+    DET_LAUNCH_SPIN(xchg_wait_kernel, 1, 32, 0, s, flags, xv.world, ep, st, kXchgTimeoutCycles);
+  }
+  switch (avec) {
 #define DET_XAPPLY(VV)                                                                                        \
   case VV: {                                                                                                   \
-    int occ = occupancy_of(xchg_apply_insert_kernel<VV>, kThreadsP);                                           \
-    if (piped && occ > 2) occ = occ - 1;   /* leave room for the sender kernel of the next chunk */            \
-    DET_LAUNCH(xchg_apply_insert_kernel<VV>, g->sm_count * occ, kThreadsP, 0, sa, xv, tv, ageo, np, ticket_a, ep); \
+    const int occ = occupancy_of(xchg_apply_insert_kernel<VV>, kThreadsP);                                     \
+    DET_LAUNCH(xchg_apply_insert_kernel<VV>, g->sm_count * occ, kThreadsP, 0, s, xv, tv, ageo, np, ticket_a, ep); \
   } break;
-      DET_XAPPLY(16) DET_XAPPLY(8) DET_XAPPLY(4) DET_XAPPLY(2)
-      default: {
-        const int occ = occupancy_of(xchg_apply_insert_kernel<1>, kThreadsP);
-        DET_LAUNCH(xchg_apply_insert_kernel<1>, g->sm_count * occ, kThreadsP, 0, sa, xv, tv, ageo, np, ticket_a, ep);
-      } break;
+    DET_XAPPLY(16) DET_XAPPLY(8) DET_XAPPLY(4) DET_XAPPLY(2)
+    default: {
+      const int occ = occupancy_of(xchg_apply_insert_kernel<1>, kThreadsP);
+      DET_LAUNCH(xchg_apply_insert_kernel<1>, g->sm_count * occ, kThreadsP, 0, s, xv, tv, ageo, np, ticket_a, ep);
+    } break;
 #undef DET_XAPPLY
-    }
   }
   CUDA_TRY(cudaGetLastError());
-  if (piped) {
-    CUDA_TRY(cudaEventRecord(g->ev_route, sr));
-    CUDA_TRY(cudaEventRecord(g->ev_apply, sa));
-    CUDA_TRY(cudaStreamWaitEvent(s, g->ev_route, 0));
-    CUDA_TRY(cudaStreamWaitEvent(s, g->ev_apply, 0));
-  }
-  xchg_mark(g, 1, 1, s);
-  g->tev_pending[1] = g->timing;
   peer_snapshot(g, s);
   return DET_OK;
 }
@@ -1465,12 +1372,11 @@ det_status det_peer_insert(det_peer_group* g, const int64_t* keys, const void* v
   }
   const int vec = pick_vec(g->row_bytes, values, nullptr, nullptr);
   const RowGeom geo = make_geom((unsigned)g->row_bytes, vec);
-  // register cap of the one-sided insert: at least DET_PEER_MINB resident CTAs per SM, more remote probes in flight
-  static const int minb = env_int("DET_PEER_MINB", 4);
   const unsigned char* v = (const unsigned char*)values;
   const long long* k = (const long long*)keys;
   const int np = g->n_slot_planes;
-  if (vec == 16 && minb >= 4) {
+  if (vec == 16) {
+    // register cap of the one-sided insert: at least 4 resident CTAs per SM, more remote probes in flight
     const auto kern = peer_insert_kernel<16, 4>;
     const int grid4 = grid_for(n, kThreadsP, g->sm_count, occupancy_of(kern, kThreadsP));
     DET_LAUNCH(kern, grid4, kThreadsP, 0, s, g->pv, k, v, n, geo, np);
@@ -1478,9 +1384,9 @@ det_status det_peer_insert(det_peer_group* g, const int64_t* keys, const void* v
     peer_snapshot(g, s);
     return DET_OK;
   }
+  // narrower rows: the grid of the uncapped 16 B kernel
   const int grid = grid_for(n, kThreadsP, g->sm_count, occupancy_of(peer_insert_kernel<16>, kThreadsP));
   switch (vec) {
-    case 16: DET_LAUNCH(peer_insert_kernel<16>, grid, kThreadsP, 0, s, g->pv, k, v, n, geo, np); break;
     case 8: DET_LAUNCH(peer_insert_kernel<8>, grid, kThreadsP, 0, s, g->pv, k, v, n, geo, np); break;
     case 4: DET_LAUNCH(peer_insert_kernel<4>, grid, kThreadsP, 0, s, g->pv, k, v, n, geo, np); break;
     case 2: DET_LAUNCH(peer_insert_kernel<2>, grid, kThreadsP, 0, s, g->pv, k, v, n, geo, np); break;

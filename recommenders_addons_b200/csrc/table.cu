@@ -8,7 +8,7 @@ namespace det {
 
 #ifdef DET_EMU
 extern "C" {
-unsigned long long g_det_emu_stat[4] = {0, 0, 0, 0};
+unsigned long long g_det_emu_hint_lanes = 0;
 }
 #endif
 thread_local std::string g_last_error;
@@ -65,18 +65,6 @@ int grid_for(size_t n_items, int items_per_block, int sm_count, int blocks_per_s
 // Kernels
 // ================================================================================================
 constexpr int kThreads = 256;
-// Occupancy experiments (measurement builds with -DDET_FIND_MINB=n / -DDET_INSERT_MINB=n: a minimum of n resident
-// CTAs per SM caps the registers of the headline kernels); undefined = the default.
-#ifdef DET_FIND_MINB
-#define DET_FIND_BOUNDS __launch_bounds__(kThreads, DET_FIND_MINB)
-#else
-#define DET_FIND_BOUNDS __launch_bounds__(kThreads)
-#endif
-#ifdef DET_INSERT_MINB
-#define DET_INSERT_BOUNDS __launch_bounds__(kThreads, DET_INSERT_MINB)
-#else
-#define DET_INSERT_BOUNDS __launch_bounds__(kThreads)
-#endif
 constexpr int kWarpsPerBlock = kThreads / 32;
 
 // Slot hints (host side: "slot hints" below): a find may leave {key, slot} of its key i at index i of these two arrays,
@@ -111,27 +99,11 @@ __device__ __forceinline__ void find_step(const TableView& t, long long key, siz
   warp_move_rows<VEC>(g, src, dst, lane, full_default ? nullptr : defaults);
 }
 
-// variant 0: keys read with coalesced LDG, grid-stride by warp
-template <int VEC>
-__global__ void DET_FIND_BOUNDS
-find_kernel(TableView t, const long long* __restrict__ keys, size_t n,
-            const unsigned char* __restrict__ defaults, int full_default,
-            unsigned char* __restrict__ out, unsigned char* __restrict__ exists, RowGeom g, SlotHints h) {
-  const int lane = threadIdx.x & 31;
-  const size_t warp0 = ((size_t)blockIdx.x * kThreads + threadIdx.x) >> 5;
-  const size_t nwarps = ((size_t)gridDim.x * kThreads) >> 5;
-  for (size_t base = warp0 * 32; base < n; base += nwarps * 32) {
-    const size_t i = base + lane;
-    const bool valid = i < n;
-    const long long key = valid ? __ldg(keys + i) : 0;
-    find_step<VEC>(t, key, i, valid, defaults, full_default, out, exists, g, lane, h);
-  }
-}
-
-// variant 1 (default): persistent CTAs, key tiles staged into shared memory by TMA bulk copies
-// (cp.async.bulk + mbarrier), tile i+1 in flight while tile i is probed and gathered
-template <int VEC>
-__global__ void DET_FIND_BOUNDS
+// Persistent CTAs, key tiles staged into shared memory by TMA bulk copies (cp.async.bulk + mbarrier), tile i+1 in
+// flight while tile i is probed and gathered.  TMA = false: keys that are not 16 B aligned, read with plain loads on
+// the same tile schedule.
+template <int VEC, bool TMA>
+__global__ void __launch_bounds__(kThreads)
 find_kernel_tma(TableView t, const long long* __restrict__ keys, size_t n,
                 const unsigned char* __restrict__ defaults, int full_default,
                 unsigned char* __restrict__ out, unsigned char* __restrict__ exists, RowGeom g, SlotHints h) {
@@ -139,7 +111,7 @@ find_kernel_tma(TableView t, const long long* __restrict__ keys, size_t n,
   __shared__ __align__(8) unsigned long long s_bar[kStages];
   const int lane = threadIdx.x & 31;
   KeyTiles kt;
-  kt.init(s_keys, s_bar, keys, n);
+  kt.init(s_keys, s_bar, keys, n, TMA);
   for (; kt.valid(); kt.next()) {
     size_t i;
     bool valid;
@@ -155,7 +127,7 @@ struct SlotInit {
 
 // K2: Insert (insert_or_assign).  HINTED: the host has checked that no mutation was enqueued since the find that wrote
 // `h`, so a hint whose key is this lane's key gives the slot the probe would find; the other lanes probe as usual.
-template <int VEC, bool BATCH, bool HINTED>
+template <int VEC, bool HINTED>
 __device__ __forceinline__ void insert_step(const TableView& t, long long key, size_t i, bool valid,
                                             const unsigned char* __restrict__ values, const RowGeom& g,
                                             const SlotInit& si, int lane, unsigned* s_new, unsigned* s_used,
@@ -167,10 +139,10 @@ __device__ __forceinline__ void insert_step(const TableView& t, long long key, s
     hinted = hslot != kNoHint && h.keys[i] == key;
   }
 #ifdef DET_EMU
-  if (hinted) __atomic_fetch_add(&g_det_emu_stat[3], 1ull, __ATOMIC_RELAXED);
+  if (hinted) __atomic_fetch_add(&g_det_emu_hint_lanes, 1ull, __ATOMIC_RELAXED);
 #endif
   bool is_new, from_empty;
-  long long slot = warp_find_or_claim_v<BATCH>(t, key, valid && !hinted, valid && !hinted, lane, is_new, from_empty);
+  long long slot = warp_find_or_claim(t, key, valid && !hinted, valid && !hinted, lane, is_new, from_empty);
   if (hinted) slot = (long long)hslot;
   const unsigned bn = __ballot_sync(kFull, is_new), bu = __ballot_sync(kFull, from_empty);
   if (lane == 0 && bn) {
@@ -192,34 +164,9 @@ __device__ __forceinline__ void insert_step(const TableView& t, long long key, s
       *reinterpret_cast<unsigned*>(t.planes[p] + (size_t)slot * t.dim * 4u) = kSlotUninit;
 }
 
-template <int VEC, bool BATCH = false, bool HINTED = false>
-__global__ void DET_INSERT_BOUNDS
-insert_kernel(TableView t, const long long* __restrict__ keys, const unsigned char* __restrict__ values,
-              size_t n, RowGeom g, SlotInit si, SlotHints h) {
-  __shared__ unsigned s_new, s_used;
-  if (threadIdx.x == 0) {
-    s_new = 0;
-    s_used = 0;
-  }
-  __syncthreads();
-  const int lane = threadIdx.x & 31;
-  const size_t warp0 = ((size_t)blockIdx.x * kThreads + threadIdx.x) >> 5;
-  const size_t nwarps = ((size_t)gridDim.x * kThreads) >> 5;
-  for (size_t base = warp0 * 32; base < n; base += nwarps * 32) {
-    const size_t i = base + lane;
-    const bool valid = i < n;
-    const long long key = valid ? __ldg(keys + i) : 0;
-    insert_step<VEC, BATCH, HINTED>(t, key, i, valid, values, g, si, lane, &s_new, &s_used, h);
-  }
-  __syncthreads();
-  if (threadIdx.x == 0 && s_new) {
-    atomicAdd(&t.st->size, (unsigned long long)s_new);
-    atomicAdd(&t.st->used, (unsigned long long)s_used);
-  }
-}
-
-template <int VEC, bool BATCH = false, bool HINTED = false>
-__global__ void DET_INSERT_BOUNDS
+// Key tiles as in find_kernel_tma<VEC, TMA>.
+template <int VEC, bool TMA, bool HINTED>
+__global__ void __launch_bounds__(kThreads)
 insert_kernel_tma(TableView t, const long long* __restrict__ keys, const unsigned char* __restrict__ values,
                   size_t n, RowGeom g, SlotInit si, SlotHints h) {
   __shared__ __align__(128) long long s_keys[kStages][kTileKeys];
@@ -231,12 +178,13 @@ insert_kernel_tma(TableView t, const long long* __restrict__ keys, const unsigne
   }
   const int lane = threadIdx.x & 31;
   KeyTiles kt;
-  kt.init(s_keys, s_bar, keys, n);
+  kt.init(s_keys, s_bar, keys, n, TMA);
+  if (!TMA) __syncthreads();  // init has no barrier without TMA: s_new / s_used are zeroed before any warp adds to them
   for (; kt.valid(); kt.next()) {
     size_t i;
     bool valid;
     const long long key = kt.key(i, valid);
-    insert_step<VEC, BATCH, HINTED>(t, key, i, valid, values, g, si, lane, &s_new, &s_used, h);
+    insert_step<VEC, HINTED>(t, key, i, valid, values, g, si, lane, &s_new, &s_used, h);
   }
   __syncthreads();
   if (threadIdx.x == 0 && s_new) {
@@ -984,8 +932,7 @@ static det_status launch_accum(det_table* t, const TableView& v, const long long
                                const uint8_t* exists, size_t n, const SlotInit& si, const RowGeom& g, int vec,
                                cudaStream_t s) {
   if constexpr (std::is_same<T, float>::value) {
-    static const int staged = env_int("DET_ACCUM_STAGED", 1);
-    if (staged && vec == 16 && g.vpr <= g.lpr) {
+    if (vec == 16 && g.vpr <= g.lpr) {
       const int grid = grid_for(n, kThreads, t->sm_count, occupancy_of(accum_staged_kernel, kThreads));
       DET_LAUNCH(accum_staged_kernel, grid, kThreads, 0, s, v, k, (const float*)vod, exists, n, si, g);
       return DET_OK;
@@ -1134,7 +1081,8 @@ extern "C" {
 
 int det_abi_version(void) { return 8; }
 #ifdef DET_EMU
-unsigned long long det_emu_stat(int which) { return which >= 0 && which < 4 ? det::g_det_emu_stat[which] : 0; }
+// emulator statistics by number: 3 = lanes of insert kernels that took a slot hint (no other number is in use)
+unsigned long long det_emu_stat(int which) { return which == 3 ? det::g_det_emu_hint_lanes : 0; }
 #endif
 
 const char* det_build_info(void) {
@@ -1195,11 +1143,7 @@ static det_status create_common(det_table** out, const det_config* cfg, void* re
   cudaDeviceProp prop;
   CUDA_TRY(cudaGetDeviceProperties(&prop, cfg->device));
   // Probes read one 64 B bucket and nothing near it: ask L2 not to fetch more than that per miss.
-  // DET_L2_FETCH=0 leaves the device default.
-  {
-    const int fetch = env_int("DET_L2_FETCH", 64);
-    if (fetch > 0 && cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, (size_t)fetch) != cudaSuccess) cudaGetLastError();
-  }
+  if (cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, 64) != cudaSuccess) cudaGetLastError();
   t->sm_count = prop.multiProcessorCount;
   uint64_t init = cfg->init_capacity ? cfg->init_capacity : 8192;
   if (cfg->max_capacity && init > cfg->max_capacity) init = cfg->max_capacity;
@@ -1315,21 +1259,14 @@ det_status det_find(det_table* t, const int64_t* keys, size_t n, const void* def
   std::unique_lock<std::mutex> hl(t->hint_mu, std::try_to_lock);
   const bool track = hl.owns_lock() && hints_allowed(t) && !stream_capturing(s);
   const SlotHints h = track ? find_hints(t, keys, n, s) : SlotHints{nullptr, nullptr};
-  // variant 1 (default): persistent CTAs + TMA-staged key tiles; needs 16 B aligned keys.  DET_FIND_VARIANT=0
-  // selects the plain grid-stride kernel.
-  static const int variant = env_int("DET_FIND_VARIANT", 1);
-  const bool tma = variant == 1 && (((uintptr_t)keys & 15u) == 0);
+  // TMA bulk copies of the key tiles need 16 B aligned keys
+  const bool tma = ((uintptr_t)keys & 15u) == 0;
   return dispatch_vec(vec, [&](auto V) -> det_status {
     constexpr int VV = decltype(V)::value;
-    if (tma) {
-      const int grid = grid_for(n, kTileKeys, t->sm_count, occupancy_of(find_kernel_tma<VV>, kThreads));
-      DET_LAUNCH(find_kernel_tma<VV>, grid, kThreads, 0, s, v, (const long long*)keys, n, (const unsigned char*)defaults,
-                                                    full_size_default, (unsigned char*)values_out, exists, g, h);
-    } else {
-      const int grid = grid_for(n, kThreads, t->sm_count, occupancy_of(find_kernel<VV>, kThreads));
-      DET_LAUNCH(find_kernel<VV>, grid, kThreads, 0, s, v, (const long long*)keys, n, (const unsigned char*)defaults,
-                                                full_size_default, (unsigned char*)values_out, exists, g, h);
-    }
+    const auto kern = tma ? find_kernel_tma<VV, true> : find_kernel_tma<VV, false>;
+    const int grid = grid_for(n, kTileKeys, t->sm_count, occupancy_of(kern, kThreads));
+    DET_LAUNCH(kern, grid, kThreads, 0, s, v, (const long long*)keys, n, (const unsigned char*)defaults, full_size_default,
+               (unsigned char*)values_out, exists, g, h);
     CUDA_TRY(cudaGetLastError());
     if (h.keys != nullptr) CUDA_TRY(cudaEventRecord(t->hint_ev, s));
     return DET_OK;
@@ -1362,19 +1299,13 @@ det_status insert_impl(det_table* t, const int64_t* keys, const void* values, si
   // after ensure_room: a growth it triggered has advanced the generation.  The chunks of det_insert_host run on
   // several streams of their own and take no hints.
   const SlotHints h = check_room ? insert_hints(t, keys, n, s) : SlotHints{nullptr, nullptr};
-  static const int variant = env_int("DET_INSERT_VARIANT", 1);
-  const bool tma = variant == 1 && (((uintptr_t)keys & 15u) == 0);
+  const bool tma = ((uintptr_t)keys & 15u) == 0;
   return dispatch_vec(vec, [&](auto V) -> det_status {
     constexpr int VV = decltype(V)::value;
-    // DET_CLAIM_BATCH=1: the batched-claim probe (common.cuh), a round-2 candidate for inserts of NEW keys; the
-    // default is the validated serial claim
-    const bool batch = env_int("DET_CLAIM_BATCH", 0) != 0;
-    using KernelFn = void (*)(TableView, const long long*, const unsigned char*, size_t, RowGeom, SlotInit, SlotHints);
-    KernelFn kfn = tma ? (batch ? (KernelFn)insert_kernel_tma<VV, true> : (KernelFn)insert_kernel_tma<VV, false>)
-                       : (batch ? (KernelFn)insert_kernel<VV, true> : (KernelFn)insert_kernel<VV, false>);
-    if (h.keys != nullptr && !batch)
-      kfn =tma ? (KernelFn)insert_kernel_tma<VV, false, true> : (KernelFn)insert_kernel<VV, false, true>;
-    const int grid = grid_for(n, tma ? kTileKeys : kThreads, t->sm_count, occupancy_of(kfn, kThreads));
+    const bool hinted = h.keys != nullptr;
+    const auto kfn = tma ? (hinted ? insert_kernel_tma<VV, true, true> : insert_kernel_tma<VV, true, false>)
+                         : (hinted ? insert_kernel_tma<VV, false, true> : insert_kernel_tma<VV, false, false>);
+    const int grid = grid_for(n, kTileKeys, t->sm_count, occupancy_of(kfn, kThreads));
     DET_LAUNCH(kfn, grid, kThreads, 0, s, v, (const long long*)keys, (const unsigned char*)values, n, g, si, h);
     CUDA_TRY(cudaGetLastError());
     if (check_room) note_mutation(t, n, s);

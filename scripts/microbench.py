@@ -2,7 +2,7 @@
 """Per-kernel sweep (dev tool, not the headline bench): times every table kernel with CUDA events on the torch
 stream for dim {16,64,128}, uniform and Zipf keys, several hit rates; prints one JSON line per case.
     python scripts/microbench.py [--resident 50000000] [--batch 1048576] [--reps 10]
-Env DET_FIND_VARIANT / DET_INSERT_VARIANT select experimental kernel variants inside libdetable.so."""
+DET_LIB_PATH=<path> times another build of the library (recommenders_addons_b200.build --variant)."""
 import argparse
 import json
 import os

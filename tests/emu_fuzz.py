@@ -1,17 +1,16 @@
 """CPU, no GPU: randomised differential runs of the kernels written after round 1's GPU budget was spent, on the SIMT
 emulator against the oracle -- many more cases than the test suite's property tests.
-  python tests/emu_fuzz.py [cases]      (default 400: det_segment_reduce, 250: staged segment-sum)"""
+  python tests/emu_fuzz.py [cases]      (default 400: det_segment_reduce, 250: det_lookup_sparse bags)"""
 import os
 import sys
 
 import numpy as np
-import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from oracle import oracle as O  # noqa: E402
 from tests.test_segreduce_emu import reduce_emu, rows_of  # noqa: E402
-from tests.test_segsum_staged_emu import _both, _tables  # noqa: E402
+from tests.test_lookup_sparse_bags_emu import _check, _tables  # noqa: E402
 
 
 def fuzz_segment_reduce(cases):
@@ -34,7 +33,7 @@ def fuzz_segment_reduce(cases):
   return bad
 
 
-def fuzz_staged_segment_sum(cases):
+def fuzz_lookup_sparse_bags(cases):
   rng0 = np.random.default_rng(777)
   bad = 0
   for it in range(cases):
@@ -51,16 +50,14 @@ def fuzz_staged_segment_sum(cases):
     seg = np.repeat(np.arange(batch), lens).astype(np.int32)
     ids = rng.integers(0, 1100, size=seg.shape[0]).astype(np.int64)   # some ids are not in the table: default row
     w = rng.uniform(0.25, 2.0, size=seg.shape[0]).astype(np.float32) if use_w else None
-    mp = pytest.MonkeyPatch()
     try:
-      _both(mp, t, ot, ids, seg, w, batch, combiner)
+      _check(t, ot, ids, seg, w, batch, combiner)
     except AssertionError as e:
       bad += 1
-      print("MISMATCH staged segment-sum", seed, dim, batch, maxlen, p_empty, combiner, use_w, str(e)[:200])
+      print("MISMATCH det_lookup_sparse bags", seed, dim, batch, maxlen, p_empty, combiner, use_w, str(e)[:200])
     finally:
-      mp.undo()
       t.close()
-  print("segment_sum_staged_kernel:", cases, "cases, mismatches:", bad)
+  print("det_lookup_sparse bags:", cases, "cases, mismatches:", bad)
   return bad
 
 
@@ -265,6 +262,6 @@ def fuzz_owner_side_exchange(cases):
 
 if __name__ == "__main__":
   n = int(sys.argv[1]) if len(sys.argv) > 1 else 400
-  sys.exit(1 if fuzz_segment_reduce(n) + fuzz_staged_segment_sum(max(1, n * 5 // 8)) + fuzz_lookup_one_id_per_row(max(1, n // 2)) +
+  sys.exit(1 if fuzz_segment_reduce(n) + fuzz_lookup_sparse_bags(max(1, n * 5 // 8)) + fuzz_lookup_one_id_per_row(max(1, n // 2)) +
            fuzz_apply_dup(max(1, n // 4)) + fuzz_owner_side_exchange(max(1, n // 10)) else 0)
 

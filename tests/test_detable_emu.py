@@ -508,28 +508,13 @@ def test_bounded_table_purges_tombstones_in_place_before_evicting():
   t.close()
 
 
-# ---- (3) the batched-claim candidate (DET_CLAIM_BATCH=1: probe all 4 rounds, then claim together; common.cuh) ----------
-@pytest.fixture
-def claim_batch(monkeypatch):
-  monkeypatch.setenv("DET_CLAIM_BATCH", "1")   # read by insert_impl at every call
-
-
-def test_batched_claim_standard_path(claim_batch):
-  """the whole standard-path scenario (growth, tombstones, both sentinel-valued keys, accum, export) with inserts going
-  through the batched-claim kernels"""
-  test_standard_path_growth_find_accum_remove_export()
-
-
-def test_batched_claim_contention_duplicates_and_crowded_buckets(claim_batch):
-  """what the batched claim changes is WHEN claims happen: (1) duplicates of a key inside one call -- in the same warp,
-  in different rounds, in different warps -- must still leave ONE copy; (2) many new keys of one call competing for the
-  free slots of the same few buckets (tiny table, load ~0.85): claims that lose their slot go through the serial
-  fallback; (3) tombstones are recycled.  Warps are OS threads here, so the CAS races are real."""
+def test_insert_contention_duplicates_and_crowded_buckets():
+  """claims of one call racing each other: (1) duplicates of a key inside one call -- in the same warp, in different
+  rounds, in different warps -- must still leave ONE copy; (2) many new keys of one call competing for the free slots
+  of the same few buckets (tiny table, load ~0.85) restart their probe when a CAS loses; (3) tombstones are recycled.
+  Warps are OS threads here, so the CAS races are real."""
   rng = np.random.default_rng(5)
   # (1) heavy duplication: 4096 entries over 300 distinct keys, shuffled
-  stat = L().det_emu_stat
-  stat.restype, stat.argtypes = ctypes.c_ulonglong, [ctypes.c_int]
-  steps0, pending0 = stat(0), stat(1)
   t = Table(dim=4, init=8192)
   distinct = rng.choice(1 << 40, size=300, replace=False).astype(np.int64)
   ks = rng.choice(distinct, size=4096)
@@ -570,12 +555,3 @@ def test_batched_claim_contention_duplicates_and_crowded_buckets(claim_batch):
   st = t.stats()
   assert st["error_flags"] == 0 and st["size"] == len(ref)
   t.close()
-  # the candidate path really ran, and so did its fallback (claims that lost their slot to another key)
-  assert stat(0) - steps0 >= 4096 // 32 and stat(1) - pending0 >= 1
-
-
-@settings(max_examples=15, deadline=None, suppress_health_check=[HealthCheck.too_slow, HealthCheck.data_too_large,
-                                                                 HealthCheck.function_scoped_fixture])
-@given(hst.sampled_from([16, 24, 64]), hst.sampled_from([0.0, 0.9]), _OPS)
-def test_batched_claim_random_op_streams(claim_batch, init, lf, ops):
-  test_random_op_streams_against_a_dict.hypothesis.inner_test(init, lf, ops)

@@ -31,12 +31,11 @@ def _reached(cases, fn):
 
 
 def test_case_lists_reach_every_branch():
-  lookup = _reached(K.LOOKUP_CASES, lambda c: K.lookup_kernels(c[0], out_off=c[1], one_per_row=c[2], weighted=c[3],
-                                                               staged=c[4]))
+  lookup = _reached(K.LOOKUP_CASES, lambda c: K.lookup_kernels(c[0], out_off=c[1], one_per_row=c[2], weighted=c[3]))
   assert lookup == K.LOOKUP_BRANCHES, sorted(K.LOOKUP_BRANCHES ^ lookup)
   clip = _reached(K.CLIP_CASES, lambda d: K.lookup_kernels(d, clip=True))
   assert clip == K.CLIP_BRANCHES, sorted(K.CLIP_BRANCHES ^ clip)
-  segsum = _reached(K.SEGSUM_CASES, lambda c: K.lookup_kernels(c[0], rows_off=c[1], out_off=c[2], staged=c[3]))
+  segsum = _reached(K.SEGSUM_CASES, lambda c: K.lookup_kernels(c[0], rows_off=c[1], out_off=c[2]))
   assert segsum == K.SEGSUM_BRANCHES, sorted(K.SEGSUM_BRANCHES ^ segsum)
   apply = _reached(K.APPLY_CASES, K.apply_case_kernels)
   assert apply == K.APPLY_BRANCHES, sorted(K.APPLY_BRANCHES ^ apply)
@@ -139,13 +138,13 @@ def test_f64_check_rejects_one_segment_off_by_a_row():
 
 
 # ---- the GPU bodies on the emulator ---------------------------------------------------------------------------------
-@pytest.mark.parametrize("dim,out_off,one_per_row,weighted,staged", K.LOOKUP_CASES)
-def test_lookup_sparse_paths(emu, dim, out_off, one_per_row, weighted, staged):
-  K.check_lookup_case(dim, out_off, one_per_row, weighted, staged)
+@pytest.mark.parametrize("dim,out_off,one_per_row,weighted,ids_off8", K.LOOKUP_CASES)
+def test_lookup_sparse_paths(emu, dim, out_off, one_per_row, weighted, ids_off8):
+  K.check_lookup_case(dim, out_off, one_per_row, weighted, ids_off=8 if ids_off8 else 0)
 
 
 def test_lookup_sparse_offset_ids(emu):
-  K.check_lookup_case(258, 0, False, False, False, ids_off=8)
+  K.check_lookup_case(258, 0, False, False, ids_off=8)
 
 
 @pytest.mark.parametrize("dim", [64, 6, 7])
@@ -158,9 +157,9 @@ def test_lookup_sparse_clip_paths(emu, dim):
   K.check_clip_case(dim)
 
 
-@pytest.mark.parametrize("dim,rows_off,out_off,staged", K.SEGSUM_CASES)
-def test_sparse_segment_sum_paths(emu, dim, rows_off, out_off, staged):
-  K.check_segsum_case(dim, rows_off, out_off, staged)
+@pytest.mark.parametrize("dim,rows_off,out_off,idx_off8", K.SEGSUM_CASES)
+def test_sparse_segment_sum_paths(emu, dim, rows_off, out_off, idx_off8):
+  K.check_segsum_case(dim, rows_off, out_off, idx_off=8 if idx_off8 else 0)
 
 
 @pytest.mark.parametrize("dim", [258, 1028])
@@ -169,12 +168,9 @@ def test_public_trainable_lookup_wide_rows(emu, dim, combiner):
   K.check_public_trainable(dim, combiner)
 
 
-@pytest.mark.parametrize("case", K.APPLY_CASES, ids=lambda c: "%d-%s-off%d-full%d-scored%d-%s" % (c[:5] + (c[5],)))
+@pytest.mark.parametrize("case", K.APPLY_CASES, ids=lambda c: "%d-%s-off%d-full%d-scored%d" % c)
 def test_apply_paths(emu, case):
-  if case[5] is None:
-    K.check_apply_case(*case)
-  else:
-    K.run_apply_in_child(case)
+  K.check_apply_case(*case)
 
 
 @pytest.mark.parametrize("case", K.DUP_CASES)

@@ -1,7 +1,7 @@
 """Dispatch-matrix parity of the fused kernels (csrc/fused.cu) and the table kernels they share probes with.
 
 Which kernel serves a call depends on dim, on the 16-byte alignment of the caller's pointers, on nnz == batch, on
-weights, on max_norm and on environment knobs.  The other suites take their shapes from the reference's tests and
+weights and on max_norm.  The other suites take their shapes from the reference's tests and
 pass fresh, aligned allocations, so whole branches of that tree ran in no test.  Here every branch is reached on
 purpose -- misalignment comes from views at byte offsets (`buf[1:]` of a float32 buffer is 4 B off, of an int64
 buffer 8 B off) -- and every result is checked two ways:
@@ -12,12 +12,8 @@ buffer 8 B off) -- and every result is checked two ways:
 The dispatch rules are restated in a few lines of Python below; tests/test_kernel_paths_emu.py asserts that the case
 lists reach every branch they name and that the comparison helpers reject deliberately wrong answers, and re-runs
 these bodies over the emulated library (DEV = "cpu", SCALE)."""
-import contextlib
 import ctypes
-import json
 import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -61,7 +57,7 @@ def pick_vec(row_bytes, *offsets):
   return 1
 
 
-def lookup_kernels(dim, out_off=0, rows_off=0, one_per_row=False, weighted=False, clip=False, staged=False):
+def lookup_kernels(dim, out_off=0, rows_off=0, one_per_row=False, weighted=False, clip=False):
   """lookup_sparse_impl / det_sparse_segment_sum: the kernels that serve the call (rows_off: the dense rows of
   det_sparse_segment_sum).  The identity kernel is launched IN FRONT of the general one, which then runs only when
   the device-side check fails, so both are named."""
@@ -70,12 +66,10 @@ def lookup_kernels(dim, out_off=0, rows_off=0, one_per_row=False, weighted=False
   vf = 4 if vec4 else 1
   ks = []
   ivec = pick_vec(dim * 4, out_off)
-  if one_per_row and not weighted and not clip and not staged and vpr <= lpr and ivec >= 4:
+  if one_per_row and not weighted and not clip and vpr <= lpr and ivec >= 4:
     ks.append("lookup_identity_kernel<%d>" % ivec)
   if clip:
     ks.append("segment_sum_kernel<%d,clip>" % vf if vpr <= lpr else "clip_refused")
-  elif vpr <= lpr and vec4 and staged:
-    ks.append("segment_sum_staged_kernel")
   elif vpr <= lpr:
     ks.append("segment_sum_kernel<%d>" % vf)
   else:
@@ -85,31 +79,31 @@ def lookup_kernels(dim, out_off=0, rows_off=0, one_per_row=False, weighted=False
   return tuple(ks)
 
 
-def apply_kernels(dim, grads_off=0, staged=True, ru=1, dup=False, scored=False):
+def apply_kernels(dim, grads_off=0, dup=False, scored=False):
   """apply_common: grads_off is the offset of the gradient / initializer pointer the kernel reads (for the _dup entry
   points: of init_param; their gradients are summed into an aligned workspace first)"""
   vec4 = dim % 4 == 0 and grads_off % 16 == 0
   vpr, lpr = fgeom(dim, vec4)
   if dup and not (vec4 and vpr <= lpr):
     return ("dup_refused",)
-  if (staged or dup) and vec4 and vpr <= lpr:
+  if vec4 and vpr <= lpr:
     return ("apply_staged_kernel<scored>" if scored else "apply_staged_kernel",)
-  return ("apply_kernel<%d,%d>" % (4, ru) if vec4 else "apply_kernel<1,1>",)
+  return ("apply_kernel<4>" if vec4 else "apply_kernel<1>",)
 
 
 # every branch the matrix must reach, per entry point
 LOOKUP_BRANCHES = {"segment_sum_kernel<4>", "segment_sum_kernel<1>", "segment_sum_wide_kernel<4>",
                    "segment_sum_wide_kernel<1>", "column_sweep<4>", "column_sweep<1>", "lookup_identity_kernel<16>",
-                   "lookup_identity_kernel<8>", "lookup_identity_kernel<4>", "segment_sum_staged_kernel"}
+                   "lookup_identity_kernel<8>", "lookup_identity_kernel<4>"}
 CLIP_BRANCHES = {"segment_sum_kernel<4,clip>", "segment_sum_kernel<1,clip>", "clip_refused"}
 SEGSUM_BRANCHES = {"segment_sum_kernel<4>", "segment_sum_kernel<1>", "segment_sum_wide_kernel<4>",
-                   "segment_sum_wide_kernel<1>", "column_sweep<4>", "column_sweep<1>", "segment_sum_staged_kernel"}
-APPLY_BRANCHES = {"apply_staged_kernel", "apply_staged_kernel<scored>", "apply_kernel<4,1>", "apply_kernel<4,2>",
-                  "apply_kernel<1,1>"}
+                   "segment_sum_wide_kernel<1>", "column_sweep<4>", "column_sweep<1>"}
+APPLY_BRANCHES = {"apply_staged_kernel", "apply_staged_kernel<scored>", "apply_kernel<4>", "apply_kernel<1>"}
 DUP_BRANCHES = {"apply_staged_kernel", "dup_refused"}
 
 # ---- the case lists (the coverage self-check reads these) ----
-# det_lookup_sparse: (dim, out_off, one_per_row, weighted, staged)
+# det_lookup_sparse: (dim, out_off, one_per_row, weighted, ids_off8) -- ids_off8: the ids 8 B off a 16 B boundary (key
+# tiles read by plain loads instead of TMA)
 LOOKUP_CASES = [(4, 0, False, True, False), (64, 0, False, False, False), (128, 0, False, True, False),
                 (1, 0, False, True, False), (7, 0, False, False, False), (31, 0, False, True, False),
                 (132, 0, False, True, False), (1024, 0, False, False, False),
@@ -120,21 +114,19 @@ LOOKUP_CASES = [(4, 0, False, True, False), (64, 0, False, False, False), (128, 
                 (64, 0, True, False, False), (6, 0, True, False, False), (7, 0, True, False, False),
                 (64, 0, False, True, True), (16, 0, False, False, True)]
 CLIP_CASES = [128, 31, 132, 33]
-# det_sparse_segment_sum: (dim, rows_off, out_off, staged)
+# det_sparse_segment_sum: (dim, rows_off, out_off, idx_off8) -- idx_off8: row_idx 8 B off a 16 B boundary
 SEGSUM_CASES = [(4, 0, 0, False), (64, 0, 0, False), (7, 0, 0, False), (31, 0, 0, False), (132, 0, 0, False),
                 (1024, 0, 0, False), (33, 0, 0, False), (255, 0, 0, False), (258, 0, 0, False), (301, 0, 0, False),
                 (1028, 0, 0, False), (1300, 0, 0, False), (64, 4, 0, False), (1028, 4, 0, False), (64, 0, 4, False),
                 (64, 0, 0, True)]
-# det_apply_adagrad / _adam: (dim, opt, grads_off, full_init, scored, knob) -- knob: an environment variable the library
-# caches in a function-local static, so those cases run in a child process
-APPLY_CASES = [(16, "adagrad", 0, False, False, None), (128, "adam", 0, False, False, None),
-               (132, "adagrad", 0, False, False, None), (256, "adam", 0, False, False, None),
-               (64, "adagrad", 4, False, False, None), (1, "adam", 0, False, False, None),
-               (7, "adagrad", 0, False, False, None), (16, "adam", 0, True, False, None),
-               (7, "adagrad", 0, True, False, None), (16, "adagrad", 0, False, True, None),
-               (64, "adam", 0, False, True, None),
-               (132, "adagrad", 0, False, False, "DET_APPLY_RU=2"), (132, "adam", 0, False, False, "DET_APPLY_RU=2"),
-               (64, "adagrad", 0, False, False, "DET_APPLY_STAGED=0")]
+# det_apply_adagrad / _adam: (dim, opt, grads_off, full_init, scored)
+APPLY_CASES = [(16, "adagrad", 0, False, False), (128, "adam", 0, False, False),
+               (132, "adagrad", 0, False, False), (256, "adam", 0, False, False),
+               (64, "adagrad", 4, False, False), (1, "adam", 0, False, False),
+               (7, "adagrad", 0, False, False), (16, "adam", 0, True, False),
+               (7, "adagrad", 0, True, False), (16, "adagrad", 0, False, True),
+               (64, "adam", 0, False, True), (132, "adam", 0, False, False), (132, "adagrad", 4, False, False),
+               (64, "adagrad", 0, False, False)]
 # det_apply_*_dup: (dim, opt, ids_off, grads_off, init_off)
 DUP_CASES = [(4, "adagrad", 0, 0, 0), (64, "adam", 0, 0, 0), (128, "adagrad", 0, 0, 0), (32, "adagrad", 8, 0, 0),
              (16, "adam", 0, 4, 0), (16, "adagrad", 0, 0, 4), (6, "adagrad", 0, 0, 0)]
@@ -142,9 +134,8 @@ KEY_COUNTS = [1, 2, 3, 255, 256, 257, 513, "2**20+3"]
 
 
 def apply_case_kernels(case):
-  dim, _, goff, _, scored, knob = case
-  return apply_kernels(dim, goff, staged=knob != "DET_APPLY_STAGED=0", ru=2 if knob == "DET_APPLY_RU=2" else 1,
-                       scored=scored)
+  dim, _, goff, _, scored = case
+  return apply_kernels(dim, goff, scored=scored)
 
 
 def dup_case_kernels(case):
@@ -264,22 +255,6 @@ def host(t):
   return t.cpu().numpy()
 
 
-@contextlib.contextmanager
-def env(name, value):
-  old = os.environ.get(name)
-  if value is None:
-    os.environ.pop(name, None)
-  else:
-    os.environ[name] = value
-  try:
-    yield
-  finally:
-    if old is None:
-      os.environ.pop(name, None)
-    else:
-      os.environ[name] = old
-
-
 def table(dim, planes=0, dtype=torch.float32, init=0, evict=None, max_capacity=0):
   from recommenders_addons_b200 import dynamic_embedding as de
   return de.CuckooHashTable(torch.int64, dtype, default_value=[0] * dim, init_size=init, device=DEV,
@@ -314,7 +289,7 @@ def batch_for(dim, base=400):
 # ------------------------------------------------------------------------------------------------------------------
 # Bodies (shared with the emulator twin)
 # ------------------------------------------------------------------------------------------------------------------
-def check_lookup_case(dim, out_off, one_per_row, weighted, staged, ids_off=0):
+def check_lookup_case(dim, out_off, one_per_row, weighted, ids_off=0):
   rng = np.random.default_rng(dim * 7 + out_off + 3 * one_per_row + weighted)
   batch = batch_for(dim)
   vocab = 3 * batch + 50
@@ -334,14 +309,13 @@ def check_lookup_case(dim, out_off, one_per_row, weighted, staged, ids_off=0):
   ot.insert(present, vals)
   x64 = gather64(present, vals, ids, default)
   d_ids, d_seg, d_w, d_def = dev(ids, ids_off), dev(seg), None if w is None else dev(w), dev(default)
-  with env("DET_SEGSUM_STAGED", "1" if staged else None):
-    for comb in COMBINERS:
-      out = dev_full((batch, dim), out_off)
-      ck(lookup_call(t, d_ids, d_seg, d_w, ids.shape[0], batch, comb, d_def, out))
-      got = host(out)
-      assert_bit_exact(got, O.embedding_lookup_sparse(ot, ids, seg, w, batch, comb, default=default))
-      ref, bound = segment_ref64(x64, seg, w, batch, comb)
-      check_f64(got, ref, bound, "det_lookup_sparse dim %d %s" % (dim, comb))
+  for comb in COMBINERS:
+    out = dev_full((batch, dim), out_off)
+    ck(lookup_call(t, d_ids, d_seg, d_w, ids.shape[0], batch, comb, d_def, out))
+    got = host(out)
+    assert_bit_exact(got, O.embedding_lookup_sparse(ot, ids, seg, w, batch, comb, default=default))
+    ref, bound = segment_ref64(x64, seg, w, batch, comb)
+    check_f64(got, ref, bound, "det_lookup_sparse dim %d %s" % (dim, comb))
 
 
 def check_identity_gate_sequence(dim):
@@ -417,7 +391,7 @@ def segsum_call(rows, dim, idx, seg, w, nnz, batch, combiner, default, out):
                                     P(default), P(out), P(ws), wsb, None)
 
 
-def check_segsum_case(dim, rows_off, out_off, staged):
+def check_segsum_case(dim, rows_off, out_off, idx_off=0):
   rng = np.random.default_rng(dim * 3 + rows_off + out_off)
   batch = batch_for(dim)
   n_rows = max(16, 300 // SCALE)
@@ -428,16 +402,15 @@ def check_segsum_case(dim, rows_off, out_off, staged):
   ot = O.PortTable(dim)
   ot.insert(np.arange(n_rows, dtype=np.int64), rows)
   x64 = np.where((idx >= 0)[:, None], rows[np.maximum(idx, 0)], default[None]).astype(np.float64)
-  d_rows, d_idx, d_seg, d_def = dev(rows, rows_off), dev(idx), dev(seg), dev(default)
-  with env("DET_SEGSUM_STAGED", "1" if staged else None):
-    for comb, ww in (("sum", None), ("mean", w), ("sqrtn", w), ("mean", None)):
-      out = dev_full((batch, dim), out_off)
-      ck(segsum_call(d_rows, dim, d_idx, d_seg, None if ww is None else dev(ww), idx.shape[0], batch, comb, d_def, out))
-      got = host(out)
-      assert_bit_exact(got, O.embedding_lookup_sparse(ot, np.where(idx >= 0, idx, n_rows + 7), seg, ww, batch, comb,
-                                                      default=default))
-      ref, bound = segment_ref64(x64, seg, ww, batch, comb)
-      check_f64(got, ref, bound, "det_sparse_segment_sum dim %d %s" % (dim, comb))
+  d_rows, d_idx, d_seg, d_def = dev(rows, rows_off), dev(idx, idx_off), dev(seg), dev(default)
+  for comb, ww in (("sum", None), ("mean", w), ("sqrtn", w), ("mean", None)):
+    out = dev_full((batch, dim), out_off)
+    ck(segsum_call(d_rows, dim, d_idx, d_seg, None if ww is None else dev(ww), idx.shape[0], batch, comb, d_def, out))
+    got = host(out)
+    assert_bit_exact(got, O.embedding_lookup_sparse(ot, np.where(idx >= 0, idx, n_rows + 7), seg, ww, batch, comb,
+                                                    default=default))
+    ref, bound = segment_ref64(x64, seg, ww, batch, comb)
+    check_f64(got, ref, bound, "det_sparse_segment_sum dim %d %s" % (dim, comb))
 
 
 def check_public_trainable(dim, combiner):
@@ -506,7 +479,7 @@ def assert_planes_equal(t, tabs, slot_init):
     assert (v[~stepped] == np.float32(slot_init)).all()
 
 
-def check_apply_case(dim, opt, grads_off, full_init, scored, knob=None):
+def check_apply_case(dim, opt, grads_off, full_init, scored):
   """three steps on one table: keys new, keys stepped before, keys written by insert (no slot state yet); one step
   passes its keys 8 B off a 16 B boundary (the plain-load tile schedule instead of TMA)"""
   rng = np.random.default_rng(dim * 11 + len(opt) + grads_off + 2 * full_init + 5 * scored)
@@ -532,34 +505,6 @@ def check_apply_case(dim, opt, grads_off, full_init, scored, knob=None):
     ck(apply_call(t, opt, dev(keys, 8 if step == 2 else 0), dev(g, grads_off), n, dev(init, grads_off if full_init else 0),
                   full_init, step))
   assert_planes_equal(t, tabs, 0.1 if opt == "adagrad" else 0.0)
-
-
-def run_apply_in_child(case):
-  """DET_APPLY_RU / DET_APPLY_STAGED are read once per process (function-local statics): a fresh interpreter with the
-  variable set runs the case and exits"""
-  dim, opt, goff, full, scored, knob = case
-  name, value = knob.split("=")
-  payload = json.dumps({"dev": DEV, "scale": SCALE, "case": [dim, opt, goff, full, scored, knob]})
-  code = "import sys; sys.path.insert(0, %r); from tests import test_kernel_paths_gpu as K; K.child_main()" % ROOT
-  e = dict(os.environ)
-  e[name] = value
-  e["DET_KERNEL_PATHS_CHILD"] = payload
-  r = subprocess.run([sys.executable, "-c", code], cwd=ROOT, env=e, capture_output=True, text=True, timeout=600)
-  assert r.returncode == 0, "child exited with %d:\n%s\n%s" % (r.returncode, r.stdout[-3000:], r.stderr[-3000:])
-  assert "apply case passed" in r.stdout
-
-
-def child_main():
-  global DEV, SCALE
-  p = json.loads(os.environ["DET_KERNEL_PATHS_CHILD"])
-  DEV, SCALE = p["dev"], p["scale"]
-  if DEV == "cpu":
-    from tests.emu import backend
-    with backend.installed():
-      check_apply_case(*p["case"])
-  else:
-    check_apply_case(*p["case"])
-  print("apply case passed")
 
 
 def ws_aligned(nbytes):
@@ -801,14 +746,13 @@ def check_accum_dtype(name):
 # ------------------------------------------------------------------------------------------------------------------
 # GPU tests
 # ------------------------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("dim,out_off,one_per_row,weighted,staged", LOOKUP_CASES)
-def test_lookup_sparse_paths(dim, out_off, one_per_row, weighted, staged):
-  check_lookup_case(dim, out_off, one_per_row, weighted, staged)
+@pytest.mark.parametrize("dim,out_off,one_per_row,weighted,ids_off8", LOOKUP_CASES)
+def test_lookup_sparse_paths(dim, out_off, one_per_row, weighted, ids_off8):
+  check_lookup_case(dim, out_off, one_per_row, weighted, ids_off=8 if ids_off8 else 0)
 
 
 def test_lookup_sparse_tma_off_ids():
-  check_lookup_case(64, 0, False, True, False, ids_off=8)
-  check_lookup_case(258, 0, False, False, False, ids_off=8)
+  check_lookup_case(258, 0, False, False, ids_off=8)     # dim 64 with offset ids is a LOOKUP_CASES entry
 
 
 @pytest.mark.parametrize("dim", [64, 6, 7])
@@ -821,9 +765,9 @@ def test_lookup_sparse_clip_paths(dim):
   check_clip_case(dim)
 
 
-@pytest.mark.parametrize("dim,rows_off,out_off,staged", SEGSUM_CASES)
-def test_sparse_segment_sum_paths(dim, rows_off, out_off, staged):
-  check_segsum_case(dim, rows_off, out_off, staged)
+@pytest.mark.parametrize("dim,rows_off,out_off,idx_off8", SEGSUM_CASES)
+def test_sparse_segment_sum_paths(dim, rows_off, out_off, idx_off8):
+  check_segsum_case(dim, rows_off, out_off, idx_off=8 if idx_off8 else 0)
 
 
 @pytest.mark.parametrize("dim", [258, 1028])
@@ -832,12 +776,9 @@ def test_public_trainable_lookup_wide_rows(dim, combiner):
   check_public_trainable(dim, combiner)
 
 
-@pytest.mark.parametrize("case", APPLY_CASES, ids=lambda c: "%d-%s-off%d-full%d-scored%d-%s" % (c[:5] + (c[5],)))
+@pytest.mark.parametrize("case", APPLY_CASES, ids=lambda c: "%d-%s-off%d-full%d-scored%d" % c)
 def test_apply_paths(case):
-  if case[5] is None:
-    check_apply_case(*case)
-  else:
-    run_apply_in_child(case)
+  check_apply_case(*case)
 
 
 @pytest.mark.parametrize("case", DUP_CASES)
