@@ -235,7 +235,11 @@ det_status det_sparse_segment_sum(const float* rows, size_t dim, const int64_t* 
  * copy and the segment_sum input are never materialised:
  * out[b,:] = combine_{i in segment b} w_i * row(ids[i]); missing ids use `default_row` [dim]
  * (broadcast default).  segment_ids are sorted ascending (canonical SparseTensor order);
- * weights may be NULL (all 1).  Rows of `out` without ids are zero.  fp32 tables only.
+ * weights may be NULL (all 1).  Rows of `out` without ids are zero.  Tables of DET_FLOAT32, DET_FLOAT16 or
+ * DET_BFLOAT16 rows (DET_UNIMPLEMENTED for the other dtypes); fp16 / bf16 rows are widened to fp32 as they are read
+ * (exact), so the result is bit-identical to an fp32 table holding the widened rows.  `default_row`, `weights` and `out`
+ * are fp32 whatever the table's dtype, and default_row is used exactly as given: for the reference's result (which casts
+ * the looked-up rows, defaults included, to fp32) pass the table's default row widened to fp32.
  * Uses the table's scratch buffer: one stream per table at a time. */
 det_status det_lookup_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids,
                              const float* weights, size_t nnz, size_t batch, int combiner,
@@ -244,7 +248,9 @@ det_status det_lookup_sparse(det_table* t, const int64_t* ids, const int32_t* se
 /* The same with `max_norm` (embedding_lookup_sparse(..., max_norm); tf.clip_by_norm of every looked-up row BEFORE it is
  * weighted, python/ops/embedding_weights.py:497-521): row <- row * max_norm / max(||row||_2, max_norm), folded into the
  * gather.  max_norm == 0: no clipping (= det_lookup_sparse).  Rows of at most 32 vectors (dim <= 128 when dim % 4 == 0,
- * else dim <= 32); DET_UNIMPLEMENTED beyond.  ABI >= 3. */
+ * else dim <= 32); DET_UNIMPLEMENTED beyond.  max_norm > 0 on a DET_FLOAT16 / DET_BFLOAT16 table is DET_UNIMPLEMENTED:
+ * the reference clips in the table's dtype, which a clip folded into the fp32 gather would not reproduce; use the
+ * composed path (find, clip, det_sparse_segment_sum).  ABI >= 3. */
 det_status det_lookup_sparse_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
                                   const float* weights, size_t nnz, size_t batch, int combiner,
                                   const float* default_row, float max_norm, float* out, det_stream_t stream);

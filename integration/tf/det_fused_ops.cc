@@ -18,8 +18,9 @@ REGISTER_OP("TFRA>DetLookupSparse")
     .Input("ids: int64")           // [nnz] SparseTensor.values
     .Input("segment_ids: int32")   // [nnz] SparseTensor.indices[:, 0], ascending
     .Input("weights: float")       // [nnz] or [0] = all ones
-    .Input("default_row: float")   // [dim]
-    .Output("output: float")       // [batch, dim]
+    .Input("default_row: float")   // [dim]; for a half / bfloat16 table: its default row cast to float
+    .Output("output: float")       // [batch, dim]: float for every table dtype (float, half, bfloat16), as the
+                                   // reference casts the looked-up rows to float (dynamic_embedding_ops.py:232-233)
     .Attr("batch: int >= 0")
     .Attr("combiner: {'sum', 'mean', 'sqrtn'} = 'mean'")
     .Attr("max_norm: float = 0.0");  // > 0: clip every looked-up row to this l2-norm before it is weighted
@@ -77,6 +78,16 @@ REGISTER_OP("TFRA>DetSegmentReduce")
 
 using Table = DetHashTableOfTensorsGpu<int64, float>;
 
+// The library handle of a table whose rows the fused lookup reads (float, half, bfloat16), or nullptr
+static det_table* LookupSparseHandle(tensorflow::lookup::LookupInterface* table) {
+  switch (table->value_dtype()) {
+    case DT_FLOAT: return static_cast<DetHashTableOfTensorsGpu<int64, float>*>(table)->handle();
+    case DT_HALF: return static_cast<DetHashTableOfTensorsGpu<int64, Eigen::half>*>(table)->handle();
+    case DT_BFLOAT16: return static_cast<DetHashTableOfTensorsGpu<int64, bfloat16>*>(table)->handle();
+    default: return nullptr;
+  }
+}
+
 static det_stream_t StreamOf(OpKernelContext* ctx) { return (det_stream_t)ctx->eigen_device<GPUDevice>().stream(); }
 
 class DetLookupSparseOp : public OpKernel {
@@ -94,12 +105,14 @@ class DetLookupSparseOp : public OpKernel {
     tensorflow::lookup::LookupInterface* table = nullptr;
     OP_REQUIRES_OK(ctx, GetLookupTable("table_handle", ctx, &table));
     core::ScopedUnref unref_me(table);
-    Table* t = static_cast<Table*>(table);
+    det_table* handle = LookupSparseHandle(table);
+    OP_REQUIRES(ctx, handle != nullptr,
+                errors::InvalidArgument("DetLookupSparse: the table's value dtype must be float, half or bfloat16"));
     const Tensor& ids = ctx->input(1);
     const Tensor& seg = ctx->input(2);
     const Tensor& w = ctx->input(3);
     const Tensor& def = ctx->input(4);
-    const int64 dim = t->value_shape().dim_size(0);
+    const int64 dim = table->value_shape().dim_size(0);
     OP_REQUIRES(ctx, seg.NumElements() == ids.NumElements(), errors::InvalidArgument("ids and segment_ids differ in length"));
     OP_REQUIRES(ctx, w.NumElements() == 0 || w.NumElements() == ids.NumElements(),
                 errors::InvalidArgument("weights must be empty or have one entry per id"));
@@ -107,7 +120,7 @@ class DetLookupSparseOp : public OpKernel {
     Tensor* out = nullptr;
     OP_REQUIRES_OK(ctx, ctx->allocate_output("output", TensorShape({batch_, dim}), &out));
     OP_REQUIRES_OK(ctx, ToStatus(det_lookup_sparse_clip(
-                            t->handle(), reinterpret_cast<const int64_t*>(ids.flat<int64>().data()),
+                            handle, reinterpret_cast<const int64_t*>(ids.flat<int64>().data()),
                             seg.flat<int32>().data(), w.NumElements() ? w.flat<float>().data() : nullptr,
                             static_cast<size_t>(ids.NumElements()), static_cast<size_t>(batch_), combiner_,
                             def.flat<float>().data(), max_norm_, out->flat<float>().data(), StreamOf(ctx))));

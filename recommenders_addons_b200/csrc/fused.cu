@@ -280,10 +280,152 @@ lookup_identity_kernel(TableView t, const long long* __restrict__ ids, const int
   }
 }
 
+// ---- fp16 / bf16 tables: rows are read in their storage type and widened to fp32 in registers (exact) --------------
+#ifdef DET_EMU
+// The SIMT emulator (tests/emu/) keeps __half / __nv_bfloat16 as 16-bit storage structs and converts them with
+// emu_half_to_float / emu_bf16_to_float; the intrinsics and vector helpers the widening loads call are restated here.
+struct __half2 {
+  __half x, y;
+};
+static inline float __half2float(__half h) { return emu_half_to_float(h); }
+static inline float __bfloat162float(__nv_bfloat16 h) { return emu_bf16_to_float(h); }
+static inline float __low2float(__half2 h) { return emu_half_to_float(h.x); }
+static inline float __high2float(__half2 h) { return emu_half_to_float(h.y); }
+static inline int __float_as_int(float f) {
+  int i;
+  memcpy(&i, &f, 4);
+  return i;
+}
+static inline float __int_as_float(int i) {
+  float f;
+  memcpy(&f, &i, 4);
+  return f;
+}
+static inline int4 make_int4(int x, int y, int z, int w) { return int4{x, y, z, w}; }
+static inline int2 make_int2(int x, int y) { return int2{x, y}; }
+#endif
+__device__ __forceinline__ float widen(__half h) { return __half2float(h); }
+__device__ __forceinline__ float widen(__nv_bfloat16 h) { return __bfloat162float(h); }
+// fp32 bits of element `k` (0 = low half) of a 32-bit word of two 16-bit values.  fp16 converts through __half2, so the
+// conversion reads the half in place (no extract first); a bf16 value is the upper 16 bits of its fp32 value.
+template <typename H> __device__ __forceinline__ int widen_bits(unsigned w, int k);
+template <> __device__ __forceinline__ int widen_bits<__half>(unsigned w, int k) {
+  __half2 h;
+  memcpy(&h, &w, sizeof(h));
+  return __float_as_int(k ? __high2float(h) : __low2float(h));
+}
+template <> __device__ __forceinline__ int widen_bits<__nv_bfloat16>(unsigned w, int k) {
+  return (int)(k ? w & 0xffff0000u : w << 16);
+}
+
+// one OV-byte fp32 vector from the OV / 2 bytes of half row it widens
+template <typename H, int OV> struct WidenVec;
+template <typename H> struct WidenVec<H, 16> {
+  static __device__ __forceinline__ int4 of(int2 r) {
+    return make_int4(widen_bits<H>((unsigned)r.x, 0), widen_bits<H>((unsigned)r.x, 1), widen_bits<H>((unsigned)r.y, 0),
+                     widen_bits<H>((unsigned)r.y, 1));
+  }
+};
+template <typename H> struct WidenVec<H, 8> {
+  static __device__ __forceinline__ int2 of(int r) {
+    return make_int2(widen_bits<H>((unsigned)r, 0), widen_bits<H>((unsigned)r, 1));
+  }
+};
+template <typename H> struct WidenVec<H, 4> {
+  static __device__ __forceinline__ int of(short r) { return widen_bits<H>((unsigned short)r, 0); }
+};
+
+// warp_move_rows for a half table into an fp32 output: lane j's src is a half row (or DET_SRC_DEFAULT = the fp32
+// broadcast row `bdef`), its dst an fp32 row.  g is the geometry of the fp32 OUTPUT row in OV-byte vectors; vector c of
+// the output comes from bytes [c * OV / 2, (c + 1) * OV / 2) of the half row.  Same schedule as warp_move_rows.
+template <typename H, int OV>
+__device__ __forceinline__ void warp_widen_rows(const RowGeom& g, const unsigned char* my_src, unsigned char* my_dst,
+                                                int lane, const unsigned char* bdef) {
+  constexpr int IV = OV / 2;
+  using V = typename VecT<OV>::type;
+  const unsigned rows_per_step = 32u >> g.lpr_shift;
+  const unsigned sub = (unsigned)lane >> g.lpr_shift;
+  const unsigned c0 = (unsigned)lane & (g.lpr - 1u);
+  if (g.vpr == g.lpr) {
+    const V defv = ld_cached<OV>(bdef + c0 * OV);
+    for (unsigned j0 = 0; j0 < 32u; j0 += rows_per_step * 4u) {
+      const unsigned char* s[4];
+      unsigned char* d[4];
+      V v[4];
+#pragma unroll
+      for (int u = 0; u < 4; ++u) {
+        const unsigned j = j0 + u * rows_per_step + sub;
+        const unsigned jj = j & 31u;
+        s[u] = (const unsigned char*)shfl_ll((long long)my_src, jj);
+        d[u] = (unsigned char*)shfl_ll((long long)my_dst, jj);
+        if (j >= 32u) s[u] = nullptr;
+      }
+#pragma unroll
+      for (int u = 0; u < 4; ++u) {
+        v[u] = defv;
+        if (s[u] > DET_SRC_DEFAULT && d[u]) v[u] = WidenVec<H, OV>::of(ld_row<IV>(s[u] + c0 * IV));
+      }
+#pragma unroll
+      for (int u = 0; u < 4; ++u)
+        if (s[u] && d[u]) st_row<OV>(d[u] + c0 * OV, v[u]);
+    }
+  } else {
+    for (unsigned j0 = 0; j0 < 32u; j0 += rows_per_step) {
+      const unsigned j = j0 + sub;
+      const unsigned char* s = (const unsigned char*)shfl_ll((long long)my_src, j & 31u);
+      unsigned char* d = (unsigned char*)shfl_ll((long long)my_dst, j & 31u);
+      if (s && d) {
+        if (s == DET_SRC_DEFAULT) {
+          for (unsigned c = c0; c < g.vpr; c += g.lpr) st_row<OV>(d + c * OV, ld_cached<OV>(bdef + c * OV));
+        } else {
+          for (unsigned c = c0; c < g.vpr; c += g.lpr) st_row<OV>(d + c * OV, WidenVec<H, OV>::of(ld_row<IV>(s + c * IV)));
+        }
+      }
+    }
+  }
+}
+
+// lookup_identity_kernel on a half table: the same gate, key tiles and probe; rows are widened on the way to `out`.
+// g: geometry of the fp32 output row in OV-byte vectors (the half row is read in OV / 2-byte vectors).
+template <typename H, int OV>
+__global__ void __launch_bounds__(kThreadsF)
+lookup_identity_widen_kernel(TableView t, const long long* __restrict__ ids, const int* __restrict__ seg, size_t n,
+                             const unsigned char* __restrict__ default_row, unsigned char* __restrict__ out, RowGeom g,
+                             int use_tma, unsigned* __restrict__ not_identity, unsigned epoch) {
+  __shared__ __align__(128) long long s_keys[kStages][kTileKeys];
+  __shared__ __align__(8) unsigned long long s_bar[kStages];
+  const int lane = threadIdx.x & 31;
+  KeyTiles kt;
+  kt.init(s_keys, s_bar, ids, n, use_tma != 0);
+  for (; kt.valid(); kt.next()) {
+    size_t i;
+    bool valid;
+    const long long key = kt.key(i, valid);
+    const bool off_row = valid && __ldg(seg + i) != (int)i;
+    if (__any_sync(kFull, off_row) && lane == 0) *not_identity = epoch;
+    const long long slot = warp_find_slots<false>(t, key, valid, lane);
+    const unsigned char* src = nullptr;
+    unsigned char* dst = nullptr;
+    if (valid) {
+      src = slot >= 0 ? t.planes[0] + (size_t)slot * t.row_bytes : DET_SRC_DEFAULT;
+      dst = out + i * g.row_bytes;
+    }
+    warp_widen_rows<H, OV>(g, src, dst, lane, default_row);
+  }
+}
+
 template <int VF> struct FVec;
 template <> struct FVec<4> {
   float4 v;
   __device__ __forceinline__ void load(const float* p) { v = *reinterpret_cast<const float4*>(p); }
+  // 4 halves = 8 B (rows of a half table with dim % 4 == 0 are 8 B aligned)
+  template <typename H> __device__ __forceinline__ void load_half(const H* p) {
+    const int2 r = *reinterpret_cast<const int2*>(p);
+    v = make_float4(__int_as_float(widen_bits<H>((unsigned)r.x, 0)), __int_as_float(widen_bits<H>((unsigned)r.x, 1)),
+                    __int_as_float(widen_bits<H>((unsigned)r.y, 0)), __int_as_float(widen_bits<H>((unsigned)r.y, 1)));
+  }
+  __device__ __forceinline__ void load(const __half* p) { load_half(p); }
+  __device__ __forceinline__ void load(const __nv_bfloat16* p) { load_half(p); }
   __device__ __forceinline__ void store(float* p) const { *reinterpret_cast<float4*>(p) = v; }
   __device__ __forceinline__ void zero() { v = make_float4(0.f, 0.f, 0.f, 0.f); }
   __device__ __forceinline__ void fill(float x) { v = make_float4(x, x, x, x); }
@@ -293,11 +435,49 @@ template <> struct FVec<4> {
 template <> struct FVec<1> {
   float v;
   __device__ __forceinline__ void load(const float* p) { v = *p; }
+  __device__ __forceinline__ void load(const __half* p) { v = widen(*p); }
+  __device__ __forceinline__ void load(const __nv_bfloat16* p) { v = widen(*p); }
   __device__ __forceinline__ void store(float* p) const { *p = v; }
   __device__ __forceinline__ void zero() { v = 0.f; }
   __device__ __forceinline__ void fill(float x) { v = x; }
   template <typename F> __device__ __forceinline__ void apply(F f) { f(v); }
   template <typename F> __device__ __forceinline__ void zip(const FVec& o, F f) { f(v, o.v); }
+};
+
+// The row vector segment_sum_kernel holds while its loads are in flight.  An fp32 lane holds the row (or the default
+// row, kept in registers) itself.  A half lane holds the raw 16-bit elements, half the registers, widens them when they
+// are added, and reads the default row from L1 when an id is missing: widening early or keeping the fp32 default row
+// live spills at the kernel's register cap.
+template <int VF, typename H> struct HalfRowVec;
+template <int VF, typename T> struct RowVec : HalfRowVec<VF, T> {};
+template <int VF> struct RowVec<VF, float> : FVec<VF> {
+  __device__ __forceinline__ void init(const FVec<VF>& def) { FVec<VF>::operator=(def); }
+  __device__ __forceinline__ const FVec<VF>& get(const FVec<VF>&, const float*, bool) const { return *this; }
+};
+template <typename H> struct HalfRowVec<4, H> {
+  int2 r;
+  __device__ __forceinline__ void init(const FVec<4>&) {}
+  __device__ __forceinline__ void load(const H* p) { r = *reinterpret_cast<const int2*>(p); }
+  __device__ __forceinline__ FVec<4> get(const FVec<4>&, const float* def, bool loaded) const {
+    FVec<4> x;
+    if (!loaded) {
+      x.v = __ldg(reinterpret_cast<const float4*>(def));
+      return x;
+    }
+    x.v = make_float4(__int_as_float(widen_bits<H>((unsigned)r.x, 0)), __int_as_float(widen_bits<H>((unsigned)r.x, 1)),
+                      __int_as_float(widen_bits<H>((unsigned)r.y, 0)), __int_as_float(widen_bits<H>((unsigned)r.y, 1)));
+    return x;
+  }
+};
+template <typename H> struct HalfRowVec<1, H> {
+  H r;
+  __device__ __forceinline__ void init(const FVec<1>&) {}
+  __device__ __forceinline__ void load(const H* p) { r = *p; }
+  __device__ __forceinline__ FVec<1> get(const FVec<1>&, const float* def, bool loaded) const {
+    FVec<1> x;
+    x.v = loaded ? widen(r) : __ldg(def);
+    return x;
+  }
 };
 
 constexpr int kMaxVecPerLane = 8;
@@ -317,7 +497,9 @@ template <> struct ClipArg<true> { float max_norm; };
 template <bool CLIP> __device__ __forceinline__ float clip_norm_of(const ClipArg<CLIP>&) { return 0.f; }
 template <> __device__ __forceinline__ float clip_norm_of<true>(const ClipArg<true>& c) { return c.max_norm; }
 
-template <int VF, bool CLIP = false>
+// T: the table's row storage type (float, __half or __nv_bfloat16); the lane geometry is that of the fp32 output row,
+// so a lane that reads a 16 B float4 of an fp32 row reads 8 B of a half row.
+template <int VF, bool CLIP = false, typename T = float>
 __global__ void __launch_bounds__(kThreadsF, kSegMinBlocks)
 segment_sum_kernel(TableView t, const long long* __restrict__ slots, const long long* __restrict__ seg_start,
                    const float* __restrict__ weights, size_t batch, int combiner,
@@ -333,10 +515,12 @@ segment_sum_kernel(TableView t, const long long* __restrict__ slots, const long 
   const bool lane_on = gl < vpr;
   const size_t warp0 = ((size_t)blockIdx.x * kThreadsF + threadIdx.x) >> 5;
   const size_t nwarps = ((size_t)gridDim.x * kThreadsF) >> 5;
-  const float* table = (const float*)t.planes[0];
+  const T* table = (const T*)t.planes[0];
   FVec<VF> defv;
   defv.zero();
   if (lane_on) defv.load(default_row + (size_t)gl * VF);
+  // where a half lane reads the default row; lanes beyond the row read (and never store) its first vector
+  const float* def_lane = default_row + (lane_on ? (size_t)gl * VF : 0);
   for (size_t sb = warp0 * gpw * U; sb < batch; sb += nwarps * gpw * U) {
     const size_t b0 = sb + (size_t)gidx * U;
     long long st[U], en[U];
@@ -358,7 +542,7 @@ segment_sum_kernel(TableView t, const long long* __restrict__ slots, const long 
       if (!__any_sync(kFull, any)) break;
       long long sl[U];
       float w[U];
-      FVec<VF> x[U];
+      RowVec<VF, T> x[U];
 #pragma unroll
       for (int u = 0; u < U; ++u) {
         const bool act = st[u] + k < en[u];
@@ -367,10 +551,10 @@ segment_sum_kernel(TableView t, const long long* __restrict__ slots, const long 
       }
 #pragma unroll
       for (int u = 0; u < U; ++u) {
-        x[u] = defv;
+        x[u].init(defv);
         if (sl[u] >= 0 && lane_on) x[u].load(table + (size_t)sl[u] * dim + (size_t)gl * VF);
       }
-      if (CLIP) {
+      if constexpr (CLIP) {   // fp32 tables only
         // row <- row * max_norm / max(||row||, max_norm): the squared norm is summed over the lanes of the group
         // (lanes beyond the row hold zeros); every lane of the warp takes part in the shuffles (uniform loop)
         const float mx = clip_norm_of(clip);
@@ -387,7 +571,7 @@ segment_sum_kernel(TableView t, const long long* __restrict__ slots, const long 
       for (int u = 0; u < U; ++u) {
         if (sl[u] != -2) {
           const float wu = w[u];
-          acc[u].zip(x[u], [wu](float& a, float xv) { a = a + xv * wu; });
+          acc[u].zip(x[u].get(defv, def_lane, sl[u] >= 0 && lane_on), [wu](float& a, float xv) { a = a + xv * wu; });
           wsum[u] = wsum[u] + wu;
           wsq[u] = wsq[u] + wu * wu;
         }
@@ -410,7 +594,25 @@ segment_sum_kernel(TableView t, const long long* __restrict__ slots, const long 
 // kMaxVecPerLane vectors, so a row wider than kMaxVecPerLane * lpr vectors is swept in column chunks of that width;
 // every chunk re-walks the segment's ids in order (same per-column summation order, same wsum / wsq), so the result
 // does not depend on the chunking.  Rows of up to one chunk run the loop body once.
-template <int VF>
+// The row one id of the wide kernel reads: its table row, or the fp32 default row of a missing id.  An fp32 table
+// selects one pointer; a half table keeps the two apart, their element types differ.
+template <typename T> struct WideSrc {
+  const T* row;
+  const float* def;
+  __device__ __forceinline__ WideSrc(const T* table, long long slot, unsigned dim, const float* default_row)
+      : row(slot >= 0 ? table + (size_t)slot * dim : nullptr), def(default_row) {}
+  template <int VF> __device__ __forceinline__ void load(FVec<VF>& x, size_t off) const {
+    if (row) x.load(row + off); else x.load(def + off);
+  }
+};
+template <> struct WideSrc<float> {
+  const float* src;
+  __device__ __forceinline__ WideSrc(const float* table, long long slot, unsigned dim, const float* default_row)
+      : src(slot >= 0 ? table + (size_t)slot * dim : default_row) {}
+  template <int VF> __device__ __forceinline__ void load(FVec<VF>& x, size_t off) const { x.load(src + off); }
+};
+
+template <int VF, typename T = float>
 __global__ void __launch_bounds__(kThreadsF)
 segment_sum_wide_kernel(TableView t, const long long* __restrict__ slots, const long long* __restrict__ seg_start,
                         const float* __restrict__ weights, size_t batch, int combiner,
@@ -424,7 +626,7 @@ segment_sum_wide_kernel(TableView t, const long long* __restrict__ slots, const 
   const unsigned chunk = (unsigned)kMaxVecPerLane * lpr;   // vectors per column chunk
   const size_t warp0 = ((size_t)blockIdx.x * kThreadsF + threadIdx.x) >> 5;
   const size_t nwarps = ((size_t)gridDim.x * kThreadsF) >> 5;
-  const float* table = (const float*)t.planes[0];
+  const T* table = (const T*)t.planes[0];
   for (size_t sb = warp0 * gpw; sb < batch; sb += nwarps * gpw) {
     const size_t b = sb + gidx;
     const bool act_seg = b < batch;
@@ -438,13 +640,13 @@ segment_sum_wide_kernel(TableView t, const long long* __restrict__ slots, const 
       for (long long i = start; i < end; ++i) {
         const long long slot = __ldg(slots + i);
         const float w = weights ? __ldg(weights + i) : 1.f;
-        const float* src = slot >= 0 ? table + (size_t)slot * dim : default_row;
+        const WideSrc<T> src(table, slot, dim, default_row);
 #pragma unroll
         for (int v = 0; v < kMaxVecPerLane; ++v) {
           const unsigned c = c0 + (unsigned)gl + (unsigned)v * lpr;
           if (c < vpr) {
             FVec<VF> x;
-            x.load(src + (size_t)c * VF);
+            src.load(x, (size_t)c * VF);
             acc[v].zip(x, [w](float& a, float xv) { a = a + xv * w; });
           }
         }
@@ -1287,6 +1489,52 @@ static size_t seg_reduce_layout(size_t n, size_t n_groups, unsigned char* base, 
   return off;
 }
 
+// K6 kernels of a table whose rows are T: float, or __half / __nv_bfloat16 rows the kernels widen to fp32
+using IdentityKernel = void (*)(TableView, const long long*, const int*, size_t, const unsigned char*, unsigned char*,
+                                RowGeom, int, unsigned*, unsigned);
+template <typename T> static IdentityKernel identity_kernel(int vec) {
+  if constexpr (std::is_same<T, float>::value) {
+    switch (vec) {
+      case 16: return lookup_identity_kernel<16>;
+      case 8: return lookup_identity_kernel<8>;
+      case 4: return lookup_identity_kernel<4>;
+    }
+  } else {
+    switch (vec) {
+      case 16: return lookup_identity_widen_kernel<T, 16>;
+      case 8: return lookup_identity_widen_kernel<T, 8>;
+      case 4: return lookup_identity_widen_kernel<T, 4>;
+    }
+  }
+  return nullptr;
+}
+
+// K6 phase B without clipping
+template <typename T>
+static void launch_segment_sum(det_table* t, const long long* slots, const long long* seg_start, const float* weights,
+                               size_t batch, int combiner, const float* default_row, float* out, bool vec4, unsigned vpr,
+                               unsigned lpr, unsigned sh, const unsigned* gate, unsigned epoch, cudaStream_t s) {
+  const unsigned gpw = 32u >> sh;
+  if (vpr <= lpr) {
+    const ClipArg<false> noclip;
+    const auto k4 = segment_sum_kernel<4, false, T>;
+    const auto k1 = segment_sum_kernel<1, false, T>;
+    const int occ = vec4 ? occupancy_of(k4, kThreadsF) : occupancy_of(k1, kThreadsF);
+    const int grid = grid_for(batch, (int)(gpw * kSegPerGroup * (kThreadsF / 32)), t->sm_count, occ);
+    if (vec4)
+      DET_LAUNCH(k4, grid, kThreadsF, 0, s, t->view, slots, seg_start, weights, batch, combiner, default_row, out, vpr, lpr, sh, noclip, gate, epoch);
+    else
+      DET_LAUNCH(k1, grid, kThreadsF, 0, s, t->view, slots, seg_start, weights, batch, combiner, default_row, out, vpr, lpr, sh, noclip, gate, epoch);
+  } else {
+    // rows wider than kMaxVecPerLane vectors per lane are swept in column chunks by the same kernel
+    const int grid = grid_for(batch, (int)(gpw * (kThreadsF / 32)), t->sm_count, 8);
+    if (vec4)
+      DET_LAUNCH((segment_sum_wide_kernel<4, T>), grid, kThreadsF, 0, s, t->view, slots, seg_start, weights, batch, combiner, default_row, out, vpr, lpr, sh);
+    else
+      DET_LAUNCH((segment_sum_wide_kernel<1, T>), grid, kThreadsF, 0, s, t->view, slots, seg_start, weights, batch, combiner, default_row, out, vpr, lpr, sh);
+  }
+}
+
 }  // namespace det
 
 using namespace det;
@@ -1331,7 +1579,13 @@ static det_status lookup_sparse_impl(det_table* t, const int64_t* ids, const int
   if (!t) return fail(DET_INVALID_ARGUMENT, "det_lookup_sparse: null table");
   if (!(max_norm >= 0.f)) return fail(DET_INVALID_ARGUMENT, "det_lookup_sparse: max_norm must be >= 0 (0 = no clipping)");
   det::MutLock _lk(t);
-  if (t->cfg.value_dtype != DET_FLOAT32) return fail(DET_UNIMPLEMENTED, "det_lookup_sparse: float32 tables only");
+  const int vt = t->cfg.value_dtype;
+  if (vt != DET_FLOAT32 && vt != DET_FLOAT16 && vt != DET_BFLOAT16)
+    return fail(DET_UNIMPLEMENTED, "det_lookup_sparse: float32, float16 and bfloat16 tables only");
+  // the reference clips in the table's own dtype; a clip folded into the fp32 gather would round differently
+  if (vt != DET_FLOAT32 && max_norm > 0.f)
+    return fail(DET_UNIMPLEMENTED, "det_lookup_sparse_clip: max_norm on float16 / bfloat16 tables is not fused; use the "
+                                   "composed path (lookup, clip in the table's dtype, segment sum)");
   if (combiner < DET_COMBINER_SUM || combiner > DET_COMBINER_SQRTN)
     return fail(DET_INVALID_ARGUMENT, "combiner must be one of 'mean', 'sqrtn' or 'sum'");
   if (batch == 0) return DET_OK;
@@ -1357,7 +1611,9 @@ static det_status lookup_sparse_impl(det_table* t, const int64_t* ids, const int
   // One id per output row and no weights (the Criteo shape: 26 features x batch, one id each): the op is a Find into the
   // dense output.  Whether the segment ids really are 0..nnz-1 is only known on the DEVICE (segment_offsets_kernel
   // computes it): the find-shaped kernel and the general pair are both launched, the flag lets exactly one of them work.
-  const int ivec = pick_vec(t->row_bytes, default_row, out, nullptr);
+  // vector width and geometry of the fp32 OUTPUT row (a half table's rows are read at half that width)
+  const size_t out_row_bytes = (size_t)dim * sizeof(float);
+  const int ivec = pick_vec(out_row_bytes, default_row, out, nullptr);
   const bool try_identity = nnz == batch && nnz > 0 && weights == nullptr && !(max_norm > 0.f) && vpr <= lpr && ivec >= 4;
   const unsigned* gate = try_identity ? not_identity : nullptr;
   // the flag word is compared with a per-table call counter instead of being reset by a memset launch per call
@@ -1370,22 +1626,16 @@ static det_status lookup_sparse_impl(det_table* t, const int64_t* ids, const int
     }
     epoch = ++t->sparse_epoch;
     if (epoch == 0) epoch = ++t->sparse_epoch;
-    const int vec = ivec;
-    const RowGeom g = make_geom((unsigned)t->row_bytes, vec);
+    const RowGeom g = make_geom((unsigned)out_row_bytes, ivec);
     const int tma = (((uintptr_t)ids & 15u) == 0) ? 1 : 0;
     const long long* k = (const long long*)ids;
     const unsigned char* d = (const unsigned char*)default_row;
     unsigned char* o = (unsigned char*)out;
-#define DET_IDENT(VV)                                                                                              \
-  case VV: {                                                                                                        \
-    const int grid = grid_for(nnz, kTileKeys, t->sm_count, occupancy_of(lookup_identity_kernel<VV>, kThreadsF));   \
-    DET_LAUNCH(lookup_identity_kernel<VV>, grid, kThreadsF, 0, s, t->view, k, segment_ids, nnz, d, o, g, tma, not_identity, epoch); \
-  } break;
-    switch (vec) {
-      DET_IDENT(16) DET_IDENT(8) DET_IDENT(4)
-      default: break;
-    }
-#undef DET_IDENT
+    const IdentityKernel kern = vt == DET_FLOAT32   ? identity_kernel<float>(ivec)
+                                : vt == DET_FLOAT16 ? identity_kernel<__half>(ivec)
+                                                    : identity_kernel<__nv_bfloat16>(ivec);
+    const int grid = grid_for(nnz, kTileKeys, t->sm_count, occupancy_of(kern, kThreadsF));
+    DET_LAUNCH(kern, grid, kThreadsF, 0, s, t->view, k, segment_ids, nnz, d, o, g, tma, not_identity, epoch);
   }
   DET_LAUNCH(segment_offsets_kernel, (int)((nnz + 1 + 255) / 256), 256, 0, s, segment_ids, nnz, batch, seg_start, t->view.st, gate, epoch);
   if (nnz)
@@ -1406,21 +1656,12 @@ static det_status lookup_sparse_impl(det_table* t, const int64_t* ids, const int
   } else if (max_norm > 0.f) {
     rc = fail(DET_UNIMPLEMENTED, "det_lookup_sparse_clip: max_norm is fused for rows of at most 32 vectors (dim <= 128 when "
                                  "dim % 4 == 0, else dim <= 32); use the composed path for wider rows");
-  } else if (vpr <= lpr) {
-    const ClipArg<false> noclip;
-    const int occ = vec4 ? occupancy_of(segment_sum_kernel<4>, kThreadsF) : occupancy_of(segment_sum_kernel<1>, kThreadsF);
-    const int grid = grid_for(batch, (int)(gpw * kSegPerGroup * (kThreadsF / 32)), t->sm_count, occ);
-    if (vec4)
-      DET_LAUNCH(segment_sum_kernel<4>, grid, kThreadsF, 0, s, t->view, slots, seg_start, weights, batch, combiner, default_row, out, vpr, lpr, sh, noclip, gate, epoch);
-    else
-      DET_LAUNCH(segment_sum_kernel<1>, grid, kThreadsF, 0, s, t->view, slots, seg_start, weights, batch, combiner, default_row, out, vpr, lpr, sh, noclip, gate, epoch);
+  } else if (vt == DET_FLOAT32) {
+    launch_segment_sum<float>(t, slots, seg_start, weights, batch, combiner, default_row, out, vec4, vpr, lpr, sh, gate, epoch, s);
+  } else if (vt == DET_FLOAT16) {
+    launch_segment_sum<__half>(t, slots, seg_start, weights, batch, combiner, default_row, out, vec4, vpr, lpr, sh, gate, epoch, s);
   } else {
-    // rows wider than kMaxVecPerLane vectors per lane are swept in column chunks by the same kernel
-    const int grid = grid_for(batch, (int)(gpw * (kThreadsF / 32)), t->sm_count, 8);
-    if (vec4)
-      DET_LAUNCH(segment_sum_wide_kernel<4>, grid, kThreadsF, 0, s, t->view, slots, seg_start, weights, batch, combiner, default_row, out, vpr, lpr, sh);
-    else
-      DET_LAUNCH(segment_sum_wide_kernel<1>, grid, kThreadsF, 0, s, t->view, slots, seg_start, weights, batch, combiner, default_row, out, vpr, lpr, sh);
+    launch_segment_sum<__nv_bfloat16>(t, slots, seg_start, weights, batch, combiner, default_row, out, vec4, vpr, lpr, sh, gate, epoch, s);
   }
   if (rc == DET_OK && cudaGetLastError() != cudaSuccess) rc = fail(DET_CUDA_ERROR, "det_lookup_sparse: launch failed");
   return rc;

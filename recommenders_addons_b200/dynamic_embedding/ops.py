@@ -22,17 +22,26 @@ def _table_device_types():
   return table._DEVICE_TYPES   # ("cuda",): the library only ever sees device memory
 
 
+# row dtypes det_lookup_sparse reads; float16 / bfloat16 rows are widened to fp32 in the kernel (exact)
+_FUSED_DTYPES = (torch.float32, torch.float16, torch.bfloat16)
+
+
 def _fused_ok(params, default_rows):
-  return (params.shard_num == 1 and params.value_dtype == torch.float32 and default_rows.numel() == params.dim)
+  return (params.shard_num == 1 and params.value_dtype in _FUSED_DTYPES and default_rows.numel() == params.dim)
 
 
-def _clip_fusable(dim):
-  """rows the fused max_norm covers (det_lookup_sparse_clip): one vector per lane of a 32-lane group"""
+def _clip_fusable(dim, value_dtype=torch.float32):
+  """rows the fused max_norm covers (det_lookup_sparse_clip): one vector per lane of a 32-lane group, fp32 tables only
+  (the reference clips half rows in their own dtype, which a clip in the fp32 gather would not reproduce)"""
+  if value_dtype != torch.float32:
+    return False
   return dim <= 128 if dim % 4 == 0 else dim <= 32
 
 
 def lookup_sparse_fused(params, ids, segment_ids, weights, batch, combiner, default_row=None, max_norm=None):
-  """K6: one kernel does find -> [clip] -> *weight -> per-segment sum -> normalise (det_lookup_sparse[_clip])."""
+  """K6: one kernel does find -> [clip] -> *weight -> per-segment sum -> normalise (det_lookup_sparse[_clip]).
+  float32, float16 and bfloat16 variables (clipping: float32 only); the result is float32, and the default row is the
+  table's default widened to float32, as the reference casts the looked-up rows right after the lookup."""
   table = params.tables[0]
   dev = table.device
   ids = ids.reshape(-1).to(dev).contiguous()
@@ -106,8 +115,10 @@ def embedding_lookup_sparse(params, sp_ids, sp_weights, partition_strategy=None,
   the dense matrix represented by sp_ids, combine (sum / mean / sqrtn) the weighted embeddings of its ids.
   Result: [dense_shape[0], dim] float32.
 
-  Forward-only calls on a single-shard fp32 variable with a constant default row run the fused kernel (with
-  `max_norm` folded into the gather for rows of up to 32 vectors);
+  Forward-only calls on a single-shard float32, float16 or bfloat16 variable with a constant default row run the fused
+  kernel, which widens half rows to float32 as it reads them (the reference casts them right after the lookup, so the
+  result is the same).  `max_norm` is folded into the gather for float32 rows of up to 32 vectors; a half variable with
+  `max_norm` takes the composed path, which clips in the variable's dtype as the reference does;
   `return_trainable=True`, sharded variables and random initializers take the composed
   path (unique -> lookup -> gather*weights -> segment sum), exactly the reference's op sequence."""
   if combiner not in ("mean", "sqrtn", "sum"):
@@ -128,7 +139,7 @@ def embedding_lookup_sparse(params, sp_ids, sp_weights, partition_strategy=None,
   weights = None if ignore_weights else sp_weights.values
   static_default = params.initializer is None or not callable(params.initializer)
   if not return_trainable and static_default and _fused_ok(params, params.tables[0]._default_value) and \
-      (max_norm is None or (float(max_norm) > 0 and _clip_fusable(params.dim))):
+      (max_norm is None or (float(max_norm) > 0 and _clip_fusable(params.dim, params.value_dtype))):
     return lookup_sparse_fused(params, ids, segment_ids, weights, batch, combiner, max_norm=max_norm)
 
   uniq, idx = unique(ids)
