@@ -57,24 +57,6 @@ static det_status read_dev(det_table* t, cudaStream_t s) {
   return DET_OK;
 }
 
-static det_status read_state_e(det_table* t, cudaStream_t s, DevState* out) {
-  CUDA_TRY(cudaMemcpyAsync(t->h_state, t->view.st, sizeof(DevState), cudaMemcpyDeviceToHost, s));
-  CUDA_TRY(cudaStreamSynchronize(s));
-  *out = *t->h_state;
-  return DET_OK;
-}
-
-template <typename F>
-static det_status dispatch_vec_e(int vec, F&& f) {
-  switch (vec) {
-    case 16: return f(std::integral_constant<int, 16>());
-    case 8: return f(std::integral_constant<int, 8>());
-    case 4: return f(std::integral_constant<int, 4>());
-    case 2: return f(std::integral_constant<int, 2>());
-    default: return f(std::integral_constant<int, 1>());
-  }
-}
-
 det_status evict_attach(det_table* t, int strategy) {
   if (strategy < DET_EVICT_LRU || strategy > DET_EVICT_CUSTOMIZED)
     return fail(DET_INVALID_ARGUMENT, "det_table_create: unknown eviction strategy in cfg.flags");
@@ -163,14 +145,12 @@ static det_status repair_rounds(det_table* t, cudaStream_t s) {
   EvictState* ev = t->ev;
   const TableView v = t->view;
   const size_t cap = v.capacity();
-  const int vec = pick_vec(t->row_bytes, nullptr, nullptr, nullptr);
-  const RowGeom g = make_geom((unsigned)t->row_bytes, vec);
   const RowGeom gs = make_geom((unsigned)t->cfg.dim * 4u, 4);
   const int np = t->cfg.num_slot_planes;
   const int rgrid = grid_for(cap, kThreadsE, t->sm_count, 8);
   for (int round = 0; round < 256; ++round) {
     CUDA_TRY(cudaMemsetAsync(&ev->dev->n_moved, 0, 2 * sizeof(unsigned long long), s));  // n_moved, n_erased
-    dispatch_vec_e(vec, [&](auto V) -> det_status {
+    dispatch_vec(t->row_bytes, {}, [&](auto V, const RowGeom& g) -> det_status {
       DET_LAUNCH(repair_move_kernel<decltype(V)::value>, rgrid, kThreadsE, 0, s, v, ev->scores, g, gs, np, ev->dev);
       return DET_OK;
     });
@@ -244,7 +224,7 @@ det_status evict_room(det_table* t, const long long* keys, size_t n, cudaStream_
     return DET_OK;
   }
   DevState ds;
-  det_status st = read_state_e(t, s, &ds);
+  det_status st = read_state(t, s, &ds);
   if (st != DET_OK) return st;
   t->snap_inflight = false;
   t->used_ub = ds.used;
@@ -283,7 +263,7 @@ det_status evict_room(det_table* t, const long long* keys, size_t n, cudaStream_
   if (ds.used > live) {   // tombstones of user removes: purge them in place before any key is evicted for room
     st = purge_tombstones(t, s);
     if (st != DET_OK) return st;
-    st = read_state_e(t, s, &ds);
+    st = read_state(t, s, &ds);
     if (st != DET_OK) return st;
     t->last_used_snap = ds.used;
     if (ds.used + n_adm <= limit) {
@@ -298,7 +278,7 @@ det_status evict_room(det_table* t, const long long* keys, size_t n, cudaStream_
   if (k > live) k = live;
   st = evict_lowest(t, k, s);
   if (st != DET_OK) return st;
-  st = read_state_e(t, s, &ds);
+  st = read_state(t, s, &ds);
   if (st != DET_OK) return st;
   t->last_used_snap = ds.used;
   if (ds.used + n_adm > hard)
@@ -322,8 +302,6 @@ det_status evict_insert(det_table* t, const int64_t* keys, const void* values, c
   const uint64_t max_cap = ((t->cfg.max_capacity + kBucket - 1) / kBucket) * kBucket;
   uint64_t chunk = t->cfg.max_capacity ? (uint64_t)((double)max_cap * t->max_lf) / 4 : (uint64_t)n;
   if (chunk < 1) chunk = 1;
-  const int vec = pick_vec(t->row_bytes, values, nullptr, nullptr);
-  const RowGeom g = make_geom((unsigned)t->row_bytes, vec);
   for (size_t off = 0; off < n; off += chunk) {
     const size_t m = (n - off < chunk) ? n - off : (size_t)chunk;
     const long long* k = (const long long*)keys + off;
@@ -341,7 +319,7 @@ det_status evict_insert(det_table* t, const int64_t* keys, const void* values, c
     const TableView v = t->view;
     const ScoreRule rule = rule_of(t);
     const int np = t->cfg.num_slot_planes;
-    st = dispatch_vec_e(vec, [&](auto V) -> det_status {
+    st = dispatch_vec(t->row_bytes, {{vals, "det_insert: values"}}, [&](auto V, const RowGeom& g) -> det_status {
       constexpr int VV = decltype(V)::value;
       const int grid = grid_for(m, kThreadsE, t->sm_count, occupancy_of(insert_scored_kernel<VV>, kThreadsE));
       DET_LAUNCH(insert_scored_kernel<VV>, grid, kThreadsE, 0, s, v, k, vals, sc_in, mask, m, g, np, ev->scores, rule);
@@ -403,7 +381,7 @@ det_status det_evict(det_table* t, uint64_t n_evict, int64_t* n_evicted_out_host
   if (st != DET_OK) return st;
   if (n_evicted_out_host) *n_evicted_out_host = (int64_t)(t->ev->n_evicted - before);
   DevState ds;
-  st = read_state_e(t, s, &ds);
+  st = read_state(t, s, &ds);
   if (st != DET_OK) return st;
   t->snap_inflight = false;
   t->used_ub = ds.used;

@@ -183,28 +183,21 @@ __global__ void unique_idx_kernel(UniqueWs w, size_t n, int* __restrict__ idx_ou
   idx_out[i] = (int)((s == 0xffffffffu) ? w.special[1] : w.hmin[s]);
 }
 
-static size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
-
 static size_t unique_ws_layout(size_t n, unsigned char* base, UniqueWs* w) {
   const size_t hcap = unique_hcap(n);
   const size_t nblocks = (n + kScanBlock - 1) / kScanBlock;
-  size_t off = 0;
-  auto take = [&](size_t bytes) {
-    unsigned char* p = base ? base + off : nullptr;
-    off += align256(bytes);
-    return p;
-  };
-  long long* hkeys = (long long*)take(hcap * 8);
-  unsigned* hmin = (unsigned*)take(hcap * 4);
-  unsigned* myslot = (unsigned*)take(n * 4);
-  unsigned* flags = (unsigned*)take(n * 4);
-  unsigned* bs = (unsigned*)take((nblocks + 1) * 4);
-  unsigned* sp = (unsigned*)take(16);
+  WsCarver c(base);
+  long long* hkeys = c.take<long long>(hcap * 8);
+  unsigned* hmin = c.take<unsigned>(hcap * 4);
+  unsigned* myslot = c.take<unsigned>(n * 4);
+  unsigned* flags = c.take<unsigned>(n * 4);
+  unsigned* bs = c.take<unsigned>((nblocks + 1) * 4);
+  unsigned* sp = c.take<unsigned>(16);
   if (w) {
     w->hkeys = hkeys; w->hmin = hmin; w->myslot = myslot; w->flags = flags;
     w->block_sums = bs; w->special = sp; w->hcap = hcap;
   }
-  return off;
+  return c.off;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1466,72 +1459,59 @@ struct SegReduceWs {
 
 static size_t seg_reduce_layout(size_t n, size_t n_groups, unsigned char* base, SegReduceWs* w) {
   const size_t nblocks = (n + kRadixTile - 1) / kRadixTile;
-  size_t off = 0;
-  auto take = [&](size_t bytes) {
-    unsigned char* p = base ? base + off : nullptr;
-    off += align256(bytes);
-    return (unsigned*)p;
-  };
-  unsigned* ka = take(n * 4);
-  unsigned* kb = take(n * 4);
-  unsigned* pa = take(n * 4);
-  unsigned* pb = take(n * 4);
-  unsigned* hist = take((size_t)kRadixBins * nblocks * 4);
-  unsigned* totals = take(kRadixBins * 4);
-  unsigned* starts = take((n_groups + 2) * 4);
-  unsigned* ll = take((n / kLongGroup + 2) * 4);
-  unsigned* hl = take((n / kHugeGroup + 2) * 4);
-  unsigned* nl = take(16);
+  WsCarver c(base);
+  unsigned* ka = c.take<unsigned>(n * 4);
+  unsigned* kb = c.take<unsigned>(n * 4);
+  unsigned* pa = c.take<unsigned>(n * 4);
+  unsigned* pb = c.take<unsigned>(n * 4);
+  unsigned* hist = c.take<unsigned>((size_t)kRadixBins * nblocks * 4);
+  unsigned* totals = c.take<unsigned>(kRadixBins * 4);
+  unsigned* starts = c.take<unsigned>((n_groups + 2) * 4);
+  unsigned* ll = c.take<unsigned>((n / kLongGroup + 2) * 4);
+  unsigned* hl = c.take<unsigned>((n / kHugeGroup + 2) * 4);
+  unsigned* nl = c.take<unsigned>(16);
   if (w) {
     w->keys_a = ka; w->keys_b = kb; w->pos_a = pa; w->pos_b = pb; w->hist = hist; w->totals = totals;
     w->starts = starts; w->long_list = ll; w->huge_list = hl; w->n_long = nl;
   }
-  return off;
+  return c.off;
 }
 
-// K6 kernels of a table whose rows are T: float, or __half / __nv_bfloat16 rows the kernels widen to fp32
+// K6 one-id-per-row kernel of a table whose rows are T: float, or __half / __nv_bfloat16 rows it widens to fp32
 using IdentityKernel = void (*)(TableView, const long long*, const int*, size_t, const unsigned char*, unsigned char*,
                                 RowGeom, int, unsigned*, unsigned);
-template <typename T> static IdentityKernel identity_kernel(int vec) {
-  if constexpr (std::is_same<T, float>::value) {
-    switch (vec) {
-      case 16: return lookup_identity_kernel<16>;
-      case 8: return lookup_identity_kernel<8>;
-      case 4: return lookup_identity_kernel<4>;
-    }
-  } else {
-    switch (vec) {
-      case 16: return lookup_identity_widen_kernel<T, 16>;
-      case 8: return lookup_identity_widen_kernel<T, 8>;
-      case 4: return lookup_identity_widen_kernel<T, 4>;
-    }
-  }
-  return nullptr;
+template <typename T, int V> static IdentityKernel identity_kernel() {
+  if constexpr (std::is_same<T, float>::value)
+    return lookup_identity_kernel<V>;
+  else
+    return lookup_identity_widen_kernel<T, V>;
 }
 
-// K6 phase B without clipping
-template <typename T>
-static void launch_segment_sum(det_table* t, const long long* slots, const long long* seg_start, const float* weights,
-                               size_t batch, int combiner, const float* default_row, float* out, bool vec4, unsigned vpr,
-                               unsigned lpr, unsigned sh, const unsigned* gate, unsigned epoch, cudaStream_t s) {
+// K6 phase B: the weighted segment sum of rows of type T gathered through `slots` from the view's plane 0 -- the looked-up
+// table rows of det_lookup_sparse, or the dense matrix of det_sparse_segment_sum.  sms: SM count the grid is sized for.
+// A clipping launch (CLIP) needs rows of at most 32 vectors (vpr <= lpr).
+template <typename T, bool CLIP>
+static void launch_segment_sum(const TableView& v, int sms, const long long* slots, const long long* seg_start,
+                               const float* weights, size_t batch, int combiner, const float* default_row, float* out,
+                               bool vec4, unsigned vpr, unsigned lpr, unsigned sh, const ClipArg<CLIP>& clip,
+                               const unsigned* gate, unsigned epoch, cudaStream_t s) {
   const unsigned gpw = 32u >> sh;
   if (vpr <= lpr) {
-    const ClipArg<false> noclip;
-    const auto k4 = segment_sum_kernel<4, false, T>;
-    const auto k1 = segment_sum_kernel<1, false, T>;
+    const auto k4 = segment_sum_kernel<4, CLIP, T>;
+    const auto k1 = segment_sum_kernel<1, CLIP, T>;
     const int occ = vec4 ? occupancy_of(k4, kThreadsF) : occupancy_of(k1, kThreadsF);
-    const int grid = grid_for(batch, (int)(gpw * kSegPerGroup * (kThreadsF / 32)), t->sm_count, occ);
+    const int grid = grid_for(batch, (int)(gpw * kSegPerGroup * (kThreadsF / 32)), sms, occ);
     if (vec4)
-      DET_LAUNCH(k4, grid, kThreadsF, 0, s, t->view, slots, seg_start, weights, batch, combiner, default_row, out, vpr, lpr, sh, noclip, gate, epoch);
+      DET_LAUNCH(k4, grid, kThreadsF, 0, s, v, slots, seg_start, weights, batch, combiner, default_row, out, vpr, lpr, sh, clip, gate, epoch);
     else
-      DET_LAUNCH(k1, grid, kThreadsF, 0, s, t->view, slots, seg_start, weights, batch, combiner, default_row, out, vpr, lpr, sh, noclip, gate, epoch);
+      DET_LAUNCH(k1, grid, kThreadsF, 0, s, v, slots, seg_start, weights, batch, combiner, default_row, out, vpr, lpr, sh, clip, gate, epoch);
   } else {
     // rows wider than kMaxVecPerLane vectors per lane are swept in column chunks by the same kernel
-    const int grid = grid_for(batch, (int)(gpw * (kThreadsF / 32)), t->sm_count, 8);
+    const int grid = grid_for(batch, (int)(gpw * (kThreadsF / 32)), sms, 8);
     if (vec4)
-      DET_LAUNCH((segment_sum_wide_kernel<4, T>), grid, kThreadsF, 0, s, t->view, slots, seg_start, weights, batch, combiner, default_row, out, vpr, lpr, sh);
+      DET_LAUNCH((segment_sum_wide_kernel<4, T>), grid, kThreadsF, 0, s, v, slots, seg_start, weights, batch, combiner, default_row, out, vpr, lpr, sh);
     else
-      DET_LAUNCH((segment_sum_wide_kernel<1, T>), grid, kThreadsF, 0, s, t->view, slots, seg_start, weights, batch, combiner, default_row, out, vpr, lpr, sh);
+      DET_LAUNCH((segment_sum_wide_kernel<1, T>), grid, kThreadsF, 0, s, v, slots, seg_start, weights, batch, combiner, default_row, out, vpr, lpr, sh);
   }
 }
 
@@ -1597,7 +1577,7 @@ static det_status lookup_sparse_impl(det_table* t, const int64_t* ids, const int
   unsigned* not_identity = nullptr;
   {
     void* sc = nullptr;
-    const size_t seg_bytes = ((batch + 1) * sizeof(long long) + 255) & ~(size_t)255;
+    const size_t seg_bytes = align256((batch + 1) * sizeof(long long));
     det_status sst = table_scratch(t, 256 + seg_bytes + (nnz ? nnz : 1) * sizeof(long long), &sc);
     if (sst != DET_OK) return sst;
     not_identity = (unsigned*)sc;
@@ -1613,7 +1593,7 @@ static det_status lookup_sparse_impl(det_table* t, const int64_t* ids, const int
   // computes it): the find-shaped kernel and the general pair are both launched, the flag lets exactly one of them work.
   // vector width and geometry of the fp32 OUTPUT row (a half table's rows are read at half that width)
   const size_t out_row_bytes = (size_t)dim * sizeof(float);
-  const int ivec = pick_vec(out_row_bytes, default_row, out, nullptr);
+  const int ivec = vec_width(out_row_bytes | (uintptr_t)default_row | (uintptr_t)out);
   const bool try_identity = nnz == batch && nnz > 0 && weights == nullptr && !(max_norm > 0.f) && vpr <= lpr && ivec >= 4;
   const unsigned* gate = try_identity ? not_identity : nullptr;
   // the flag word is compared with a per-table call counter instead of being reset by a memset launch per call
@@ -1626,42 +1606,43 @@ static det_status lookup_sparse_impl(det_table* t, const int64_t* ids, const int
     }
     epoch = ++t->sparse_epoch;
     if (epoch == 0) epoch = ++t->sparse_epoch;
-    const RowGeom g = make_geom((unsigned)out_row_bytes, ivec);
     const int tma = (((uintptr_t)ids & 15u) == 0) ? 1 : 0;
     const long long* k = (const long long*)ids;
     const unsigned char* d = (const unsigned char*)default_row;
     unsigned char* o = (unsigned char*)out;
-    const IdentityKernel kern = vt == DET_FLOAT32   ? identity_kernel<float>(ivec)
-                                : vt == DET_FLOAT16 ? identity_kernel<__half>(ivec)
-                                                    : identity_kernel<__nv_bfloat16>(ivec);
-    const int grid = grid_for(nnz, kTileKeys, t->sm_count, occupancy_of(kern, kThreadsF));
-    DET_LAUNCH(kern, grid, kThreadsF, 0, s, t->view, k, segment_ids, nnz, d, o, g, tma, not_identity, epoch);
+    dispatch_vec<4>(out_row_bytes, {{default_row, "det_lookup_sparse: default_row"}, {out, "det_lookup_sparse: out"}},
+                    [&](auto V, const RowGeom& g) -> det_status {
+      constexpr int VV = decltype(V)::value;
+      const IdentityKernel kern = vt == DET_FLOAT32   ? identity_kernel<float, VV>()
+                                  : vt == DET_FLOAT16 ? identity_kernel<__half, VV>()
+                                                      : identity_kernel<__nv_bfloat16, VV>();
+      const int grid = grid_for(nnz, kTileKeys, t->sm_count, occupancy_of(kern, kThreadsF));
+      DET_LAUNCH(kern, grid, kThreadsF, 0, s, t->view, k, segment_ids, nnz, d, o, g, tma, not_identity, epoch);
+      return DET_OK;
+    });
   }
   DET_LAUNCH(segment_offsets_kernel, (int)((nnz + 1 + 255) / 256), 256, 0, s, segment_ids, nnz, batch, seg_start, t->view.st, gate, epoch);
   if (nnz)
     DET_LAUNCH(resolve_slots_kernel, grid_for(nnz, kTileKeys, t->sm_count, occupancy_of(resolve_slots_kernel, kThreadsF)), kThreadsF, 0, s, t->view, (const long long*)ids, nnz, slots, (((uintptr_t)ids & 15u) == 0) ? 1 : 0, gate, epoch);
   det_status rc = DET_OK;
-  const unsigned gpw = 32u >> sh;
+  const ClipArg<false> noclip;
   if (vpr <= lpr && max_norm > 0.f) {
     ClipArg<true> clip;
     clip.max_norm = max_norm;
-    const auto k4 = segment_sum_kernel<4, true>;
-    const auto k1 = segment_sum_kernel<1, true>;
-    const int occ = vec4 ? occupancy_of(k4, kThreadsF) : occupancy_of(k1, kThreadsF);
-    const int grid = grid_for(batch, (int)(gpw * kSegPerGroup * (kThreadsF / 32)), t->sm_count, occ);
-    if (vec4)
-      DET_LAUNCH(k4, grid, kThreadsF, 0, s, t->view, slots, seg_start, weights, batch, combiner, default_row, out, vpr, lpr, sh, clip, (const unsigned*)nullptr, 0u);
-    else
-      DET_LAUNCH(k1, grid, kThreadsF, 0, s, t->view, slots, seg_start, weights, batch, combiner, default_row, out, vpr, lpr, sh, clip, (const unsigned*)nullptr, 0u);
+    launch_segment_sum<float>(t->view, t->sm_count, slots, seg_start, weights, batch, combiner, default_row, out, vec4, vpr,
+                              lpr, sh, clip, gate, epoch, s);
   } else if (max_norm > 0.f) {
     rc = fail(DET_UNIMPLEMENTED, "det_lookup_sparse_clip: max_norm is fused for rows of at most 32 vectors (dim <= 128 when "
                                  "dim % 4 == 0, else dim <= 32); use the composed path for wider rows");
   } else if (vt == DET_FLOAT32) {
-    launch_segment_sum<float>(t, slots, seg_start, weights, batch, combiner, default_row, out, vec4, vpr, lpr, sh, gate, epoch, s);
+    launch_segment_sum<float>(t->view, t->sm_count, slots, seg_start, weights, batch, combiner, default_row, out, vec4, vpr,
+                              lpr, sh, noclip, gate, epoch, s);
   } else if (vt == DET_FLOAT16) {
-    launch_segment_sum<__half>(t, slots, seg_start, weights, batch, combiner, default_row, out, vec4, vpr, lpr, sh, gate, epoch, s);
+    launch_segment_sum<__half>(t->view, t->sm_count, slots, seg_start, weights, batch, combiner, default_row, out, vec4, vpr,
+                               lpr, sh, noclip, gate, epoch, s);
   } else {
-    launch_segment_sum<__nv_bfloat16>(t, slots, seg_start, weights, batch, combiner, default_row, out, vec4, vpr, lpr, sh, gate, epoch, s);
+    launch_segment_sum<__nv_bfloat16>(t->view, t->sm_count, slots, seg_start, weights, batch, combiner, default_row, out,
+                                      vec4, vpr, lpr, sh, noclip, gate, epoch, s);
   }
   if (rc == DET_OK && cudaGetLastError() != cudaSuccess) rc = fail(DET_CUDA_ERROR, "det_lookup_sparse: launch failed");
   return rc;
@@ -1707,45 +1688,37 @@ static det_status apply_common(det_table* t, const int64_t* keys, const float* g
     const int ns = opt == 0 ? 3 : 4;
     const size_t smem = (size_t)(kThreadsF / 32) * 2 * kStageSteps * ns * 32 * 16;
     const int tma = (((uintptr_t)keys & 15u) == 0) ? 1 : 0;
-    int occ = 1;
-    const bool scored = t->ev != nullptr;
-#define DET_LAUNCH_STAGED(OPT_, SCORED_, SA_)                                                                       \
-  {                                                                                                               \
-    const auto kern = apply_staged_kernel<OPT_, SCORED_>;                                                         \
-    CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));                 \
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, kThreadsF, smem) != cudaSuccess || occ < 1) occ = 1; \
-    DET_LAUNCH(kern, grid_for(n, kTileKeys, t->sm_count, occ), kThreadsF, smem, s, v, k, grads, n, h, init_param, \
-               full_init, vpr, lpr, sh, tma, SA_, n_dev);                                                         \
-  }
-    if (scored) {
-      ScoreArg<true> sa;
-      sa.sc = evict_scores(t);
-      sa.rule = evict_rule(t);
-      if (opt == 0) DET_LAUNCH_STAGED(0, true, sa) else DET_LAUNCH_STAGED(1, true, sa)
-    } else {
-      const ScoreArg<false> sa;
-      if (opt == 0) DET_LAUNCH_STAGED(0, false, sa) else DET_LAUNCH_STAGED(1, false, sa)
-    }
-#undef DET_LAUNCH_STAGED
+    st = dispatch_bit(t->ev != nullptr, [&](auto SCORED) -> det_status {
+      return dispatch_bit(opt != 0, [&](auto OPT) -> det_status {
+        constexpr bool kScored = decltype(SCORED)::value;
+        ScoreArg<kScored> sa;
+        if constexpr (kScored) {
+          sa.sc = evict_scores(t);
+          sa.rule = evict_rule(t);
+        }
+        const auto kern = apply_staged_kernel<decltype(OPT)::value, kScored>;
+        CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        int occ = 1;
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, kThreadsF, smem) != cudaSuccess || occ < 1) occ = 1;
+        DET_LAUNCH(kern, grid_for(n, kTileKeys, t->sm_count, occ), kThreadsF, smem, s, v, k, grads, n, h, init_param,
+                   full_init, vpr, lpr, sh, tma, sa, n_dev);
+        return DET_OK;
+      });
+    });
+    if (st != DET_OK) return st;
     CUDA_TRY(cudaGetLastError());
     note_mutation(t, n, s);
     return DET_OK;   // scores of a table with an eviction strategy were written by the kernel itself
   }
-#define DET_LAUNCH_APPLY(VF_, OPT_)                                                                           \
-  {                                                                                                           \
-    const int grid = grid_for(n, kTileKeys, t->sm_count, occupancy_of(apply_kernel<VF_, OPT_>, kThreadsF));   \
-    const auto kern = apply_kernel<VF_, OPT_>;                                                                \
-    DET_LAUNCH(kern, grid, kThreadsF, 0, s, v, k, grads, n, h, init_param, full_init, vpr, lpr, sh,                   \
-                                    (((uintptr_t)keys & 15u) == 0) ? 1 : 0);                                  \
-  }
-  if (opt == 0) {
-    if (vec4) DET_LAUNCH_APPLY(4, 0)
-    else DET_LAUNCH_APPLY(1, 0)
-  } else {
-    if (vec4) DET_LAUNCH_APPLY(4, 1)
-    else DET_LAUNCH_APPLY(1, 1)
-  }
-#undef DET_LAUNCH_APPLY
+  dispatch_bit(opt != 0, [&](auto OPT) -> det_status {
+    return dispatch_bit(vec4, [&](auto VEC4) -> det_status {
+      const auto kern = apply_kernel<decltype(VEC4)::value ? 4 : 1, decltype(OPT)::value>;
+      const int grid = grid_for(n, kTileKeys, t->sm_count, occupancy_of(kern, kThreadsF));
+      DET_LAUNCH(kern, grid, kThreadsF, 0, s, v, k, grads, n, h, init_param, full_init, vpr, lpr, sh,
+                 (((uintptr_t)keys & 15u) == 0) ? 1 : 0);
+      return DET_OK;
+    });
+  });
   CUDA_TRY(cudaGetLastError());
   note_mutation(t, n, s);
   if (t->ev) return evict_touch(t, k, nullptr, n, s);
@@ -1800,29 +1773,17 @@ static det_status permute_rows(const void* in, const int32_t* perm, size_t n, si
                                cudaStream_t s) {
   if (n == 0) return DET_OK;
   if (!in || !perm || !out || row_bytes == 0) return fail(DET_INVALID_ARGUMENT, "det_*_rows: null argument");
-  const int vec = pick_vec(row_bytes, in, out, nullptr);
-  const RowGeom g = make_geom((unsigned)row_bytes, vec);
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  const int grid = grid_for(n, kThreadsF, sms, 8);
+  const int grid = grid_for(n, kThreadsF, current_sm_count(), 8);
   const unsigned char* i = (const unsigned char*)in;
   unsigned char* o = (unsigned char*)out;
-#define LAUNCH(V)                                                        \
-  {                                                                      \
-    const auto ks = permute_rows_kernel<V, true>;                        \
-    const auto kg = permute_rows_kernel<V, false>;                       \
-    if (scatter) DET_LAUNCH(ks, grid, kThreadsF, 0, s, i, perm, n, o, g);        \
-    else DET_LAUNCH(kg, grid, kThreadsF, 0, s, i, perm, n, o, g);                \
-  }
-  switch (vec) {
-    case 16: LAUNCH(16) break;
-    case 8: LAUNCH(8) break;
-    case 4: LAUNCH(4) break;
-    case 2: LAUNCH(2) break;
-    default: LAUNCH(1) break;
-  }
-#undef LAUNCH
+  dispatch_vec(row_bytes, {{in, "det_*_rows: rows_in"}, {out, "det_*_rows: rows_out"}}, [&](auto V, const RowGeom& g) -> det_status {
+    constexpr int VV = decltype(V)::value;
+    const auto ks = permute_rows_kernel<VV, true>;
+    const auto kg = permute_rows_kernel<VV, false>;
+    if (scatter) DET_LAUNCH(ks, grid, kThreadsF, 0, s, i, perm, n, o, g);
+    else DET_LAUNCH(kg, grid, kThreadsF, 0, s, i, perm, n, o, g);
+    return DET_OK;
+  });
   CUDA_TRY(cudaGetLastError());
   return DET_OK;
 }
@@ -1865,30 +1826,14 @@ det_status det_sparse_segment_sum(const float* rows, size_t dim, const int64_t* 
   v.dim = (unsigned)dim;
   v.row_bytes = (unsigned)dim * 4u;
   v.st = st;
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  const int sms = current_sm_count();
   DET_LAUNCH(segment_offsets_kernel, (int)((nnz + 1 + 255) / 256), 256, 0, s, segment_ids, nnz, batch, seg_start, st, (const unsigned*)nullptr, 0u);
   const long long* slots = (const long long*)row_idx;
   const bool vec4 = (dim % 4 == 0) && ((((uintptr_t)default_row | (uintptr_t)out | (uintptr_t)rows) & 15u) == 0);
   unsigned vpr, lpr, sh;
   fgeom((unsigned)dim, vec4, 1, &vpr, &lpr, &sh);
-  const unsigned gpw = 32u >> sh;
-  if (vpr <= lpr) {
-    const ClipArg<false> noclip;
-    const int occ = vec4 ? occupancy_of(segment_sum_kernel<4>, kThreadsF) : occupancy_of(segment_sum_kernel<1>, kThreadsF);
-    const int grid = grid_for(batch, (int)(gpw * kSegPerGroup * (kThreadsF / 32)), sms, occ);
-    if (vec4)
-      DET_LAUNCH(segment_sum_kernel<4>, grid, kThreadsF, 0, s, v, slots, seg_start, weights, batch, combiner, default_row, out, vpr, lpr, sh, noclip, (const unsigned*)nullptr, 0u);
-    else
-      DET_LAUNCH(segment_sum_kernel<1>, grid, kThreadsF, 0, s, v, slots, seg_start, weights, batch, combiner, default_row, out, vpr, lpr, sh, noclip, (const unsigned*)nullptr, 0u);
-  } else {
-    const int grid = grid_for(batch, (int)(gpw * (kThreadsF / 32)), sms, 8);
-    if (vec4)
-      DET_LAUNCH(segment_sum_wide_kernel<4>, grid, kThreadsF, 0, s, v, slots, seg_start, weights, batch, combiner, default_row, out, vpr, lpr, sh);
-    else
-      DET_LAUNCH(segment_sum_wide_kernel<1>, grid, kThreadsF, 0, s, v, slots, seg_start, weights, batch, combiner, default_row, out, vpr, lpr, sh);
-  }
+  launch_segment_sum<float>(v, sms, slots, seg_start, weights, batch, combiner, default_row, out, vec4, vpr, lpr, sh,
+                            ClipArg<false>(), nullptr, 0u, s);
   CUDA_TRY(cudaGetLastError());
   return DET_OK;
 }
@@ -1933,9 +1878,7 @@ static det_status seg_reduce_run(const float* rows, const int32_t* idx, size_t n
     pout = (pout == w.pos_a) ? w.pos_b : w.pos_a;
   }
   DET_LAUNCH(group_starts_kernel, (int)((n + 1 + 255) / 256), 256, 0, s, kin, n, ng, w.starts, ngd, n_dev, w.n_long);
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  const int sms = current_sm_count();
   const bool vec4 = (dim % 4 == 0) && ((((uintptr_t)rows | (uintptr_t)out) & 15u) == 0);
   // rows that can be cut into 16-column slices (the double-buffered cp.async staging moves 16 B vectors)
   const int sliceable = (vec4 && dim % kSliceCols == 0 && dim > (size_t)kSliceCols) ? 1 : 0;
@@ -1985,24 +1928,19 @@ struct DupWs {
   size_t sws_bytes;
 };
 static size_t dup_layout(size_t n, size_t dim, unsigned char* base, DupWs* w) {
-  size_t off = 0;
-  auto take = [&](size_t bytes) {
-    unsigned char* p = base ? base + off : nullptr;
-    off += align256(bytes);
-    return p;
-  };
+  WsCarver c(base);
   const size_t ub = unique_ws_layout(n, nullptr, nullptr), sb = seg_reduce_layout(n, n, nullptr, nullptr);
-  unsigned char* uniq = take(n * 8);
-  unsigned char* idx = take(n * 4);
-  unsigned char* cnt = take(16);
-  unsigned char* uws = take(ub);
-  unsigned char* gsum = take(n * dim * 4);
-  unsigned char* sws = take(sb);
+  long long* uniq = c.take<long long>(n * 8);
+  int* idx = c.take<int>(n * 4);
+  long long* cnt = c.take<long long>(16);
+  unsigned char* uws = c.take(ub);
+  float* gsum = c.take<float>(n * dim * 4);
+  unsigned char* sws = c.take(sb);
   if (w) {
-    w->uniq = (long long*)uniq; w->idx = (int*)idx; w->cnt = (long long*)cnt; w->uws = uws; w->uws_bytes = ub;
-    w->gsum = (float*)gsum; w->sws = sws; w->sws_bytes = sb;
+    w->uniq = uniq; w->idx = idx; w->cnt = cnt; w->uws = uws; w->uws_bytes = ub;
+    w->gsum = gsum; w->sws = sws; w->sws_bytes = sb;
   }
-  return off;
+  return c.off;
 }
 
 size_t det_apply_dup_workspace_bytes(size_t n, size_t dim) { return dup_layout(n ? n : 1, dim ? dim : 1, nullptr, nullptr); }

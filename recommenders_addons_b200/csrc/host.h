@@ -9,6 +9,7 @@
 #include <stdlib.h>
 
 #include <atomic>
+#include <initializer_list>
 #include <mutex>
 #include <shared_mutex>
 #include <string>
@@ -96,8 +97,79 @@ struct EvictState;  // score plane + eviction bookkeeping of a table with an evi
 
 size_t dtype_size(int dt);
 RowGeom make_geom(unsigned row_bytes, int vec);
-int pick_vec(size_t row_bytes, const void* a, const void* b, const void* c);
 int grid_for(size_t n_items, int items_per_block, int sm_count, int blocks_per_sm);
+
+inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
+
+// Consecutive 256 B aligned regions of a workspace.  With base == nullptr, take() returns nullptr and `off` adds up the
+// size a caller has to provide.
+struct WsCarver {
+  unsigned char* base;
+  size_t off = 0;
+  explicit WsCarver(void* b) : base((unsigned char*)b) {}
+  template <typename T = unsigned char>
+  T* take(size_t bytes) {
+    unsigned char* p = base ? base + off : nullptr;
+    off += align256(bytes);
+    return (T*)p;
+  }
+};
+
+// SM count of the current device (entry points without a table)
+inline int current_sm_count() {
+  int dev = 0, sms = 132;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  return sms;
+}
+
+// Widest vector width (16, 8, 4, 2 or 1 bytes) that divides `bits`: a row size OR-ed with the addresses of the rows.
+inline int vec_width(uintptr_t bits) {
+  if ((bits & 15u) == 0) return 16;
+  if ((bits & 7u) == 0) return 8;
+  if ((bits & 3u) == 0) return 4;
+  if ((bits & 1u) == 0) return 2;
+  return 1;
+}
+
+// A row operand of a launch: its address and the name an error message gives it.
+struct RowArg {
+  const void* p;
+  const char* name;
+};
+
+template <int V, int MinVec, typename F>
+det_status call_vec(int vec, const RowGeom& g, F& f) {
+  if constexpr (V > MinVec) {
+    if (vec < V) return call_vec<V / 2, MinVec>(vec, g, f);
+  }
+  return f(std::integral_constant<int, V>(), g);
+}
+
+// The launch dispatch over row vector widths.  V is the widest width that divides row_bytes and the address of every
+// operand; f receives std::integral_constant<int, V> together with make_geom(row_bytes, V), so a kernel never runs with
+// the geometry of another width.  Only the widths 16 down to MinVec are instantiated: when V is narrower, nothing is
+// launched and the call fails with DET_INVALID_ARGUMENT naming the operand that is not MinVec-byte aligned.
+template <int MinVec = 1, typename F>
+det_status dispatch_vec(size_t row_bytes, std::initializer_list<RowArg> ops, F&& f) {
+  uintptr_t bits = (uintptr_t)row_bytes;
+  for (const RowArg& a : ops) bits |= (uintptr_t)a.p;
+  const int vec = vec_width(bits);
+  if (vec < MinVec) {
+    for (const RowArg& a : ops)
+      if ((uintptr_t)a.p % MinVec != 0)
+        return fail(DET_INVALID_ARGUMENT, std::string(a.name) + " must be " + std::to_string(MinVec) + "-byte aligned");
+    return fail(DET_INVALID_ARGUMENT, "detable: rows of " + std::to_string(row_bytes) + " bytes are not a multiple of " +
+                                          std::to_string(MinVec) + " bytes");
+  }
+  return call_vec<16, MinVec>(vec, make_geom((unsigned)row_bytes, vec), f);
+}
+
+// f(std::integral_constant<int, 0 or 1>): a run-time choice between two instantiations of a kernel
+template <typename F>
+det_status dispatch_bit(bool b, F&& f) {
+  return b ? f(std::integral_constant<int, 1>()) : f(std::integral_constant<int, 0>());
+}
 
 }  // namespace det
 
@@ -167,6 +239,14 @@ struct MutLock {
   MutLock(const MutLock&) = delete;
   MutLock& operator=(const MutLock&) = delete;
 };
+
+// the table's DevState, read synchronously through its pinned mirror
+inline det_status read_state(det_table* t, cudaStream_t s, DevState* out) {
+  CUDA_TRY(cudaMemcpyAsync(t->h_state, t->view.st, sizeof(DevState), cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaStreamSynchronize(s));
+  *out = *t->h_state;
+  return DET_OK;
+}
 }  // namespace det
 
 namespace det {

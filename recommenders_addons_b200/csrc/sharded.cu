@@ -826,11 +826,9 @@ det_status det_peer_group_create_regions(det_peer_group** out, det_table* local,
   return DET_OK;
 }
 
-static size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
-
 size_t det_peer_inbox_bytes(int world, size_t max_items, size_t row_bytes) {
   if (world < 1 || world > kMaxPeers) return 0;
-  return 256 + (size_t)world * (al256(max_items * 8) + al256(max_items * row_bytes));
+  return 256 + (size_t)world * (align256(max_items * 8) + align256(max_items * row_bytes));
 }
 
 // inbox_ptrs[p] = where THIS process sees rank p's inbox (det_peer_inbox_bytes each, zero-initialised by the owner)
@@ -843,8 +841,8 @@ det_status det_peer_inbox_attach(det_peer_group* g, const void* const* inbox_ptr
   }
   g->inbox_cap = max_items;
   g->inbox_row_bytes = row_bytes;
-  g->inbox_seg_keys = al256(max_items * 8);
-  g->inbox_seg_rows = al256(max_items * row_bytes);
+  g->inbox_seg_keys = align256(max_items * 8);
+  g->inbox_seg_rows = align256(max_items * row_bytes);
   if (!g->cursor) {
     CUDA_TRY(cudaMalloc((void**)&g->cursor, kMaxPeers * sizeof(unsigned long long)));
     CUDA_TRY(cudaMemset(g->cursor, 0, kMaxPeers * sizeof(unsigned long long)));
@@ -873,19 +871,15 @@ det_status det_peer_route(det_peer_group* g, const int64_t* keys, const void* ro
   det::DevGuard _dg(g->device);
   const InboxView ib = inbox_view(g, g->pv.rank);
   if (n) {
-    const int vec = pick_vec(g->inbox_row_bytes, rows, nullptr, nullptr);
-    const RowGeom geo = make_geom((unsigned)g->inbox_row_bytes, vec);
     const int grid = grid_for(n, kThreadsP, g->sm_count, 4);
     const long long* k = (const long long*)keys;
     const unsigned char* r = (const unsigned char*)rows;
     DevState* st = g->local->view.st;
-    switch (vec) {
-      case 16: DET_LAUNCH(peer_route_kernel<16>, grid, kThreadsP, 0, s, ib, g->pv.world, g->pv.gpu_mode, k, r, n, geo, g->cursor, st); break;
-      case 8: DET_LAUNCH(peer_route_kernel<8>, grid, kThreadsP, 0, s, ib, g->pv.world, g->pv.gpu_mode, k, r, n, geo, g->cursor, st); break;
-      case 4: DET_LAUNCH(peer_route_kernel<4>, grid, kThreadsP, 0, s, ib, g->pv.world, g->pv.gpu_mode, k, r, n, geo, g->cursor, st); break;
-      case 2: DET_LAUNCH(peer_route_kernel<2>, grid, kThreadsP, 0, s, ib, g->pv.world, g->pv.gpu_mode, k, r, n, geo, g->cursor, st); break;
-      default: DET_LAUNCH(peer_route_kernel<1>, grid, kThreadsP, 0, s, ib, g->pv.world, g->pv.gpu_mode, k, r, n, geo, g->cursor, st); break;
-    }
+    dispatch_vec(g->inbox_row_bytes, {{rows, "det_peer_route: rows"}}, [&](auto V, const RowGeom& geo) -> det_status {
+      DET_LAUNCH(peer_route_kernel<decltype(V)::value>, grid, kThreadsP, 0, s, ib, g->pv.world, g->pv.gpu_mode, k, r, n, geo,
+                 g->cursor, st);
+      return DET_OK;
+    });
   }
   DET_LAUNCH(peer_publish_counts_kernel, 1, 32, 0, s, ib, g->pv.world, g->pv.rank, g->cursor);
   CUDA_TRY(cudaGetLastError());
@@ -927,12 +921,12 @@ det_status det_peer_inbox_gather(det_peer_group* g, int shard, const int64_t* co
 // ---- owner-side exchange: host entry points ----------------------------------------------------------------------
 static void xchg_layout(int world, size_t cap, size_t rb, XchgView* xv) {
   size_t off = kXchgHeader;
-  xv->seg_req_keys = al256(cap * 8);
-  xv->seg_req_idx = al256(cap * 4);
-  xv->seg_ins_keys = al256(cap * 8);
-  xv->seg_ins_rows = al256(cap * rb);
-  xv->out_bytes = al256(cap * rb);
-  xv->ex_bytes = al256(cap);
+  xv->seg_req_keys = align256(cap * 8);
+  xv->seg_req_idx = align256(cap * 4);
+  xv->seg_ins_keys = align256(cap * 8);
+  xv->seg_ins_rows = align256(cap * rb);
+  xv->out_bytes = align256(cap * rb);
+  xv->ex_bytes = align256(cap);
   xv->off_req_keys = off; off += (size_t)world * xv->seg_req_keys;
   xv->off_req_idx = off;  off += (size_t)world * xv->seg_req_idx;
   xv->off_ins_keys = off; off += 2 * (size_t)world * xv->seg_ins_keys;   // two sets (epoch parity)
@@ -1023,6 +1017,56 @@ static void peer_snapshot(det_peer_group* g, cudaStream_t s) {
     cudaGetLastError();
 }
 
+}  // extern "C"
+
+// One epoch of the insert exchange (det_peer_xchg_insert, det_peer_xchg_apply_*) up to the owner side: wait until the
+// owners have consumed the segment set this epoch is about to overwrite (epoch ep - 2), route the (key, row) pairs to
+// their owners, then wait until every source has published its count of this epoch.  Rows narrower than MinVec bytes
+// aligned are refused before anything is launched or the epoch advances.  *ep: the epoch.
+template <int MinVec>
+static det_status xchg_send(det_peer_group* g, const int64_t* keys, const void* rows, size_t n, const char* rows_name,
+                            cudaStream_t s, unsigned long long* ep) {
+  unsigned* ticket_r = reinterpret_cast<unsigned*>(g->xcursor + kMaxPeers);
+  return dispatch_vec<MinVec>(g->row_bytes, {{rows, rows_name}}, [&](auto V, const RowGeom& geo) -> det_status {
+    const unsigned long long e = *ep = ++g->ep_ins;
+    if (e > 2) xchg_wait(g, kFlagAck, e - 2, s);
+    const int grid = grid_for(n, kThreadsP * kRouteKpt, g->sm_count, 4);
+    DET_LAUNCH((xchg_route_kernel<true, decltype(V)::value>), grid, kThreadsP, 0, s, g->xv, (const long long*)keys,
+               (const unsigned char*)rows, n, geo, g->xcursor, ticket_r, e, g->local->view.st);
+    xchg_wait(g, (e & 1ull) ? kFlagIns1 : kFlagIns, e, s);
+    return DET_OK;
+  });
+}
+
+// The pairs every source sent to this owner in one epoch, compacted into a workspace: keys | rows | count, each 256 B
+// aligned, room for world x max_items pairs.
+struct Inbound {
+  long long* keys;
+  unsigned char* rows;
+  long long* n_dev;
+};
+
+static Inbound inbound_layout(const det_peer_group* g, WsCarver& c) {
+  const size_t bound = (size_t)g->pv.world * g->xv.cap;
+  Inbound in;
+  in.keys = c.take<long long>(bound * 8);
+  in.rows = c.take(bound * g->row_bytes);
+  in.n_dev = c.take<long long>(sizeof(long long));
+  return in;
+}
+
+// owner side of epoch ep: compact what arrived into `in` (rows of whole 4-byte words)
+static det_status xchg_compact(det_peer_group* g, const Inbound& in, unsigned long long ep, cudaStream_t s) {
+  unsigned* ticket_a = reinterpret_cast<unsigned*>(g->xcursor + kMaxPeers + 1);
+  return dispatch_vec<4>(g->row_bytes, {}, [&](auto V, const RowGeom& cgeo) -> det_status {
+    DET_LAUNCH(xchg_compact_kernel<decltype(V)::value>, g->sm_count * 4, kThreadsP, 0, s, g->xv, in.keys, in.rows, cgeo,
+               in.n_dev, ticket_a, ep);
+    return DET_OK;
+  });
+}
+
+extern "C" {
+
 // Sharded Find through the owners.  COLLECTIVE: every rank of the group calls it (n may differ, 0 allowed), in the same
 // order as its peers.  Rows land in this rank's output ring (2 entries): *rows_view (if non-null) receives the device
 // pointer of the n rows, valid until the next-but-one det_peer_xchg_find; values_out (if non-null) additionally gets a
@@ -1043,47 +1087,33 @@ det_status det_peer_xchg_find(det_peer_group* g, const int64_t* keys, size_t n, 
   unsigned char* out = xv.base[xv.rank] + xv.off_out + (size_t)parity * xv.out_bytes;
   unsigned char* ex = xv.base[xv.rank] + xv.off_exists + (size_t)parity * xv.ex_bytes;
   const int want_exists = (exists_out != nullptr || full_size_default) ? 1 : 0;
-  // serve: table row or the broadcast default row -> the requester's ring (256 B aligned); fill: per-key defaults -> ring
-  const int v = pick_vec(g->row_bytes, full_size_default ? nullptr : defaults, nullptr, nullptr);
-  const RowGeom geo = make_geom((unsigned)g->row_bytes, v);
   unsigned* ticket = reinterpret_cast<unsigned*>(g->xcursor + kMaxPeers);
   DevState* st = g->local->view.st;
   const long long* k = (const long long*)keys;
   {
     const int grid = grid_for(n, kThreadsP * kRouteKpt, g->sm_count, 4);
-    DET_LAUNCH((xchg_route_kernel<false, 16>), grid, kThreadsP, 0, s, xv, k, (const unsigned char*)nullptr, n, geo, g->xcursor, ticket, ep, st);
+    // requests carry no rows: the kernel does not read the geometry
+    DET_LAUNCH((xchg_route_kernel<false, 16>), grid, kThreadsP, 0, s, xv, k, (const unsigned char*)nullptr, n, RowGeom{},
+               g->xcursor, ticket, ep, st);
   }
   xchg_wait(g, kFlagReq, ep, s);
-  {
-    const unsigned char* d = (const unsigned char*)defaults;
-    const TableView tv = g->local->view;
-    switch (v) {
-#define DET_XSERVE(VV)                                                                                                   \
-  case VV: {                                                                                                              \
-    const int grid = g->sm_count * occupancy_of(xchg_serve_find_kernel<VV>, kThreadsP);                                   \
-    DET_LAUNCH(xchg_serve_find_kernel<VV>, grid, kThreadsP, 0, s, xv, tv, d, full_size_default, want_exists, parity, geo, ticket + 2, ep); \
-  } break;
-      DET_XSERVE(16) DET_XSERVE(8) DET_XSERVE(4) DET_XSERVE(2)
-      default: {
-        const int grid = g->sm_count * occupancy_of(xchg_serve_find_kernel<1>, kThreadsP);
-        DET_LAUNCH(xchg_serve_find_kernel<1>, grid, kThreadsP, 0, s, xv, tv, d, full_size_default, want_exists, parity, geo, ticket + 2, ep);
-      } break;
-#undef DET_XSERVE
-    }
-  }
+  // serve: table row or the broadcast default row -> the requester's ring (256 B aligned); fill: per-key defaults -> ring
+  const unsigned char* d = (const unsigned char*)defaults;
+  const TableView tv = g->local->view;
+  dispatch_vec(g->row_bytes, {{full_size_default ? nullptr : defaults, "det_peer_xchg_find: default_value"}},
+               [&](auto V, const RowGeom& geo) -> det_status {
+    const auto kern = xchg_serve_find_kernel<decltype(V)::value>;
+    const int grid = g->sm_count * occupancy_of(kern, kThreadsP);
+    DET_LAUNCH(kern, grid, kThreadsP, 0, s, xv, tv, d, full_size_default, want_exists, parity, geo, ticket + 2, ep);
+    return DET_OK;
+  });
   xchg_wait(g, kFlagDone, ep, s);
   if (full_size_default && n) {
     const int grid = grid_for(n, kThreadsP, g->sm_count, 4);
-    const unsigned char* d = (const unsigned char*)defaults;
-    const int vf = pick_vec(g->row_bytes, defaults, nullptr, nullptr);
-    const RowGeom gf = make_geom((unsigned)g->row_bytes, vf);
-    switch (vf) {
-      case 16: DET_LAUNCH(xchg_fill_missing_kernel<16>, grid, kThreadsP, 0, s, ex, d, out, n, gf); break;
-      case 8: DET_LAUNCH(xchg_fill_missing_kernel<8>, grid, kThreadsP, 0, s, ex, d, out, n, gf); break;
-      case 4: DET_LAUNCH(xchg_fill_missing_kernel<4>, grid, kThreadsP, 0, s, ex, d, out, n, gf); break;
-      case 2: DET_LAUNCH(xchg_fill_missing_kernel<2>, grid, kThreadsP, 0, s, ex, d, out, n, gf); break;
-      default: DET_LAUNCH(xchg_fill_missing_kernel<1>, grid, kThreadsP, 0, s, ex, d, out, n, gf); break;
-    }
+    dispatch_vec(g->row_bytes, {{defaults, "det_peer_xchg_find: default_value"}}, [&](auto V, const RowGeom& gf) -> det_status {
+      DET_LAUNCH(xchg_fill_missing_kernel<decltype(V)::value>, grid, kThreadsP, 0, s, ex, d, out, n, gf);
+      return DET_OK;
+    });
   }
   CUDA_TRY(cudaGetLastError());
   if (values_out && n) CUDA_TRY(cudaMemcpyAsync(values_out, out, n * g->row_bytes, cudaMemcpyDeviceToDevice, s));
@@ -1106,57 +1136,25 @@ static det_status xchg_insert_evicting(det_peer_group* g, const int64_t* keys, c
   det::DevGuard _dg(g->device);
   det_status rs = peer_room(g, "det_peer_xchg_insert");
   if (rs != DET_OK) return rs;
-  const XchgView& xv = g->xv;
-  const size_t bound = (size_t)g->pv.world * xv.cap;
-  const size_t off_rows = al256(bound * 8), off_n = off_rows + al256(bound * g->row_bytes);
   if (!g->ins_ws) {
-    CUDA_TRY(cudaMalloc((void**)&g->ins_ws, off_n + 256));
+    WsCarver size(nullptr);
+    inbound_layout(g, size);
+    CUDA_TRY(cudaMalloc((void**)&g->ins_ws, size.off));
     CUDA_TRY(cudaMallocHost((void**)&g->h_ins_n, sizeof(long long)));
   }
-  const unsigned long long ep = ++g->ep_ins;
-  unsigned* ticket_r = reinterpret_cast<unsigned*>(g->xcursor + kMaxPeers);
-  unsigned* ticket_a = reinterpret_cast<unsigned*>(g->xcursor + kMaxPeers + 1);
-  DevState* st = t->view.st;
-  if (ep > 2) {
-    const unsigned long long* flags = reinterpret_cast<const unsigned long long*>(xv.base[xv.rank] + kFlagAck * 64);
-    DET_LAUNCH_SPIN(xchg_wait_kernel, 1, 32, 0, s, flags, xv.world, ep - 2, st, kXchgTimeoutCycles);
-  }
-  {
-    const int vec = pick_vec(g->row_bytes, values, nullptr, nullptr);
-    const RowGeom geo = make_geom((unsigned)g->row_bytes, vec);
-    const int grid = grid_for(n, kThreadsP * kRouteKpt, g->sm_count, 4);
-    const long long* k = (const long long*)keys;
-    const unsigned char* r = (const unsigned char*)values;
-    switch (vec) {
-      case 16: DET_LAUNCH((xchg_route_kernel<true, 16>), grid, kThreadsP, 0, s, xv, k, r, n, geo, g->xcursor, ticket_r, ep, st); break;
-      case 8: DET_LAUNCH((xchg_route_kernel<true, 8>), grid, kThreadsP, 0, s, xv, k, r, n, geo, g->xcursor, ticket_r, ep, st); break;
-      default: DET_LAUNCH((xchg_route_kernel<true, 4>), grid, kThreadsP, 0, s, xv, k, r, n, geo, g->xcursor, ticket_r, ep, st); break;
-    }
-  }
-  {
-    const unsigned long long* flags = reinterpret_cast<const unsigned long long*>(xv.base[xv.rank] + ((ep & 1ull) ? kFlagIns1 : kFlagIns) * 64);
-    DET_LAUNCH_SPIN(xchg_wait_kernel, 1, 32, 0, s, flags, xv.world, ep, st, kXchgTimeoutCycles);
-  }
-  long long* ckeys = (long long*)g->ins_ws;
-  unsigned char* crows = g->ins_ws + off_rows;
-  long long* n_dev = (long long*)(g->ins_ws + off_n);
-  {
-    const int cvec = pick_vec(g->row_bytes, nullptr, nullptr, nullptr);
-    const RowGeom cgeo = make_geom((unsigned)g->row_bytes, cvec);
-    const int grid = g->sm_count * 4;
-    switch (cvec) {
-      case 16: DET_LAUNCH(xchg_compact_kernel<16>, grid, kThreadsP, 0, s, xv, ckeys, crows, cgeo, n_dev, ticket_a, ep); break;
-      case 8: DET_LAUNCH(xchg_compact_kernel<8>, grid, kThreadsP, 0, s, xv, ckeys, crows, cgeo, n_dev, ticket_a, ep); break;
-      default: DET_LAUNCH(xchg_compact_kernel<4>, grid, kThreadsP, 0, s, xv, ckeys, crows, cgeo, n_dev, ticket_a, ep); break;
-    }
-  }
+  WsCarver c(g->ins_ws);
+  const Inbound in = inbound_layout(g, c);
+  unsigned long long ep = 0;
+  det_status st = xchg_send<1>(g, keys, values, n, "det_peer_xchg_insert: values", s, &ep);
+  if (st == DET_OK) st = xchg_compact(g, in, ep, s);
+  if (st != DET_OK) return st;
   CUDA_TRY(cudaGetLastError());
-  CUDA_TRY(cudaMemcpyAsync(g->h_ins_n, n_dev, sizeof(long long), cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaMemcpyAsync(g->h_ins_n, in.n_dev, sizeof(long long), cudaMemcpyDeviceToHost, s));
   CUDA_TRY(cudaStreamSynchronize(s));
   const long long m = *g->h_ins_n;
-  if (m < 0 || (size_t)m > bound) return fail(DET_INTERNAL, "det_peer_xchg_insert: inbound count out of range");
+  if (m < 0 || (size_t)m > (size_t)g->pv.world * g->xv.cap) return fail(DET_INTERNAL, "det_peer_xchg_insert: inbound count out of range");
   if (m == 0) return DET_OK;
-  return det::evict_insert(t, (const int64_t*)ckeys, crows, nullptr, (size_t)m, s);
+  return det::evict_insert(t, (const int64_t*)in.keys, in.rows, nullptr, (size_t)m, s);
 }
 
 
@@ -1176,52 +1174,17 @@ det_status det_peer_xchg_insert(det_peer_group* g, const int64_t* keys, const vo
   det_status rs = peer_room(g, "det_peer_xchg_insert");
   if (rs != DET_OK) return rs;
   det::MutLock _lk(g->local);
-  const XchgView& xv = g->xv;
-  const int vec = pick_vec(g->row_bytes, values, nullptr, nullptr);
-  const RowGeom geo = make_geom((unsigned)g->row_bytes, vec);
-  const int avec = pick_vec(g->row_bytes, nullptr, nullptr, nullptr);
-  const RowGeom ageo = make_geom((unsigned)g->row_bytes, avec);
-  unsigned* ticket_r = reinterpret_cast<unsigned*>(g->xcursor + kMaxPeers);
+  unsigned long long ep = 0;
+  det_status st = xchg_send<1>(g, keys, values, n, "det_peer_xchg_insert: values", s, &ep);
+  if (st != DET_OK) return st;
+  // owner side: apply what arrived to the local shard
   unsigned* ticket_a = reinterpret_cast<unsigned*>(g->xcursor + kMaxPeers + 1);
-  DevState* st = g->local->view.st;
-  const TableView tv = g->local->view;
-  const int np = g->n_slot_planes;
-  const long long* k = (const long long*)keys;
-  const unsigned char* r = (const unsigned char*)values;
-  const unsigned long long ep = ++g->ep_ins;
-  // sender side: the owners have consumed the segment set this epoch is about to overwrite (epoch ep - 2)
-  if (ep > 2) {
-    const unsigned long long* flags = reinterpret_cast<const unsigned long long*>(xv.base[xv.rank] + kFlagAck * 64);
-    DET_LAUNCH_SPIN(xchg_wait_kernel, 1, 32, 0, s, flags, xv.world, ep - 2, st, kXchgTimeoutCycles);
-  }
-  {
-    const int grid = grid_for(n, kThreadsP * kRouteKpt, g->sm_count, 4);
-    switch (vec) {
-      case 16: DET_LAUNCH((xchg_route_kernel<true, 16>), grid, kThreadsP, 0, s, xv, k, r, n, geo, g->xcursor, ticket_r, ep, st); break;
-      case 8: DET_LAUNCH((xchg_route_kernel<true, 8>), grid, kThreadsP, 0, s, xv, k, r, n, geo, g->xcursor, ticket_r, ep, st); break;
-      case 4: DET_LAUNCH((xchg_route_kernel<true, 4>), grid, kThreadsP, 0, s, xv, k, r, n, geo, g->xcursor, ticket_r, ep, st); break;
-      case 2: DET_LAUNCH((xchg_route_kernel<true, 2>), grid, kThreadsP, 0, s, xv, k, r, n, geo, g->xcursor, ticket_r, ep, st); break;
-      default: DET_LAUNCH((xchg_route_kernel<true, 1>), grid, kThreadsP, 0, s, xv, k, r, n, geo, g->xcursor, ticket_r, ep, st); break;
-    }
-  }
-  // owner side: every source has published its count of this epoch
-  {
-    const unsigned long long* flags = reinterpret_cast<const unsigned long long*>(xv.base[xv.rank] + ((ep & 1ull) ? kFlagIns1 : kFlagIns) * 64);
-    DET_LAUNCH_SPIN(xchg_wait_kernel, 1, 32, 0, s, flags, xv.world, ep, st, kXchgTimeoutCycles);
-  }
-  switch (avec) {
-#define DET_XAPPLY(VV)                                                                                        \
-  case VV: {                                                                                                   \
-    const int occ = occupancy_of(xchg_apply_insert_kernel<VV>, kThreadsP);                                     \
-    DET_LAUNCH(xchg_apply_insert_kernel<VV>, g->sm_count * occ, kThreadsP, 0, s, xv, tv, ageo, np, ticket_a, ep); \
-  } break;
-    DET_XAPPLY(16) DET_XAPPLY(8) DET_XAPPLY(4) DET_XAPPLY(2)
-    default: {
-      const int occ = occupancy_of(xchg_apply_insert_kernel<1>, kThreadsP);
-      DET_LAUNCH(xchg_apply_insert_kernel<1>, g->sm_count * occ, kThreadsP, 0, s, xv, tv, ageo, np, ticket_a, ep);
-    } break;
-#undef DET_XAPPLY
-  }
+  dispatch_vec(g->row_bytes, {}, [&](auto V, const RowGeom& ageo) -> det_status {
+    const auto kern = xchg_apply_insert_kernel<decltype(V)::value>;
+    const int occ = occupancy_of(kern, kThreadsP);
+    DET_LAUNCH(kern, g->sm_count * occ, kThreadsP, 0, s, g->xv, g->local->view, ageo, g->n_slot_planes, ticket_a, ep);
+    return DET_OK;
+  });
   CUDA_TRY(cudaGetLastError());
   peer_snapshot(g, s);
   return DET_OK;
@@ -1235,19 +1198,16 @@ det_status det_peer_xchg_insert(det_peer_group* g, const int64_t* keys, const vo
 // sender's order) and runs the fused find-or-insert optimizer step on its shard.  Every count stays on the device:
 // no cudaStreamSynchronize, no host round trip for split sizes (the reference negotiates them on the host).
 // workspace: det_peer_xchg_apply_workspace_bytes(g) bytes of device memory, 256 B aligned.
-static size_t xchg_apply_layout(const det_peer_group* g, size_t* off_rows, size_t* off_n, size_t* off_dup, size_t* dup_bytes) {
-  const size_t bound = (size_t)g->pv.world * g->xv.cap;
-  const size_t dim = g->row_bytes / 4;
-  size_t off = 0;
-  off += al256(bound * 8);
-  if (off_rows) *off_rows = off;
-  off += al256(bound * g->row_bytes);
-  if (off_n) *off_n = off;
-  off += 256;
-  if (off_dup) *off_dup = off;
-  const size_t db = det_apply_dup_workspace_bytes(bound, dim);
+// Its layout: the inbound pairs, then the workspace of det_apply_*_dup over them (a multiple of 256 B).
+static size_t xchg_apply_layout(const det_peer_group* g, void* base, Inbound* in, unsigned char** dup, size_t* dup_bytes) {
+  WsCarver c(base);
+  const Inbound i = inbound_layout(g, c);
+  const size_t db = det_apply_dup_workspace_bytes((size_t)g->pv.world * g->xv.cap, g->row_bytes / 4);
+  unsigned char* d = c.take(db);
+  if (in) *in = i;
+  if (dup) *dup = d;
   if (dup_bytes) *dup_bytes = db;
-  return off + db;
+  return c.off;
 }
 
 size_t det_peer_xchg_apply_workspace_bytes(det_peer_group* g) {
@@ -1263,55 +1223,22 @@ static det_status xchg_apply(det_peer_group* g, const int64_t* keys, const float
   if (n > g->xv.cap) return fail(DET_INVALID_ARGUMENT, "det_peer_xchg_apply: batch larger than the mailbox (max_items)");
   if (!init_param || !workspace || (n && (!keys || !grads))) return fail(DET_INVALID_ARGUMENT, "det_peer_xchg_apply: null argument");
   if (((uintptr_t)workspace & 255u) != 0) return fail(DET_INVALID_ARGUMENT, "det_peer_xchg_apply: workspace must be 256 B aligned");
-  size_t off_rows, off_n, off_dup, dup_bytes;
-  if (workspace_bytes < xchg_apply_layout(g, &off_rows, &off_n, &off_dup, &dup_bytes))
+  Inbound in;
+  unsigned char* dup;
+  size_t dup_bytes;
+  if (workspace_bytes < xchg_apply_layout(g, workspace, &in, &dup, &dup_bytes))
     return fail(DET_INVALID_ARGUMENT, "det_peer_xchg_apply: workspace too small");
   det::DevGuard _dg(g->device);
   det_status rs = peer_room(g, "det_peer_xchg_apply");
   if (rs != DET_OK) return rs;
-  const XchgView& xv = g->xv;
-  const unsigned long long ep = ++g->ep_ins;
-  unsigned* ticket_r = reinterpret_cast<unsigned*>(g->xcursor + kMaxPeers);
-  unsigned* ticket_a = reinterpret_cast<unsigned*>(g->xcursor + kMaxPeers + 1);
-  DevState* st = g->local->view.st;
-  const int vec = pick_vec(g->row_bytes, grads, nullptr, nullptr);
-  const RowGeom geo = make_geom((unsigned)g->row_bytes, vec);
-  if (ep > 2) {
-    const unsigned long long* flags = reinterpret_cast<const unsigned long long*>(xv.base[xv.rank] + kFlagAck * 64);
-    DET_LAUNCH_SPIN(xchg_wait_kernel, 1, 32, 0, s, flags, xv.world, ep - 2, st, kXchgTimeoutCycles);
-  }
-  {
-    const int grid = grid_for(n, kThreadsP * kRouteKpt, g->sm_count, 4);
-    const long long* k = (const long long*)keys;
-    const unsigned char* r = (const unsigned char*)grads;
-    switch (vec) {
-      case 16: DET_LAUNCH((xchg_route_kernel<true, 16>), grid, kThreadsP, 0, s, xv, k, r, n, geo, g->xcursor, ticket_r, ep, st); break;
-      case 8: DET_LAUNCH((xchg_route_kernel<true, 8>), grid, kThreadsP, 0, s, xv, k, r, n, geo, g->xcursor, ticket_r, ep, st); break;
-      default: DET_LAUNCH((xchg_route_kernel<true, 4>), grid, kThreadsP, 0, s, xv, k, r, n, geo, g->xcursor, ticket_r, ep, st); break;
-    }
-  }
-  {
-    const unsigned long long* flags = reinterpret_cast<const unsigned long long*>(xv.base[xv.rank] + ((ep & 1ull) ? kFlagIns1 : kFlagIns) * 64);
-    DET_LAUNCH_SPIN(xchg_wait_kernel, 1, 32, 0, s, flags, xv.world, ep, st, kXchgTimeoutCycles);
-  }
-  unsigned char* ws = (unsigned char*)workspace;
-  long long* ckeys = (long long*)ws;
-  unsigned char* crows = ws + off_rows;
-  long long* n_dev = (long long*)(ws + off_n);
-  {
-    const int cvec = pick_vec(g->row_bytes, nullptr, nullptr, nullptr);
-    const RowGeom cgeo = make_geom((unsigned)g->row_bytes, cvec);
-    const int grid = g->sm_count * 4;
-    switch (cvec) {
-      case 16: DET_LAUNCH(xchg_compact_kernel<16>, grid, kThreadsP, 0, s, xv, ckeys, crows, cgeo, n_dev, ticket_a, ep); break;
-      case 8: DET_LAUNCH(xchg_compact_kernel<8>, grid, kThreadsP, 0, s, xv, ckeys, crows, cgeo, n_dev, ticket_a, ep); break;
-      default: DET_LAUNCH(xchg_compact_kernel<4>, grid, kThreadsP, 0, s, xv, ckeys, crows, cgeo, n_dev, ticket_a, ep); break;
-    }
-  }
+  unsigned long long ep = 0;
+  det_status rc = xchg_send<4>(g, keys, grads, n, "det_peer_xchg_apply: grads", s, &ep);
+  if (rc == DET_OK) rc = xchg_compact(g, in, ep, s);
+  if (rc != DET_OK) return rc;
   CUDA_TRY(cudaGetLastError());
   const size_t bound = (size_t)g->pv.world * g->xv.cap;
-  det_status rc = det::apply_dup_on_device_count(g->local, (const int64_t*)ckeys, (const float*)crows, bound, n_dev, opt, lr, eps,
-                                                 beta1, beta2, init_slot, init_param, ws + off_dup, dup_bytes, s);
+  rc = det::apply_dup_on_device_count(g->local, (const int64_t*)in.keys, (const float*)in.rows, bound, in.n_dev, opt, lr,
+                                      eps, beta1, beta2, init_slot, init_param, dup, dup_bytes, s);
   if (rc != DET_OK) return rc;
   peer_snapshot(g, s);
   return DET_OK;
@@ -1339,19 +1266,15 @@ det_status det_peer_find(det_peer_group* g, const int64_t* keys, size_t n, const
   if (!keys || !values_out || !defaults) return fail(DET_INVALID_ARGUMENT, "det_peer_find: null argument");
   cudaStream_t s = (cudaStream_t)stream;
   det::DevGuard _dg(g->device);
-  const int vec = pick_vec(g->row_bytes, defaults, values_out, nullptr);
-  const RowGeom geo = make_geom((unsigned)g->row_bytes, vec);
   const int grid = grid_for(n, kThreadsP, g->sm_count, occupancy_of(peer_find_kernel<16>, kThreadsP));
   const unsigned char* d = (const unsigned char*)defaults;
   unsigned char* o = (unsigned char*)values_out;
   const long long* k = (const long long*)keys;
-  switch (vec) {
-    case 16: DET_LAUNCH(peer_find_kernel<16>, grid, kThreadsP, 0, s, g->pv, k, n, d, full_size_default, o, exists, geo); break;
-    case 8: DET_LAUNCH(peer_find_kernel<8>, grid, kThreadsP, 0, s, g->pv, k, n, d, full_size_default, o, exists, geo); break;
-    case 4: DET_LAUNCH(peer_find_kernel<4>, grid, kThreadsP, 0, s, g->pv, k, n, d, full_size_default, o, exists, geo); break;
-    case 2: DET_LAUNCH(peer_find_kernel<2>, grid, kThreadsP, 0, s, g->pv, k, n, d, full_size_default, o, exists, geo); break;
-    default: DET_LAUNCH(peer_find_kernel<1>, grid, kThreadsP, 0, s, g->pv, k, n, d, full_size_default, o, exists, geo); break;
-  }
+  dispatch_vec(g->row_bytes, {{defaults, "det_peer_find: default_value"}, {values_out, "det_peer_find: values"}},
+               [&](auto V, const RowGeom& geo) -> det_status {
+    DET_LAUNCH(peer_find_kernel<decltype(V)::value>, grid, kThreadsP, 0, s, g->pv, k, n, d, full_size_default, o, exists, geo);
+    return DET_OK;
+  });
   CUDA_TRY(cudaGetLastError());
   return DET_OK;
 }
@@ -1370,28 +1293,23 @@ det_status det_peer_insert(det_peer_group* g, const int64_t* keys, const void* v
     det_status rs = peer_room(g, "det_peer_insert");
     if (rs != DET_OK) return rs;
   }
-  const int vec = pick_vec(g->row_bytes, values, nullptr, nullptr);
-  const RowGeom geo = make_geom((unsigned)g->row_bytes, vec);
   const unsigned char* v = (const unsigned char*)values;
   const long long* k = (const long long*)keys;
   const int np = g->n_slot_planes;
-  if (vec == 16) {
-    // register cap of the one-sided insert: at least 4 resident CTAs per SM, more remote probes in flight
-    const auto kern = peer_insert_kernel<16, 4>;
-    const int grid4 = grid_for(n, kThreadsP, g->sm_count, occupancy_of(kern, kThreadsP));
-    DET_LAUNCH(kern, grid4, kThreadsP, 0, s, g->pv, k, v, n, geo, np);
-    CUDA_TRY(cudaGetLastError());
-    peer_snapshot(g, s);
+  dispatch_vec(g->row_bytes, {{values, "det_peer_insert: values"}}, [&](auto V, const RowGeom& geo) -> det_status {
+    constexpr int VV = decltype(V)::value;
+    if constexpr (VV == 16) {
+      // register cap of the one-sided insert: at least 4 resident CTAs per SM, more remote probes in flight
+      const auto kern = peer_insert_kernel<16, 4>;
+      const int grid4 = grid_for(n, kThreadsP, g->sm_count, occupancy_of(kern, kThreadsP));
+      DET_LAUNCH(kern, grid4, kThreadsP, 0, s, g->pv, k, v, n, geo, np);
+    } else {
+      // narrower rows: the grid of the uncapped 16 B kernel
+      const int grid = grid_for(n, kThreadsP, g->sm_count, occupancy_of(peer_insert_kernel<16>, kThreadsP));
+      DET_LAUNCH(peer_insert_kernel<VV>, grid, kThreadsP, 0, s, g->pv, k, v, n, geo, np);
+    }
     return DET_OK;
-  }
-  // narrower rows: the grid of the uncapped 16 B kernel
-  const int grid = grid_for(n, kThreadsP, g->sm_count, occupancy_of(peer_insert_kernel<16>, kThreadsP));
-  switch (vec) {
-    case 8: DET_LAUNCH(peer_insert_kernel<8>, grid, kThreadsP, 0, s, g->pv, k, v, n, geo, np); break;
-    case 4: DET_LAUNCH(peer_insert_kernel<4>, grid, kThreadsP, 0, s, g->pv, k, v, n, geo, np); break;
-    case 2: DET_LAUNCH(peer_insert_kernel<2>, grid, kThreadsP, 0, s, g->pv, k, v, n, geo, np); break;
-    default: DET_LAUNCH(peer_insert_kernel<1>, grid, kThreadsP, 0, s, g->pv, k, v, n, geo, np); break;
-  }
+  });
   CUDA_TRY(cudaGetLastError());
   peer_snapshot(g, s);
   return DET_OK;

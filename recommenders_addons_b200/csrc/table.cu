@@ -45,15 +45,6 @@ RowGeom make_geom(unsigned row_bytes, int vec) {
   return g;
 }
 
-int pick_vec(size_t row_bytes, const void* a, const void* b, const void* c) {
-  uintptr_t bits = (uintptr_t)row_bytes | (uintptr_t)a | (uintptr_t)b | (uintptr_t)c;
-  if ((bits & 15u) == 0) return 16;
-  if ((bits & 7u) == 0) return 8;
-  if ((bits & 3u) == 0) return 4;
-  if ((bits & 1u) == 0) return 2;
-  return 1;
-}
-
 int grid_for(size_t n_items, int items_per_block, int sm_count, int blocks_per_sm) {
   size_t need = (n_items + (size_t)items_per_block - 1) / (size_t)items_per_block;
   size_t cap = (size_t)sm_count * (size_t)blocks_per_sm;
@@ -745,24 +736,6 @@ det_status table_clear_async(det_table* t, cudaStream_t s) {
   return DET_OK;
 }
 
-template <typename F>
-static det_status dispatch_vec(int vec, F&& f) {
-  switch (vec) {
-    case 16: return f(std::integral_constant<int, 16>());
-    case 8: return f(std::integral_constant<int, 8>());
-    case 4: return f(std::integral_constant<int, 4>());
-    case 2: return f(std::integral_constant<int, 2>());
-    default: return f(std::integral_constant<int, 1>());
-  }
-}
-
-static det_status read_state(det_table* t, cudaStream_t s, DevState* out) {
-  CUDA_TRY(cudaMemcpyAsync(t->h_state, t->view.st, sizeof(DevState), cudaMemcpyDeviceToHost, s));
-  CUDA_TRY(cudaStreamSynchronize(s));
-  *out = *t->h_state;
-  return DET_OK;
-}
-
 det_status rehash_to(det_table* t, uint64_t new_nb, cudaStream_t s) {
   if (t->external) return fail(DET_TABLE_FULL, "detable: a table living in a caller-provided region cannot grow");
   TableView nv;
@@ -772,12 +745,10 @@ det_status rehash_to(det_table* t, uint64_t new_nb, cudaStream_t s) {
   const size_t ncap = new_nb * kBucket;
   DET_LAUNCH(fill_keys_kernel, grid_for(ncap, 4096, t->sm_count, 8), 1024, 0, s, nv.keys, ncap, kEmptyKey);
   const TableView ov = t->view;
-  const int vec = pick_vec(t->row_bytes, nullptr, nullptr, nullptr);
-  const RowGeom g = make_geom((unsigned)t->row_bytes, vec);
   const RowGeom gs = make_geom((unsigned)t->cfg.dim * 4u, 4);
   const int np = t->cfg.num_slot_planes;
   const int grid = grid_for(ov.capacity(), kThreads, t->sm_count, 8);
-  dispatch_vec(vec, [&](auto V) -> det_status {
+  dispatch_vec(t->row_bytes, {}, [&](auto V, const RowGeom& g) -> det_status {
     DET_LAUNCH(rehash_kernel<decltype(V)::value>, grid, kThreads, 0, s, ov, nv, g, gs, np);
     return DET_OK;
   });
@@ -917,39 +888,25 @@ void note_mutation(det_table* t, size_t n, cudaStream_t s) {
   }
 }
 
-template <typename T, int VEC>
-static det_status launch_accum_v(det_table* t, const TableView& v, const long long* k, const void* vod,
-                                 const uint8_t* exists, size_t n, const SlotInit& si, const RowGeom& g,
-                                 cudaStream_t s) {
-  const int grid = grid_for(n, kThreads, t->sm_count, occupancy_of(accum_kernel<T, VEC>, kThreads));
-  const auto kern = accum_kernel<T, VEC>;
-  DET_LAUNCH(kern, grid, kThreads, 0, s, v, k, (const T*)vod, exists, n, si, g);
-  return DET_OK;
-}
-
+// values_or_deltas must be aligned to the value dtype: the narrowest width is the element size
 template <typename T>
 static det_status launch_accum(det_table* t, const TableView& v, const long long* k, const void* vod,
-                               const uint8_t* exists, size_t n, const SlotInit& si, const RowGeom& g, int vec,
-                               cudaStream_t s) {
-  if constexpr (std::is_same<T, float>::value) {
-    if (vec == 16 && g.vpr <= g.lpr) {
-      const int grid = grid_for(n, kThreads, t->sm_count, occupancy_of(accum_staged_kernel, kThreads));
-      DET_LAUNCH(accum_staged_kernel, grid, kThreads, 0, s, v, k, (const float*)vod, exists, n, si, g);
-      return DET_OK;
+                               const uint8_t* exists, size_t n, const SlotInit& si, cudaStream_t s) {
+  return dispatch_vec<(int)sizeof(T)>(t->row_bytes, {{vod, "det_accum: values_or_deltas"}},
+                                      [&](auto V, const RowGeom& g) -> det_status {
+    constexpr int VV = decltype(V)::value;
+    if constexpr (std::is_same<T, float>::value && VV == 16) {
+      if (g.vpr <= g.lpr) {
+        const int grid = grid_for(n, kThreads, t->sm_count, occupancy_of(accum_staged_kernel, kThreads));
+        DET_LAUNCH(accum_staged_kernel, grid, kThreads, 0, s, v, k, (const float*)vod, exists, n, si, g);
+        return DET_OK;
+      }
     }
-  }
-  switch (vec) {
-    case 16: return launch_accum_v<T, 16>(t, v, k, vod, exists, n, si, g, s);
-    case 8:
-      if constexpr (sizeof(T) <= 8) return launch_accum_v<T, 8>(t, v, k, vod, exists, n, si, g, s);
-    case 4:
-      if constexpr (sizeof(T) <= 4) return launch_accum_v<T, 4>(t, v, k, vod, exists, n, si, g, s);
-    case 2:
-      if constexpr (sizeof(T) <= 2) return launch_accum_v<T, 2>(t, v, k, vod, exists, n, si, g, s);
-    case 1:
-      if constexpr (sizeof(T) <= 1) return launch_accum_v<T, 1>(t, v, k, vod, exists, n, si, g, s);
-    default: return fail(DET_INVALID_ARGUMENT, "det_accum: unsupported alignment");
-  }
+    const int grid = grid_for(n, kThreads, t->sm_count, occupancy_of(accum_kernel<T, VV>, kThreads));
+    const auto kern = accum_kernel<T, VV>;
+    DET_LAUNCH(kern, grid, kThreads, 0, s, v, k, (const T*)vod, exists, n, si, g);
+    return DET_OK;
+  });
 }
 
 det_status table_scratch(det_table* t, size_t bytes, void** out) {
@@ -1095,8 +1052,6 @@ const char* det_last_error(void) { return g_last_error.c_str(); }
 
 namespace det {
 
-static size_t align256u(size_t x) { return (x + 255) & ~(size_t)255; }
-
 // Fixed layout of a table inside ONE caller-provided region (every peer of a sharded group uses the same
 // layout, so a peer's planes are found at the same offsets from its region base):
 //   [DevState 256 B][peer barrier flags 256 B][keys][values (+2 rows)][slot planes ...], each 256 B aligned
@@ -1111,12 +1066,12 @@ void region_layout(const det_config& cfg, RegionLayout* L) {
   L->off_bar = off;
   off += 256;
   L->off_keys = off;
-  off += align256u(cap * sizeof(long long));
+  off += align256(cap * sizeof(long long));
   L->off_plane[0] = off;
-  off += align256u((cap + 2) * es * (size_t)cfg.dim);
+  off += align256((cap + 2) * es * (size_t)cfg.dim);
   for (int p = 1; p < kMaxPlanes; ++p) {
     L->off_plane[p] = off;
-    if (p <= cfg.num_slot_planes) off += align256u((cap + 2) * (size_t)cfg.dim * 4u);
+    if (p <= cfg.num_slot_planes) off += align256((cap + 2) * (size_t)cfg.dim * 4u);
   }
   L->bytes = off;
 }
@@ -1250,8 +1205,6 @@ det_status det_find(det_table* t, const int64_t* keys, size_t n, const void* def
   if (!keys || !values_out || !defaults) return fail(DET_INVALID_ARGUMENT, "det_find: null keys/values/default_value");
   cudaStream_t s = (cudaStream_t)stream;
   det::DevGuard _dg(t->cfg.device);
-  const int vec = pick_vec(t->row_bytes, defaults, values_out, nullptr);
-  const RowGeom g = make_geom((unsigned)t->row_bytes, vec);
   std::shared_lock<std::shared_mutex> _vl(t->view_mu);   // vs a concurrent growth on another host thread (host.h)
   const TableView v = t->view;
   // slot hints: bookkeeping only when the hint lock is free right now (a find never waits) and the stream is not
@@ -1261,7 +1214,8 @@ det_status det_find(det_table* t, const int64_t* keys, size_t n, const void* def
   const SlotHints h = track ? find_hints(t, keys, n, s) : SlotHints{nullptr, nullptr};
   // TMA bulk copies of the key tiles need 16 B aligned keys
   const bool tma = ((uintptr_t)keys & 15u) == 0;
-  return dispatch_vec(vec, [&](auto V) -> det_status {
+  return dispatch_vec(t->row_bytes, {{defaults, "det_find: default_value"}, {values_out, "det_find: values"}},
+                      [&](auto V, const RowGeom& g) -> det_status {
     constexpr int VV = decltype(V)::value;
     const auto kern = tma ? find_kernel_tma<VV, true> : find_kernel_tma<VV, false>;
     const int grid = grid_for(n, kTileKeys, t->sm_count, occupancy_of(kern, kThreads));
@@ -1292,15 +1246,13 @@ det_status insert_impl(det_table* t, const int64_t* keys, const void* values, si
     det_status st = ensure_room(t, (const long long*)keys, n, s);
     if (st != DET_OK) return st;
   }
-  const int vec = pick_vec(t->row_bytes, values, nullptr, nullptr);
-  const RowGeom g = make_geom((unsigned)t->row_bytes, vec);
   const TableView v = t->view;
   const SlotInit si = slot_init_of(t);
   // after ensure_room: a growth it triggered has advanced the generation.  The chunks of det_insert_host run on
   // several streams of their own and take no hints.
   const SlotHints h = check_room ? insert_hints(t, keys, n, s) : SlotHints{nullptr, nullptr};
   const bool tma = ((uintptr_t)keys & 15u) == 0;
-  return dispatch_vec(vec, [&](auto V) -> det_status {
+  return dispatch_vec(t->row_bytes, {{values, "det_insert: values"}}, [&](auto V, const RowGeom& g) -> det_status {
     constexpr int VV = decltype(V)::value;
     const bool hinted = h.keys != nullptr;
     const auto kfn = tma ? (hinted ? insert_kernel_tma<VV, true, true> : insert_kernel_tma<VV, true, false>)
@@ -1330,18 +1282,14 @@ static det_status accum_impl(det_table* t, const int64_t* keys, const void* vod,
   const TableView v = t->view;
   const SlotInit si = slot_init_of(t);
   const long long* k = (const long long*)keys;
-  int vec = pick_vec(t->row_bytes, vod, nullptr, nullptr);
-  const int es = (int)dtype_size(t->cfg.value_dtype);
-  if (vec < es) return fail(DET_INVALID_ARGUMENT, "det_accum: values_or_deltas is not aligned to the value dtype");
-  const RowGeom g = make_geom((unsigned)t->row_bytes, vec);
   switch (t->cfg.value_dtype) {
-    case DET_FLOAT32: st = launch_accum<float>(t, v, k, vod, exists, n, si, g, vec, s); break;
-    case DET_FLOAT64: st = launch_accum<double>(t, v, k, vod, exists, n, si, g, vec, s); break;
-    case DET_INT32: st = launch_accum<int>(t, v, k, vod, exists, n, si, g, vec, s); break;
-    case DET_INT64: st = launch_accum<long long>(t, v, k, vod, exists, n, si, g, vec, s); break;
-    case DET_INT8: st = launch_accum<signed char>(t, v, k, vod, exists, n, si, g, vec, s); break;
-    case DET_FLOAT16: st = launch_accum<__half>(t, v, k, vod, exists, n, si, g, vec, s); break;
-    case DET_BFLOAT16: st = launch_accum<__nv_bfloat16>(t, v, k, vod, exists, n, si, g, vec, s); break;
+    case DET_FLOAT32: st = launch_accum<float>(t, v, k, vod, exists, n, si, s); break;
+    case DET_FLOAT64: st = launch_accum<double>(t, v, k, vod, exists, n, si, s); break;
+    case DET_INT32: st = launch_accum<int>(t, v, k, vod, exists, n, si, s); break;
+    case DET_INT64: st = launch_accum<long long>(t, v, k, vod, exists, n, si, s); break;
+    case DET_INT8: st = launch_accum<signed char>(t, v, k, vod, exists, n, si, s); break;
+    case DET_FLOAT16: st = launch_accum<__half>(t, v, k, vod, exists, n, si, s); break;
+    case DET_BFLOAT16: st = launch_accum<__nv_bfloat16>(t, v, k, vod, exists, n, si, s); break;
     default: return fail(DET_UNIMPLEMENTED, "det_accum: dtype");
   }
   if (st != DET_OK) return st;
@@ -1435,7 +1383,7 @@ det_status det_export_window(det_table* t, int plane, uint64_t first, int64_t* k
   unsigned long long* offs = nullptr;
   {
     void* sc = nullptr;
-    const size_t off_bytes = (n_tiles * sizeof(unsigned) + 255) & ~(size_t)255;
+    const size_t off_bytes = align256(n_tiles * sizeof(unsigned));
     det_status sst = table_scratch(t, off_bytes + n_tiles * sizeof(unsigned long long), &sc);
     if (sst != DET_OK) return sst;
     counts = (unsigned*)sc;
@@ -1445,9 +1393,7 @@ det_status det_export_window(det_table* t, int plane, uint64_t first, int64_t* k
   DET_LAUNCH(export_count_kernel, grid, kThreads, 0, s, v, counts, n_tiles);
   DET_LAUNCH(export_scan_kernel, 1, 1024, 0, s, counts, offs, n_tiles, v.st);
   const unsigned prb = plane == 0 ? (unsigned)t->row_bytes : (unsigned)t->cfg.dim * 4u;
-  const int vec = pick_vec(prb, values_out, nullptr, nullptr);
-  const RowGeom g = make_geom(prb, vec);
-  dispatch_vec(vec, [&](auto V) -> det_status {
+  dispatch_vec(prb, {{values_out, "det_export: values"}}, [&](auto V, const RowGeom& g) -> det_status {
     DET_LAUNCH(export_write_kernel<decltype(V)::value>, grid, kThreads, 0, s, 
         v, plane, prb, offs, n_tiles, (long long*)keys_out, (unsigned char*)values_out, (size_t)first, max_n, g);
     return DET_OK;
@@ -1481,11 +1427,9 @@ det_status det_import_plane(det_table* t, int plane, const int64_t* keys, const 
   cudaStream_t s = (cudaStream_t)stream;
   det::DevGuard _dg(t->cfg.device);
   const size_t rb = (size_t)t->cfg.dim * 4u;
-  const int vec = pick_vec(rb, rows, nullptr, nullptr);
-  const RowGeom g = make_geom((unsigned)rb, vec);
   const int grid = grid_for(n, kThreads, t->sm_count, 8);
   const TableView v = t->view;
-  dispatch_vec(vec, [&](auto V) -> det_status {
+  dispatch_vec(rb, {{rows, "det_import_plane: rows"}}, [&](auto V, const RowGeom& g) -> det_status {
     DET_LAUNCH(set_plane_kernel<decltype(V)::value>, grid, kThreads, 0, s, v, plane, (const long long*)keys,
                (const unsigned char*)rows, n, g);
     return DET_OK;
