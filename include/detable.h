@@ -82,7 +82,8 @@ typedef struct det_config {
   int32_t value_dtype;      /* DET_FLOAT32 ... */
   int32_t dim;              /* value_shape[0] */
   int32_t device;           /* CUDA device ordinal */
-  int32_t num_slot_planes;  /* 0..3 optimizer slot planes co-indexed with the value rows (fp32 only) */
+  int32_t num_slot_planes;  /* 0..3 optimizer slot planes co-indexed with the value rows: fp32 rows of 4 * dim bytes
+                             * beside DET_FLOAT32, DET_FLOAT16 or DET_BFLOAT16 value rows (other dtypes: 0 only) */
   uint64_t init_capacity;   /* keys; 0 -> 8192 (TF_HASHTABLE_INIT_SIZE default, cuckoo_hashtable_op.cc:199-205) */
   uint64_t max_capacity;    /* SLOTS (HKV's max_capacity); 0 -> grow without bound (cuckoo semantics); else the table
                              * holds at most max_load_factor * max_capacity keys and answers DET_TABLE_FULL beyond */
@@ -262,7 +263,11 @@ det_status det_lookup_sparse_clip(det_table* t, const int64_t* ids, const int32_
  * Adagrad: a += g*g; p -= lr*g/(sqrt(a)+eps)   (eps = 0: TF1 AdagradOptimizer; 1e-7: Keras)
  *   slot plane 1 = accumulator.
  * Adam   : m += (g-m)(1-b1); v += (g*g-v)(1-b2); p -= m*alpha/(sqrt(v)+eps),
- *   alpha = lr*sqrt(1-b2^t)/(1-b1^t) computed by the caller;  plane 1 = m, plane 2 = v. */
+ *   alpha = lr*sqrt(1-b2^t)/(1-b1^t) computed by the caller;  plane 1 = m, plane 2 = v.
+ * Tables of DET_FLOAT32, DET_FLOAT16 and DET_BFLOAT16 values (other dtypes: DET_UNIMPLEMENTED).  On a half table the
+ * stored param is widened to fp32 (exact), stepped by the fp32 rule above, and rounded to nearest even into the table's
+ * dtype once (overflow to +-inf, subnormals kept, NaN stays NaN); the slot planes stay fp32.  grads and init_param are
+ * fp32 whatever the table's dtype (a half initializer row widened to fp32 is exact). */
 det_status det_apply_adagrad(det_table* t, const int64_t* keys, const float* grads, size_t n,
                              float lr, float epsilon, const float* init_param, int full_size_init,
                              float init_accum, det_stream_t stream);
@@ -297,7 +302,8 @@ det_status det_host_sync_pipe(det_table* t, int which);
  * ids int64[n] (repeats allowed), grads f32[n, dim]; new keys start from the broadcast row init_param[dim].
  * workspace: det_apply_dup_workspace_bytes(n, dim) bytes of device memory, 256 B aligned, stream-ordered scratch.
  * n_unique_dev_out (nullable): device int64 that receives the number of distinct ids.
- * DET_UNIMPLEMENTED for rows that are not 16-byte vectors (use det_unique + det_segment_reduce + det_apply_*). */
+ * DET_UNIMPLEMENTED for rows that are not 16-byte vectors (use det_unique + det_segment_reduce + det_apply_*).
+ * Value dtypes and the narrowing of a half table's param: as det_apply_adagrad / det_apply_adam. */
 size_t det_apply_dup_workspace_bytes(size_t n, size_t dim);
 det_status det_apply_adagrad_dup(det_table* t, const int64_t* ids, const float* grads, size_t n, float lr, float epsilon,
                                  const float* init_param, float init_accum, void* workspace, size_t workspace_bytes,

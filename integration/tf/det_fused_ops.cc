@@ -76,10 +76,9 @@ REGISTER_OP("TFRA>DetSegmentReduce")
     .Input("num_segments: int32")    // scalar, host memory
     .Output("output: float");        // [num_segments, dim]
 
-using Table = DetHashTableOfTensorsGpu<int64, float>;
-
-// The library handle of a table whose rows the fused lookup reads (float, half, bfloat16), or nullptr
-static det_table* LookupSparseHandle(tensorflow::lookup::LookupInterface* table) {
+// The library handle of a table the fused lookup and optimizer ops serve (float, half or bfloat16 rows), or nullptr.
+// The optimizer ops keep fp32 gradients, initializer rows and slot planes whatever the row dtype.
+static det_table* FusedHandle(tensorflow::lookup::LookupInterface* table) {
   switch (table->value_dtype()) {
     case DT_FLOAT: return static_cast<DetHashTableOfTensorsGpu<int64, float>*>(table)->handle();
     case DT_HALF: return static_cast<DetHashTableOfTensorsGpu<int64, Eigen::half>*>(table)->handle();
@@ -105,7 +104,7 @@ class DetLookupSparseOp : public OpKernel {
     tensorflow::lookup::LookupInterface* table = nullptr;
     OP_REQUIRES_OK(ctx, GetLookupTable("table_handle", ctx, &table));
     core::ScopedUnref unref_me(table);
-    det_table* handle = LookupSparseHandle(table);
+    det_table* handle = FusedHandle(table);
     OP_REQUIRES(ctx, handle != nullptr,
                 errors::InvalidArgument("DetLookupSparse: the table's value dtype must be float, half or bfloat16"));
     const Tensor& ids = ctx->input(1);
@@ -142,17 +141,19 @@ class DetApplyAdagradOp : public OpKernel {
     tensorflow::lookup::LookupInterface* table = nullptr;
     OP_REQUIRES_OK(ctx, GetLookupTable("table_handle", ctx, &table));
     core::ScopedUnref unref_me(table);
-    Table* t = static_cast<Table*>(table);
+    det_table* handle = FusedHandle(table);
+    OP_REQUIRES(ctx, handle != nullptr,
+                errors::InvalidArgument("DetApplyAdagrad: the table's value dtype must be float, half or bfloat16"));
     const Tensor& keys = ctx->input(1);
     const Tensor& grads = ctx->input(2);
     const Tensor& lr = ctx->input(3);
     const Tensor& init = ctx->input(4);
-    const int64 n = keys.NumElements(), dim = t->value_shape().dim_size(0);
+    const int64 n = keys.NumElements(), dim = table->value_shape().dim_size(0);
     OP_REQUIRES(ctx, grads.NumElements() == n * dim, errors::InvalidArgument("grads must have shape [n, dim]"));
     OP_REQUIRES(ctx, init.NumElements() == dim || init.NumElements() == n * dim,
                 errors::InvalidArgument("init_param must have shape [dim] or [n, dim]"));
     OP_REQUIRES_OK(ctx, ToStatus(det_apply_adagrad(
-                            t->handle(), reinterpret_cast<const int64_t*>(keys.flat<int64>().data()),
+                            handle, reinterpret_cast<const int64_t*>(keys.flat<int64>().data()),
                             grads.flat<float>().data(), static_cast<size_t>(n), lr.scalar<float>()(), epsilon_,
                             init.flat<float>().data(), init.NumElements() == dim ? 0 : 1,
                             init_accum_, StreamOf(ctx))));
@@ -173,17 +174,19 @@ class DetApplyAdamOp : public OpKernel {
     tensorflow::lookup::LookupInterface* table = nullptr;
     OP_REQUIRES_OK(ctx, GetLookupTable("table_handle", ctx, &table));
     core::ScopedUnref unref_me(table);
-    Table* t = static_cast<Table*>(table);
+    det_table* handle = FusedHandle(table);
+    OP_REQUIRES(ctx, handle != nullptr,
+                errors::InvalidArgument("DetApplyAdam: the table's value dtype must be float, half or bfloat16"));
     const Tensor& keys = ctx->input(1);
     const Tensor& grads = ctx->input(2);
     const Tensor& alpha = ctx->input(3);
     const Tensor& init = ctx->input(4);
-    const int64 n = keys.NumElements(), dim = t->value_shape().dim_size(0);
+    const int64 n = keys.NumElements(), dim = table->value_shape().dim_size(0);
     OP_REQUIRES(ctx, grads.NumElements() == n * dim, errors::InvalidArgument("grads must have shape [n, dim]"));
     OP_REQUIRES(ctx, init.NumElements() == dim || init.NumElements() == n * dim,
                 errors::InvalidArgument("init_param must have shape [dim] or [n, dim]"));
     OP_REQUIRES_OK(ctx, ToStatus(det_apply_adam(
-                            t->handle(), reinterpret_cast<const int64_t*>(keys.flat<int64>().data()),
+                            handle, reinterpret_cast<const int64_t*>(keys.flat<int64>().data()),
                             grads.flat<float>().data(), static_cast<size_t>(n), alpha.scalar<float>()(), beta1_,
                             beta2_, epsilon_, init.flat<float>().data(), init.NumElements() == dim ? 0 : 1,
                             StreamOf(ctx))));
@@ -210,12 +213,14 @@ class DetApplyDuplicateIndicesOp : public OpKernel {
     tensorflow::lookup::LookupInterface* table = nullptr;
     OP_REQUIRES_OK(ctx, GetLookupTable("table_handle", ctx, &table));
     core::ScopedUnref unref_me(table);
-    Table* t = static_cast<Table*>(table);
+    det_table* handle = FusedHandle(table);
+    OP_REQUIRES(ctx, handle != nullptr,
+                errors::InvalidArgument("DetApply*DuplicateIndices: the table's value dtype must be float, half or bfloat16"));
     const Tensor& ids = ctx->input(1);
     const Tensor& grads = ctx->input(2);
     const Tensor& step = ctx->input(3);
     const Tensor& init = ctx->input(4);
-    const int64 n = ids.NumElements(), dim = t->value_shape().dim_size(0);
+    const int64 n = ids.NumElements(), dim = table->value_shape().dim_size(0);
     OP_REQUIRES(ctx, grads.NumElements() == n * dim, errors::InvalidArgument("grads must have shape [n, dim]"));
     OP_REQUIRES(ctx, init.NumElements() == dim, errors::InvalidArgument("init_param must have shape [dim]"));
     if (n == 0) return;
@@ -228,11 +233,11 @@ class DetApplyDuplicateIndicesOp : public OpKernel {
     const int64_t* k = reinterpret_cast<const int64_t*>(ids.flat<int64>().data());
     const float* g = grads.flat<float>().data();
     if (OPT == 0) {
-      OP_REQUIRES_OK(ctx, ToStatus(det_apply_adagrad_dup(t->handle(), k, g, static_cast<size_t>(n), step.scalar<float>()(),
+      OP_REQUIRES_OK(ctx, ToStatus(det_apply_adagrad_dup(handle, k, g, static_cast<size_t>(n), step.scalar<float>()(),
                                                          epsilon_, init.flat<float>().data(), init_accum_, aligned,
                                                          ws_bytes, nullptr, StreamOf(ctx))));
     } else {
-      OP_REQUIRES_OK(ctx, ToStatus(det_apply_adam_dup(t->handle(), k, g, static_cast<size_t>(n), step.scalar<float>()(),
+      OP_REQUIRES_OK(ctx, ToStatus(det_apply_adam_dup(handle, k, g, static_cast<size_t>(n), step.scalar<float>()(),
                                                       beta1_, beta2_, epsilon_, init.flat<float>().data(), aligned,
                                                       ws_bytes, nullptr, StreamOf(ctx))));
     }

@@ -117,9 +117,12 @@ class DetHashTableOfTensorsGpu final : public LookupInterface {
     cfg.dim = static_cast<int32_t>(runtime_dim_);
     cfg.device = ctx->device_ordinal();   // TF: ctx->device()->tensorflow_accelerator_device_info()->gpu_id
     // optimizer slot planes co-indexed with the rows (needed by TFRA>DetApplyAdagrad / Adam): no attr of the
-    // reference op carries this, so it is an environment override like TFRA_GPU_HASHTABLE_UPLIMIT_SIZE (:102-113)
+    // reference op carries this, so it is an environment override like TFRA_GPU_HASHTABLE_UPLIMIT_SIZE (:102-113).
+    // The planes are fp32 beside float, half or bfloat16 rows; tables of other dtypes get none.
     const char* planes = std::getenv("TFRA_DET_SLOT_PLANES");
-    cfg.num_slot_planes = (planes && cfg.value_dtype == DET_FLOAT32) ? std::atoi(planes) : 0;
+    const bool fused_dtype = cfg.value_dtype == DET_FLOAT32 || cfg.value_dtype == DET_FLOAT16 ||
+                             cfg.value_dtype == DET_BFLOAT16;
+    cfg.num_slot_planes = (planes && fused_dtype) ? std::atoi(planes) : 0;
     cfg.init_capacity = static_cast<uint64_t>(init_capacity);
     cfg.max_capacity = static_cast<uint64_t>(max_capacity);
     cfg.max_load_factor = 0.f;

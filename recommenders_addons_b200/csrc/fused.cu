@@ -296,6 +296,29 @@ static inline float __int_as_float(int i) {
 }
 static inline int4 make_int4(int x, int y, int z, int w) { return int4{x, y, z, w}; }
 static inline int2 make_int2(int x, int y) { return int2{x, y}; }
+// the narrowing of the fused optimizer step: round to nearest even, overflow to +-inf, subnormals kept, NaN stays NaN
+static inline __half __float2half_rn(float f) { return emu_float_to_half(f); }
+static inline __nv_bfloat16 __float2bfloat16_rn(float f) {
+  unsigned bits;
+  memcpy(&bits, &f, 4);
+  __nv_bfloat16 r;
+  if ((bits & 0x7fffffffu) > 0x7f800000u) {
+    r.x = 0x7fffu;                      // the device's canonical bf16 NaN
+  } else {
+    bits += 0x7fffu + ((bits >> 16) & 1u);
+    r.x = (unsigned short)(bits >> 16);
+  }
+  return r;
+}
+static inline unsigned short __half_as_ushort(__half h) { return h.x; }
+static inline unsigned short __bfloat16_as_ushort(__nv_bfloat16 h) { return h.x; }
+// the emulator completes an asynchronous copy at once
+static inline void cp_async8(void* smem_dst, const void* gsrc) { memcpy(smem_dst, gsrc, 8); }
+#else
+// 8 B asynchronous copy global -> shared (the param vector of a half row; .cg takes 16 B only)
+__device__ __forceinline__ void cp_async8(void* smem_dst, const void* gsrc) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(smem_u32(smem_dst)), "l"(gsrc) : "memory");
+}
 #endif
 __device__ __forceinline__ float widen(__half h) { return __half2float(h); }
 __device__ __forceinline__ float widen(__nv_bfloat16 h) { return __bfloat162float(h); }
@@ -309,6 +332,12 @@ template <> __device__ __forceinline__ int widen_bits<__half>(unsigned w, int k)
 }
 template <> __device__ __forceinline__ int widen_bits<__nv_bfloat16>(unsigned w, int k) {
   return (int)(k ? w & 0xffff0000u : w << 16);
+}
+// the 16 bits of `f` rounded to nearest even into H (the one rounding of the fused optimizer step on a half table)
+template <typename H> __device__ __forceinline__ unsigned narrow_bits(float f);
+template <> __device__ __forceinline__ unsigned narrow_bits<__half>(float f) { return __half_as_ushort(__float2half_rn(f)); }
+template <> __device__ __forceinline__ unsigned narrow_bits<__nv_bfloat16>(float f) {
+  return __bfloat16_as_ushort(__float2bfloat16_rn(f));
 }
 
 // one OV-byte fp32 vector from the OV / 2 bytes of half row it widens
@@ -420,6 +449,13 @@ template <> struct FVec<4> {
   __device__ __forceinline__ void load(const __half* p) { load_half(p); }
   __device__ __forceinline__ void load(const __nv_bfloat16* p) { load_half(p); }
   __device__ __forceinline__ void store(float* p) const { *reinterpret_cast<float4*>(p) = v; }
+  // rounded to 4 halves, one 8 B store
+  template <typename H> __device__ __forceinline__ void store_half(H* p) const {
+    *reinterpret_cast<int2*>(p) = make_int2((int)(narrow_bits<H>(v.x) | narrow_bits<H>(v.y) << 16),
+                                            (int)(narrow_bits<H>(v.z) | narrow_bits<H>(v.w) << 16));
+  }
+  __device__ __forceinline__ void store(__half* p) const { store_half(p); }
+  __device__ __forceinline__ void store(__nv_bfloat16* p) const { store_half(p); }
   __device__ __forceinline__ void zero() { v = make_float4(0.f, 0.f, 0.f, 0.f); }
   __device__ __forceinline__ void fill(float x) { v = make_float4(x, x, x, x); }
   template <typename F> __device__ __forceinline__ void apply(F f) { f(v.x); f(v.y); f(v.z); f(v.w); }
@@ -431,6 +467,8 @@ template <> struct FVec<1> {
   __device__ __forceinline__ void load(const __half* p) { v = widen(*p); }
   __device__ __forceinline__ void load(const __nv_bfloat16* p) { v = widen(*p); }
   __device__ __forceinline__ void store(float* p) const { *p = v; }
+  __device__ __forceinline__ void store(__half* p) const { *p = __float2half_rn(v); }
+  __device__ __forceinline__ void store(__nv_bfloat16* p) const { *p = __float2bfloat16_rn(v); }
   __device__ __forceinline__ void zero() { v = 0.f; }
   __device__ __forceinline__ void fill(float x) { v = x; }
   template <typename F> __device__ __forceinline__ void apply(F f) { f(v); }
@@ -677,7 +715,11 @@ struct OptHyper {
   float init_slot;  // adagrad initial accumulator
 };
 
-template <int VF, int OPT>
+// T: the table's param row storage type (float, __half or __nv_bfloat16).  Slot planes are fp32 whatever T is, and the
+// lane geometry is that of the fp32 gradient row: a half lane reads and writes 8 B of param row where an fp32 lane
+// moves 16 B.  A half param is widened after its load (exact), stepped in fp32, and rounded to nearest even into T
+// once, at its store.
+template <int VF, int OPT, typename T = float>
 __global__ void __launch_bounds__(kThreadsF)
 apply_kernel(TableView t, const long long* __restrict__ keys, const float* __restrict__ grads, size_t n,
              OptHyper h, const float* __restrict__ init_param, int full_init, unsigned vpr, unsigned lpr,
@@ -695,7 +737,7 @@ apply_kernel(TableView t, const long long* __restrict__ keys, const float* __res
   const unsigned rows_per_step = 32u >> lpr_shift;
   const unsigned sub = (unsigned)lane >> lpr_shift;
   const unsigned c0 = (unsigned)lane & (lpr - 1u);
-  float* P = (float*)t.planes[0];
+  T* P = (T*)t.planes[0];
   float* S1 = (float*)t.planes[1];
   float* S2 = (float*)t.planes[2];
   const float omb1 = 1.f - h.beta1, omb2 = 1.f - h.beta2;
@@ -807,7 +849,9 @@ __device__ __forceinline__ void score_touch<true>(const ScoreArg<true>& sa, long
   if (valid && slot >= 0) sa.sc[slot] = rule_score(sa.rule, is_new ? 0ull : sa.sc[slot], false, 0ull, now_ns());
 }
 
-template <int OPT, bool SCORED = false>
+// T: the param row storage type, as in apply_kernel.  An existing key's half param vector is one 8 B cp.async into the
+// first half of its 16 B stage slot; a new key's is the 16 B fp32 init_param vector, as on an fp32 table.
+template <int OPT, bool SCORED = false, typename T = float>
 __global__ void __launch_bounds__(kThreadsF)
 apply_staged_kernel(TableView t, const long long* __restrict__ keys, const float* __restrict__ grads, size_t n,
                     OptHyper h, const float* __restrict__ init_param, int full_init, unsigned vpr, unsigned lpr,
@@ -829,7 +873,7 @@ apply_staged_kernel(TableView t, const long long* __restrict__ keys, const float
   const unsigned sub = (unsigned)lane >> lpr_shift;
   const unsigned c0 = (unsigned)lane & (lpr - 1u);
   const bool lane_on = c0 < vpr;
-  float* P = (float*)t.planes[0];
+  T* P = (T*)t.planes[0];
   float* S1 = (float*)t.planes[1];
   float* S2 = (float*)t.planes[2];
   const float omb1 = 1.f - h.beta1, omb2 = 1.f - h.beta2;
@@ -870,7 +914,12 @@ apply_staged_kernel(TableView t, const long long* __restrict__ keys, const float
         if (ok) {
           const size_t ro = (size_t)sl * dim + (size_t)c0 * 4;
           cp_async16(sm(stage, st, 0), grads + gi * dim + (size_t)c0 * 4);
-          cp_async16(sm(stage, st, 1), nw ? (full_init ? init_param + gi * dim : init_param) + (size_t)c0 * 4 : P + ro);
+          if constexpr (std::is_same<T, float>::value)
+            cp_async16(sm(stage, st, 1), nw ? (full_init ? init_param + gi * dim : init_param) + (size_t)c0 * 4 : P + ro);
+          else if (nw)
+            cp_async16(sm(stage, st, 1), (full_init ? init_param + gi * dim : init_param) + (size_t)c0 * 4);
+          else
+            cp_async8(sm(stage, st, 1), P + ro);
           if (!nw) {
             cp_async16(sm(stage, st, 2), S1 + ro);
             if (OPT == 1) cp_async16(sm(stage, st, 3), S2 + ro);
@@ -903,7 +952,9 @@ apply_staged_kernel(TableView t, const long long* __restrict__ keys, const float
           const size_t ro = (size_t)sl * dim + (size_t)c0 * 4;
           FVec<4> g, p, a, b2;
           g.v = *sm(stage, st, 0);
-          p.v = *sm(stage, st, 1);
+          if constexpr (std::is_same<T, float>::value) p.v = *sm(stage, st, 1);
+          else if (nw) p.v = *sm(stage, st, 1);
+          else p.load(reinterpret_cast<const T*>(sm(stage, st, 1)));
           if (OPT == 0) {
             if (fresh) a.fill(h.init_slot); else a.v = *sm(stage, st, 2);
             a.zip(g, [](float& av, float gv) { av = av + gv * gv; });
@@ -1515,6 +1566,16 @@ static void launch_segment_sum(const TableView& v, int sms, const long long* slo
   }
 }
 
+// K7: f(row) with decltype(row)::type the param row storage type of a float32, float16 or bfloat16 table (the caller
+// has refused every other dtype)
+template <typename T> struct RowType { using type = T; };
+template <typename F>
+static det_status dispatch_row_type(int value_dtype, F&& f) {
+  if (value_dtype == DET_FLOAT16) return f(RowType<__half>());
+  if (value_dtype == DET_BFLOAT16) return f(RowType<__nv_bfloat16>());
+  return f(RowType<float>());
+}
+
 }  // namespace det
 
 using namespace det;
@@ -1667,7 +1728,9 @@ static det_status apply_common(det_table* t, const int64_t* keys, const float* g
                                const long long* n_dev = nullptr) {
   if (!t) return fail(DET_INVALID_ARGUMENT, "det_apply: null table");
   det::MutLock _lk(t);
-  if (t->cfg.value_dtype != DET_FLOAT32) return fail(DET_UNIMPLEMENTED, "det_apply: float32 tables only");
+  const int vt = t->cfg.value_dtype;
+  if (vt != DET_FLOAT32 && vt != DET_FLOAT16 && vt != DET_BFLOAT16)
+    return fail(DET_UNIMPLEMENTED, "det_apply: float32, float16 and bfloat16 tables only");
   if (t->cfg.num_slot_planes < (opt == 0 ? 1 : 2))
     return fail(DET_INVALID_ARGUMENT, "det_apply: table was created with too few optimizer slot planes");
   if (n == 0) return DET_OK;
@@ -1688,21 +1751,23 @@ static det_status apply_common(det_table* t, const int64_t* keys, const float* g
     const int ns = opt == 0 ? 3 : 4;
     const size_t smem = (size_t)(kThreadsF / 32) * 2 * kStageSteps * ns * 32 * 16;
     const int tma = (((uintptr_t)keys & 15u) == 0) ? 1 : 0;
-    st = dispatch_bit(t->ev != nullptr, [&](auto SCORED) -> det_status {
-      return dispatch_bit(opt != 0, [&](auto OPT) -> det_status {
-        constexpr bool kScored = decltype(SCORED)::value;
-        ScoreArg<kScored> sa;
-        if constexpr (kScored) {
-          sa.sc = evict_scores(t);
-          sa.rule = evict_rule(t);
-        }
-        const auto kern = apply_staged_kernel<decltype(OPT)::value, kScored>;
-        CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        int occ = 1;
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, kThreadsF, smem) != cudaSuccess || occ < 1) occ = 1;
-        DET_LAUNCH(kern, grid_for(n, kTileKeys, t->sm_count, occ), kThreadsF, smem, s, v, k, grads, n, h, init_param,
-                   full_init, vpr, lpr, sh, tma, sa, n_dev);
-        return DET_OK;
+    st = dispatch_row_type(vt, [&](auto row) -> det_status {
+      return dispatch_bit(t->ev != nullptr, [&](auto SCORED) -> det_status {
+        return dispatch_bit(opt != 0, [&](auto OPT) -> det_status {
+          constexpr bool kScored = decltype(SCORED)::value;
+          ScoreArg<kScored> sa;
+          if constexpr (kScored) {
+            sa.sc = evict_scores(t);
+            sa.rule = evict_rule(t);
+          }
+          const auto kern = apply_staged_kernel<decltype(OPT)::value, kScored, typename decltype(row)::type>;
+          CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+          int occ = 1;
+          if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, kThreadsF, smem) != cudaSuccess || occ < 1) occ = 1;
+          DET_LAUNCH(kern, grid_for(n, kTileKeys, t->sm_count, occ), kThreadsF, smem, s, v, k, grads, n, h, init_param,
+                     full_init, vpr, lpr, sh, tma, sa, n_dev);
+          return DET_OK;
+        });
       });
     });
     if (st != DET_OK) return st;
@@ -1710,13 +1775,15 @@ static det_status apply_common(det_table* t, const int64_t* keys, const float* g
     note_mutation(t, n, s);
     return DET_OK;   // scores of a table with an eviction strategy were written by the kernel itself
   }
-  dispatch_bit(opt != 0, [&](auto OPT) -> det_status {
-    return dispatch_bit(vec4, [&](auto VEC4) -> det_status {
-      const auto kern = apply_kernel<decltype(VEC4)::value ? 4 : 1, decltype(OPT)::value>;
-      const int grid = grid_for(n, kTileKeys, t->sm_count, occupancy_of(kern, kThreadsF));
-      DET_LAUNCH(kern, grid, kThreadsF, 0, s, v, k, grads, n, h, init_param, full_init, vpr, lpr, sh,
-                 (((uintptr_t)keys & 15u) == 0) ? 1 : 0);
-      return DET_OK;
+  dispatch_row_type(vt, [&](auto row) -> det_status {
+    return dispatch_bit(opt != 0, [&](auto OPT) -> det_status {
+      return dispatch_bit(vec4, [&](auto VEC4) -> det_status {
+        const auto kern = apply_kernel<decltype(VEC4)::value ? 4 : 1, decltype(OPT)::value, typename decltype(row)::type>;
+        const int grid = grid_for(n, kTileKeys, t->sm_count, occupancy_of(kern, kThreadsF));
+        DET_LAUNCH(kern, grid, kThreadsF, 0, s, v, k, grads, n, h, init_param, full_init, vpr, lpr, sh,
+                   (((uintptr_t)keys & 15u) == 0) ? 1 : 0);
+        return DET_OK;
+      });
     });
   });
   CUDA_TRY(cudaGetLastError());

@@ -1083,8 +1083,10 @@ static det_status create_common(det_table** out, const det_config* cfg, void* re
   if (cfg->dim <= 0) return fail(DET_INVALID_ARGUMENT, "det_table_create: dim must be positive (value_shape must be a vector)");
   if (cfg->num_slot_planes < 0 || cfg->num_slot_planes >= kMaxPlanes)
     return fail(DET_INVALID_ARGUMENT, "det_table_create: num_slot_planes must be in [0,3]");
-  if (cfg->num_slot_planes > 0 && cfg->value_dtype != DET_FLOAT32)
-    return fail(DET_INVALID_ARGUMENT, "det_table_create: optimizer slot planes need float32 values");
+  // slot planes are fp32 rows of 4 * dim bytes beside value rows of fp32, fp16 or bf16 (the fused optimizer step)
+  if (cfg->num_slot_planes > 0 && cfg->value_dtype != DET_FLOAT32 && cfg->value_dtype != DET_FLOAT16 &&
+      cfg->value_dtype != DET_BFLOAT16)
+    return fail(DET_INVALID_ARGUMENT, "det_table_create: optimizer slot planes need float32, float16 or bfloat16 values");
   int ndev = 0;
   CUDA_TRY(cudaGetDeviceCount(&ndev));
   if (cfg->device < 0 || cfg->device >= ndev) return fail(DET_INVALID_ARGUMENT, "det_table_create: bad device ordinal");

@@ -5,13 +5,17 @@ of the UNIQUE rows from the table, autograd produces the gradient of that scratc
 writes the update back with the fused find-or-insert + optimizer kernel."""
 import torch
 
-from .optimizer import ComposedOptimizer, _FusedBase
+from .optimizer import _FUSED_DTYPES, ComposedOptimizer, _FusedBase
 from .sharded import PeerShardedVariable, ShardedVariable
 from .variable import Variable, default_partition_fn, embedding_lookup_unique, gather_unique, unique
 
 
 class Embedding(torch.nn.Module):
-  """de.keras.layers.Embedding: dynamic embedding space, arbitrary ids shape -> ids.shape + [embedding_size]."""
+  """de.keras.layers.Embedding: dynamic embedding space, arbitrary ids shape -> ids.shape + [embedding_size].
+
+  num_slot_planes: float32 optimizer slot planes beside the rows, for the fused Adagrad / Adam step; kept for float32,
+  float16 and bfloat16 rows (the step widens a half row, updates it in float32 and rounds it once), 0 for any other
+  value_dtype."""
 
   def __init__(self, embedding_size, key_dtype=torch.int64, value_dtype=torch.float32, combiner="sum", initializer=None,
                devices=None, name="DynamicEmbeddingLayer", with_unique=True, trainable=True, bp_v2=False,
@@ -27,7 +31,7 @@ class Embedding(torch.nn.Module):
     self.params = Variable(key_dtype=key_dtype, value_dtype=value_dtype, dim=self.embedding_size, devices=devices,
                            partitioner=partitioner, name=name, initializer=initializer, trainable=trainable,
                            init_size=init_capacity, kv_creator=kv_creator, bp_v2=bp_v2, restrict_policy=restrict_policy,
-                           num_slot_planes=num_slot_planes if value_dtype == torch.float32 else 0,
+                           num_slot_planes=num_slot_planes if value_dtype in _FUSED_DTYPES else 0,
                            short_file_name=short_file_name)
     self._wrappers = []
 
