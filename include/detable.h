@@ -274,6 +274,22 @@ det_status det_apply_adagrad(det_table* t, const int64_t* keys, const float* gra
 det_status det_apply_adam(det_table* t, const int64_t* keys, const float* grads, size_t n,
                           float alpha, float beta1, float beta2, float epsilon,
                           const float* init_param, int full_size_init, det_stream_t stream);
+/* The same step for SGD, momentum and FTRL, each fp32 operation rounded on its own, in the order written (TF's sparse
+ * CPU kernels).  Keys, init_param, value dtypes, eviction scores: as det_apply_adagrad.  A key the step creates gets
+ * the "no slot state" marker in every slot plane the step does not write, as det_insert gives it.
+ * SGD     (momentum == 0): p = p - lr*g;  no slot plane needed.
+ * Momentum (TF1 MomentumOptimizer; torch SGD(momentum, dampening=0)): a = a*m + g;  p = p - a*lr, or with nesterov
+ *   p = p - ((g*lr) + ((a*m)*lr));  plane 1 = momentum (initial 0).  nesterov with momentum == 0: DET_INVALID_ARGUMENT.
+ * FTRL    (learning_rate_power = -0.5): gs = l2_shrinkage > 0 ? g + (2*l2_shrinkage)*p : g;  nn = n + g*g;
+ *   z = z + (gs - (((sqrt(nn) - sqrt(n)) / lr) * p));  p = (min(max(z, -l1), l1) - z) / (sqrt(nn)/lr + 2*l2);  n = nn
+ *   (p is +0 exactly when |z| <= l1);  plane 1 = accumulator n (initial init_accum), plane 2 = linear z (initial 0).
+ *   lr <= 0 or a negative l1, l2, l2_shrinkage or init_accum: DET_INVALID_ARGUMENT.
+ * Additive to ABI 8. */
+det_status det_apply_sgd(det_table* t, const int64_t* keys, const float* grads, size_t n, float lr, float momentum,
+                         int nesterov, const float* init_param, int full_size_init, det_stream_t stream);
+det_status det_apply_ftrl(det_table* t, const int64_t* keys, const float* grads, size_t n, float lr, float l1, float l2,
+                          float l2_shrinkage, const float* init_param, int full_size_init, float init_accum,
+                          det_stream_t stream);
 
 /* ---- HOST-buffer entry points (the op placed on host tensors; used for end-to-end timing):
  * pinned or pageable HOST pointers; chunked H2D -> kernel -> D2H pipeline on internal streams;
@@ -310,6 +326,12 @@ det_status det_apply_adagrad_dup(det_table* t, const int64_t* ids, const float* 
                                  int64_t* n_unique_dev_out, det_stream_t stream);
 det_status det_apply_adam_dup(det_table* t, const int64_t* ids, const float* grads, size_t n, float alpha, float beta1,
                               float beta2, float epsilon, const float* init_param, void* workspace,
+                              size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_sgd_dup(det_table* t, const int64_t* ids, const float* grads, size_t n, float lr, float momentum,
+                             int nesterov, const float* init_param, void* workspace, size_t workspace_bytes,
+                             int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_ftrl_dup(det_table* t, const int64_t* ids, const float* grads, size_t n, float lr, float l1,
+                              float l2, float l2_shrinkage, const float* init_param, float init_accum, void* workspace,
                               size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream);
 
 /* ---- key-hash sharding across GPUs (python/ops/dynamic_embedding_variable.py:165-197 default_partition_fn,

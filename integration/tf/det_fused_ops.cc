@@ -66,6 +66,49 @@ REGISTER_OP("TFRA>DetApplyAdamDuplicateIndices")
     .Attr("beta2: float = 0.999")
     .Attr("epsilon: float = 1e-8");
 
+// SGD (momentum == 0) and momentum (TF1 MomentumOptimizer / ResourceSparseApplyMomentum), and FTRL
+// (ResourceSparseApplyFtrl(V2) with learning_rate_power = -0.5), as det_apply_sgd / det_apply_ftrl.  Keras' beta enters
+// the FTRL op as l2 + beta / (2 * lr), folded by the caller.
+REGISTER_OP("TFRA>DetApplySgd")
+    .Input("table_handle: resource")
+    .Input("keys: int64")          // [n] unique
+    .Input("grads: float")         // [n, dim]
+    .Input("lr: float")
+    .Input("init_param: float")    // [dim] or [n, dim]
+    .Attr("momentum: float = 0.0")
+    .Attr("nesterov: int = 0");    // 1: Nesterov momentum (needs momentum > 0)
+
+REGISTER_OP("TFRA>DetApplyFtrl")
+    .Input("table_handle: resource")
+    .Input("keys: int64")
+    .Input("grads: float")
+    .Input("lr: float")
+    .Input("init_param: float")
+    .Attr("l1: float = 0.0")
+    .Attr("l2: float = 0.0")
+    .Attr("l2_shrinkage: float = 0.0")
+    .Attr("initial_accumulator_value: float = 0.1");
+
+REGISTER_OP("TFRA>DetApplySgdDuplicateIndices")
+    .Input("table_handle: resource")
+    .Input("ids: int64")
+    .Input("grads: float")
+    .Input("lr: float")
+    .Input("init_param: float")    // [dim]
+    .Attr("momentum: float = 0.0")
+    .Attr("nesterov: int = 0");    // 1: Nesterov momentum (needs momentum > 0)
+
+REGISTER_OP("TFRA>DetApplyFtrlDuplicateIndices")
+    .Input("table_handle: resource")
+    .Input("ids: int64")
+    .Input("grads: float")
+    .Input("lr: float")
+    .Input("init_param: float")    // [dim]
+    .Attr("l1: float = 0.0")
+    .Attr("l2: float = 0.0")
+    .Attr("l2_shrinkage: float = 0.0")
+    .Attr("initial_accumulator_value: float = 0.1");
+
 // The gradient dedupe in front of the sparse optimizer step: unsorted_segment_sum(values, idx, num_segments) as
 // _deduplicate_indexed_slices calls it before _resource_apply_sparse_duplicate_indices
 // (python/ops/dynamic_embedding_optimizer.py:150,184), with the rows of one segment added in position order
@@ -247,6 +290,72 @@ class DetApplyDuplicateIndicesOp : public OpKernel {
   float epsilon_ = 0.f, init_accum_ = 0.1f, beta1_ = 0.9f, beta2_ = 0.999f;
 };
 
+// SGD / momentum (OPT 0) and FTRL (OPT 1), unique keys (DUP false) or repeated ids in one call (DUP true)
+template <int OPT, bool DUP>
+class DetApplySgdFtrlOp : public OpKernel {
+ public:
+  explicit DetApplySgdFtrlOp(OpKernelConstruction* ctx) : OpKernel(ctx) {
+    if (OPT == 0) {
+      OP_REQUIRES_OK(ctx, ctx->GetAttr("momentum", &momentum_));
+      OP_REQUIRES_OK(ctx, ctx->GetAttr("nesterov", &nesterov_));
+    } else {
+      OP_REQUIRES_OK(ctx, ctx->GetAttr("l1", &l1_));
+      OP_REQUIRES_OK(ctx, ctx->GetAttr("l2", &l2_));
+      OP_REQUIRES_OK(ctx, ctx->GetAttr("l2_shrinkage", &l2_shrinkage_));
+      OP_REQUIRES_OK(ctx, ctx->GetAttr("initial_accumulator_value", &init_accum_));
+    }
+  }
+  void Compute(OpKernelContext* ctx) override {
+    tensorflow::lookup::LookupInterface* table = nullptr;
+    OP_REQUIRES_OK(ctx, GetLookupTable("table_handle", ctx, &table));
+    core::ScopedUnref unref_me(table);
+    det_table* handle = FusedHandle(table);
+    OP_REQUIRES(ctx, handle != nullptr,
+                errors::InvalidArgument(string(OPT == 0 ? "DetApplySgd" : "DetApplyFtrl") +
+                                        ": the table's value dtype must be float, half or bfloat16"));
+    const Tensor& keys = ctx->input(1);
+    const Tensor& grads = ctx->input(2);
+    const Tensor& lr = ctx->input(3);
+    const Tensor& init = ctx->input(4);
+    const int64 n = keys.NumElements(), dim = table->value_shape().dim_size(0);
+    OP_REQUIRES(ctx, grads.NumElements() == n * dim, errors::InvalidArgument("grads must have shape [n, dim]"));
+    OP_REQUIRES(ctx, init.NumElements() == dim || (!DUP && init.NumElements() == n * dim),
+                errors::InvalidArgument(DUP ? "init_param must have shape [dim]" : "init_param must have shape [dim] or [n, dim]"));
+    const int64_t* k = reinterpret_cast<const int64_t*>(keys.flat<int64>().data());
+    const float* g = grads.flat<float>().data();
+    const float* ip = init.flat<float>().data();
+    const float step = lr.scalar<float>()();
+    if (!DUP) {
+      const int full = init.NumElements() == dim ? 0 : 1;
+      if (OPT == 0) {
+        OP_REQUIRES_OK(ctx, ToStatus(det_apply_sgd(handle, k, g, static_cast<size_t>(n), step, momentum_, nesterov_,
+                                                   ip, full, StreamOf(ctx))));
+      } else {
+        OP_REQUIRES_OK(ctx, ToStatus(det_apply_ftrl(handle, k, g, static_cast<size_t>(n), step, l1_, l2_, l2_shrinkage_, ip,
+                                                    full, init_accum_, StreamOf(ctx))));
+      }
+      return;
+    }
+    if (n == 0) return;
+    const size_t ws_bytes = det_apply_dup_workspace_bytes(static_cast<size_t>(n), static_cast<size_t>(dim));
+    Tensor ws;
+    OP_REQUIRES_OK(ctx, ctx->allocate_temp(DT_INT8, TensorShape({static_cast<int64>(ws_bytes + 256)}), &ws));
+    int8* raw = ws.flat<int8>().data();
+    void* aligned = raw + ((256 - (reinterpret_cast<uintptr_t>(raw) & 255u)) & 255u);
+    if (OPT == 0) {
+      OP_REQUIRES_OK(ctx, ToStatus(det_apply_sgd_dup(handle, k, g, static_cast<size_t>(n), step, momentum_, nesterov_,
+                                                     ip, aligned, ws_bytes, nullptr, StreamOf(ctx))));
+    } else {
+      OP_REQUIRES_OK(ctx, ToStatus(det_apply_ftrl_dup(handle, k, g, static_cast<size_t>(n), step, l1_, l2_, l2_shrinkage_,
+                                                      ip, init_accum_, aligned, ws_bytes, nullptr, StreamOf(ctx))));
+    }
+  }
+
+ private:
+  float momentum_ = 0.f, l1_ = 0.f, l2_ = 0.f, l2_shrinkage_ = 0.f, init_accum_ = 0.1f;
+  int nesterov_ = 0;
+};
+
 class DetSegmentReduceOp : public OpKernel {
  public:
   explicit DetSegmentReduceOp(OpKernelConstruction* ctx) : OpKernel(ctx) {}
@@ -279,6 +388,12 @@ REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplyAdagradDuplicateIndices").Device(DEVI
                         DetApplyDuplicateIndicesOp<0>);
 REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplyAdamDuplicateIndices").Device(DEVICE_GPU).HostMemory("alpha"),
                         DetApplyDuplicateIndicesOp<1>);
+REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplySgd").Device(DEVICE_GPU).HostMemory("lr"), DetApplySgdFtrlOp<0, false>);
+REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplyFtrl").Device(DEVICE_GPU).HostMemory("lr"), DetApplySgdFtrlOp<1, false>);
+REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplySgdDuplicateIndices").Device(DEVICE_GPU).HostMemory("lr"),
+                        DetApplySgdFtrlOp<0, true>);
+REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplyFtrlDuplicateIndices").Device(DEVICE_GPU).HostMemory("lr"),
+                        DetApplySgdFtrlOp<1, true>);
 
 }  // namespace det_shim
 }  // namespace lookup

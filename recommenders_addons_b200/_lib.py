@@ -68,6 +68,12 @@ SIGNATURES = {
     "det_apply_adagrad_dup": (_i, [_vp, _vp, _vp, _sz, ctypes.c_float, ctypes.c_float, _vp, ctypes.c_float, _vp, _sz, _vp, _vp]),
     "det_apply_adam_dup": (_i, [_vp, _vp, _vp, _sz, ctypes.c_float, ctypes.c_float, ctypes.c_float, ctypes.c_float, _vp, _vp,
                                 _sz, _vp, _vp]),
+    "det_apply_sgd": (_i, [_vp, _vp, _vp, _sz, ctypes.c_float, ctypes.c_float, _i, _vp, _i, _vp]),
+    "det_apply_ftrl": (_i, [_vp, _vp, _vp, _sz, ctypes.c_float, ctypes.c_float, ctypes.c_float, ctypes.c_float, _vp, _i,
+                            ctypes.c_float, _vp]),
+    "det_apply_sgd_dup": (_i, [_vp, _vp, _vp, _sz, ctypes.c_float, ctypes.c_float, _i, _vp, _vp, _sz, _vp, _vp]),
+    "det_apply_ftrl_dup": (_i, [_vp, _vp, _vp, _sz, ctypes.c_float, ctypes.c_float, ctypes.c_float, ctypes.c_float, _vp,
+                                ctypes.c_float, _vp, _sz, _vp, _vp]),
     "det_find_host": (_i, [_vp, _vp, _sz, _vp, _i, _vp, _vp]),
     "det_insert_host": (_i, [_vp, _vp, _vp, _sz]),
     "det_find_host_async": (_i, [_vp, _vp, _sz, _vp, _i, _vp, _vp]),

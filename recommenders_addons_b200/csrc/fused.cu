@@ -708,22 +708,93 @@ segment_sum_wide_kernel(TableView t, const long long* __restrict__ slots, const 
 // ------------------------------------------------------------------------------------------------
 // K7: fused find-or-insert + optimizer update
 // ------------------------------------------------------------------------------------------------
+// The optimizer of a K7 launch (template parameter OPT) and its hyper-parameters.  The fields mean, per optimizer:
+//   OPT 0 Adagrad : lr,    eps = epsilon,                             init_slot = initial accumulator
+//   OPT 1 Adam    : lr = alpha, eps = epsilon, beta1, beta2
+//   OPT 2 SGD     : lr
+//   OPT 3 Momentum: lr,    eps = 1 for nesterov (else 0), beta1 = momentum
+//   OPT 4 FTRL    : lr,    eps = l1, beta1 = 2*l2, beta2 = 2*l2_shrinkage, init_slot = initial accumulator
 struct OptHyper {
-  float lr;       // adagrad lr | adam alpha
-  float eps;
+  float lr;       // adagrad lr | adam alpha | sgd, momentum and ftrl lr
+  float eps;      // adagrad / adam epsilon | momentum: nesterov flag | ftrl l1
   float beta1, beta2;
-  float init_slot;  // adagrad initial accumulator
+  float init_slot;  // adagrad / ftrl initial accumulator
 };
+
+// slot planes an optimizer reads and writes (planes 1 .. opt_slots(OPT)): momentum = plane 1; FTRL accumulator n =
+// plane 1, linear z = plane 2
+__host__ __device__ constexpr int opt_slots(int opt) { return opt == 1 || opt == 4 ? 2 : opt == 2 ? 0 : 1; }
+
+// SGD, momentum and FTRL on one fp32 element, one IEEE operation per operation in the order written (the library is
+// built with --fmad=false): p param, a slot 1, b slot 2, updated in place.  These restate TF's sparse CPU kernels
+// (ResourceSparseApplyMomentum, ResourceSparseApplyFtrl(V2) with learning_rate_power = -0.5).
+template <int OPT>
+__device__ __forceinline__ void opt_elem(const OptHyper& h, float g, float& p, float& a, float& b) {
+  if (OPT == 2) {
+    p = p - h.lr * g;
+  } else if (OPT == 3) {
+    a = a * h.beta1 + g;
+    if (h.eps != 0.f) p = p - ((g * h.lr) + ((a * h.beta1) * h.lr));   // nesterov
+    else p = p - a * h.lr;
+  } else {
+    // l2_shrinkage == 0 is FTRL V1: the gradient is used as it is (0 * inf must not make NaN)
+    const float gs = h.beta2 > 0.f ? g + h.beta2 * p : g;
+    const float nn = a + g * g;
+    const float sn = sqrtf(nn);
+    b = b + (gs - (((sn - sqrtf(a)) / h.lr) * p));
+    // min(max(z, -l1), l1) - z, with z kept as it is inside [-l1, l1]: the difference is then +0 exactly
+    const float c = b < -h.eps ? -h.eps : (b > h.eps ? h.eps : b);
+    const float x = c - b;
+    const float y = sn / h.lr + h.beta1;
+    p = x / y;
+    a = nn;
+  }
+}
+template <int OPT, int VF>
+__device__ __forceinline__ void opt_step(const OptHyper& h, const FVec<VF>& g, FVec<VF>& p, FVec<VF>& a, FVec<VF>& b) {
+  const float* gv = reinterpret_cast<const float*>(&g.v);
+  float* pv = reinterpret_cast<float*>(&p.v);
+  float* av = reinterpret_cast<float*>(&a.v);
+  float* bv = reinterpret_cast<float*>(&b.v);
+#pragma unroll
+  for (int e = 0; e < VF; ++e) opt_elem<OPT>(h, gv[e], pv[e], av[e], bv[e]);
+}
+
+// The slot-plane count of the table, for the optimizers that mark the slot planes they do not write (SGD, momentum,
+// FTRL): a key such a step creates gets kSlotUninit in the first word of its row in every other slot plane, as insert
+// gives it (table.cu insert_step).  An EMPTY trailing parameter for Adagrad and Adam keeps their kernels unchanged.
+template <int OPT> struct SlotPlanes { int n; };
+template <> struct SlotPlanes<0> {};
+template <> struct SlotPlanes<1> {};
+template <int OPT>
+__device__ __forceinline__ void mark_unwritten(const TableView& t, const SlotPlanes<OPT>& sp, long long slot) {
+  // unrolled: a plane index known at compile time keeps the TableView parameter out of local memory
+#pragma unroll
+  for (int p = 1 + opt_slots(OPT); p < kMaxPlanes; ++p)
+    if (p <= sp.n) *reinterpret_cast<unsigned*>(t.planes[p] + (size_t)slot * t.dim * 4u) = kSlotUninit;
+}
+constexpr int kNumOpts = 5;   // OPT 0 .. 4
+template <int OPT>
+static SlotPlanes<OPT> slot_planes_arg(const det_table* t) {
+  SlotPlanes<OPT> sp;
+  if constexpr (OPT >= 2) sp.n = t->cfg.num_slot_planes;
+  return sp;
+}
 
 // T: the table's param row storage type (float, __half or __nv_bfloat16).  Slot planes are fp32 whatever T is, and the
 // lane geometry is that of the fp32 gradient row: a half lane reads and writes 8 B of param row where an fp32 lane
 // moves 16 B.  A half param is widened after its load (exact), stepped in fp32, and rounded to nearest even into T
 // once, at its store.
+// FTRL's two square roots and three divisions per element: left to its own heuristics ptxas spills the probe's
+// first-bucket loads to reach 4 CTAs per SM; asking for 3 (the register-held Adagrad / Adam kernels' occupancy) keeps
+// them in registers.  0 = no minimum, the other optimizers' kernels as before.
+template <int OPT> constexpr int kApplyMinBlocks = OPT == 4 ? 3 : 0;
+
 template <int VF, int OPT, typename T = float>
-__global__ void __launch_bounds__(kThreadsF)
+__global__ void __launch_bounds__(kThreadsF, kApplyMinBlocks<OPT>)
 apply_kernel(TableView t, const long long* __restrict__ keys, const float* __restrict__ grads, size_t n,
              OptHyper h, const float* __restrict__ init_param, int full_init, unsigned vpr, unsigned lpr,
-             unsigned lpr_shift, int use_tma) {
+             unsigned lpr_shift, int use_tma, SlotPlanes<OPT> sp) {
   __shared__ __align__(128) long long s_keys[kStages][kTileKeys];
   __shared__ __align__(8) unsigned long long s_bar[kStages];
   __shared__ unsigned s_new, s_used;
@@ -773,7 +844,10 @@ apply_kernel(TableView t, const long long* __restrict__ keys, const float* __res
         ro[u] = ok[u] ? (size_t)s * dim : 0;
         // slot state absent: key created in this launch, or created by insert/accum and never stepped.
         // Every lane reads the marker word BEFORE any lane of the row's group overwrites it.
-        mark[u] = ok[u] ? __float_as_uint(S1[ro[u]]) : 0u;
+        mark[u] = ok[u] && opt_slots(OPT) > 0 ? __float_as_uint(S1[ro[u]]) : 0u;
+        if constexpr (OPT >= 2) {
+          if (ok[u] && nwv[u] && c0 == 0) mark_unwritten(t, sp, s);
+        }
       }
       __syncwarp();
 #pragma unroll
@@ -789,8 +863,12 @@ apply_kernel(TableView t, const long long* __restrict__ keys, const float* __res
           else p[u].load(P + ro[u] + o);
           if (OPT == 0) {
             if (fresh[u]) a[u].fill(h.init_slot); else a[u].load(S1 + ro[u] + o);
-          } else {
+          } else if (OPT == 1) {
             if (fresh[u]) { a[u].zero(); b[u].zero(); } else { a[u].load(S1 + ro[u] + o); b[u].load(S2 + ro[u] + o); }
+          } else if (OPT == 3) {
+            if (fresh[u]) a[u].zero(); else a[u].load(S1 + ro[u] + o);
+          } else if (OPT == 4) {
+            if (fresh[u]) { a[u].fill(h.init_slot); b[u].zero(); } else { a[u].load(S1 + ro[u] + o); b[u].load(S2 + ro[u] + o); }
           }
         }
 #pragma unroll
@@ -804,7 +882,7 @@ apply_kernel(TableView t, const long long* __restrict__ keys, const float* __res
             p[u].zip(upd, [](float& pv, float x) { pv = pv - x; });
             a[u].store(S1 + ro[u] + o);
             p[u].store(P + ro[u] + o);
-          } else {
+          } else if (OPT == 1) {
             // m += (g-m)(1-b1) ; v += (g*g-v)(1-b2) ; var -= (m*alpha)/(sqrt(v)+eps)
             a[u].zip(g[u], [omb1](float& mv, float gv) { mv = mv + (gv - mv) * omb1; });
             b[u].zip(g[u], [omb2](float& vv, float gv) { vv = vv + (gv * gv - vv) * omb2; });
@@ -813,6 +891,11 @@ apply_kernel(TableView t, const long long* __restrict__ keys, const float* __res
             p[u].zip(upd, [](float& pv, float x) { pv = pv - x; });
             a[u].store(S1 + ro[u] + o);
             b[u].store(S2 + ro[u] + o);
+            p[u].store(P + ro[u] + o);
+          } else {
+            opt_step<OPT>(h, g[u], p[u], a[u], b[u]);
+            if (opt_slots(OPT) > 0) a[u].store(S1 + ro[u] + o);
+            if (opt_slots(OPT) > 1) b[u].store(S2 + ro[u] + o);
             p[u].store(P + ro[u] + o);
           }
         }
@@ -855,9 +938,10 @@ template <int OPT, bool SCORED = false, typename T = float>
 __global__ void __launch_bounds__(kThreadsF)
 apply_staged_kernel(TableView t, const long long* __restrict__ keys, const float* __restrict__ grads, size_t n,
                     OptHyper h, const float* __restrict__ init_param, int full_init, unsigned vpr, unsigned lpr,
-                    unsigned lpr_shift, int use_tma, ScoreArg<SCORED> sa, const long long* __restrict__ n_dev) {
+                    unsigned lpr_shift, int use_tma, ScoreArg<SCORED> sa, const long long* __restrict__ n_dev,
+                    SlotPlanes<OPT> sp) {
   if (n_dev) n = (size_t)*n_dev;        // key count produced on the device (det_apply_*_dup); the grid covers the bound
-  constexpr int NS = OPT == 0 ? 3 : 4;  // streams per row: grad, param, slot1 (, slot2)
+  constexpr int NS = 2 + opt_slots(OPT);  // streams per row: grad, param (, slot1 (, slot2))
   DET_DYN_SHARED(dyn_smem);
   __shared__ __align__(128) long long s_keys[kStages][kTileKeys];
   __shared__ __align__(8) unsigned long long s_bar[kStages];
@@ -920,9 +1004,9 @@ apply_staged_kernel(TableView t, const long long* __restrict__ keys, const float
             cp_async16(sm(stage, st, 1), (full_init ? init_param + gi * dim : init_param) + (size_t)c0 * 4);
           else
             cp_async8(sm(stage, st, 1), P + ro);
-          if (!nw) {
+          if (!nw && NS > 2) {
             cp_async16(sm(stage, st, 2), S1 + ro);
-            if (OPT == 1) cp_async16(sm(stage, st, 3), S2 + ro);
+            if (NS > 3) cp_async16(sm(stage, st, 3), S2 + ro);
           }
         }
       }
@@ -947,7 +1031,7 @@ apply_staged_kernel(TableView t, const long long* __restrict__ keys, const float
         const size_t gi = base + (j & 31u);
         const bool row_ok = step < steps_total && gi < n && sl >= 0;
         // slot state absent: key created in this launch, or created by insert/accum and never stepped
-        const bool fresh = nw || (row_ok && __float_as_uint(*sm_mark(stage, st)) == kSlotUninit);
+        const bool fresh = nw || (NS > 2 && row_ok && __float_as_uint(*sm_mark(stage, st)) == kSlotUninit);
         if (row_ok && lane_on) {
           const size_t ro = (size_t)sl * dim + (size_t)c0 * 4;
           FVec<4> g, p, a, b2;
@@ -963,7 +1047,7 @@ apply_staged_kernel(TableView t, const long long* __restrict__ keys, const float
             p.zip(upd, [](float& pv, float x) { pv = pv - x; });
             a.store(S1 + ro);
             p.store(P + ro);
-          } else {
+          } else if (OPT == 1) {
             if (fresh) { a.zero(); b2.zero(); } else { a.v = *sm(stage, st, 2); b2.v = *sm(stage, st, 3); }
             a.zip(g, [omb1](float& mv, float gv) { mv = mv + (gv - mv) * omb1; });
             b2.zip(g, [omb2](float& vv, float gv) { vv = vv + (gv * gv - vv) * omb2; });
@@ -973,6 +1057,19 @@ apply_staged_kernel(TableView t, const long long* __restrict__ keys, const float
             a.store(S1 + ro);
             b2.store(S2 + ro);
             p.store(P + ro);
+          } else {
+            if (OPT == 3) {
+              if (fresh) a.zero(); else a.v = *sm(stage, st, 2);
+            } else if (OPT == 4) {
+              if (fresh) { a.fill(h.init_slot); b2.zero(); } else { a.v = *sm(stage, st, 2); b2.v = *sm(stage, st, 3); }
+            }
+            opt_step<OPT>(h, g, p, a, b2);
+            if (opt_slots(OPT) > 0) a.store(S1 + ro);
+            if (opt_slots(OPT) > 1) b2.store(S2 + ro);
+            p.store(P + ro);
+            if constexpr (OPT >= 2) {
+              if (nw && c0 == 0) mark_unwritten(t, sp, sl);
+            }
           }
         }
       }
@@ -1731,7 +1828,7 @@ static det_status apply_common(det_table* t, const int64_t* keys, const float* g
   const int vt = t->cfg.value_dtype;
   if (vt != DET_FLOAT32 && vt != DET_FLOAT16 && vt != DET_BFLOAT16)
     return fail(DET_UNIMPLEMENTED, "det_apply: float32, float16 and bfloat16 tables only");
-  if (t->cfg.num_slot_planes < (opt == 0 ? 1 : 2))
+  if (t->cfg.num_slot_planes < opt_slots(opt))
     return fail(DET_INVALID_ARGUMENT, "det_apply: table was created with too few optimizer slot planes");
   if (n == 0) return DET_OK;
   if (!keys || !grads || !init_param) return fail(DET_INVALID_ARGUMENT, "det_apply: null argument");
@@ -1748,12 +1845,12 @@ static det_status apply_common(det_table* t, const int64_t* keys, const float* g
   const long long* k = (const long long*)keys;
   if (vec4 && vpr <= lpr) {
     // cp.async-staged variant: 2 stages x kStageSteps x streams x 512 B per warp of dynamic shared memory
-    const int ns = opt == 0 ? 3 : 4;
+    const int ns = 2 + opt_slots(opt);
     const size_t smem = (size_t)(kThreadsF / 32) * 2 * kStageSteps * ns * 32 * 16;
     const int tma = (((uintptr_t)keys & 15u) == 0) ? 1 : 0;
     st = dispatch_row_type(vt, [&](auto row) -> det_status {
       return dispatch_bit(t->ev != nullptr, [&](auto SCORED) -> det_status {
-        return dispatch_bit(opt != 0, [&](auto OPT) -> det_status {
+        return dispatch_int<kNumOpts>(opt, [&](auto OPT) -> det_status {
           constexpr bool kScored = decltype(SCORED)::value;
           ScoreArg<kScored> sa;
           if constexpr (kScored) {
@@ -1765,7 +1862,7 @@ static det_status apply_common(det_table* t, const int64_t* keys, const float* g
           int occ = 1;
           if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, kThreadsF, smem) != cudaSuccess || occ < 1) occ = 1;
           DET_LAUNCH(kern, grid_for(n, kTileKeys, t->sm_count, occ), kThreadsF, smem, s, v, k, grads, n, h, init_param,
-                     full_init, vpr, lpr, sh, tma, sa, n_dev);
+                     full_init, vpr, lpr, sh, tma, sa, n_dev, slot_planes_arg<decltype(OPT)::value>(t));
           return DET_OK;
         });
       });
@@ -1776,12 +1873,12 @@ static det_status apply_common(det_table* t, const int64_t* keys, const float* g
     return DET_OK;   // scores of a table with an eviction strategy were written by the kernel itself
   }
   dispatch_row_type(vt, [&](auto row) -> det_status {
-    return dispatch_bit(opt != 0, [&](auto OPT) -> det_status {
+    return dispatch_int<kNumOpts>(opt, [&](auto OPT) -> det_status {
       return dispatch_bit(vec4, [&](auto VEC4) -> det_status {
         const auto kern = apply_kernel<decltype(VEC4)::value ? 4 : 1, decltype(OPT)::value, typename decltype(row)::type>;
         const int grid = grid_for(n, kTileKeys, t->sm_count, occupancy_of(kern, kThreadsF));
         DET_LAUNCH(kern, grid, kThreadsF, 0, s, v, k, grads, n, h, init_param, full_init, vpr, lpr, sh,
-                   (((uintptr_t)keys & 15u) == 0) ? 1 : 0);
+                   (((uintptr_t)keys & 15u) == 0) ? 1 : 0, slot_planes_arg<decltype(OPT)::value>(t));
         return DET_OK;
       });
     });
@@ -1806,6 +1903,48 @@ det_status det_apply_adam(det_table* t, const int64_t* keys, const float* grads,
   OptHyper h;
   h.lr = alpha; h.eps = epsilon; h.beta1 = beta1; h.beta2 = beta2; h.init_slot = 0.f;
   return apply_common(t, keys, grads, n, h, init_param, full_size_init, 1, (cudaStream_t)stream);
+}
+
+// SGD (momentum == 0, OPT 2) or momentum (OPT 3); sets *opt.  A momentum table's unstepped keys export 0.
+static det_status sgd_hyper(det_table* t, float lr, float momentum, int nesterov, OptHyper* h, int* opt) {
+  if (nesterov && momentum == 0.f) return fail(DET_INVALID_ARGUMENT, "det_apply_sgd: nesterov needs a momentum");
+  h->lr = lr; h->eps = nesterov ? 1.f : 0.f; h->beta1 = momentum; h->beta2 = 0.f; h->init_slot = 0.f;
+  *opt = momentum == 0.f ? 2 : 3;
+  if (t && *opt == 3) t->slot_init[1] = 0.f;
+  return DET_OK;
+}
+
+// FTRL (OPT 4): lr > 0 and l1, l2, l2_shrinkage, init_accum >= 0 as TF's ApplyFtrl checks them; 2*l2 and
+// 2*l2_shrinkage are exact in fp32
+static det_status ftrl_hyper(det_table* t, float lr, float l1, float l2, float l2_shrinkage, float init_accum,
+                             OptHyper* h) {
+  if (!(lr > 0.f)) return fail(DET_INVALID_ARGUMENT, "det_apply_ftrl: lr must be positive");
+  if (!(l1 >= 0.f) || !(l2 >= 0.f) || !(l2_shrinkage >= 0.f) || !(init_accum >= 0.f))
+    return fail(DET_INVALID_ARGUMENT, "det_apply_ftrl: l1, l2, l2_shrinkage and init_accum must be >= 0");
+  h->lr = lr; h->eps = l1; h->beta1 = 2.f * l2; h->beta2 = 2.f * l2_shrinkage; h->init_slot = init_accum;
+  if (t) {
+    t->slot_init[1] = init_accum;
+    t->slot_init[2] = 0.f;
+  }
+  return DET_OK;
+}
+
+det_status det_apply_sgd(det_table* t, const int64_t* keys, const float* grads, size_t n, float lr, float momentum,
+                         int nesterov, const float* init_param, int full_size_init, det_stream_t stream) {
+  OptHyper h;
+  int opt = 2;
+  const det_status st = sgd_hyper(t, lr, momentum, nesterov, &h, &opt);
+  if (st != DET_OK) return st;
+  return apply_common(t, keys, grads, n, h, init_param, full_size_init, opt, (cudaStream_t)stream);
+}
+
+det_status det_apply_ftrl(det_table* t, const int64_t* keys, const float* grads, size_t n, float lr, float l1, float l2,
+                          float l2_shrinkage, const float* init_param, int full_size_init, float init_accum,
+                          det_stream_t stream) {
+  OptHyper h;
+  const det_status st = ftrl_hyper(t, lr, l1, l2, l2_shrinkage, init_accum, &h);
+  if (st != DET_OK) return st;
+  return apply_common(t, keys, grads, n, h, init_param, full_size_init, 4, (cudaStream_t)stream);
 }
 
 size_t det_partition_workspace_bytes(size_t n, int num_shards) {
@@ -2051,6 +2190,25 @@ det_status det_apply_adam_dup(det_table* t, const int64_t* ids, const float* gra
   OptHyper h;
   h.lr = alpha; h.eps = epsilon; h.beta1 = beta1; h.beta2 = beta2; h.init_slot = 0.f;
   return apply_dup(t, ids, grads, n, h, init_param, 1, workspace, workspace_bytes, n_unique_dev_out, (cudaStream_t)stream);
+}
+
+det_status det_apply_sgd_dup(det_table* t, const int64_t* ids, const float* grads, size_t n, float lr, float momentum,
+                             int nesterov, const float* init_param, void* workspace, size_t workspace_bytes,
+                             int64_t* n_unique_dev_out, det_stream_t stream) {
+  OptHyper h;
+  int opt = 2;
+  const det_status st = sgd_hyper(t, lr, momentum, nesterov, &h, &opt);
+  if (st != DET_OK) return st;
+  return apply_dup(t, ids, grads, n, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out, (cudaStream_t)stream);
+}
+
+det_status det_apply_ftrl_dup(det_table* t, const int64_t* ids, const float* grads, size_t n, float lr, float l1, float l2,
+                              float l2_shrinkage, const float* init_param, float init_accum, void* workspace,
+                              size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream) {
+  OptHyper h;
+  const det_status st = ftrl_hyper(t, lr, l1, l2, l2_shrinkage, init_accum, &h);
+  if (st != DET_OK) return st;
+  return apply_dup(t, ids, grads, n, h, init_param, 4, workspace, workspace_bytes, n_unique_dev_out, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -165,10 +165,19 @@ det_status dispatch_vec(size_t row_bytes, std::initializer_list<RowArg> ops, F&&
   return call_vec<16, MinVec>(vec, make_geom((unsigned)row_bytes, vec), f);
 }
 
-// f(std::integral_constant<int, 0 or 1>): a run-time choice between two instantiations of a kernel
+// f(std::integral_constant<int, v>) for a run-time v in [0, N): a run-time choice between N instantiations of a kernel
+template <int N, int I = 0, typename F>
+det_status dispatch_int(int v, F&& f) {
+  if constexpr (I + 1 < N) {
+    if (v != I) return dispatch_int<N, I + 1>(v, f);
+  }
+  return f(std::integral_constant<int, I>());
+}
+
+// f(std::integral_constant<int, 0 or 1>): the two-way form
 template <typename F>
 det_status dispatch_bit(bool b, F&& f) {
-  return b ? f(std::integral_constant<int, 1>()) : f(std::integral_constant<int, 0>());
+  return dispatch_int<2>(b ? 1 : 0, f);
 }
 
 }  // namespace det

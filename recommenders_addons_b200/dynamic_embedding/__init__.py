@@ -7,7 +7,7 @@ from .variable import (GraphKeys, ModelMode, TrainableWrapper, Variable, default
                        embedding_lookup_unique, enable_inference_mode, enable_train_mode, get_model_mode, get_variable,
                        load_de_variable_from_file_system, make_partition, segment_reduce, trainable_wrapper_filter, unique)
 from .ops import SparseIds, embedding_lookup_sparse, safe_embedding_lookup_sparse
-from .optimizer import ComposedOptimizer, DynamicEmbeddingOptimizer, FusedAdagrad, FusedAdam, SlotPlane
+from .optimizer import ComposedOptimizer, DynamicEmbeddingOptimizer, FusedAdagrad, FusedAdam, FusedFtrl, FusedSGD, SlotPlane
 from .restrict_policies import FrequencyRestrictPolicy, RestrictPolicy, TimestampRestrictPolicy
 from .sharded import PeerShardedVariable, ShardedVariable
 from . import layers
@@ -20,7 +20,7 @@ __all__ = [
     "CuckooHashTable", "CuckooHashTableConfig", "CuckooHashTableCreator", "HkvEvictStrategy", "HkvHashTable", "HkvHashTableConfig",
     "HkvHashTableCreator", "KVCreator", "Variable", "default_partition_fn", "embedding_lookup",
     "embedding_lookup_unique", "get_variable", "unique", "segment_reduce", "SparseIds", "embedding_lookup_sparse",
-    "safe_embedding_lookup_sparse", "DynamicEmbeddingOptimizer", "FusedAdagrad", "FusedAdam", "ShardedVariable", "PeerShardedVariable", "layers",
+    "safe_embedding_lookup_sparse", "DynamicEmbeddingOptimizer", "FusedAdagrad", "FusedAdam", "FusedSGD", "FusedFtrl", "ShardedVariable", "PeerShardedVariable", "layers",
     "RestrictPolicy", "TimestampRestrictPolicy", "FrequencyRestrictPolicy", "TrainableWrapper", "ModelMode",
     "enable_inference_mode", "enable_train_mode", "get_model_mode", "trainable_wrapper_filter", "shadow_ops",
     "ComposedOptimizer", "SlotPlane", "math", "data_flow", "keras", "GraphKeys", "FileSystemSaver", "FileSystemSaverConfig", "DynamicEmbeddingSaver",

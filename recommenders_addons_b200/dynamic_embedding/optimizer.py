@@ -256,6 +256,84 @@ class FusedAdam(_FusedBase):
                                              _stream_ptr(table.device)))
 
 
+class FusedSGD(_FusedBase):
+  """SGD and momentum on dynamic-embedding rows (TF1 GradientDescent / MomentumOptimizer; torch SGD(momentum,
+  dampening=0) has the same algebra): momentum == 0: var -= lr*g; else a = a*m + g; var -= a*lr, with nesterov
+  var -= (g*lr) + ((a*m)*lr).  One slot ("momentum") when momentum != 0, none otherwise."""
+  opt_name = "SGD"
+
+  def __init__(self, learning_rate=0.01, momentum=0.0, nesterov=False):
+    super().__init__()
+    if learning_rate < 0:
+      raise ValueError("Invalid learning_rate: %r" % (learning_rate,))
+    if momentum < 0:
+      raise ValueError("Invalid momentum: %r" % (momentum,))
+    if nesterov and momentum == 0:
+      raise ValueError("Nesterov momentum requires a momentum")
+    self.learning_rate = float(learning_rate)
+    self.momentum = float(momentum)
+    self.nesterov = bool(nesterov)
+    self.n_slots = 0 if self.momentum == 0 else 1
+    self.slot_plane_names = () if self.momentum == 0 else ("momentum",)
+
+  def _apply_table(self, params, table, keys, grads):
+    n = keys.numel()
+    init, full = _init_rows(params, n, table.device)
+    _lib.check(_lib.lib().det_apply_sgd(table.handle, _ptr(keys), _ptr(grads), n, self.learning_rate, self.momentum,
+                                        int(self.nesterov), _ptr(init), full, _stream_ptr(table.device)))
+
+  def _apply_table_dup(self, table, ids, grads, n, init, ws):
+    _lib.check(_lib.lib().det_apply_sgd_dup(table.handle, _ptr(ids), _ptr(grads), n, self.learning_rate, self.momentum,
+                                            int(self.nesterov), _ptr(init), _ptr(ws), ws.numel(), None,
+                                            _stream_ptr(table.device)))
+
+
+class FusedFtrl(_FusedBase):
+  """FTRL-Proximal on dynamic-embedding rows, with Keras' signature (tf.keras.optimizers.Ftrl; TF1 FtrlOptimizer is
+  l2_shrinkage_regularization_strength = beta = 0).  Slots: "accumulator" (starts at initial_accumulator_value) and
+  "linear" (starts at 0).  Only learning_rate_power = -0.5 is supported; Keras' beta enters as
+  l2 + beta / (2 * learning_rate), computed in float32."""
+  n_slots = 2
+  opt_name = "Ftrl"
+  slot_plane_names = ("accumulator", "linear")
+
+  def __init__(self, learning_rate=0.001, learning_rate_power=-0.5, initial_accumulator_value=0.1,
+               l1_regularization_strength=0.0, l2_regularization_strength=0.0, l2_shrinkage_regularization_strength=0.0,
+               beta=0.0):
+    super().__init__()
+    if learning_rate_power != -0.5:
+      raise ValueError("FusedFtrl supports learning_rate_power=-0.5 only, got %r" % (learning_rate_power,))
+    if not learning_rate > 0:
+      raise ValueError("learning_rate must be positive, got %r" % (learning_rate,))
+    for name, v in (("initial_accumulator_value", initial_accumulator_value),
+                    ("l1_regularization_strength", l1_regularization_strength),
+                    ("l2_regularization_strength", l2_regularization_strength),
+                    ("l2_shrinkage_regularization_strength", l2_shrinkage_regularization_strength),
+                    ("beta", beta)):
+      if not v >= 0:
+        raise ValueError("%s must be >= 0, got %r" % (name, v))
+    f = np.float32
+    self.learning_rate = float(learning_rate)
+    self.learning_rate_power = -0.5
+    self.initial_accumulator_value = float(initial_accumulator_value)
+    self.l1 = float(l1_regularization_strength)
+    self.l2 = float(f(l2_regularization_strength) + f(beta) / (f(2) * f(learning_rate)))
+    self.l2_shrinkage = float(l2_shrinkage_regularization_strength)
+    self.beta = float(beta)
+
+  def _apply_table(self, params, table, keys, grads):
+    n = keys.numel()
+    init, full = _init_rows(params, n, table.device)
+    _lib.check(_lib.lib().det_apply_ftrl(table.handle, _ptr(keys), _ptr(grads), n, self.learning_rate, self.l1, self.l2,
+                                         self.l2_shrinkage, _ptr(init), full, self.initial_accumulator_value,
+                                         _stream_ptr(table.device)))
+
+  def _apply_table_dup(self, table, ids, grads, n, init, ws):
+    _lib.check(_lib.lib().det_apply_ftrl_dup(table.handle, _ptr(ids), _ptr(grads), n, self.learning_rate, self.l1,
+                                             self.l2, self.l2_shrinkage, _ptr(init), self.initial_accumulator_value,
+                                             _ptr(ws), ws.numel(), None, _stream_ptr(table.device)))
+
+
 class ComposedOptimizer(object):
   """ANY torch.optim optimizer on dynamic-embedding rows, the way the reference patches a stock optimizer
   (dynamic_embedding_optimizer.py:137-204 `apply_grad_to_update_var`, :870-958 `create_slots`): per step and per
@@ -263,7 +341,8 @@ class ComposedOptimizer(object):
   named `<var>/<Optimizer>/<slot>` like the reference's slot tables), run the stock dense rule on the [U, dim] scratch,
   write param and slots back (`TrainableWrapper.update_op`, embedding_weights.py:434-444).  Table passes per step:
   (1 + slots) finds + (1 + slots) upserts, all through the validated table kernels; Adagrad / Adam have the fused
-  single-kernel path (FusedAdagrad / FusedAdam), which DynamicEmbeddingOptimizer picks by default.
+  single-kernel path (FusedAdagrad / FusedAdam), which DynamicEmbeddingOptimizer picks by default.  SGD, momentum and
+  FTRL have fused steps too (FusedSGD / FusedFtrl), used when passed explicitly.
 
   A key without slot state starts from the state a fresh torch optimizer gives a new parameter (zeros; Adagrad's
   `sum` from initial_accumulator_value) -- the reference's slot initializers.  State that is not per row (`step`,

@@ -1,0 +1,199 @@
+"""The fused SGD, momentum and FTRL steps next to the fused Adagrad and Adam steps, timed in one process.
+
+Two variables, fp32 and bf16, hold the same --resident keys (bf16 rows, so both start from the same numbers) and two
+fp32 slot planes each.  Every optimizer steps its own 2^20 unique resident keys, so no optimizer reads another's slot
+rows.  Timed with CUDA events, in rounds that alternate the dtype order, median of the rounds:
+  * sgd, momentum (0.9), ftrl, adagrad, adam -- det_apply_* on 2^20 unique resident keys;
+  * sgd_dup (momentum 0.9), ftrl_dup        -- det_apply_*_dup at the c3 backward shape (26 x 65536 Zipf ids);
+  * composed_momentum -- ComposedOptimizer(torch.optim.SGD(momentum=0.9)): unique ids, finds of the param and slot
+    rows, torch's dense rule, upserts -- on an fp32 variable of --composed-resident rows, next to FusedSGD(0.9) on it.
+Before the timing, the first step of each new optimizer on a sample of its keys (rows written by insert, no slot state
+yet) is checked bit for bit against tests/optimizer_oracle.py: params of both dtypes (bf16: the fp32 result rounded).
+
+Bytes per key are what the unique-key step must move at dim 64: key 8 + probed bucket 64 + fp32 gradient 256 + param
+row read and write + fp32 slot rows read and write.  The rate is against the H100 SXM data-sheet HBM3 bandwidth of
+3.35 TB/s (a data-sheet figure, not a measured peak).  Prints one JSON line.
+
+  python scripts/fused_optimizer_microbench.py [--resident 9000000] [--rounds 5] [--calls 10]
+"""
+import argparse
+import ctypes
+import json
+import os
+import subprocess
+import sys
+
+import numpy as np
+import torch
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+DATASHEET_HBM_BPS = 3.35e12
+DIM = 64
+BUCKET_BYTES = 64          # one probed 8-slot bucket of int64 keys
+N_UNIQUE = 1 << 20
+N_DUP = 26 * 65536
+N_SAMPLE = 1 << 16
+SLOTS = {"sgd": 0, "momentum": 1, "ftrl": 2, "adagrad": 1, "adam": 2}
+FTRL = dict(lr=0.05, l1=0.001, l2=0.01, l2_shrinkage=0.0)
+
+
+def card():
+  q = "name,power.limit,clocks.max.sm"
+  try:
+    out = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=" + q, "--format=csv,noheader"], capture_output=True,
+                         text=True, timeout=30).stdout.strip()
+    name, pl, clk = [s.strip() for s in out.split(",")]
+    return {"name": name, "power_limit": pl, "max_sm_clock": clk}
+  except Exception as ex:   # noqa: BLE001
+    return {"name": torch.cuda.get_device_name(0), "error": repr(ex)}
+
+
+def bytes_per_key(opt, elem_bytes):
+  return 8 + BUCKET_BYTES + DIM * 4 + 2 * DIM * elem_bytes + SLOTS[opt] * 2 * DIM * 4
+
+
+def mix_keys(r):
+  return (r * -7046029254386353131) & 0x7FFFFFFFFFFFFFFF   # golden-ratio multiplier (0x9E3779B97F4A7C15) as int64
+
+
+def main():
+  ap = argparse.ArgumentParser()
+  ap.add_argument("--resident", type=int, default=9_000_000)
+  ap.add_argument("--composed-resident", type=int, default=1 << 22)
+  ap.add_argument("--rounds", type=int, default=5)
+  ap.add_argument("--calls", type=int, default=10)
+  args = ap.parse_args()
+  if not torch.cuda.is_available():
+    raise SystemExit("fused_optimizer_microbench.py needs a GPU")
+  from recommenders_addons_b200 import _lib
+  from recommenders_addons_b200 import dynamic_embedding as de
+  from tests import optimizer_oracle as OO
+  lib = _lib.lib()
+  P = lambda t: ctypes.c_void_p(t.data_ptr())   # noqa: E731
+  dev = torch.device("cuda", 0)
+  torch.cuda.set_device(0)
+  info = card()
+  R = args.resident
+  dts = {"float32": torch.float32, "bfloat16": torch.bfloat16}
+  vars_ = {n: de.Variable(value_dtype=dt, dim=DIM, init_size=2 * R, initializer=0.0, name="fob_" + n,
+                          num_slot_planes=2) for n, dt in dts.items()}
+  gen = torch.Generator(device=dev).manual_seed(7)
+
+  def fill(variables, n_rows):
+    for b in range(0, n_rows, 1 << 22):
+      k = mix_keys(torch.arange(b, min(n_rows, b + (1 << 22)), dtype=torch.int64, device=dev))
+      x = torch.randn(k.numel(), DIM, device=dev, generator=gen).to(torch.bfloat16)
+      for v in variables:
+        v.tables[0].insert(k, x.to(v.value_dtype))
+      del x
+  fill(list(vars_.values()), R)
+  torch.cuda.synchronize()
+
+  # one range of R // 8 resident keys per optimizer and per duplicate-id shape
+  part = R // 8
+  opts = ("sgd", "momentum", "ftrl", "adagrad", "adam")
+  keys = {o: mix_keys(i * part + torch.randperm(part, device=dev, generator=gen)[:N_UNIQUE]) for i, o in enumerate(opts)}
+  zipf = np.random.default_rng(3).zipf(1.2, N_DUP) - 1
+  ids_dup = {"sgd_dup": mix_keys(5 * part + torch.as_tensor(zipf % part, device=dev)),
+             "ftrl_dup": mix_keys(6 * part + torch.as_tensor(zipf % part, device=dev))}
+  g_dup = torch.randn(N_DUP, DIM, device=dev, generator=gen) * 0.01
+  g_uni = torch.randn(N_UNIQUE, DIM, device=dev, generator=gen) * 0.01
+  init = torch.zeros(DIM, device=dev)
+  wsb = int(lib.det_apply_dup_workspace_bytes(N_DUP, DIM))
+  ws = torch.empty(wsb + 256, dtype=torch.uint8, device=dev)
+  ws = ws[(-ws.data_ptr()) % 256:][:wsb]
+
+  def step(name, shape, k=None, g=None, n=N_UNIQUE):
+    h = vars_[name].tables[0].handle
+    k = keys.get(shape) if k is None else k
+    g = g_uni if g is None else g
+    if shape == "sgd":
+      st = lib.det_apply_sgd(h, P(k), P(g), n, 0.01, 0.0, 0, P(init), 0, None)
+    elif shape == "momentum":
+      st = lib.det_apply_sgd(h, P(k), P(g), n, 0.01, 0.9, 0, P(init), 0, None)
+    elif shape == "ftrl":
+      st = lib.det_apply_ftrl(h, P(k), P(g), n, FTRL["lr"], FTRL["l1"], FTRL["l2"], FTRL["l2_shrinkage"], P(init), 0,
+                              0.1, None)
+    elif shape == "adagrad":
+      st = lib.det_apply_adagrad(h, P(k), P(g), n, 0.01, 0.0, P(init), 0, 0.1, None)
+    elif shape == "adam":
+      st = lib.det_apply_adam(h, P(k), P(g), n, 0.003, 0.9, 0.999, 1e-8, P(init), 0, None)
+    elif shape == "sgd_dup":
+      st = lib.det_apply_sgd_dup(h, P(ids_dup[shape]), P(g_dup), N_DUP, 0.01, 0.9, 0, P(init), P(ws), wsb, None, None)
+    else:
+      st = lib.det_apply_ftrl_dup(h, P(ids_dup[shape]), P(g_dup), N_DUP, FTRL["lr"], FTRL["l1"], FTRL["l2"],
+                                  FTRL["l2_shrinkage"], P(init), 0.1, P(ws), wsb, None, None)
+    _lib.check(st)
+
+  # in-run check: the first step on a sample of each new optimizer's keys (insert-written rows, no slot state yet)
+  mismatches = {}
+  for shape in ("sgd", "momentum", "ftrl"):
+    k = keys[shape][:N_SAMPLE].contiguous()
+    g = g_uni[:N_SAMPLE].contiguous()
+    bad = 0
+    for name, dt in dts.items():
+      p0 = vars_[name].lookup(k).float().cpu().numpy()
+      step(name, shape, k, g, N_SAMPLE)
+      got = vars_[name].lookup(k).float().cpu().numpy()
+      gn = g.cpu().numpy()
+      if shape == "ftrl":
+        exp, _, _ = OO.ftrl_dense(p0, np.full_like(p0, 0.1), np.zeros_like(p0), gn, FTRL["lr"], FTRL["l1"], FTRL["l2"],
+                                  FTRL["l2_shrinkage"])
+      else:
+        exp, _ = OO.sgd_dense(p0, np.zeros_like(p0), gn, 0.01, 0.9 if shape == "momentum" else 0.0)
+      exp = torch.from_numpy(exp).to(dt).float().numpy()
+      bad += int((got.view(np.uint32) != exp.view(np.uint32)).sum())
+    mismatches[shape] = bad
+
+  def timed(fn, calls):
+    fn()
+    torch.cuda.synchronize()
+    a, z = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    a.record()
+    for _ in range(calls):
+      fn()
+    z.record()
+    z.synchronize()
+    return a.elapsed_time(z) / calls
+
+  # composed momentum (torch.optim.SGD through ComposedOptimizer) and FusedSGD(0.9) on one fp32 variable
+  Rc = args.composed_resident
+  small = de.Variable(dim=DIM, init_size=2 * Rc, initializer=0.0, name="fob_small", num_slot_planes=1)
+  fill([small], Rc)
+  keys_small = mix_keys(torch.randperm(Rc, device=dev, generator=gen)[:N_UNIQUE])
+  comp = de.DynamicEmbeddingOptimizer(torch.optim.SGD([torch.nn.Parameter(torch.zeros(1))], lr=0.01, momentum=0.9))
+  fused_small = de.FusedSGD(0.01, 0.9)
+
+  shapes = opts + ("sgd_dup", "ftrl_dup")
+  ms = {(n, s): [] for n in dts for s in shapes}
+  ms_comp, ms_fused_small = [], []
+  for r in range(args.rounds):
+    order = list(dts) if r % 2 == 0 else list(reversed(list(dts)))
+    for shape in shapes:
+      for n in order:
+        ms[(n, shape)].append(timed(lambda: step(n, shape), args.calls))
+    ms_comp.append(timed(lambda: comp.apply_sparse(small, keys_small, g_uni), max(2, args.calls // 2)))
+    ms_fused_small.append(timed(lambda: fused_small.apply_sparse(small, keys_small, g_uni), args.calls))
+  res = {}
+  for shape in shapes:
+    row = {}
+    for n, dt in dts.items():
+      t = float(np.median(ms[(n, shape)]))
+      row[n] = {"ms": round(t, 4), "ms_spread": [round(min(ms[(n, shape)]), 4), round(max(ms[(n, shape)]), 4)]}
+      if not shape.endswith("_dup"):
+        bpk = bytes_per_key(shape, torch.empty(0, dtype=dt).element_size())
+        row[n].update({"bytes_per_key": bpk, "GB_s": round(bpk * N_UNIQUE / t / 1e6, 1),
+                       "of_datasheet_hbm": round(bpk * N_UNIQUE / (t * 1e-3) / DATASHEET_HBM_BPS, 3)})
+    row["ids"] = N_DUP if shape.endswith("_dup") else N_UNIQUE
+    res[shape] = row
+  res["composed_vs_fused_fp32_momentum"] = {"resident": Rc, "keys": N_UNIQUE, "composed_is": type(comp).__name__,
+                                            "composed_ms": round(float(np.median(ms_comp)), 4),
+                                            "fused_ms": round(float(np.median(ms_fused_small)), 4)}
+  print(json.dumps({"metric": "fused optimizer step ms per call (median of rounds, CUDA events)", "card": info,
+                    "resident": R, "dim": DIM, "rounds": args.rounds, "calls": args.calls,
+                    "datasheet_hbm_TB_s": DATASHEET_HBM_BPS / 1e12, "oracle_mismatches": mismatches, "shapes": res}))
+
+
+if __name__ == "__main__":
+  main()
