@@ -127,6 +127,26 @@ const char* det_last_error(void);
 int det_abi_version(void);
 const char* det_build_info(void);
 
+/* Keyed random initializer: the row of a missing key is a pure function of (seed, key, column), computed by the kernels
+ * where they find the key missing.  Element j of the row of key k: x = Philox4x32-10(counter = (lo32 k, hi32 k, j >> 2,
+ * 0), key = (lo32 seed, hi32 seed))[j & 3], u = ((x >> 8) | 1) * 2^-24, then
+ *   DET_INIT_UNIFORM           u * (b - a) + a                                   (a, b) = (minval, maxval)
+ *   DET_INIT_NORMAL            sqrt(2) * erfinv(2u - 1) * b + a                   (a, b) = (mean, stddev)
+ *   DET_INIT_TRUNCATED_NORMAL  sqrt(2) * erfinv(erf(sqrt 2) * (2u - 1)) * b + a   (the law of N(a, b) inside a +- 2b)
+ * in fp32 (erfinv: Giles' single-precision approximation), rounded to nearest even into the table's dtype.  The row does
+ * not depend on the batch, call order, capacity or device.  With an initializer set, a NULL row pointer means "generate"
+ * in det_find (defaults, full_size_default 0), det_lookup_sparse(_clip) (default_row), det_apply_* (init_param,
+ * full_size_init 0) and det_apply_*_dup (init_param); without one NULL stays DET_INVALID_ARGUMENT.  The host-buffer
+ * finds and the det_peer_* calls do not generate rows.  Float32, float16 and bfloat16 tables; `init` NULL clears. */
+enum { DET_INIT_UNIFORM = 1, DET_INIT_NORMAL = 2, DET_INIT_TRUNCATED_NORMAL = 3 };
+typedef struct det_initializer {
+  int32_t kind;
+  int32_t reserved;
+  uint64_t seed;
+  float a, b;
+} det_initializer;
+det_status det_table_set_initializer(det_table* t, const det_initializer* init);
+
 /* ---- LookupInterface surface (kernels/cuckoo_hashtable_op.cc:211-308; GPU twin
  *      kernels/hkv_hashtable_op_gpu.cu.cc:181-470) ---- */
 

@@ -35,6 +35,15 @@ class DetStats(ctypes.Structure):
               ("evicted_keys", ctypes.c_uint64), ("host_bytes", ctypes.c_uint64)]
 
 
+# det_initializer.kind
+INIT_KINDS = {"uniform": 1, "normal": 2, "truncated_normal": 3}
+
+
+class DetInitializer(ctypes.Structure):
+  _fields_ = [("kind", ctypes.c_int32), ("reserved", ctypes.c_int32), ("seed", ctypes.c_uint64), ("a", ctypes.c_float),
+              ("b", ctypes.c_float)]
+
+
 # name -> (restype, argtypes); must list EVERY function include/detable.h declares
 SIGNATURES = {
     "det_table_create": (_i, [ctypes.POINTER(_vp), ctypes.POINTER(DetConfig)]),
@@ -42,6 +51,7 @@ SIGNATURES = {
     "det_last_error": (ctypes.c_char_p, []),
     "det_abi_version": (_i, []),
     "det_build_info": (ctypes.c_char_p, []),
+    "det_table_set_initializer": (_i, [_vp, ctypes.POINTER(DetInitializer)]),
     "det_find": (_i, [_vp, _vp, _sz, _vp, _i, _vp, _vp, _vp]),
     "det_insert": (_i, [_vp, _vp, _vp, _sz, _vp]),
     "det_accum": (_i, [_vp, _vp, _vp, _vp, _sz, _vp]),

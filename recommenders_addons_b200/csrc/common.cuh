@@ -440,16 +440,240 @@ __device__ __forceinline__ char ld_cached<1>(const unsigned char* p) {
   return __ldg(reinterpret_cast<const char*>(p));
 }
 
+// ---- keyed random initializer (det_table_set_initializer) ------------------------------------------------------------
+// Element j of the row of key k is a pure function of (seed, k, j): x = Philox4x32-10(counter = (lo32 k, hi32 k, j >> 2,
+// 0), key = seed)[j & 3] (Salmon et al. 2011, as in Random123 and curand), u = ((x >> 8) | 1) * 2^-24 in (0, 1), then
+//   kind 1 uniform         v = u * (b - a) + a
+//   kind 2 normal          v = sqrt(2) * erfinv(2u - 1) * b + a
+//   kind 3 truncated normal v = sqrt(2) * erfinv(erf(sqrt 2) * (2u - 1)) * b + a   (the law of resampling outside 2 sigma)
+// rounded to nearest even into the table's dtype.  Every step is an integer op or one IEEE fp32 add, sub, mul, div or
+// sqrt (the library is built with --fmad=false), so tests/keyed_init_oracle.py restates it bit for bit.
+struct KeyedInit {
+  int kind;   // DET_INIT_UNIFORM, DET_INIT_NORMAL or DET_INIT_TRUNCATED_NORMAL
+  int elem;   // stored element: 0 fp32, 1 fp16, 2 bf16
+  unsigned seed_lo, seed_hi;
+  float a, b;
+};
+// The trailing kernel argument of the kernels that fill missing rows: EMPTY when the table has no keyed initializer, so
+// those instantiations keep their code.
+template <bool KEYED> struct InitArg {};
+template <> struct InitArg<true> : KeyedInit {
+  const long long* ids;   // det_lookup_sparse's segment-sum kernels: the ids behind their slots (they see no keys)
+};
+
+__device__ __forceinline__ float keyed_as_float(unsigned u) {
+#ifdef DET_EMU
+  float f;
+  memcpy(&f, &u, 4);
+  return f;
+#else
+  return __uint_as_float(u);
+#endif
+}
+
+__device__ __forceinline__ void philox4x32_10(unsigned c[4], unsigned k0, unsigned k1) {
+#pragma unroll
+  for (int r = 0; r < 10; ++r) {
+    // 64-bit products (not __umulhi): the emulator's g++ build compiles the same code
+    const unsigned long long p0 = 0xD2511F53ull * c[0], p1 = 0xCD9E8D57ull * c[2];
+    const unsigned n0 = (unsigned)(p1 >> 32) ^ c[1] ^ k0, n2 = (unsigned)(p0 >> 32) ^ c[3] ^ k1;
+    c[0] = n0;
+    c[1] = (unsigned)p1;
+    c[2] = n2;
+    c[3] = (unsigned)p0;
+    k0 += 0x9E3779B9u;
+    k1 += 0xBB67AE85u;
+  }
+}
+
+// natural log of y > 0 (normal): y = 2^e m with m in [sqrt(1/2), sqrt 2), log m = 2 atanh(s), s = (m - 1) / (m + 1)
+__device__ __forceinline__ float keyed_log(float y) {
+  const unsigned bits = __float_as_uint(y);
+  int e = (int)((bits >> 23) & 0xffu) - 127;
+  float m = keyed_as_float((bits & 0x7fffffu) | (127u << 23));
+  if (m > 1.41421356f) {
+    m = m * 0.5f;
+    e += 1;
+  }
+  const float s = (m - 1.f) / (m + 1.f);
+  const float z = s * s;
+  float p = 0.111111111f;
+  p = p * z + 0.142857143f;
+  p = p * z + 0.2f;
+  p = p * z + 0.333333333f;
+  p = p * z + 1.f;
+  const float lm = (2.f * s) * p;
+  const float ef = (float)e;
+  return ef * 0.693145752f + (ef * 1.42860677e-06f + lm);
+}
+
+// Giles, "Approximating the erfinv function" (GPU Computing Gems, 2010), single precision, x in (-1, 1)
+__device__ __forceinline__ float keyed_erfinv(float x) {
+  float w = -keyed_log((1.f - x) * (1.f + x));
+  float p;
+  if (w < 5.f) {
+    w = w - 2.5f;
+    p = 2.81022636e-08f;
+    p = 3.43273939e-07f + p * w;
+    p = -3.5233877e-06f + p * w;
+    p = -4.39150654e-06f + p * w;
+    p = 0.00021858087f + p * w;
+    p = -0.00125372503f + p * w;
+    p = -0.00417768164f + p * w;
+    p = 0.246640727f + p * w;
+    p = 1.50140941f + p * w;
+  } else {
+    w = sqrtf(w) - 3.f;
+    p = -0.000200214257f;
+    p = 0.000100950558f + p * w;
+    p = 0.00134934322f + p * w;
+    p = -0.00367342844f + p * w;
+    p = 0.00573950773f + p * w;
+    p = -0.0076224613f + p * w;
+    p = 0.00943887047f + p * w;
+    p = 1.00167406f + p * w;
+    p = 2.83297682f + p * w;
+  }
+  return p * x;
+}
+
+// fp32 -> fp16 / bf16 bits, round to nearest even (overflow to +-inf; the generated values are never NaN)
+__device__ __forceinline__ unsigned keyed_f16_bits(float f) {
+  const unsigned bits = __float_as_uint(f);
+  const unsigned s = (bits >> 16) & 0x8000u;
+  const int e = (int)((bits >> 23) & 0xffu) - 127 + 15;
+  unsigned m = bits & 0x7fffffu;
+  if (e >= 31) return s | 0x7c00u;
+  if (e <= 0) {
+    if (e < -10) return s;
+    m |= 0x800000u;
+    const int shift = 14 - e;
+    unsigned r = m >> shift;
+    const unsigned rem = m & ((1u << shift) - 1u), half = 1u << (shift - 1);
+    if (rem > half || (rem == half && (r & 1u))) ++r;
+    return s | r;
+  }
+  unsigned r = ((unsigned)e << 10) | (m >> 13);
+  const unsigned rem = m & 0x1fffu;
+  if (rem > 0x1000u || (rem == 0x1000u && (r & 1u))) ++r;   // a carry into the exponent is the right result
+  return s | r;
+}
+__device__ __forceinline__ unsigned keyed_bf16_bits(float f) {
+  const unsigned bits = __float_as_uint(f);
+  return (bits + 0x7fffu + ((bits >> 16) & 1u)) >> 16;
+}
+// fp32 value of fp16 bits
+__device__ __forceinline__ float keyed_f16_value(unsigned h) {
+  const unsigned s = (h & 0x8000u) << 16, e = (h >> 10) & 0x1fu, m = h & 0x3ffu;
+  if (e == 31) return keyed_as_float(s | 0x7f800000u | (m << 13));
+  if (e == 0) {
+    const float v = (float)m * 5.96046448e-08f;   // subnormal: m * 2^-24, exact
+    return s ? -v : v;
+  }
+  return keyed_as_float(s | ((e + 112u) << 23) | (m << 13));
+}
+
+// The two generator steps are out-of-line calls with scalar arguments and results: a kernel pays for them only in the
+// lanes of missing rows, keeps just the four words of one Philox block live across them, and holds one copy of Philox,
+// log and erfinv instead of one per unrolled row.
+#ifdef DET_EMU
+#define DET_NOINLINE __attribute__((noinline))
+#else
+#define DET_NOINLINE __noinline__
+#endif
+struct KeyedWords {
+  unsigned x0, x1, x2, x3;
+};
+// the four Philox words of elements 4q .. 4q + 3 of the row of key (klo, khi)
+static __device__ DET_NOINLINE KeyedWords keyed_philox(unsigned klo, unsigned khi, unsigned q, unsigned s0, unsigned s1) {
+  unsigned c[4] = {klo, khi, q, 0u};
+  philox4x32_10(c, s0, s1);
+  return KeyedWords{c[0], c[1], c[2], c[3]};
+}
+// the stored bits (fp32 bits, or the 16 bits of a half element) of the value of one Philox word
+static __device__ DET_NOINLINE unsigned keyed_word_bits(int kind, int elem, float a, float b, unsigned x) {
+  const float u = (float)((x >> 8) | 1u) * 5.96046448e-08f;   // * 2^-24: exact
+  float v;
+  if (kind == DET_INIT_UNIFORM) {
+    v = u * (b - a) + a;
+  } else {
+    float t = 2.f * u - 1.f;                                  // exact
+    if (kind == DET_INIT_TRUNCATED_NORMAL) t = 0.954499736f * t;
+    v = (1.41421356f * keyed_erfinv(t)) * b + a;
+  }
+  return elem == 0 ? __float_as_uint(v) : elem == 1 ? keyed_f16_bits(v) : keyed_bf16_bits(v);
+}
+__device__ __forceinline__ KeyedWords keyed_block(const KeyedInit& ki, long long key, unsigned q) {
+  return keyed_philox((unsigned)(unsigned long long)key, (unsigned)((unsigned long long)key >> 32), q, ki.seed_lo,
+                      ki.seed_hi);
+}
+__device__ __forceinline__ unsigned pick4(const KeyedWords& w, unsigned i) {
+  return i == 0 ? w.x0 : i == 1 ? w.x1 : i == 2 ? w.x2 : w.x3;
+}
+__device__ __forceinline__ unsigned keyed_bits(const KeyedInit& ki, unsigned x) {
+  return keyed_word_bits(ki.kind, ki.elem, ki.a, ki.b, x);
+}
+// the fp32 value a find of the element returns, widened from the table's dtype
+__device__ __forceinline__ float keyed_widen(const KeyedInit& ki, unsigned bits) {
+  return ki.elem == 0 ? keyed_as_float(bits) : ki.elem == 1 ? keyed_f16_value(bits) : keyed_as_float(bits << 16);
+}
+// fp32 value (as stored, widened) of element `col`, and of elements col .. col + 3 (col % 4 == 0): the fused kernels' rows
+__device__ __forceinline__ float keyed_f32x1(const KeyedInit& ki, long long key, unsigned col) {
+  return keyed_widen(ki, keyed_bits(ki, pick4(keyed_block(ki, key, col >> 2), col & 3u)));
+}
+__device__ __forceinline__ float4 keyed_f32x4(const KeyedInit& ki, long long key, unsigned col) {
+  const KeyedWords w = keyed_block(ki, key, col >> 2);
+  return make_float4(keyed_widen(ki, keyed_bits(ki, w.x0)), keyed_widen(ki, keyed_bits(ki, w.x1)),
+                     keyed_widen(ki, keyed_bits(ki, w.x2)), keyed_widen(ki, keyed_bits(ki, w.x3)));
+}
+
+// The VEC bytes at byte offset `off` (a multiple of VEC) of the generated row of `key`, in the table's dtype.
+template <int VEC>
+__device__ __forceinline__ typename VecT<VEC>::type keyed_vec(const KeyedInit& ki, long long key, unsigned off) {
+  using V = typename VecT<VEC>::type;
+  if constexpr (VEC >= 4) {
+    unsigned w[VEC / 4];
+    KeyedWords x;
+    if (ki.elem == 0) {
+      // VEC / 4 elements from col = off / 4, all in one Philox block
+      const unsigned col = off / 4u;
+      x = keyed_block(ki, key, col >> 2);
+#pragma unroll
+      for (int k = 0; k < VEC / 4; ++k) w[k] = keyed_bits(ki, pick4(x, (col & 3u) + k));
+    } else {
+      // VEC / 2 half elements from col = off / 2: one Philox block per 4 of them
+      const unsigned col = off / 2u;
+#pragma unroll
+      for (int k = 0; k < VEC / 2; ++k) {
+        if (k % 4 == 0) x = keyed_block(ki, key, (col + k) >> 2);
+        const unsigned h = keyed_bits(ki, pick4(x, (col + k) & 3u));
+        w[k / 2] = (k & 1) ? (w[k / 2] | (h << 16)) : h;
+      }
+    }
+    V r;
+    memcpy(&r, w, VEC);
+    return r;
+  } else {
+    // a 1- or 2-byte piece of one element
+    const unsigned es = ki.elem == 0 ? 4u : 2u;
+    const unsigned col = off / es;
+    const unsigned bits = keyed_bits(ki, pick4(keyed_block(ki, key, col >> 2), col & 3u));
+    return (V)(bits >> (8u * (off % es)));
+  }
+}
+
 // marker a lane passes as its row's source to say "the broadcast default row"
 #define DET_SRC_DEFAULT (reinterpret_cast<const unsigned char*>(uintptr_t(1)))
 
 // For each of the warp's 32 items (item j held by lane j): copy one row from src_j to dst_j.
 // Lane j provides its row's src/dst pointers (nullptr src or dst = skip; src == DET_SRC_DEFAULT = copy the
-// broadcast row `bdef`, which each lane keeps in a register / L1).
-template <int VEC>
+// broadcast row `bdef`, which each lane keeps in a register / L1).  KEYED: src == DET_SRC_DEFAULT instead generates the
+// row of the lane's key `my_key` from the table's keyed initializer `ki` (bdef is unused).
+template <int VEC, bool KEYED = false>
 __device__ __forceinline__ void warp_move_rows(const RowGeom& g, const unsigned char* my_src,
                                                unsigned char* my_dst, int lane,
-                                               const unsigned char* bdef = nullptr) {
+                                               const unsigned char* bdef = nullptr,
+                                               const InitArg<KEYED>& ki = InitArg<KEYED>(), long long my_key = 0) {
   using V = typename VecT<VEC>::type;
   const unsigned rows_per_step = 32u >> g.lpr_shift;
   const unsigned sub = (unsigned)lane >> g.lpr_shift;        // which row of the step
@@ -475,6 +699,14 @@ __device__ __forceinline__ void warp_move_rows(const RowGeom& g, const unsigned 
         v[u] = defv;
         if (s[u] > DET_SRC_DEFAULT && d[u]) v[u] = ld_row<VEC>(s[u] + c0 * VEC);
       }
+      if constexpr (KEYED) {
+        // only the lanes of missing rows run the generator
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+          const long long k = shfl_ll(my_key, (int)((j0 + u * rows_per_step + sub) & 31u));
+          if (s[u] == DET_SRC_DEFAULT && d[u]) v[u] = keyed_vec<VEC>(ki, k, c0 * VEC);
+        }
+      }
 #pragma unroll
       for (int u = 0; u < 4; ++u)
         if (s[u] && d[u]) st_row<VEC>(d[u] + c0 * VEC, v[u]);
@@ -484,9 +716,15 @@ __device__ __forceinline__ void warp_move_rows(const RowGeom& g, const unsigned 
       const unsigned j = j0 + sub;
       const unsigned char* s = (const unsigned char*)shfl_ll((long long)my_src, j & 31u);
       unsigned char* d = (unsigned char*)shfl_ll((long long)my_dst, j & 31u);
+      long long k = 0;
+      if constexpr (KEYED) k = shfl_ll(my_key, (int)(j & 31u));
       if (s && d) {
         if (s == DET_SRC_DEFAULT) {
-          for (unsigned c = c0; c < g.vpr; c += g.lpr) st_row<VEC>(d + c * VEC, ld_cached<VEC>(bdef + c * VEC));
+          if constexpr (KEYED) {
+            for (unsigned c = c0; c < g.vpr; c += g.lpr) st_row<VEC>(d + c * VEC, keyed_vec<VEC>(ki, k, c * VEC));
+          } else {
+            for (unsigned c = c0; c < g.vpr; c += g.lpr) st_row<VEC>(d + c * VEC, ld_cached<VEC>(bdef + c * VEC));
+          }
         } else {
           for (unsigned c = c0; c < g.vpr; c += g.lpr) st_row<VEC>(d + c * VEC, ld_row<VEC>(s + c * VEC));
         }

@@ -246,11 +246,12 @@ resolve_slots_kernel(TableView t, const long long* __restrict__ ids, size_t nnz,
 // scratch and no per-row segment bookkeeping.  Launched on spec IN FRONT of the general kernels (nnz == batch, no weights):
 // it checks segment_ids[i] == i for the ids it serves and raises `not_identity` otherwise; the general kernels
 // (segment_offsets, resolve_slots, segment_sum) run only when the flag is set and then rewrite every output row.
-template <int VEC>
+// KEYED: missing rows are generated from the table's keyed initializer (default_row is NULL).
+template <int VEC, bool KEYED = false>
 __global__ void __launch_bounds__(kThreadsF)
 lookup_identity_kernel(TableView t, const long long* __restrict__ ids, const int* __restrict__ seg, size_t n,
                        const unsigned char* __restrict__ default_row, unsigned char* __restrict__ out, RowGeom g, int use_tma,
-                       unsigned* __restrict__ not_identity, unsigned epoch) {
+                       unsigned* __restrict__ not_identity, unsigned epoch, InitArg<KEYED> ki = InitArg<KEYED>()) {
   __shared__ __align__(128) long long s_keys[kStages][kTileKeys];
   __shared__ __align__(8) unsigned long long s_bar[kStages];
   const int lane = threadIdx.x & 31;
@@ -269,7 +270,7 @@ lookup_identity_kernel(TableView t, const long long* __restrict__ ids, const int
       src = slot >= 0 ? t.planes[0] + (size_t)slot * g.row_bytes : DET_SRC_DEFAULT;
       dst = out + i * g.row_bytes;
     }
-    warp_move_rows<VEC>(g, src, dst, lane, default_row);
+    warp_move_rows<VEC, KEYED>(g, src, dst, lane, default_row, ki, key);
   }
 }
 
@@ -360,16 +361,32 @@ template <typename H> struct WidenVec<H, 4> {
 // warp_move_rows for a half table into an fp32 output: lane j's src is a half row (or DET_SRC_DEFAULT = the fp32
 // broadcast row `bdef`), its dst an fp32 row.  g is the geometry of the fp32 OUTPUT row in OV-byte vectors; vector c of
 // the output comes from bytes [c * OV / 2, (c + 1) * OV / 2) of the half row.  Same schedule as warp_move_rows.
-template <typename H, int OV>
+// the OV bytes at byte offset `off` of the fp32 (widened) generated row of `key`
+template <int OV>
+__device__ __forceinline__ typename VecT<OV>::type keyed_out_vec(const KeyedInit& ki, long long key, unsigned off) {
+  if constexpr (OV == 16) {
+    const float4 f = keyed_f32x4(ki, key, off / 4u);
+    return make_int4(__float_as_int(f.x), __float_as_int(f.y), __float_as_int(f.z), __float_as_int(f.w));
+  } else if constexpr (OV == 8) {
+    return make_int2(__float_as_int(keyed_f32x1(ki, key, off / 4u)), __float_as_int(keyed_f32x1(ki, key, off / 4u + 1)));
+  } else {
+    return __float_as_int(keyed_f32x1(ki, key, off / 4u));
+  }
+}
+
+// KEYED: a missing row (DET_SRC_DEFAULT) is generated from `ki` for the lane's key `my_key` instead (bdef is unused)
+template <typename H, int OV, bool KEYED = false>
 __device__ __forceinline__ void warp_widen_rows(const RowGeom& g, const unsigned char* my_src, unsigned char* my_dst,
-                                                int lane, const unsigned char* bdef) {
+                                                int lane, const unsigned char* bdef,
+                                                const InitArg<KEYED>& ki = InitArg<KEYED>(), long long my_key = 0) {
   constexpr int IV = OV / 2;
   using V = typename VecT<OV>::type;
   const unsigned rows_per_step = 32u >> g.lpr_shift;
   const unsigned sub = (unsigned)lane >> g.lpr_shift;
   const unsigned c0 = (unsigned)lane & (g.lpr - 1u);
   if (g.vpr == g.lpr) {
-    const V defv = ld_cached<OV>(bdef + c0 * OV);
+    V defv = V();
+    if constexpr (!KEYED) defv = ld_cached<OV>(bdef + c0 * OV);
     for (unsigned j0 = 0; j0 < 32u; j0 += rows_per_step * 4u) {
       const unsigned char* s[4];
       unsigned char* d[4];
@@ -387,6 +404,13 @@ __device__ __forceinline__ void warp_widen_rows(const RowGeom& g, const unsigned
         v[u] = defv;
         if (s[u] > DET_SRC_DEFAULT && d[u]) v[u] = WidenVec<H, OV>::of(ld_row<IV>(s[u] + c0 * IV));
       }
+      if constexpr (KEYED) {
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+          const long long k = shfl_ll(my_key, (int)((j0 + u * rows_per_step + sub) & 31u));
+          if (s[u] == DET_SRC_DEFAULT && d[u]) v[u] = keyed_out_vec<OV>(ki, k, c0 * OV);
+        }
+      }
 #pragma unroll
       for (int u = 0; u < 4; ++u)
         if (s[u] && d[u]) st_row<OV>(d[u] + c0 * OV, v[u]);
@@ -396,9 +420,15 @@ __device__ __forceinline__ void warp_widen_rows(const RowGeom& g, const unsigned
       const unsigned j = j0 + sub;
       const unsigned char* s = (const unsigned char*)shfl_ll((long long)my_src, j & 31u);
       unsigned char* d = (unsigned char*)shfl_ll((long long)my_dst, j & 31u);
+      long long k = 0;
+      if constexpr (KEYED) k = shfl_ll(my_key, (int)(j & 31u));
       if (s && d) {
         if (s == DET_SRC_DEFAULT) {
-          for (unsigned c = c0; c < g.vpr; c += g.lpr) st_row<OV>(d + c * OV, ld_cached<OV>(bdef + c * OV));
+          if constexpr (KEYED) {
+            for (unsigned c = c0; c < g.vpr; c += g.lpr) st_row<OV>(d + c * OV, keyed_out_vec<OV>(ki, k, c * OV));
+          } else {
+            for (unsigned c = c0; c < g.vpr; c += g.lpr) st_row<OV>(d + c * OV, ld_cached<OV>(bdef + c * OV));
+          }
         } else {
           for (unsigned c = c0; c < g.vpr; c += g.lpr) st_row<OV>(d + c * OV, WidenVec<H, OV>::of(ld_row<IV>(s + c * IV)));
         }
@@ -409,11 +439,12 @@ __device__ __forceinline__ void warp_widen_rows(const RowGeom& g, const unsigned
 
 // lookup_identity_kernel on a half table: the same gate, key tiles and probe; rows are widened on the way to `out`.
 // g: geometry of the fp32 output row in OV-byte vectors (the half row is read in OV / 2-byte vectors).
-template <typename H, int OV>
+template <typename H, int OV, bool KEYED = false>
 __global__ void __launch_bounds__(kThreadsF)
 lookup_identity_widen_kernel(TableView t, const long long* __restrict__ ids, const int* __restrict__ seg, size_t n,
                              const unsigned char* __restrict__ default_row, unsigned char* __restrict__ out, RowGeom g,
-                             int use_tma, unsigned* __restrict__ not_identity, unsigned epoch) {
+                             int use_tma, unsigned* __restrict__ not_identity, unsigned epoch,
+                             InitArg<KEYED> ki = InitArg<KEYED>()) {
   __shared__ __align__(128) long long s_keys[kStages][kTileKeys];
   __shared__ __align__(8) unsigned long long s_bar[kStages];
   const int lane = threadIdx.x & 31;
@@ -432,7 +463,7 @@ lookup_identity_widen_kernel(TableView t, const long long* __restrict__ ids, con
       src = slot >= 0 ? t.planes[0] + (size_t)slot * t.row_bytes : DET_SRC_DEFAULT;
       dst = out + i * g.row_bytes;
     }
-    warp_widen_rows<H, OV>(g, src, dst, lane, default_row);
+    warp_widen_rows<H, OV, KEYED>(g, src, dst, lane, default_row, ki, key);
   }
 }
 
@@ -457,12 +488,15 @@ template <> struct FVec<4> {
   __device__ __forceinline__ void store(__half* p) const { store_half(p); }
   __device__ __forceinline__ void store(__nv_bfloat16* p) const { store_half(p); }
   __device__ __forceinline__ void zero() { v = make_float4(0.f, 0.f, 0.f, 0.f); }
+  __device__ __forceinline__ void keyed(const KeyedInit& ki, long long key, unsigned col) { v = keyed_f32x4(ki, key, col); }
   __device__ __forceinline__ void fill(float x) { v = make_float4(x, x, x, x); }
   template <typename F> __device__ __forceinline__ void apply(F f) { f(v.x); f(v.y); f(v.z); f(v.w); }
   template <typename F> __device__ __forceinline__ void zip(const FVec& o, F f) { f(v.x, o.v.x); f(v.y, o.v.y); f(v.z, o.v.z); f(v.w, o.v.w); }
 };
 template <> struct FVec<1> {
   float v;
+  // elements col .. col + VF - 1 of the row of `key` from the table's keyed initializer
+  __device__ __forceinline__ void keyed(const KeyedInit& ki, long long key, unsigned col) { v = keyed_f32x1(ki, key, col); }
   __device__ __forceinline__ void load(const float* p) { v = *p; }
   __device__ __forceinline__ void load(const __half* p) { v = widen(*p); }
   __device__ __forceinline__ void load(const __nv_bfloat16* p) { v = widen(*p); }
@@ -483,12 +517,15 @@ template <int VF, typename H> struct HalfRowVec;
 template <int VF, typename T> struct RowVec : HalfRowVec<VF, T> {};
 template <int VF> struct RowVec<VF, float> : FVec<VF> {
   __device__ __forceinline__ void init(const FVec<VF>& def) { FVec<VF>::operator=(def); }
+  // the row's bits as stored (a generated row, keyed initializer)
+  template <typename B> __device__ __forceinline__ void set_bits(const B& b) { memcpy(&this->v, &b, sizeof(this->v)); }
   __device__ __forceinline__ const FVec<VF>& get(const FVec<VF>&, const float*, bool) const { return *this; }
 };
 template <typename H> struct HalfRowVec<4, H> {
   int2 r;
   __device__ __forceinline__ void init(const FVec<4>&) {}
   __device__ __forceinline__ void load(const H* p) { r = *reinterpret_cast<const int2*>(p); }
+  __device__ __forceinline__ void set_bits(int2 b) { r = b; }
   __device__ __forceinline__ FVec<4> get(const FVec<4>&, const float* def, bool loaded) const {
     FVec<4> x;
     if (!loaded) {
@@ -504,6 +541,7 @@ template <typename H> struct HalfRowVec<1, H> {
   H r;
   __device__ __forceinline__ void init(const FVec<1>&) {}
   __device__ __forceinline__ void load(const H* p) { r = *p; }
+  __device__ __forceinline__ void set_bits(short b) { memcpy(&r, &b, sizeof(r)); }
   __device__ __forceinline__ FVec<1> get(const FVec<1>&, const float* def, bool loaded) const {
     FVec<1> x;
     x.v = loaded ? widen(r) : __ldg(def);
@@ -530,12 +568,16 @@ template <> __device__ __forceinline__ float clip_norm_of<true>(const ClipArg<tr
 
 // T: the table's row storage type (float, __half or __nv_bfloat16); the lane geometry is that of the fp32 output row,
 // so a lane that reads a 16 B float4 of an fp32 row reads 8 B of a half row.
-template <int VF, bool CLIP = false, typename T = float>
-__global__ void __launch_bounds__(kThreadsF, kSegMinBlocks)
+// KEYED: a missing id's row is generated from the table's keyed initializer for ki.ids[i] (default_row is NULL).
+// A keyed instantiation keeps the generator's out-of-line calls inside the unrolled body: the registers live across
+// them need a budget above the 80 that 3 CTAs per SM leave, so it is built for 2.
+template <int VF, bool CLIP = false, typename T = float, bool KEYED = false>
+__global__ void __launch_bounds__(kThreadsF, KEYED ? 2 : kSegMinBlocks)
 segment_sum_kernel(TableView t, const long long* __restrict__ slots, const long long* __restrict__ seg_start,
                    const float* __restrict__ weights, size_t batch, int combiner,
                    const float* __restrict__ default_row, float* __restrict__ out, unsigned vpr, unsigned lpr,
-                   unsigned lpr_shift, ClipArg<CLIP> clip, const unsigned* __restrict__ run_if_set, unsigned epoch) {
+                   unsigned lpr_shift, ClipArg<CLIP> clip, const unsigned* __restrict__ run_if_set, unsigned epoch,
+                   InitArg<KEYED> ki = InitArg<KEYED>()) {
   if (run_if_set && *run_if_set != epoch) return;   // the one-id-per-row kernel has served this call
   constexpr int U = kSegPerGroup;
   const int lane = threadIdx.x & 31;
@@ -549,7 +591,7 @@ segment_sum_kernel(TableView t, const long long* __restrict__ slots, const long 
   const T* table = (const T*)t.planes[0];
   FVec<VF> defv;
   defv.zero();
-  if (lane_on) defv.load(default_row + (size_t)gl * VF);
+  if (!KEYED && lane_on) defv.load(default_row + (size_t)gl * VF);
   // where a half lane reads the default row; lanes beyond the row read (and never store) its first vector
   const float* def_lane = default_row + (lane_on ? (size_t)gl * VF : 0);
   for (size_t sb = warp0 * gpw * U; sb < batch; sb += nwarps * gpw * U) {
@@ -585,6 +627,18 @@ segment_sum_kernel(TableView t, const long long* __restrict__ slots, const long 
         x[u].init(defv);
         if (sl[u] >= 0 && lane_on) x[u].load(table + (size_t)sl[u] * dim + (size_t)gl * VF);
       }
+      if constexpr (KEYED) {
+        // a missing id's row, in the table's storage type; every other lane that loaded nothing holds zeros
+        constexpr int VB = VF * (int)sizeof(T);
+#pragma unroll
+        for (int u = 0; u < U; ++u) {
+          if (!(sl[u] >= 0 && lane_on)) {
+            typename VecT<VB>::type b = typename VecT<VB>::type();
+            if (sl[u] == -1 && lane_on) b = keyed_vec<VB>(ki, __ldg(ki.ids + st[u] + k), gl * (unsigned)VB);
+            x[u].set_bits(b);
+          }
+        }
+      }
       if constexpr (CLIP) {   // fp32 tables only
         // row <- row * max_norm / max(||row||, max_norm): the squared norm is summed over the lanes of the group
         // (lanes beyond the row hold zeros); every lane of the warp takes part in the shuffles (uniform loop)
@@ -602,7 +656,7 @@ segment_sum_kernel(TableView t, const long long* __restrict__ slots, const long 
       for (int u = 0; u < U; ++u) {
         if (sl[u] != -2) {
           const float wu = w[u];
-          acc[u].zip(x[u].get(defv, def_lane, sl[u] >= 0 && lane_on), [wu](float& a, float xv) { a = a + xv * wu; });
+          acc[u].zip(x[u].get(defv, def_lane, KEYED || (sl[u] >= 0 && lane_on)), [wu](float& a, float xv) { a = a + xv * wu; });
           wsum[u] = wsum[u] + wu;
           wsq[u] = wsq[u] + wu * wu;
         }
@@ -643,12 +697,12 @@ template <> struct WideSrc<float> {
   template <int VF> __device__ __forceinline__ void load(FVec<VF>& x, size_t off) const { x.load(src + off); }
 };
 
-template <int VF, typename T = float>
+template <int VF, typename T = float, bool KEYED = false>
 __global__ void __launch_bounds__(kThreadsF)
 segment_sum_wide_kernel(TableView t, const long long* __restrict__ slots, const long long* __restrict__ seg_start,
                         const float* __restrict__ weights, size_t batch, int combiner,
                         const float* __restrict__ default_row, float* __restrict__ out, unsigned vpr, unsigned lpr,
-                        unsigned lpr_shift) {
+                        unsigned lpr_shift, InitArg<KEYED> ki = InitArg<KEYED>()) {
   const int lane = threadIdx.x & 31;
   const int gl = lane & (int)(lpr - 1);
   const unsigned gpw = 32u >> lpr_shift;
@@ -672,12 +726,19 @@ segment_sum_wide_kernel(TableView t, const long long* __restrict__ slots, const 
         const long long slot = __ldg(slots + i);
         const float w = weights ? __ldg(weights + i) : 1.f;
         const WideSrc<T> src(table, slot, dim, default_row);
+        long long key = 0;
+        if constexpr (KEYED) key = slot < 0 ? __ldg(ki.ids + i) : 0;
 #pragma unroll
         for (int v = 0; v < kMaxVecPerLane; ++v) {
           const unsigned c = c0 + (unsigned)gl + (unsigned)v * lpr;
           if (c < vpr) {
             FVec<VF> x;
-            src.load(x, (size_t)c * VF);
+            if constexpr (KEYED) {
+              if (slot < 0) x.keyed(ki, key, c * (unsigned)VF);
+              else src.load(x, (size_t)c * VF);
+            } else {
+              src.load(x, (size_t)c * VF);
+            }
             acc[v].zip(x, [w](float& a, float xv) { a = a + xv * w; });
           }
         }
@@ -790,11 +851,13 @@ static SlotPlanes<OPT> slot_planes_arg(const det_table* t) {
 // them in registers.  0 = no minimum, the other optimizers' kernels as before.
 template <int OPT> constexpr int kApplyMinBlocks = OPT == 4 ? 3 : 0;
 
-template <int VF, int OPT, typename T = float>
-__global__ void __launch_bounds__(kThreadsF, kApplyMinBlocks<OPT>)
+// KEYED: a new key's param starts from its row of the table's keyed initializer (init_param is NULL).
+// (keyed: 2 CTAs per SM, the register budget the generator's calls need without spilling, as segment_sum_kernel)
+template <int VF, int OPT, typename T = float, bool KEYED = false>
+__global__ void __launch_bounds__(kThreadsF, KEYED ? 2 : kApplyMinBlocks<OPT>)
 apply_kernel(TableView t, const long long* __restrict__ keys, const float* __restrict__ grads, size_t n,
              OptHyper h, const float* __restrict__ init_param, int full_init, unsigned vpr, unsigned lpr,
-             unsigned lpr_shift, int use_tma, SlotPlanes<OPT> sp) {
+             unsigned lpr_shift, int use_tma, SlotPlanes<OPT> sp, InitArg<KEYED> ki = InitArg<KEYED>()) {
   __shared__ __align__(128) long long s_keys[kStages][kTileKeys];
   __shared__ __align__(8) unsigned long long s_bar[kStages];
   __shared__ unsigned s_new, s_used;
@@ -833,11 +896,13 @@ apply_kernel(TableView t, const long long* __restrict__ keys, const float* __res
       bool ok[RU], nwv[RU], fresh[RU];
       size_t ro[RU], gi[RU];
       unsigned mark[RU];
+      long long kj[RU];
 #pragma unroll
       for (int u = 0; u < RU; ++u) {
         const unsigned j = j0 + (unsigned)u * rows_per_step + sub;
         const unsigned jj = j & 31u;
         const long long s = shfl_ll(slot, (int)jj);
+        kj[u] = KEYED ? shfl_ll(key, (int)jj) : 0;
         nwv[u] = (bn >> jj) & 1u;
         gi[u] = base + jj;
         ok[u] = (j < 32u) && (gi[u] < n) && s >= 0;
@@ -859,8 +924,13 @@ apply_kernel(TableView t, const long long* __restrict__ keys, const float* __res
         for (int u = 0; u < RU; ++u) {
           if (!ok[u]) continue;
           g[u].load(grads + gi[u] * dim + o);
-          if (nwv[u]) p[u].load((full_init ? init_param + gi[u] * dim : init_param) + o);
-          else p[u].load(P + ro[u] + o);
+          if constexpr (KEYED) {
+            if (nwv[u]) p[u].keyed(ki, kj[u], c * (unsigned)VF);
+            else p[u].load(P + ro[u] + o);
+          } else {
+            if (nwv[u]) p[u].load((full_init ? init_param + gi[u] * dim : init_param) + o);
+            else p[u].load(P + ro[u] + o);
+          }
           if (OPT == 0) {
             if (fresh[u]) a[u].fill(h.init_slot); else a[u].load(S1 + ro[u] + o);
           } else if (OPT == 1) {
@@ -934,12 +1004,14 @@ __device__ __forceinline__ void score_touch<true>(const ScoreArg<true>& sa, long
 
 // T: the param row storage type, as in apply_kernel.  An existing key's half param vector is one 8 B cp.async into the
 // first half of its 16 B stage slot; a new key's is the 16 B fp32 init_param vector, as on an fp32 table.
-template <int OPT, bool SCORED = false, typename T = float>
+// KEYED: a new key's param vector is generated in registers from the table's keyed initializer instead of copied from
+// init_param (NULL); the key travels with the slot through the row-step shuffles.
+template <int OPT, bool SCORED = false, typename T = float, bool KEYED = false>
 __global__ void __launch_bounds__(kThreadsF)
 apply_staged_kernel(TableView t, const long long* __restrict__ keys, const float* __restrict__ grads, size_t n,
                     OptHyper h, const float* __restrict__ init_param, int full_init, unsigned vpr, unsigned lpr,
                     unsigned lpr_shift, int use_tma, ScoreArg<SCORED> sa, const long long* __restrict__ n_dev,
-                    SlotPlanes<OPT> sp) {
+                    SlotPlanes<OPT> sp, InitArg<KEYED> ki = InitArg<KEYED>()) {
   if (n_dev) n = (size_t)*n_dev;        // key count produced on the device (det_apply_*_dup); the grid covers the bound
   constexpr int NS = 2 + opt_slots(OPT);  // streams per row: grad, param (, slot1 (, slot2))
   DET_DYN_SHARED(dyn_smem);
@@ -998,12 +1070,14 @@ apply_staged_kernel(TableView t, const long long* __restrict__ keys, const float
         if (ok) {
           const size_t ro = (size_t)sl * dim + (size_t)c0 * 4;
           cp_async16(sm(stage, st, 0), grads + gi * dim + (size_t)c0 * 4);
-          if constexpr (std::is_same<T, float>::value)
-            cp_async16(sm(stage, st, 1), nw ? (full_init ? init_param + gi * dim : init_param) + (size_t)c0 * 4 : P + ro);
-          else if (nw)
-            cp_async16(sm(stage, st, 1), (full_init ? init_param + gi * dim : init_param) + (size_t)c0 * 4);
-          else
-            cp_async8(sm(stage, st, 1), P + ro);
+          if (!(KEYED && nw)) {   // a keyed new row is generated when it is consumed
+            if constexpr (std::is_same<T, float>::value)
+              cp_async16(sm(stage, st, 1), nw ? (full_init ? init_param + gi * dim : init_param) + (size_t)c0 * 4 : P + ro);
+            else if (nw)
+              cp_async16(sm(stage, st, 1), (full_init ? init_param + gi * dim : init_param) + (size_t)c0 * 4);
+            else
+              cp_async8(sm(stage, st, 1), P + ro);
+          }
           if (!nw && NS > 2) {
             cp_async16(sm(stage, st, 2), S1 + ro);
             if (NS > 3) cp_async16(sm(stage, st, 3), S2 + ro);
@@ -1027,6 +1101,7 @@ apply_staged_kernel(TableView t, const long long* __restrict__ keys, const float
         const unsigned step = b * kStageSteps + st;
         const unsigned j = step * rows_per_step + sub;
         const long long sl = shfl_ll(slot, (int)(j & 31u));
+        const long long kj = KEYED ? shfl_ll(key, (int)(j & 31u)) : 0;
         const bool nw = (bn >> (j & 31u)) & 1u;
         const size_t gi = base + (j & 31u);
         const bool row_ok = step < steps_total && gi < n && sl >= 0;
@@ -1036,9 +1111,15 @@ apply_staged_kernel(TableView t, const long long* __restrict__ keys, const float
           const size_t ro = (size_t)sl * dim + (size_t)c0 * 4;
           FVec<4> g, p, a, b2;
           g.v = *sm(stage, st, 0);
-          if constexpr (std::is_same<T, float>::value) p.v = *sm(stage, st, 1);
-          else if (nw) p.v = *sm(stage, st, 1);
-          else p.load(reinterpret_cast<const T*>(sm(stage, st, 1)));
+          if constexpr (KEYED) {
+            if (nw) p.keyed(ki, kj, c0 * 4u);
+            else if constexpr (std::is_same<T, float>::value) p.v = *sm(stage, st, 1);
+            else p.load(reinterpret_cast<const T*>(sm(stage, st, 1)));
+          } else {
+            if constexpr (std::is_same<T, float>::value) p.v = *sm(stage, st, 1);
+            else if (nw) p.v = *sm(stage, st, 1);
+            else p.load(reinterpret_cast<const T*>(sm(stage, st, 1)));
+          }
           if (OPT == 0) {
             if (fresh) a.fill(h.init_slot); else a.v = *sm(stage, st, 2);
             a.zip(g, [](float& av, float gv) { av = av + gv * gv; });
@@ -1627,7 +1708,7 @@ static size_t seg_reduce_layout(size_t n, size_t n_groups, unsigned char* base, 
 
 // K6 one-id-per-row kernel of a table whose rows are T: float, or __half / __nv_bfloat16 rows it widens to fp32
 using IdentityKernel = void (*)(TableView, const long long*, const int*, size_t, const unsigned char*, unsigned char*,
-                                RowGeom, int, unsigned*, unsigned);
+                                RowGeom, int, unsigned*, unsigned, InitArg<false>);
 template <typename T, int V> static IdentityKernel identity_kernel() {
   if constexpr (std::is_same<T, float>::value)
     return lookup_identity_kernel<V>;
@@ -1650,9 +1731,11 @@ static void launch_segment_sum(const TableView& v, int sms, const long long* slo
     const int occ = vec4 ? occupancy_of(k4, kThreadsF) : occupancy_of(k1, kThreadsF);
     const int grid = grid_for(batch, (int)(gpw * kSegPerGroup * (kThreadsF / 32)), sms, occ);
     if (vec4)
-      DET_LAUNCH(k4, grid, kThreadsF, 0, s, v, slots, seg_start, weights, batch, combiner, default_row, out, vpr, lpr, sh, clip, gate, epoch);
+      DET_LAUNCH(k4, grid, kThreadsF, 0, s, v, slots, seg_start, weights, batch, combiner, default_row, out, vpr, lpr, sh, clip, gate, epoch,
+                 InitArg<false>());
     else
-      DET_LAUNCH(k1, grid, kThreadsF, 0, s, v, slots, seg_start, weights, batch, combiner, default_row, out, vpr, lpr, sh, clip, gate, epoch);
+      DET_LAUNCH(k1, grid, kThreadsF, 0, s, v, slots, seg_start, weights, batch, combiner, default_row, out, vpr, lpr, sh, clip, gate, epoch,
+                 InitArg<false>());
   } else {
     // rows wider than kMaxVecPerLane vectors per lane are swept in column chunks by the same kernel
     const int grid = grid_for(batch, (int)(gpw * (kThreadsF / 32)), sms, 8);
@@ -1661,6 +1744,41 @@ static void launch_segment_sum(const TableView& v, int sms, const long long* slo
     else
       DET_LAUNCH((segment_sum_wide_kernel<1, T>), grid, kThreadsF, 0, s, v, slots, seg_start, weights, batch, combiner, default_row, out, vpr, lpr, sh);
   }
+}
+
+// launch_segment_sum of a table with a keyed initializer and no default row: the kernels generate missing ids' rows
+template <typename T, bool CLIP>
+static void launch_segment_sum_keyed(const TableView& v, int sms, const long long* slots, const long long* seg_start,
+                                     const float* weights, size_t batch, int combiner, float* out, bool vec4, unsigned vpr,
+                                     unsigned lpr, unsigned sh, const ClipArg<CLIP>& clip, const unsigned* gate,
+                                     unsigned epoch, const InitArg<true>& ki, cudaStream_t s) {
+  const unsigned gpw = 32u >> sh;
+  const float* nodef = nullptr;
+  if (vpr <= lpr) {
+    const auto k4 = segment_sum_kernel<4, CLIP, T, true>;
+    const auto k1 = segment_sum_kernel<1, CLIP, T, true>;
+    const int occ = vec4 ? occupancy_of(k4, kThreadsF) : occupancy_of(k1, kThreadsF);
+    const int grid = grid_for(batch, (int)(gpw * kSegPerGroup * (kThreadsF / 32)), sms, occ);
+    if (vec4)
+      DET_LAUNCH(k4, grid, kThreadsF, 0, s, v, slots, seg_start, weights, batch, combiner, nodef, out, vpr, lpr, sh, clip, gate, epoch, ki);
+    else
+      DET_LAUNCH(k1, grid, kThreadsF, 0, s, v, slots, seg_start, weights, batch, combiner, nodef, out, vpr, lpr, sh, clip, gate, epoch, ki);
+  } else {
+    const int grid = grid_for(batch, (int)(gpw * (kThreadsF / 32)), sms, 8);
+    if (vec4)
+      DET_LAUNCH((segment_sum_wide_kernel<4, T, true>), grid, kThreadsF, 0, s, v, slots, seg_start, weights, batch, combiner, nodef, out, vpr, lpr, sh, ki);
+    else
+      DET_LAUNCH((segment_sum_wide_kernel<1, T, true>), grid, kThreadsF, 0, s, v, slots, seg_start, weights, batch, combiner, nodef, out, vpr, lpr, sh, ki);
+  }
+}
+
+using IdentityKernelKeyed = void (*)(TableView, const long long*, const int*, size_t, const unsigned char*, unsigned char*,
+                                     RowGeom, int, unsigned*, unsigned, InitArg<true>);
+template <typename T, int V> static IdentityKernelKeyed identity_kernel_keyed() {
+  if constexpr (std::is_same<T, float>::value)
+    return lookup_identity_kernel<V, true>;
+  else
+    return lookup_identity_widen_kernel<T, V, true>;
 }
 
 // K7: f(row) with decltype(row)::type the param row storage type of a float32, float16 or bfloat16 table (the caller
@@ -1727,7 +1845,14 @@ static det_status lookup_sparse_impl(det_table* t, const int64_t* ids, const int
   if (combiner < DET_COMBINER_SUM || combiner > DET_COMBINER_SQRTN)
     return fail(DET_INVALID_ARGUMENT, "combiner must be one of 'mean', 'sqrtn' or 'sum'");
   if (batch == 0) return DET_OK;
-  if (!out || !default_row || (nnz && (!ids || !segment_ids))) return fail(DET_INVALID_ARGUMENT, "det_lookup_sparse: null argument");
+  if (!out || (nnz && (!ids || !segment_ids))) return fail(DET_INVALID_ARGUMENT, "det_lookup_sparse: null argument");
+  // NULL default_row: missing ids' rows come from the table's keyed initializer
+  const bool keyed = default_row == nullptr;
+  if (keyed && !t->keyed)
+    return fail(DET_INVALID_ARGUMENT, "det_lookup_sparse: null default_row (the table has no keyed initializer)");
+  InitArg<true> ki{};
+  static_cast<KeyedInit&>(ki) = t->init;
+  ki.ids = (const long long*)ids;
   cudaStream_t s = (cudaStream_t)stream;
   det::DevGuard _dg(t->cfg.device);
   long long* seg_start = nullptr;
@@ -1771,11 +1896,19 @@ static det_status lookup_sparse_impl(det_table* t, const int64_t* ids, const int
     dispatch_vec<4>(out_row_bytes, {{default_row, "det_lookup_sparse: default_row"}, {out, "det_lookup_sparse: out"}},
                     [&](auto V, const RowGeom& g) -> det_status {
       constexpr int VV = decltype(V)::value;
+      if (keyed) {
+        const IdentityKernelKeyed kern = vt == DET_FLOAT32   ? identity_kernel_keyed<float, VV>()
+                                         : vt == DET_FLOAT16 ? identity_kernel_keyed<__half, VV>()
+                                                             : identity_kernel_keyed<__nv_bfloat16, VV>();
+        const int grid = grid_for(nnz, kTileKeys, t->sm_count, occupancy_of(kern, kThreadsF));
+        DET_LAUNCH(kern, grid, kThreadsF, 0, s, t->view, k, segment_ids, nnz, d, o, g, tma, not_identity, epoch, ki);
+        return DET_OK;
+      }
       const IdentityKernel kern = vt == DET_FLOAT32   ? identity_kernel<float, VV>()
                                   : vt == DET_FLOAT16 ? identity_kernel<__half, VV>()
                                                       : identity_kernel<__nv_bfloat16, VV>();
       const int grid = grid_for(nnz, kTileKeys, t->sm_count, occupancy_of(kern, kThreadsF));
-      DET_LAUNCH(kern, grid, kThreadsF, 0, s, t->view, k, segment_ids, nnz, d, o, g, tma, not_identity, epoch);
+      DET_LAUNCH(kern, grid, kThreadsF, 0, s, t->view, k, segment_ids, nnz, d, o, g, tma, not_identity, epoch, InitArg<false>());
       return DET_OK;
     });
   }
@@ -1784,7 +1917,23 @@ static det_status lookup_sparse_impl(det_table* t, const int64_t* ids, const int
     DET_LAUNCH(resolve_slots_kernel, grid_for(nnz, kTileKeys, t->sm_count, occupancy_of(resolve_slots_kernel, kThreadsF)), kThreadsF, 0, s, t->view, (const long long*)ids, nnz, slots, (((uintptr_t)ids & 15u) == 0) ? 1 : 0, gate, epoch);
   det_status rc = DET_OK;
   const ClipArg<false> noclip;
-  if (vpr <= lpr && max_norm > 0.f) {
+  if (keyed && !(max_norm > 0.f && !(vpr <= lpr))) {
+    if (max_norm > 0.f) {
+      ClipArg<true> clip;
+      clip.max_norm = max_norm;
+      launch_segment_sum_keyed<float>(t->view, t->sm_count, slots, seg_start, weights, batch, combiner, out, vec4, vpr, lpr,
+                                      sh, clip, gate, epoch, ki, s);
+    } else if (vt == DET_FLOAT32) {
+      launch_segment_sum_keyed<float>(t->view, t->sm_count, slots, seg_start, weights, batch, combiner, out, vec4, vpr, lpr,
+                                      sh, noclip, gate, epoch, ki, s);
+    } else if (vt == DET_FLOAT16) {
+      launch_segment_sum_keyed<__half>(t->view, t->sm_count, slots, seg_start, weights, batch, combiner, out, vec4, vpr, lpr,
+                                       sh, noclip, gate, epoch, ki, s);
+    } else {
+      launch_segment_sum_keyed<__nv_bfloat16>(t->view, t->sm_count, slots, seg_start, weights, batch, combiner, out, vec4,
+                                              vpr, lpr, sh, noclip, gate, epoch, ki, s);
+    }
+  } else if (vpr <= lpr && max_norm > 0.f) {
     ClipArg<true> clip;
     clip.max_norm = max_norm;
     launch_segment_sum<float>(t->view, t->sm_count, slots, seg_start, weights, batch, combiner, default_row, out, vec4, vpr,
@@ -1831,7 +1980,15 @@ static det_status apply_common(det_table* t, const int64_t* keys, const float* g
   if (t->cfg.num_slot_planes < opt_slots(opt))
     return fail(DET_INVALID_ARGUMENT, "det_apply: table was created with too few optimizer slot planes");
   if (n == 0) return DET_OK;
-  if (!keys || !grads || !init_param) return fail(DET_INVALID_ARGUMENT, "det_apply: null argument");
+  if (!keys || !grads) return fail(DET_INVALID_ARGUMENT, "det_apply: null argument");
+  // NULL init_param: new keys start from their rows of the table's keyed initializer
+  const bool keyed = init_param == nullptr;
+  if (keyed && !t->keyed) return fail(DET_INVALID_ARGUMENT, "det_apply: null init_param (the table has no keyed initializer)");
+  if (keyed && full_init)
+    return fail(DET_INVALID_ARGUMENT, "det_apply: full_size_init needs init_param rows (NULL generates them)");
+  InitArg<true> ki{};
+  static_cast<KeyedInit&>(ki) = t->init;
+  ki.ids = nullptr;
   det::DevGuard _dg(t->cfg.device);
   const unsigned dim = (unsigned)t->cfg.dim;
   const bool vec4 = (dim % 4 == 0) && ((((uintptr_t)grads | (uintptr_t)init_param) & 15u) == 0);
@@ -1857,12 +2014,21 @@ static det_status apply_common(det_table* t, const int64_t* keys, const float* g
             sa.sc = evict_scores(t);
             sa.rule = evict_rule(t);
           }
+          if (keyed) {
+            const auto kern = apply_staged_kernel<decltype(OPT)::value, kScored, typename decltype(row)::type, true>;
+            CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            int occ = 1;
+            if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, kThreadsF, smem) != cudaSuccess || occ < 1) occ = 1;
+            DET_LAUNCH(kern, grid_for(n, kTileKeys, t->sm_count, occ), kThreadsF, smem, s, v, k, grads, n, h, init_param,
+                       0, vpr, lpr, sh, tma, sa, n_dev, slot_planes_arg<decltype(OPT)::value>(t), ki);
+            return DET_OK;
+          }
           const auto kern = apply_staged_kernel<decltype(OPT)::value, kScored, typename decltype(row)::type>;
           CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
           int occ = 1;
           if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, kThreadsF, smem) != cudaSuccess || occ < 1) occ = 1;
           DET_LAUNCH(kern, grid_for(n, kTileKeys, t->sm_count, occ), kThreadsF, smem, s, v, k, grads, n, h, init_param,
-                     full_init, vpr, lpr, sh, tma, sa, n_dev, slot_planes_arg<decltype(OPT)::value>(t));
+                     full_init, vpr, lpr, sh, tma, sa, n_dev, slot_planes_arg<decltype(OPT)::value>(t), InitArg<false>());
           return DET_OK;
         });
       });
@@ -1875,10 +2041,17 @@ static det_status apply_common(det_table* t, const int64_t* keys, const float* g
   dispatch_row_type(vt, [&](auto row) -> det_status {
     return dispatch_int<kNumOpts>(opt, [&](auto OPT) -> det_status {
       return dispatch_bit(vec4, [&](auto VEC4) -> det_status {
+        if (keyed) {
+          const auto kern = apply_kernel<decltype(VEC4)::value ? 4 : 1, decltype(OPT)::value, typename decltype(row)::type, true>;
+          const int grid = grid_for(n, kTileKeys, t->sm_count, occupancy_of(kern, kThreadsF));
+          DET_LAUNCH(kern, grid, kThreadsF, 0, s, v, k, grads, n, h, init_param, 0, vpr, lpr, sh,
+                     (((uintptr_t)keys & 15u) == 0) ? 1 : 0, slot_planes_arg<decltype(OPT)::value>(t), ki);
+          return DET_OK;
+        }
         const auto kern = apply_kernel<decltype(VEC4)::value ? 4 : 1, decltype(OPT)::value, typename decltype(row)::type>;
         const int grid = grid_for(n, kTileKeys, t->sm_count, occupancy_of(kern, kThreadsF));
         DET_LAUNCH(kern, grid, kThreadsF, 0, s, v, k, grads, n, h, init_param, full_init, vpr, lpr, sh,
-                   (((uintptr_t)keys & 15u) == 0) ? 1 : 0, slot_planes_arg<decltype(OPT)::value>(t));
+                   (((uintptr_t)keys & 15u) == 0) ? 1 : 0, slot_planes_arg<decltype(OPT)::value>(t), InitArg<false>());
         return DET_OK;
       });
     });
@@ -2156,7 +2329,15 @@ static det_status apply_dup(det_table* t, const int64_t* ids, const float* grads
                             int64_t* n_unique_dev_out, cudaStream_t s, const long long* n_items_dev = nullptr) {
   if (!t) return fail(DET_INVALID_ARGUMENT, "det_apply_dup: null table");
   if (n == 0) return DET_OK;
-  if (!ids || !grads || !init_param || !workspace) return fail(DET_INVALID_ARGUMENT, "det_apply_dup: null argument");
+  if (!ids || !grads || !workspace) return fail(DET_INVALID_ARGUMENT, "det_apply_dup: null argument");
+  if (!init_param) {
+    bool keyed;
+    {
+      std::lock_guard<std::mutex> lk(t->mu);   // set_initializer writes it under the same lock
+      keyed = t->keyed;
+    }
+    if (!keyed) return fail(DET_INVALID_ARGUMENT, "det_apply_dup: null init_param (the table has no keyed initializer)");
+  }
   if (n >= 0x7fffffffull) return fail(DET_INVALID_ARGUMENT, "det_apply_dup: n too large");
   const size_t dim = (size_t)t->cfg.dim;
   if (workspace_bytes < det_apply_dup_workspace_bytes(n, dim)) return fail(DET_INVALID_ARGUMENT, "det_apply_dup: workspace too small");
@@ -2223,6 +2404,8 @@ det_status apply_dup_on_device_count(det_table* t, const int64_t* ids, const flo
   OptHyper h;
   h.lr = lr; h.eps = eps; h.beta1 = beta1; h.beta2 = beta2; h.init_slot = init_slot;
   if (t && opt == 0) t->slot_init[1] = init_slot;
+  // the owner side does not generate rows: the exchange always passes the initial param row
+  if (!init_param) return fail(DET_INVALID_ARGUMENT, "det_peer_xchg_apply: null init_param");
   return apply_dup(t, ids, grads, n_bound, h, init_param, opt, workspace, workspace_bytes, nullptr, s, n_items_dev);
 }
 }  // namespace det

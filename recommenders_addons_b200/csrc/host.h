@@ -205,6 +205,8 @@ struct det_table {
   uint64_t n_since_snap = 0;         // keys of mutating calls issued after the snapshot in flight
   uint32_t rehash_count = 0;
   float slot_init[det::kMaxPlanes];  // value given to slot-plane rows of keys created by insert/accum
+  bool keyed = false;                // det_table_set_initializer: missing rows come from `init` where a NULL row is passed
+  det::KeyedInit init{};
   det::HostPipe* pipe = nullptr;   // host-buffer pipeline of det_find_host
   det::HostPipe* pipe2 = nullptr;  // ... of det_insert_host (separate streams: the two directions overlap)
   void* scratch = nullptr;           // per-table device scratch reused by det_lookup_sparse / det_export

@@ -2,6 +2,8 @@
 // remove / clear / size / export / rehash).  sm_90a only.  See DESIGN.md for layout and rooflines.
 #include <stdlib.h>
 
+#include <cmath>
+
 #include "host.h"
 
 namespace det {
@@ -69,11 +71,13 @@ constexpr unsigned kNoHint = 0xffffffffu;
 
 // K1: Find / FindWithExists with the default-row fill folded in (replaces HKV find +
 // gpu_fill_default_values, lookup_table_op_hkv.h:317-327, 719-732).  One warp-step = 32 keys.
-template <int VEC>
+// KEYED: missing rows are generated from the table's keyed initializer `ki` (defaults is NULL).
+template <int VEC, bool KEYED = false>
 __device__ __forceinline__ void find_step(const TableView& t, long long key, size_t i, bool valid,
                                           const unsigned char* __restrict__ defaults, int full_default,
                                           unsigned char* __restrict__ out, unsigned char* __restrict__ exists,
-                                          const RowGeom& g, int lane, const SlotHints& h) {
+                                          const RowGeom& g, int lane, const SlotHints& h,
+                                          const InitArg<KEYED>& ki = InitArg<KEYED>()) {
   const long long slot = warp_find_slots<false>(t, key, valid, lane);
   if (exists != nullptr && valid) exists[i] = slot >= 0 ? 1 : 0;
   if (h.keys != nullptr && valid) {
@@ -87,17 +91,19 @@ __device__ __forceinline__ void find_step(const TableView& t, long long key, siz
                     : (full_default ? defaults + i * g.row_bytes : DET_SRC_DEFAULT);
     dst = out + i * g.row_bytes;
   }
-  warp_move_rows<VEC>(g, src, dst, lane, full_default ? nullptr : defaults);
+  warp_move_rows<VEC, KEYED>(g, src, dst, lane, full_default ? nullptr : defaults, ki, key);
 }
 
 // Persistent CTAs, key tiles staged into shared memory by TMA bulk copies (cp.async.bulk + mbarrier), tile i+1 in
 // flight while tile i is probed and gathered.  TMA = false: keys that are not 16 B aligned, read with plain loads on
 // the same tile schedule.
-template <int VEC, bool TMA>
-__global__ void __launch_bounds__(kThreads)
+// (keyed: built for 2 CTAs per SM, the register budget the generator's out-of-line calls need without spilling)
+template <int VEC, bool TMA, bool KEYED = false>
+__global__ void __launch_bounds__(kThreads, KEYED ? 2 : 0)
 find_kernel_tma(TableView t, const long long* __restrict__ keys, size_t n,
                 const unsigned char* __restrict__ defaults, int full_default,
-                unsigned char* __restrict__ out, unsigned char* __restrict__ exists, RowGeom g, SlotHints h) {
+                unsigned char* __restrict__ out, unsigned char* __restrict__ exists, RowGeom g, SlotHints h,
+                InitArg<KEYED> ki = InitArg<KEYED>()) {
   __shared__ __align__(128) long long s_keys[kStages][kTileKeys];
   __shared__ __align__(8) unsigned long long s_bar[kStages];
   const int lane = threadIdx.x & 31;
@@ -107,7 +113,7 @@ find_kernel_tma(TableView t, const long long* __restrict__ keys, size_t n,
     size_t i;
     bool valid;
     const long long key = kt.key(i, valid);
-    find_step<VEC>(t, key, i, valid, defaults, full_default, out, exists, g, lane, h);
+    find_step<VEC, KEYED>(t, key, i, valid, defaults, full_default, out, exists, g, lane, h, ki);
   }
 }
 
@@ -1204,10 +1210,15 @@ det_status det_find(det_table* t, const int64_t* keys, size_t n, const void* def
                     void* values_out, uint8_t* exists, det_stream_t stream) {
   if (!t) return fail(DET_INVALID_ARGUMENT, "det_find: null table");
   if (n == 0) return DET_OK;
-  if (!keys || !values_out || !defaults) return fail(DET_INVALID_ARGUMENT, "det_find: null keys/values/default_value");
+  if (!keys || !values_out) return fail(DET_INVALID_ARGUMENT, "det_find: null keys/values");
   cudaStream_t s = (cudaStream_t)stream;
   det::DevGuard _dg(t->cfg.device);
   std::shared_lock<std::shared_mutex> _vl(t->view_mu);   // vs a concurrent growth on another host thread (host.h)
+  // NULL defaults: the rows of missing keys come from the table's keyed initializer
+  const bool keyed = defaults == nullptr;
+  if (keyed && !t->keyed) return fail(DET_INVALID_ARGUMENT, "det_find: null default_value (the table has no keyed initializer)");
+  if (keyed && full_size_default)
+    return fail(DET_INVALID_ARGUMENT, "det_find: full_size_default needs default values (NULL generates the rows)");
   const TableView v = t->view;
   // slot hints: bookkeeping only when the hint lock is free right now (a find never waits) and the stream is not
   // being captured into a graph
@@ -1219,14 +1230,50 @@ det_status det_find(det_table* t, const int64_t* keys, size_t n, const void* def
   return dispatch_vec(t->row_bytes, {{defaults, "det_find: default_value"}, {values_out, "det_find: values"}},
                       [&](auto V, const RowGeom& g) -> det_status {
     constexpr int VV = decltype(V)::value;
-    const auto kern = tma ? find_kernel_tma<VV, true> : find_kernel_tma<VV, false>;
-    const int grid = grid_for(n, kTileKeys, t->sm_count, occupancy_of(kern, kThreads));
-    DET_LAUNCH(kern, grid, kThreads, 0, s, v, (const long long*)keys, n, (const unsigned char*)defaults, full_size_default,
-               (unsigned char*)values_out, exists, g, h);
+    if (keyed) {
+      const auto kern = tma ? find_kernel_tma<VV, true, true> : find_kernel_tma<VV, false, true>;
+      InitArg<true> ki{};
+      static_cast<KeyedInit&>(ki) = t->init;
+      const int grid = grid_for(n, kTileKeys, t->sm_count, occupancy_of(kern, kThreads));
+      DET_LAUNCH(kern, grid, kThreads, 0, s, v, (const long long*)keys, n, nullptr, 0, (unsigned char*)values_out, exists, g,
+                 h, ki);
+    } else {
+      const auto kern = tma ? find_kernel_tma<VV, true> : find_kernel_tma<VV, false>;
+      const int grid = grid_for(n, kTileKeys, t->sm_count, occupancy_of(kern, kThreads));
+      DET_LAUNCH(kern, grid, kThreads, 0, s, v, (const long long*)keys, n, (const unsigned char*)defaults, full_size_default,
+                 (unsigned char*)values_out, exists, g, h, InitArg<false>());
+    }
     CUDA_TRY(cudaGetLastError());
     if (h.keys != nullptr) CUDA_TRY(cudaEventRecord(t->hint_ev, s));
     return DET_OK;
   });
+}
+
+det_status det_table_set_initializer(det_table* t, const det_initializer* init) {
+  if (!t) return fail(DET_INVALID_ARGUMENT, "det_table_set_initializer: null table");
+  if (init) {
+    const int vt = t->cfg.value_dtype;
+    if (vt != DET_FLOAT32 && vt != DET_FLOAT16 && vt != DET_BFLOAT16)
+      return fail(DET_INVALID_ARGUMENT, "det_table_set_initializer: float32, float16 and bfloat16 tables only");
+    if (init->kind < DET_INIT_UNIFORM || init->kind > DET_INIT_TRUNCATED_NORMAL)
+      return fail(DET_INVALID_ARGUMENT, "det_table_set_initializer: unknown kind " + std::to_string(init->kind));
+    if (!std::isfinite(init->a) || !std::isfinite(init->b))
+      return fail(DET_INVALID_ARGUMENT, "det_table_set_initializer: parameters must be finite");
+    if (init->kind != DET_INIT_UNIFORM && init->b < 0.f)
+      return fail(DET_INVALID_ARGUMENT, "det_table_set_initializer: stddev must be >= 0");
+  }
+  det::MutLock _lk(t);
+  std::unique_lock<std::shared_mutex> _vl(t->view_mu);   // a find copies the initializer under the shared lock
+  t->keyed = init != nullptr;
+  if (init) {
+    t->init.kind = init->kind;
+    t->init.elem = t->cfg.value_dtype == DET_FLOAT32 ? 0 : t->cfg.value_dtype == DET_FLOAT16 ? 1 : 2;
+    t->init.seed_lo = (unsigned)(init->seed & 0xffffffffull);
+    t->init.seed_hi = (unsigned)(init->seed >> 32);
+    t->init.a = init->a;
+    t->init.b = init->b;
+  }
+  return DET_OK;
 }
 
 det_status det_insert(det_table* t, const int64_t* keys, const void* values, size_t n, det_stream_t stream) {

@@ -6,6 +6,7 @@ from .table import (CuckooHashTable, CuckooHashTableConfig, CuckooHashTableCreat
 from .variable import (GraphKeys, ModelMode, TrainableWrapper, Variable, default_partition_fn, embedding_lookup,
                        embedding_lookup_unique, enable_inference_mode, enable_train_mode, get_model_mode, get_variable,
                        load_de_variable_from_file_system, make_partition, segment_reduce, trainable_wrapper_filter, unique)
+from .keyed_init import KeyedRandomNormal, KeyedRandomUniform, KeyedTruncatedNormal
 from .ops import SparseIds, embedding_lookup_sparse, safe_embedding_lookup_sparse
 from .optimizer import ComposedOptimizer, DynamicEmbeddingOptimizer, FusedAdagrad, FusedAdam, FusedFtrl, FusedSGD, SlotPlane
 from .restrict_policies import FrequencyRestrictPolicy, RestrictPolicy, TimestampRestrictPolicy
@@ -24,4 +25,5 @@ __all__ = [
     "RestrictPolicy", "TimestampRestrictPolicy", "FrequencyRestrictPolicy", "TrainableWrapper", "ModelMode",
     "enable_inference_mode", "enable_train_mode", "get_model_mode", "trainable_wrapper_filter", "shadow_ops",
     "ComposedOptimizer", "SlotPlane", "math", "data_flow", "keras", "GraphKeys", "FileSystemSaver", "FileSystemSaverConfig", "DynamicEmbeddingSaver",
+    "KeyedRandomNormal", "KeyedRandomUniform", "KeyedTruncatedNormal",
 ]

@@ -127,6 +127,8 @@ class AllToAllEmbedding(torch.nn.Module):
     base layer's) are accepted; the world size comes from `group`, lookups always dedupe once (unique -> one-sided
     find), and a published shard has a FIXED capacity: capacity_per_shard (default: init_capacity, else 1M slots)."""
     super().__init__()
+    from .keyed_init import refuse_keyed
+    refuse_keyed(initializer, "AllToAllEmbedding")
     if key_dtype != torch.int64 or value_dtype != torch.float32:
       raise TypeError("AllToAllEmbedding: int64 keys and float32 rows")
     self.embedding_size = int(embedding_size)

@@ -47,9 +47,10 @@ def lookup_sparse_fused(params, ids, segment_ids, weights, batch, combiner, defa
   ids = ids.reshape(-1).to(dev).contiguous()
   seg = segment_ids.reshape(-1).to(device=dev, dtype=torch.int32).contiguous()
   w = None if weights is None else weights.reshape(-1).to(device=dev, dtype=torch.float32).contiguous()
-  if default_row is None:
+  if default_row is None and table.keyed_initializer is None:
     default_row = table._default_value
-  default_row = default_row.to(device=dev, dtype=torch.float32).contiguous()
+  if default_row is not None:   # None: the kernels generate missing rows from the table's keyed initializer
+    default_row = default_row.to(device=dev, dtype=torch.float32).contiguous()
   out = torch.empty((batch, params.dim), dtype=torch.float32, device=dev)
   if max_norm is not None:
     _lib.check(_lib.lib().det_lookup_sparse_clip(table.handle, _ptr(ids), _ptr(seg), _ptr(w), ids.numel(), batch,
@@ -119,7 +120,7 @@ def embedding_lookup_sparse(params, sp_ids, sp_weights, partition_strategy=None,
   kernel, which widens half rows to float32 as it reads them (the reference casts them right after the lookup, so the
   result is the same).  `max_norm` is folded into the gather for float32 rows of up to 32 vectors; a half variable with
   `max_norm` takes the composed path, which clips in the variable's dtype as the reference does;
-  `return_trainable=True`, sharded variables and random initializers take the composed
+  `return_trainable=True`, sharded variables and callable random initializers take the composed
   path (unique -> lookup -> gather*weights -> segment sum), exactly the reference's op sequence."""
   if combiner not in ("mean", "sqrtn", "sum"):
     raise ValueError("combiner must be one of 'mean', 'sqrtn' or 'sum'")
@@ -137,6 +138,7 @@ def embedding_lookup_sparse(params, sp_ids, sp_weights, partition_strategy=None,
   ids = sp_ids.values
   batch = sp_ids.dense_shape[0]
   weights = None if ignore_weights else sp_weights.values
+  # constant and keyed initializers are fusable; a callable draws per lookup and takes the composed path
   static_default = params.initializer is None or not callable(params.initializer)
   if not return_trainable and static_default and _fused_ok(params, params.tables[0]._default_value) and \
       (max_norm is None or (float(max_norm) > 0 and _clip_fusable(params.dim, params.value_dtype))):

@@ -24,7 +24,11 @@ _FUSED_DTYPES = (torch.float32, torch.float16, torch.bfloat16)
 def _init_rows(params, n, device):
   """The rows a missing key starts from: the variable's initializer, evaluated like
   Variable._create_default_values_by_initializer (one row per key when it is callable), in float32 -- the kernels take
-  init rows in float32 whatever the variable's dtype, and widening float16 / bfloat16 rows is exact."""
+  init rows in float32 whatever the variable's dtype, and widening float16 / bfloat16 rows is exact.  None for a keyed
+  initializer: the kernels generate a new key's row from it."""
+  from .keyed_init import is_keyed
+  if is_keyed(params.initializer):
+    return None, 0
   dyn = params._create_default_values_by_initializer(n, device)
   if dyn is not None and dyn.numel() == n * params.dim:
     return dyn.reshape(n, params.dim).to(torch.float32).contiguous(), 1
@@ -168,7 +172,7 @@ class _FusedBase(object):
     """one step from row gradients whose ids may repeat: gradients of the same id are summed first
     (`_resource_apply_sparse_duplicate_indices` -> `_deduplicate_indexed_slices`, the path the reference takes for
     IndexedSlices gradients, dynamic_embedding_optimizer.py:150,184), then the fused step runs on the unique ids.
-    Single-shard fp32 / fp16 / bf16 variables with a static initializer take ONE C call (det_apply_*_dup): unique -> position-order
+    Single-shard fp32 / fp16 / bf16 variables with a constant or keyed initializer take ONE C call (det_apply_*_dup): unique -> position-order
     gradient sum -> fused find-or-insert step, the unique count never leaves the device (no host synchronisation)."""
     ids = ids.reshape(-1)
     grads = grads.reshape(-1, params.dim).to(torch.float32).contiguous()
@@ -188,7 +192,7 @@ class _FusedBase(object):
         raw = torch.empty(need + need // 8 + 256, dtype=torch.uint8, device=t.device)
         off = (-raw.data_ptr()) % 256          # the C ABI wants a 256 B aligned workspace (CUDA allocations already are)
         ws = self._dup_ws = raw[off:off + need + need // 8]
-      init = t._default_value.to(device=t.device, dtype=torch.float32).contiguous()
+      init = None if t.keyed_initializer is not None else t._default_value.to(device=t.device, dtype=torch.float32).contiguous()
       self._apply_table_dup(t, ids, grads, n, init, ws)
       return
     from .variable import combine_rows, unique

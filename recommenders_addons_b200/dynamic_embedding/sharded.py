@@ -54,6 +54,8 @@ class ShardedVariable(object):
 
   def __init__(self, local_variable, group=None, partition_impl=None, gather_impl=None, scatter_impl=None,
                unique_impl=None):
+    from .keyed_init import refuse_keyed
+    refuse_keyed(getattr(local_variable, "initializer", None), "ShardedVariable")
     self.local = local_variable
     self._unique = unique_impl
     self.group = group
@@ -128,6 +130,8 @@ class PeerShardedVariable(object):
     det_peer_xchg_apply_* -- the step's find-or-insert makes room (evict_room) and writes the scores -- and upsert() as
     det_peer_xchg_insert, where the owner compacts what arrived and runs its own scored insert (one host sync per
     call).  The one-sided kernels are refused by the library (DESIGN.md 4b)."""
+    from .keyed_init import refuse_keyed
+    refuse_keyed(initializer, "PeerShardedVariable")
     import torch.distributed._symmetric_memory as symm_mem
     from .table import CuckooHashTable
     from .variable import Variable
@@ -235,6 +239,8 @@ class PeerShardedVariable(object):
 
   def _init_common(self, local_variable, group, gpu_mode):
     from .. import _lib
+    from .keyed_init import refuse_keyed
+    refuse_keyed(getattr(local_variable, "initializer", None), "PeerShardedVariable")
     self._lib = _lib.lib()
     self._libmod = _lib
     self.local = local_variable

@@ -280,13 +280,30 @@ class CuckooHashTable(object):
   def clear(self, name=None):
     _lib.check(self._lib.det_clear(self._h, _stream_ptr(self._device)))
 
+  def set_initializer(self, initializer):
+    """a keyed random initializer (de.KeyedRandomNormal, ...) the kernels generate missing rows from, or None to clear it"""
+    _lib.check(self._lib.det_table_set_initializer(self._h, None if initializer is None else
+                                                   ctypes.byref(initializer.c_struct())))
+    self._keyed_init = initializer   # only once the library has accepted it
+
+  @property
+  def keyed_initializer(self):
+    return getattr(self, "_keyed_init", None)
+
   def lookup(self, keys, dynamic_default_values=None, return_exists=False, name=None):
     """Find / FindWithExists.  Values have shape keys.shape + [dim]; a missing key gets the default
-    row: dynamic_default_values[i] if it is full-size, else its first row, else the static default."""
+    row: dynamic_default_values[i] if it is full-size, else its first row, else the row of the table's keyed
+    initializer, else the static default."""
     keys = self._check_keys(keys)
     shape = tuple(keys.shape)
     flat = keys.reshape(-1)
     n = flat.numel()
+    if dynamic_default_values is None and self.keyed_initializer is not None:
+      values = torch.empty(shape + (self._dim,), dtype=self._value_dtype, device=self._device)
+      exists = torch.empty(shape, dtype=torch.bool, device=self._device) if return_exists else None
+      _lib.check(self._lib.det_find(self._h, _ptr(flat), n, None, 0, _ptr(values), _ptr(exists),
+                                    _stream_ptr(self._device)))
+      return (values, exists) if return_exists else values
     default = self._default_value if dynamic_default_values is None else dynamic_default_values
     if not torch.is_tensor(default):
       default = torch.as_tensor(default, dtype=self._value_dtype)

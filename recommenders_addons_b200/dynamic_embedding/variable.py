@@ -186,7 +186,10 @@ class Variable(object):
       raise TypeError("config should be instance of 'config', but got %s" % type(self.kv_creator))
     if key_dtype != torch.int64:
       raise TypeError("key-value dtype (%s-%s) is not support! keys must be int64 on GPU" % (key_dtype, value_dtype))
-    static_default = self._convert_anything_to_init(initializer, self.dim)
+    from .keyed_init import is_keyed
+    # a keyed initializer is set on every shard table below; the static default row is then never read
+    static_default = torch.zeros(self.dim, dtype=value_dtype) if is_keyed(initializer) else \
+        self._convert_anything_to_init(initializer, self.dim)
     self._tables = []
     for idx, dev in enumerate(self.devices):
       self._tables.append(
@@ -194,6 +197,8 @@ class Variable(object):
                                  name=self._make_name(idx), checkpoint=checkpoint,
                                  init_size=int(self.init_size / self.shard_num), device=dev,
                                  num_slot_planes=num_slot_planes))
+      if is_keyed(initializer):
+        self._tables[-1].set_initializer(initializer)
     # dynamic_embedding_variable.py:604-611
     if restrict_policy is not None:
       from .restrict_policies import RestrictPolicy
@@ -292,7 +297,8 @@ class Variable(object):
       t.clear()
 
   def _create_default_values_by_initializer(self, n, device):
-    """:919-931: a callable initializer yields one default row per looked-up key ([n, dim])."""
+    """:919-931: a callable initializer yields one default row per looked-up key ([n, dim]).  None for a constant or
+    keyed initializer (the kernels generate a keyed initializer's rows)."""
     if self.initializer is None or not callable(self.initializer):
       return None
     try:
