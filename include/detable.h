@@ -354,6 +354,49 @@ det_status det_apply_ftrl_dup(det_table* t, const int64_t* ids, const float* gra
                               float l2, float l2_shrinkage, const float* init_param, float init_accum, void* workspace,
                               size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream);
 
+/* The backward of det_lookup_sparse, fused: per-unique-id gradients straight from the output gradient (ABI >= 8).
+ * Inputs are the forward's ids int64[nnz], segment_ids int32[nnz] (ascending, in [0, batch)), weights f32[nnz] or NULL
+ * and combiner, and gout f32[batch, dim] = dL/d(output).  The rule:
+ *   den_b = the forward's normaliser of segment b, summed as the forward sums it: in id order from +0, the weights for
+ *           DET_COMBINER_MEAN, sqrtf of the weights' squares for DET_COMBINER_SQRTN; none for DET_COMBINER_SUM;
+ *   c_i   = w_i / den_{seg_i} (w_i = 1 without weights; c_i = w_i for DET_COMBINER_SUM), one IEEE division;
+ *   g_i   = gout[seg_i, :] * c_i, one multiply per element;
+ *   the gradient of a unique id (det_unique's first-occurrence order) = its g_i added in increasing position from 0.
+ * den = 0 gives what IEEE division gives (inf / NaN), as in the forward.  The [nnz, dim] g_i are never materialised.
+ * Malformed segment ids (not ascending, or outside [0, batch)) make every gradient NaN.
+ * nnz == 0 is DET_OK (the count is 0); NULL ids, segment_ids or gout, a bad combiner, or batch == 0 with nnz > 0 are
+ * DET_INVALID_ARGUMENT.
+ *
+ * det_lookup_sparse_grad: the backward alone, no table.  unique_out int64[nnz], grads_out f32[nnz, dim] (the first
+ * *n_unique_dev rows are written), n_unique_dev: device int64.  Any dim.  workspace:
+ * det_lookup_sparse_grad_workspace_bytes(nnz, batch, dim) bytes of device memory, 256 B aligned. */
+size_t det_lookup_sparse_grad_workspace_bytes(size_t nnz, size_t batch, size_t dim);
+det_status det_lookup_sparse_grad(const int64_t* ids, const int32_t* segment_ids, const float* weights, size_t nnz,
+                                  size_t batch, int combiner, const float* gout, size_t dim, int64_t* unique_out,
+                                  float* grads_out, int64_t* n_unique_dev, void* workspace, size_t workspace_bytes,
+                                  det_stream_t stream);
+/* det_apply_*_sparse: the backward above chained into the fused optimizer step of the matching det_apply_*_dup, in
+ * one call with the unique count on the device (no host synchronisation).  Hyper-parameters, init_param (NULL on a
+ * table with a keyed initializer), value dtypes, row limits, eviction scores and refusals: as det_apply_*_dup.
+ * workspace: det_apply_sparse_workspace_bytes(nnz, batch, dim) bytes, 256 B aligned. */
+size_t det_apply_sparse_workspace_bytes(size_t nnz, size_t batch, size_t dim);
+det_status det_apply_adagrad_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
+                                    size_t nnz, size_t batch, int combiner, const float* gout, float lr, float epsilon,
+                                    const float* init_param, float init_accum, void* workspace, size_t workspace_bytes,
+                                    int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_adam_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
+                                 size_t nnz, size_t batch, int combiner, const float* gout, float alpha, float beta1,
+                                 float beta2, float epsilon, const float* init_param, void* workspace,
+                                 size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_sgd_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
+                                size_t nnz, size_t batch, int combiner, const float* gout, float lr, float momentum,
+                                int nesterov, const float* init_param, void* workspace, size_t workspace_bytes,
+                                int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_ftrl_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
+                                 size_t nnz, size_t batch, int combiner, const float* gout, float lr, float l1, float l2,
+                                 float l2_shrinkage, const float* init_param, float init_accum, void* workspace,
+                                 size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream);
+
 /* ---- key-hash sharding across GPUs (python/ops/dynamic_embedding_variable.py:165-197 default_partition_fn,
  * python/ops/shadow_embedding_ops.py:397-447 alltoall exchange) ----
  * Partition n keys into num_shards contiguous groups by owner = (key & 0x7fffffff) % S (gpu_mode)

@@ -1484,13 +1484,67 @@ __global__ void group_long_kernel(const unsigned* __restrict__ starts, unsigned 
   else if (len > (unsigned)kLongGroup) long_list[atomicAdd(&ctr[0], 1u)] = (unsigned)g;
 }
 
-template <int VF>
+// The sparse backward's coefficients: for every id i of segment b, coef[i] = (b, c_i) with c_i = w_i / den_b (w_i = 1
+// without weights; c_i = w_i for "sum").  den_b is the forward's normaliser (segment_sum_kernel), summed the same way:
+// in id order from +0, sqrtf of the sum of w*w for "sqrtn".  Bags are short: one thread walks one segment.
+// Malformed segment ids (flagged in `st` by segment_offsets_kernel, which then leaves seg_start incomplete) give every
+// id the pair (0, NaN): the gradients are NaN and no row outside gout is read.
+__global__ void segment_coef_kernel(const long long* __restrict__ seg_start, const float* __restrict__ weights,
+                                    size_t nnz, size_t batch, int combiner, const DevState* __restrict__ st,
+                                    int2* __restrict__ coef) {
+  const size_t t0 = (size_t)blockIdx.x * blockDim.x + threadIdx.x, stride = (size_t)gridDim.x * blockDim.x;
+  if (st->error & kErrBadSegment) {
+    for (size_t i = t0; i < nnz; i += stride) coef[i] = make_int2(0, 0x7fc00000);
+    return;
+  }
+  for (size_t b = t0; b < batch; b += stride) {
+    const long long st = seg_start[b], en = seg_start[b + 1];
+    float den = 1.f;
+    if (combiner != DET_COMBINER_SUM) {
+      float wsum = 0.f, wsq = 0.f;
+      for (long long i = st; i < en; ++i) {
+        const float w = weights ? __ldg(weights + i) : 1.f;
+        wsum = wsum + w;
+        wsq = wsq + w * w;
+      }
+      den = combiner == DET_COMBINER_MEAN ? wsum : sqrtf(wsq);
+    }
+    for (long long i = st; i < en; ++i) {
+      const float w = weights ? __ldg(weights + i) : 1.f;
+      const float c = combiner == DET_COMBINER_SUM ? w : w / den;
+      coef[i] = make_int2((int)b, __float_as_int(c));
+    }
+  }
+}
+
+// The row source of the sparse backward (det_lookup_sparse_grad, det_apply_*_sparse): the row of position p is
+// gout[seg_p] * c_p, read through the (seg_p, c_p bits) pair segment_coef_kernel wrote -- one 8 B load per position.
+// An EMPTY trailing kernel parameter when unused, so the plain kernel (rows[p]) is unchanged.
+template <bool GATHER> struct GatherArg {};
+template <> struct GatherArg<true> { const int2* coef; };
+// positions whose coefficient one staged tile keeps in shared memory: a double-buffered tile holds up to
+// kLongTileFloats / 2 / 4 rows (4-column rows), the single-buffered one kLongTileRows
+constexpr int kCoefTileRows = kLongTileFloats / 8;
+
+// position p -> (the row index, its coefficient): the gathered source reads the pair, the plain one the position itself
+template <bool GATHER>
+__device__ __forceinline__ unsigned gather_row(const GatherArg<GATHER>& ga, unsigned p, float& c) {
+  if constexpr (GATHER) {
+    const int2 sc = __ldg(ga.coef + p);
+    c = __int_as_float(sc.y);
+    return (unsigned)sc.x;
+  } else {
+    return p;
+  }
+}
+
+template <int VF, bool GATHER = false>
 __global__ void __launch_bounds__(kThreadsF)
 segment_reduce_kernel(const float* __restrict__ rows, const unsigned* __restrict__ pos,
                       const unsigned* __restrict__ starts, unsigned n_groups, unsigned dim, unsigned vpr, unsigned lpr,
                       unsigned lpr_shift, const unsigned* __restrict__ long_list, const unsigned* __restrict__ huge_list,
                       unsigned* __restrict__ ctr, int n_long_ctas, float* __restrict__ out,
-                      const long long* __restrict__ ngd) {
+                      const long long* __restrict__ ngd, GatherArg<GATHER> ga = GatherArg<GATHER>()) {
   if (ngd) n_groups = (unsigned)*ngd;
   if ((int)blockIdx.x < n_long_ctas) {
     // ---- long groups: a CTA per work item, rows staged tile by tile, thread c adds column c in position order ----
@@ -1501,6 +1555,8 @@ segment_reduce_kernel(const float* __restrict__ rows, const unsigned* __restrict
     __shared__ __align__(16) float s_rows[kLongTileFloats];
     __shared__ unsigned s_pos[kLongTileRows];
     __shared__ unsigned s_q;
+    // GATHER: the coefficient of every staged row (two tiles of the double-buffered path, or one of kLongTileRows)
+    __shared__ float s_c[GATHER ? 2 * kCoefTileRows : 1];
     const unsigned n_long = ctr[0], n_huge = ctr[1];
     const unsigned slices = dim / (unsigned)kSliceCols;          // only used when huge groups exist (sliceable rows)
     const unsigned n_huge_items = n_huge * slices;
@@ -1535,7 +1591,8 @@ segment_reduce_kernel(const float* __restrict__ rows, const unsigned* __restrict
           constexpr unsigned kHalf = kLongTileFloats / 2;
           const unsigned rp2 = kHalf / wcols;                               // rows per tile (>= 4)
           const unsigned ntiles = (en - st + rp2 - 1) / rp2;
-          unsigned pp[4];
+          unsigned pp[4];     // the row index of every vector this thread stages (GATHER: its segment)
+          float pc[4];        // GATHER: its coefficient
           auto load_pos = [&](unsigned tile) {
             const unsigned tb = st + tile * rp2;
             const unsigned m = tile < ntiles ? (en - tb < rp2 ? en - tb : rp2) : 0u;
@@ -1543,6 +1600,7 @@ segment_reduce_kernel(const float* __restrict__ rows, const unsigned* __restrict
             for (int i = 0; i < 4; ++i) {
               const unsigned f = threadIdx.x + (unsigned)i * kThreadsF;
               pp[i] = f < m * wv ? __ldg(pos + tb + f / wv) : 0xffffffffu;
+              if (GATHER && pp[i] != 0xffffffffu) pp[i] = gather_row(ga, pp[i], pc[i]);
             }
           };
           auto issue = [&](unsigned tile) {
@@ -1551,8 +1609,11 @@ segment_reduce_kernel(const float* __restrict__ rows, const unsigned* __restrict
             for (int i = 0; i < 4; ++i) {
               const unsigned f = threadIdx.x + (unsigned)i * kThreadsF;
               const unsigned r = f / wv, cv = f - r * wv;
-              if (pp[i] != 0xffffffffu)
+              if (pp[i] != 0xffffffffu) {
                 cp_async16(buf + (size_t)r * wcols + (size_t)cv * 4, rows + (size_t)pp[i] * dim + c0 + (size_t)cv * 4);
+                // this tile's half of s_c was last read before the barrier that ended tile - 2
+                if (GATHER && cv == 0) s_c[(tile & 1u) * kCoefTileRows + r] = pc[i];
+              }
             }
             cp_async_commit();
           };
@@ -1572,7 +1633,12 @@ segment_reduce_kernel(const float* __restrict__ rows, const unsigned* __restrict
               const unsigned c = threadIdx.x + (unsigned)a * kThreadsF;
               if (c < wcols) {
                 float sacc = acc[a];
-                for (unsigned r = 0; r < m; ++r) sacc = sacc + buf[(size_t)r * wcols + c];
+                if constexpr (GATHER) {
+                  const float* cf = s_c + (j & 1u) * kCoefTileRows;
+                  for (unsigned r = 0; r < m; ++r) sacc = sacc + buf[(size_t)r * wcols + c] * cf[r];
+                } else {
+                  for (unsigned r = 0; r < m; ++r) sacc = sacc + buf[(size_t)r * wcols + c];
+                }
                 acc[a] = sacc;
               }
             }
@@ -1582,7 +1648,13 @@ segment_reduce_kernel(const float* __restrict__ rows, const unsigned* __restrict
         } else {
           for (unsigned base = st; base < en; base += rpt) {
             const unsigned m = en - base < rpt ? en - base : rpt;
-            for (unsigned r = threadIdx.x; r < m; r += kThreadsF) s_pos[r] = pos[base + r];
+            for (unsigned r = threadIdx.x; r < m; r += kThreadsF) {
+              if constexpr (GATHER) {
+                s_pos[r] = gather_row(ga, pos[base + r], s_c[r]);
+              } else {
+                s_pos[r] = pos[base + r];
+              }
+            }
             __syncthreads();
             const unsigned total = m * wv;
   #pragma unroll 4
@@ -1590,6 +1662,10 @@ segment_reduce_kernel(const float* __restrict__ rows, const unsigned* __restrict
               const unsigned r = f / wv, cv = f - r * wv;
               FVec<VF> x;
               x.load(rows + (size_t)s_pos[r] * dim + c0 + (size_t)cv * VF);
+              if constexpr (GATHER) {   // staged as the product: the sum below then adds x * c in position order
+                const float cr = s_c[r];
+                x.apply([cr](float& a) { a = a * cr; });
+              }
               x.store(s_rows + (size_t)r * wcols + (size_t)cv * VF);
             }
             __syncthreads();
@@ -1657,11 +1733,15 @@ segment_reduce_kernel(const float* __restrict__ rows, const unsigned* __restrict
         for (int u = 0; u < U; ++u) any |= st[u] + k < en[u];
         if (!__any_sync(kFull, any)) break;
         unsigned p[U][K];
+        float c[U][K];      // GATHER: the coefficient of each row
         FVec<VF> x[U][K];
 #pragma unroll
         for (int u = 0; u < U; ++u)
 #pragma unroll
-          for (int q = 0; q < K; ++q) p[u][q] = st[u] + k + q < en[u] ? __ldg(pos + st[u] + k + q) : 0xffffffffu;
+          for (int q = 0; q < K; ++q) {
+            p[u][q] = st[u] + k + q < en[u] ? __ldg(pos + st[u] + k + q) : 0xffffffffu;
+            if (GATHER && p[u][q] != 0xffffffffu) p[u][q] = gather_row(ga, p[u][q], c[u][q]);
+          }
 #pragma unroll
         for (int u = 0; u < U; ++u)
 #pragma unroll
@@ -1673,7 +1753,14 @@ segment_reduce_kernel(const float* __restrict__ rows, const unsigned* __restrict
         for (int u = 0; u < U; ++u)
 #pragma unroll
           for (int q = 0; q < K; ++q)
-            if (p[u][q] != 0xffffffffu) acc[u].zip(x[u][q], [](float& a, float xv) { a = a + xv; });
+            if (p[u][q] != 0xffffffffu) {
+              if constexpr (GATHER) {
+                const float cq = c[u][q];
+                acc[u].zip(x[u][q], [cq](float& a, float xv) { a = a + xv * cq; });
+              } else {
+                acc[u].zip(x[u][q], [](float& a, float xv) { a = a + xv; });
+              }
+            }
       }
 #pragma unroll
       for (int u = 0; u < U; ++u)
@@ -2221,10 +2308,12 @@ size_t det_segment_reduce_workspace_bytes(size_t n, size_t n_groups) {
   return seg_reduce_layout(n ? n : 1, n_groups ? n_groups : 1, nullptr, nullptr);
 }
 
-// n_groups bounds the group count (sizes, pass count, grids); with `ngd` the real count is read on the device
+// n_groups bounds the group count (sizes, pass count, grids); with `ngd` the real count is read on the device.
+// coef (nullable): the sparse backward's (segment, coefficient) pair of every position -- the row of position p is then
+// rows[seg_p] * c_p, rows being the output gradient of the forward
 static det_status seg_reduce_run(const float* rows, const int32_t* idx, size_t n, size_t n_groups, size_t dim, float* out,
                                  void* workspace, size_t workspace_bytes, const long long* ngd, cudaStream_t s,
-                                 const long long* n_dev = nullptr) {
+                                 const long long* n_dev = nullptr, const int2* coef = nullptr) {
   if (n_groups == 0 || dim == 0) return DET_OK;
   if (!out) return fail(DET_INVALID_ARGUMENT, "det_segment_reduce: null out");
   if (n >= 0x7fffffffull || n_groups >= 0x7fffffffull || dim >= 0x7fffffffull)
@@ -2268,16 +2357,22 @@ static det_status seg_reduce_run(const float* rows, const int32_t* idx, size_t n
   const unsigned gpw = 32u >> sh;
   // CTAs of the launch reserved for the long groups
   const int n_long_ctas = 2 * sms;
-  const auto k4 = segment_reduce_kernel<4>;
-  const auto k1 = segment_reduce_kernel<1>;
-  const int occ = vec4 ? occupancy_of(k4, kThreadsF) : occupancy_of(k1, kThreadsF);
   // one resident wave: the long-path CTAs (blockIdx < n_long_ctas) plus the short-group CTAs that still fit beside them
   const int long_per_sm = (n_long_ctas + sms - 1) / sms;
-  const int grid = n_long_ctas + grid_for(n_groups, (int)(gpw * 2 * (kThreadsF / 32)), sms, occ > long_per_sm ? occ - long_per_sm : 1);
-  if (vec4)
-    DET_LAUNCH(k4, grid, kThreadsF, 0, s, rows, pin, w.starts, ng, (unsigned)dim, vpr, lpr, sh, w.long_list, w.huge_list, w.n_long, n_long_ctas, out, ngd);
-  else
-    DET_LAUNCH(k1, grid, kThreadsF, 0, s, rows, pin, w.starts, ng, (unsigned)dim, vpr, lpr, sh, w.long_list, w.huge_list, w.n_long, n_long_ctas, out, ngd);
+  dispatch_bit(coef != nullptr, [&](auto G) -> det_status {
+    constexpr bool kGather = decltype(G)::value;
+    GatherArg<kGather> ga;
+    if constexpr (kGather) ga.coef = coef;
+    const auto k4 = segment_reduce_kernel<4, kGather>;
+    const auto k1 = segment_reduce_kernel<1, kGather>;
+    const int occ = vec4 ? occupancy_of(k4, kThreadsF) : occupancy_of(k1, kThreadsF);
+    const int grid = n_long_ctas + grid_for(n_groups, (int)(gpw * 2 * (kThreadsF / 32)), sms, occ > long_per_sm ? occ - long_per_sm : 1);
+    if (vec4)
+      DET_LAUNCH(k4, grid, kThreadsF, 0, s, rows, pin, w.starts, ng, (unsigned)dim, vpr, lpr, sh, w.long_list, w.huge_list, w.n_long, n_long_ctas, out, ngd, ga);
+    else
+      DET_LAUNCH(k1, grid, kThreadsF, 0, s, rows, pin, w.starts, ng, (unsigned)dim, vpr, lpr, sh, w.long_list, w.huge_list, w.n_long, n_long_ctas, out, ngd, ga);
+    return DET_OK;
+  });
   CUDA_TRY(cudaGetLastError());
   return DET_OK;
 }
@@ -2305,8 +2400,14 @@ struct DupWs {
   float* gsum;
   unsigned char* sws;
   size_t sws_bytes;
+  // the sparse backward (batch > 0): segment starts [batch + 1], the (segment, coefficient) pair of every id, and the
+  // DevState segment_offsets_kernel reports malformed segment ids into when no table is involved
+  long long* seg_start;
+  int2* coef;
+  DevState* st;
 };
-static size_t dup_layout(size_t n, size_t dim, unsigned char* base, DupWs* w) {
+// dim == 0: no gradient-sum buffer (det_lookup_sparse_grad writes the caller's)
+static size_t dup_layout(size_t n, size_t dim, unsigned char* base, DupWs* w, size_t batch = 0) {
   WsCarver c(base);
   const size_t ub = unique_ws_layout(n, nullptr, nullptr), sb = seg_reduce_layout(n, n, nullptr, nullptr);
   long long* uniq = c.take<long long>(n * 8);
@@ -2315,20 +2416,101 @@ static size_t dup_layout(size_t n, size_t dim, unsigned char* base, DupWs* w) {
   unsigned char* uws = c.take(ub);
   float* gsum = c.take<float>(n * dim * 4);
   unsigned char* sws = c.take(sb);
+  long long* seg_start = nullptr;
+  int2* coef = nullptr;
+  DevState* st = nullptr;
+  if (batch) {
+    seg_start = c.take<long long>((batch + 1) * 8);
+    coef = c.take<int2>(n * 8);
+    st = c.take<DevState>(sizeof(DevState));
+  }
   if (w) {
     w->uniq = uniq; w->idx = idx; w->cnt = cnt; w->uws = uws; w->uws_bytes = ub;
     w->gsum = gsum; w->sws = sws; w->sws_bytes = sb;
+    w->seg_start = seg_start; w->coef = coef; w->st = st;
   }
   return c.off;
 }
 
 size_t det_apply_dup_workspace_bytes(size_t n, size_t dim) { return dup_layout(n ? n : 1, dim ? dim : 1, nullptr, nullptr); }
 
+// ---- the backward of det_lookup_sparse: per-unique-id gradients straight from the output gradient ----------------
+// The forward's ids, segment ids, weights and combiner, and gout [batch, dim] = dL/d(output).  d row(id) = the sum, over
+// the positions i holding the id, in increasing i, of gout[seg_i] * c_i (segment_coef_kernel): det_unique, the
+// coefficient pass, and K9 reading the gathered rows -- the [nnz, dim] product is never materialised.
+struct SparseSrc {
+  const int32_t* seg;
+  const float* weights;
+  size_t batch;
+  int combiner;
+};
+
+static det_status check_sparse(const int64_t* ids, const SparseSrc& sp, size_t nnz, const float* gout, const char* who) {
+  const std::string w(who);
+  if (sp.combiner < DET_COMBINER_SUM || sp.combiner > DET_COMBINER_SQRTN)
+    return fail(DET_INVALID_ARGUMENT, w + ": combiner must be one of 'mean', 'sqrtn' or 'sum'");
+  if (!ids || !sp.seg || !gout) return fail(DET_INVALID_ARGUMENT, w + ": null ids, segment_ids or gout");
+  if (sp.batch == 0) return fail(DET_INVALID_ARGUMENT, w + ": batch is 0 but there are ids");
+  if (nnz >= 0x7fffffffull || sp.batch >= 0x7fffffffull) return fail(DET_INVALID_ARGUMENT, w + ": nnz / batch too large");
+  return DET_OK;
+}
+
+// unique ids -> uniq (count -> cnt, on the device); their summed gradients -> gsum [n_unique, dim]
+static det_status sparse_grad_run(const int64_t* ids, const SparseSrc& sp, size_t n, const float* gout, size_t dim,
+                                  const DupWs& w, int64_t* uniq, int64_t* cnt, float* gsum, int sms, cudaStream_t s) {
+  det_status st = unique_run(ids, n, uniq, w.idx, cnt, w.uws, w.uws_bytes, nullptr, s);
+  if (st != DET_OK) return st;
+  CUDA_TRY(cudaMemsetAsync(w.st, 0, sizeof(DevState), s));
+  DET_LAUNCH(segment_offsets_kernel, (int)((n + 1 + 255) / 256), 256, 0, s, sp.seg, n, sp.batch, w.seg_start, w.st,
+             (const unsigned*)nullptr, 0u);
+  DET_LAUNCH(segment_coef_kernel, grid_for(sp.batch > n ? sp.batch : n, 256, sms, 8), 256, 0, s, w.seg_start, sp.weights, n,
+             sp.batch, sp.combiner, w.st, w.coef);
+  return seg_reduce_run(gout, w.idx, n, n, dim, gsum, w.sws, w.sws_bytes, (const long long*)cnt, s, nullptr, w.coef);
+}
+
+size_t det_lookup_sparse_grad_workspace_bytes(size_t nnz, size_t batch, size_t dim) {
+  (void)dim;   // the gradient rows go to the caller's buffer
+  return dup_layout(nnz ? nnz : 1, 0, nullptr, nullptr, batch ? batch : 1);
+}
+
+det_status det_lookup_sparse_grad(const int64_t* ids, const int32_t* segment_ids, const float* weights, size_t nnz,
+                                  size_t batch, int combiner, const float* gout, size_t dim, int64_t* unique_out,
+                                  float* grads_out, int64_t* n_unique_dev, void* workspace, size_t workspace_bytes,
+                                  det_stream_t stream) {
+  cudaStream_t s = (cudaStream_t)stream;
+  if (!n_unique_dev) return fail(DET_INVALID_ARGUMENT, "det_lookup_sparse_grad: null n_unique");
+  if (nnz == 0) {
+    CUDA_TRY(cudaMemsetAsync(n_unique_dev, 0, sizeof(int64_t), s));
+    return DET_OK;
+  }
+  const SparseSrc sp{segment_ids, weights, batch, combiner};
+  det_status st = check_sparse(ids, sp, nnz, gout, "det_lookup_sparse_grad");
+  if (st != DET_OK) return st;
+  if (dim == 0 || dim >= 0x7fffffffull) return fail(DET_INVALID_ARGUMENT, "det_lookup_sparse_grad: dim must be in [1, 2^31)");
+  if (!unique_out || !grads_out || !workspace) return fail(DET_INVALID_ARGUMENT, "det_lookup_sparse_grad: null argument");
+  if (workspace_bytes < det_lookup_sparse_grad_workspace_bytes(nnz, batch, dim))
+    return fail(DET_INVALID_ARGUMENT, "det_lookup_sparse_grad: workspace too small");
+  if (((uintptr_t)workspace & 255u) != 0) return fail(DET_INVALID_ARGUMENT, "det_lookup_sparse_grad: workspace must be 256 B aligned");
+  DupWs w;
+  dup_layout(nnz, 0, (unsigned char*)workspace, &w, batch);
+  return sparse_grad_run(ids, sp, nnz, gout, dim, w, unique_out, n_unique_dev, grads_out, current_sm_count(), s);
+}
+
+size_t det_apply_sparse_workspace_bytes(size_t nnz, size_t batch, size_t dim) {
+  return dup_layout(nnz ? nnz : 1, dim ? dim : 1, nullptr, nullptr, batch ? batch : 1);
+}
+
+// sp (nullable): the ids are those of a det_lookup_sparse call and `grads` is its output gradient [batch, dim]
 static det_status apply_dup(det_table* t, const int64_t* ids, const float* grads, size_t n, OptHyper h,
                             const float* init_param, int opt, void* workspace, size_t workspace_bytes,
-                            int64_t* n_unique_dev_out, cudaStream_t s, const long long* n_items_dev = nullptr) {
+                            int64_t* n_unique_dev_out, cudaStream_t s, const long long* n_items_dev = nullptr,
+                            const SparseSrc* sp = nullptr) {
   if (!t) return fail(DET_INVALID_ARGUMENT, "det_apply_dup: null table");
   if (n == 0) return DET_OK;
+  if (sp) {
+    const det_status cs = check_sparse(ids, *sp, n, grads, "det_apply_*_sparse");
+    if (cs != DET_OK) return cs;
+  }
   if (!ids || !grads || !workspace) return fail(DET_INVALID_ARGUMENT, "det_apply_dup: null argument");
   if (!init_param) {
     bool keyed;
@@ -2340,15 +2522,21 @@ static det_status apply_dup(det_table* t, const int64_t* ids, const float* grads
   }
   if (n >= 0x7fffffffull) return fail(DET_INVALID_ARGUMENT, "det_apply_dup: n too large");
   const size_t dim = (size_t)t->cfg.dim;
-  if (workspace_bytes < det_apply_dup_workspace_bytes(n, dim)) return fail(DET_INVALID_ARGUMENT, "det_apply_dup: workspace too small");
+  if (workspace_bytes < (sp ? det_apply_sparse_workspace_bytes(n, sp->batch, dim) : det_apply_dup_workspace_bytes(n, dim)))
+    return fail(DET_INVALID_ARGUMENT, "det_apply_dup: workspace too small");
   if (((uintptr_t)workspace & 255u) != 0) return fail(DET_INVALID_ARGUMENT, "det_apply_dup: workspace must be 256 B aligned");
   det::DevGuard _dg(t->cfg.device);
   DupWs w;
-  dup_layout(n, dim, (unsigned char*)workspace, &w);
-  // n_items_dev: the id count itself lives on the device (owner side of the sharded backward); n is its bound
-  det_status st = unique_run(ids, n, (int64_t*)w.uniq, w.idx, (int64_t*)w.cnt, w.uws, w.uws_bytes, n_items_dev, s);
-  if (st != DET_OK) return st;
-  st = seg_reduce_run(grads, w.idx, n, n, dim, w.gsum, w.sws, w.sws_bytes, w.cnt, s, n_items_dev);
+  dup_layout(n, dim, (unsigned char*)workspace, &w, sp ? sp->batch : 0);
+  det_status st;
+  if (sp) {
+    st = sparse_grad_run(ids, *sp, n, grads, dim, w, (int64_t*)w.uniq, (int64_t*)w.cnt, w.gsum, t->sm_count, s);
+  } else {
+    // n_items_dev: the id count itself lives on the device (owner side of the sharded backward); n is its bound
+    st = unique_run(ids, n, (int64_t*)w.uniq, w.idx, (int64_t*)w.cnt, w.uws, w.uws_bytes, n_items_dev, s);
+    if (st != DET_OK) return st;
+    st = seg_reduce_run(grads, w.idx, n, n, dim, w.gsum, w.sws, w.sws_bytes, w.cnt, s, n_items_dev);
+  }
   if (st != DET_OK) return st;
   st = apply_common(t, (const int64_t*)w.uniq, w.gsum, n, h, init_param, 0, opt, s, w.cnt);
   if (st != DET_OK) return st;
@@ -2390,6 +2578,54 @@ det_status det_apply_ftrl_dup(det_table* t, const int64_t* ids, const float* gra
   const det_status st = ftrl_hyper(t, lr, l1, l2, l2_shrinkage, init_accum, &h);
   if (st != DET_OK) return st;
   return apply_dup(t, ids, grads, n, h, init_param, 4, workspace, workspace_bytes, n_unique_dev_out, (cudaStream_t)stream);
+}
+
+det_status det_apply_adagrad_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
+                                    size_t nnz, size_t batch, int combiner, const float* gout, float lr, float epsilon,
+                                    const float* init_param, float init_accum, void* workspace, size_t workspace_bytes,
+                                    int64_t* n_unique_dev_out, det_stream_t stream) {
+  OptHyper h;
+  h.lr = lr; h.eps = epsilon; h.beta1 = 0.f; h.beta2 = 0.f; h.init_slot = init_accum;
+  if (t) t->slot_init[1] = init_accum;
+  const SparseSrc sp{segment_ids, weights, batch, combiner};
+  return apply_dup(t, ids, gout, nnz, h, init_param, 0, workspace, workspace_bytes, n_unique_dev_out, (cudaStream_t)stream,
+                   nullptr, &sp);
+}
+
+det_status det_apply_adam_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
+                                 size_t nnz, size_t batch, int combiner, const float* gout, float alpha, float beta1,
+                                 float beta2, float epsilon, const float* init_param, void* workspace,
+                                 size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream) {
+  OptHyper h;
+  h.lr = alpha; h.eps = epsilon; h.beta1 = beta1; h.beta2 = beta2; h.init_slot = 0.f;
+  const SparseSrc sp{segment_ids, weights, batch, combiner};
+  return apply_dup(t, ids, gout, nnz, h, init_param, 1, workspace, workspace_bytes, n_unique_dev_out, (cudaStream_t)stream,
+                   nullptr, &sp);
+}
+
+det_status det_apply_sgd_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
+                                size_t nnz, size_t batch, int combiner, const float* gout, float lr, float momentum,
+                                int nesterov, const float* init_param, void* workspace, size_t workspace_bytes,
+                                int64_t* n_unique_dev_out, det_stream_t stream) {
+  OptHyper h;
+  int opt = 2;
+  const det_status st = sgd_hyper(t, lr, momentum, nesterov, &h, &opt);
+  if (st != DET_OK) return st;
+  const SparseSrc sp{segment_ids, weights, batch, combiner};
+  return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
+                   (cudaStream_t)stream, nullptr, &sp);
+}
+
+det_status det_apply_ftrl_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
+                                 size_t nnz, size_t batch, int combiner, const float* gout, float lr, float l1, float l2,
+                                 float l2_shrinkage, const float* init_param, float init_accum, void* workspace,
+                                 size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream) {
+  OptHyper h;
+  const det_status st = ftrl_hyper(t, lr, l1, l2, l2_shrinkage, init_accum, &h);
+  if (st != DET_OK) return st;
+  const SparseSrc sp{segment_ids, weights, batch, combiner};
+  return apply_dup(t, ids, gout, nnz, h, init_param, 4, workspace, workspace_bytes, n_unique_dev_out, (cudaStream_t)stream,
+                   nullptr, &sp);
 }
 
 }  // extern "C"

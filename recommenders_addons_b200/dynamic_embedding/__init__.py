@@ -7,7 +7,8 @@ from .variable import (GraphKeys, ModelMode, TrainableWrapper, Variable, default
                        embedding_lookup_unique, enable_inference_mode, enable_train_mode, get_model_mode, get_variable,
                        load_de_variable_from_file_system, make_partition, segment_reduce, trainable_wrapper_filter, unique)
 from .keyed_init import KeyedRandomNormal, KeyedRandomUniform, KeyedTruncatedNormal
-from .ops import SparseIds, embedding_lookup_sparse, safe_embedding_lookup_sparse
+from .ops import (SparseIds, SparseLookupTrainable, embedding_lookup_sparse, safe_embedding_lookup_sparse,
+                  trainable_embedding_lookup_sparse)
 from .optimizer import ComposedOptimizer, DynamicEmbeddingOptimizer, FusedAdagrad, FusedAdam, FusedFtrl, FusedSGD, SlotPlane
 from .restrict_policies import FrequencyRestrictPolicy, RestrictPolicy, TimestampRestrictPolicy
 from .sharded import PeerShardedVariable, ShardedVariable
@@ -25,5 +26,6 @@ __all__ = [
     "RestrictPolicy", "TimestampRestrictPolicy", "FrequencyRestrictPolicy", "TrainableWrapper", "ModelMode",
     "enable_inference_mode", "enable_train_mode", "get_model_mode", "trainable_wrapper_filter", "shadow_ops",
     "ComposedOptimizer", "SlotPlane", "math", "data_flow", "keras", "GraphKeys", "FileSystemSaver", "FileSystemSaverConfig", "DynamicEmbeddingSaver",
-    "KeyedRandomNormal", "KeyedRandomUniform", "KeyedTruncatedNormal",
+    "KeyedRandomNormal", "KeyedRandomUniform", "KeyedTruncatedNormal", "SparseLookupTrainable",
+    "trainable_embedding_lookup_sparse",
 ]

@@ -5,6 +5,7 @@ of the UNIQUE rows from the table, autograd produces the gradient of that scratc
 writes the update back with the fused find-or-insert + optimizer kernel."""
 import torch
 
+from .ops import trainable_embedding_lookup_sparse
 from .optimizer import _FUSED_DTYPES, ComposedOptimizer, _FusedBase
 from .sharded import PeerShardedVariable, ShardedVariable
 from .variable import Variable, default_partition_fn, embedding_lookup_unique, gather_unique, unique
@@ -74,6 +75,32 @@ class SquashedEmbedding(Embedding):
 
 
 BasicEmbedding = Embedding  # embedding.py:340-343
+
+
+class SparseEmbedding(Embedding):
+  """Bags of ids -> [batch, embedding_size], combined with `combiner`, trained through the fused kernels:
+  `forward(sp_ids, sp_weights=None)` is `trainable_embedding_lookup_sparse` (the fused embedding_lookup_sparse), and
+  `apply_gradients(optimizer)` steps the table from the output gradient -- one det_apply_*_sparse call per forward with
+  a fused optimizer.  One shard, float32 / float16 / bfloat16 rows, a constant or keyed initializer, embedding_size a
+  multiple of 4 up to 128."""
+
+  def __init__(self, embedding_size, combiner="mean", **kwargs):
+    super().__init__(embedding_size, combiner=combiner, **kwargs)
+
+  def forward(self, sp_ids, sp_weights=None):
+    out, h = trainable_embedding_lookup_sparse(self.params, sp_ids, sp_weights, combiner=self.combiner)
+    if self.training and self.params.trainable:
+      self._wrappers.append(h)
+    return out
+
+  def apply_gradients(self, optimizer):
+    """optimizer: a fused optimizer or DynamicEmbeddingOptimizer(torch optimizer)."""
+    if not isinstance(optimizer, (_FusedBase, ComposedOptimizer)):
+      raise TypeError("use de.DynamicEmbeddingOptimizer(...) / de.FusedAdagrad / de.FusedAdam")
+    gv = [(h.out.grad, h) for h in self._wrappers if h.out.grad is not None]
+    self._wrappers = []
+    if gv:
+      optimizer.apply_gradients(gv)
 
 
 class FieldWiseEmbedding(Embedding):

@@ -170,6 +170,87 @@ def embedding_lookup_sparse(params, sp_ids, sp_weights, partition_strategy=None,
   return (out, tw) if return_trainable else out
 
 
+class SparseLookupTrainable(object):
+  """What a training step needs from one `trainable_embedding_lookup_sparse` call: the forward's inputs (`params`,
+  `ids`, `segment_ids` int32, `weights` or None, `batch`, `combiner`) and its output `out`, whose `.grad` is dL/dout.
+  A fused optimizer turns them into one det_apply_*_sparse call; `ComposedOptimizer` into det_lookup_sparse_grad and
+  its own step."""
+
+  def __init__(self, params, ids, segment_ids, weights, batch, combiner, out):
+    self.params, self.ids, self.segment_ids, self.weights = params, ids, segment_ids, weights
+    self.batch, self.combiner, self.out = int(batch), combiner, out
+
+  def grad_rows(self, gout=None):
+    """(unique ids, their summed gradients [n_unique, dim]) from dL/dout (default: `out.grad`) -- det_lookup_sparse_grad.
+    The unique count is read on the host."""
+    gout = self.out.grad if gout is None else gout
+    dev = self.ids.device
+    gout = gout.to(device=dev, dtype=torch.float32).contiguous()
+    nnz, dim = self.ids.numel(), self.params.dim
+    uniq = torch.empty(nnz, dtype=torch.int64, device=dev)
+    grads = torch.empty((nnz, dim), dtype=torch.float32, device=dev)
+    cnt = torch.zeros(1, dtype=torch.int64, device=dev)
+    lib = _lib.lib()
+    ws_bytes = int(lib.det_lookup_sparse_grad_workspace_bytes(nnz, self.batch, dim))
+    raw = torch.empty(ws_bytes + 256, dtype=torch.uint8, device=dev)
+    off = (-raw.data_ptr()) % 256          # the C ABI wants a 256 B aligned workspace (CUDA allocations already are)
+    ws = raw[off:off + ws_bytes]
+    _lib.check(lib.det_lookup_sparse_grad(_ptr(self.ids), _ptr(self.segment_ids), _ptr(self.weights), nnz, self.batch,
+                                          _lib.COMBINERS[self.combiner], _ptr(gout), dim, _ptr(uniq), _ptr(grads), _ptr(cnt),
+                                          _ptr(ws), ws_bytes, _stream_ptr(dev)))
+    n = int(cnt.item())
+    return uniq[:n], grads[:n]
+
+
+def trainable_embedding_lookup_sparse(params, sp_ids, sp_weights=None, combiner="mean"):
+  """embedding_lookup_sparse for training through the fused kernels: returns (out, SparseLookupTrainable).
+
+  `out` [batch, dim] float32 is the fused forward (det_lookup_sparse).  In TRAIN mode on a trainable variable it is a
+  leaf that requires grad; after backward, `optimizer.apply_gradients([(out.grad, handle)])` turns dL/dout into the
+  per-id gradients and steps the table, with a fused optimizer in one call (det_apply_*_sparse, no host
+  synchronisation).  Per id i of segment b the gradient row is dL/dout[b] * w_i / den_b (den_b: the forward's
+  normaliser), summed per unique id in increasing position -- the composed path's rule, deterministic.
+
+  Single-shard float32 / float16 / bfloat16 variables with a constant or keyed initializer, dim % 4 == 0 and
+  dim <= 128; no max_norm.  Everything else takes `embedding_lookup_sparse(..., return_trainable=True)`."""
+  if combiner not in ("mean", "sqrtn", "sum"):
+    raise ValueError("combiner must be one of 'mean', 'sqrtn' or 'sum'")
+  if not isinstance(sp_ids, SparseIds):
+    raise TypeError("sp_ids must be SparseTensor")
+  if sp_weights is not None and not isinstance(sp_weights, SparseIds):
+    raise TypeError("sp_weights must be either None or SparseTensor")
+  if not isinstance(params, Variable):
+    raise TypeError("params should be a Variable instance.")
+  if params.key_dtype != sp_ids.values.dtype:
+    raise TypeError("params.key_dtype should be same with sp_ids.dtype: {} vs. {}".format(params.key_dtype,
+                                                                                           sp_ids.values.dtype))
+  if params.shard_num != 1:
+    raise ValueError("trainable_embedding_lookup_sparse: one shard only (got %d); use embedding_lookup_sparse("
+                     "return_trainable=True)" % params.shard_num)
+  if params.value_dtype not in _FUSED_DTYPES:
+    raise TypeError("trainable_embedding_lookup_sparse: float32, float16 or bfloat16 variables, got %s" % (params.value_dtype,))
+  from .keyed_init import is_keyed
+  if callable(params.initializer) and not is_keyed(params.initializer):
+    raise ValueError("trainable_embedding_lookup_sparse: a callable initializer draws rows per lookup; use a constant or "
+                     "a keyed initializer (de.KeyedRandomUniform / de.KeyedRandomNormal / de.KeyedTruncatedNormal), or the "
+                     "composed path embedding_lookup_sparse(return_trainable=True)")
+  if params.bp_v2:
+    raise ValueError("trainable_embedding_lookup_sparse: bp_v2 is not supported; use embedding_lookup_sparse("
+                     "return_trainable=True)")
+  if params.dim % 4 != 0 or params.dim > 128:
+    raise ValueError("trainable_embedding_lookup_sparse: dim must be a multiple of 4 and at most 128, got %d" % params.dim)
+  dev = params.tables[0].device
+  ids = sp_ids.values.reshape(-1).to(dev).contiguous()
+  seg = sp_ids.indices[:, 0].to(device=dev, dtype=torch.int32).contiguous()
+  w = None if sp_weights is None else sp_weights.values.reshape(-1).to(device=dev, dtype=torch.float32).contiguous()
+  batch = sp_ids.dense_shape[0]
+  out = lookup_sparse_fused(params, ids, seg, w, batch, combiner)
+  from .variable import ModelMode
+  if params.trainable and ModelMode.CURRENT_SETTING == ModelMode.TRAIN:
+    out.requires_grad_(True)
+  return out, SparseLookupTrainable(params, ids, seg, w, batch, combiner, out)
+
+
 def verify_embedding_param_weights(embedding_weights, sparse_ids, sparse_weights=None):
   """EmbeddingWeights.verify_embedding_param_weights (python/ops/embedding_weights.py:78-95)"""
   if embedding_weights is None:

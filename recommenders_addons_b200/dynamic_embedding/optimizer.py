@@ -141,9 +141,14 @@ class _FusedBase(object):
                          (params.name, t._num_slot_planes, type(self).__name__, self.n_slots))
 
   def apply_gradients(self, grads_and_vars):
-    """grads_and_vars: iterable of (grad [n, dim], TrainableWrapper) or (grad, (Variable, unique ids))."""
+    """grads_and_vars: iterable of (grad [n, dim], TrainableWrapper), (grad, (Variable, unique ids)) or
+    (dL/dout [batch, dim], SparseLookupTrainable) -- the last in one det_apply_*_sparse call."""
+    from .ops import SparseLookupTrainable
     self.iterations += 1
     for grad, var in grads_and_vars:
+      if isinstance(var, SparseLookupTrainable):
+        self._apply_lookup_sparse(var, grad)
+        continue
       if isinstance(var, TrainableWrapper):
         params, ids = var.params, var.ids
       else:
@@ -184,20 +189,38 @@ class _FusedBase(object):
       ids = ids.to(t.device).contiguous()
       grads = grads.to(t.device)
       n = ids.numel()
-      lib = _lib.lib()
-      need = int(lib.det_apply_dup_workspace_bytes(n, params.dim))
-      ws = getattr(self, "_dup_ws", None)
-      if ws is None or ws.numel() < need or ws.device != t.device:
-        # reused across steps (stream-ordered scratch): no allocation on the hot path after the first step
-        raw = torch.empty(need + need // 8 + 256, dtype=torch.uint8, device=t.device)
-        off = (-raw.data_ptr()) % 256          # the C ABI wants a 256 B aligned workspace (CUDA allocations already are)
-        ws = self._dup_ws = raw[off:off + need + need // 8]
+      ws = self._workspace(int(_lib.lib().det_apply_dup_workspace_bytes(n, params.dim)), t.device)
       init = None if t.keyed_initializer is not None else t._default_value.to(device=t.device, dtype=torch.float32).contiguous()
       self._apply_table_dup(t, ids, grads, n, init, ws)
       return
     from .variable import combine_rows, unique
     uniq, idx = unique(ids)
     self.apply_sparse(params, uniq, combine_rows(grads, idx, uniq.numel()))
+
+  def _workspace(self, need, device):
+    ws = getattr(self, "_dup_ws", None)
+    if ws is None or ws.numel() < need or ws.device != device:
+      # reused across steps (stream-ordered scratch): no allocation on the hot path after the first step
+      raw = torch.empty(need + need // 8 + 256, dtype=torch.uint8, device=device)
+      off = (-raw.data_ptr()) % 256          # the C ABI wants a 256 B aligned workspace (CUDA allocations already are)
+      ws = self._dup_ws = raw[off:off + need + need // 8]
+    return ws
+
+  def _apply_lookup_sparse(self, h, gout):
+    """one step from dL/dout of a trainable_embedding_lookup_sparse call: det_apply_*_sparse (the backward of the fused
+    lookup chained into the fused step; the unique count stays on the device)"""
+    params = h.params
+    self._check(params)
+    t = params.tables[0]
+    nnz = h.ids.numel()
+    if nnz:
+      gout = gout.to(device=t.device, dtype=torch.float32).contiguous()
+      ws = self._workspace(int(_lib.lib().det_apply_sparse_workspace_bytes(nnz, h.batch, params.dim)), t.device)
+      init = None if t.keyed_initializer is not None else t._default_value.to(device=t.device, dtype=torch.float32).contiguous()
+      self._apply_table_sparse(t, h, gout, init, ws)
+    policy = getattr(params, "restrict_policy", None)
+    if policy is not None:
+      policy.apply_update(h.ids)
 
 
 class FusedAdagrad(_FusedBase):
@@ -225,6 +248,13 @@ class FusedAdagrad(_FusedBase):
     _lib.check(_lib.lib().det_apply_adagrad_dup(table.handle, _ptr(ids), _ptr(grads), n, self.learning_rate, self.epsilon,
                                                 _ptr(init), self.initial_accumulator_value, _ptr(ws), ws.numel(), None,
                                                 _stream_ptr(table.device)))
+
+  def _apply_table_sparse(self, table, h, gout, init, ws):
+    _lib.check(_lib.lib().det_apply_adagrad_sparse(table.handle, _ptr(h.ids), _ptr(h.segment_ids), _ptr(h.weights),
+                                                   h.ids.numel(), h.batch, _lib.COMBINERS[h.combiner], _ptr(gout),
+                                                   self.learning_rate, self.epsilon, _ptr(init),
+                                                   self.initial_accumulator_value, _ptr(ws), ws.numel(), None,
+                                                   _stream_ptr(table.device)))
 
 
 class FusedAdam(_FusedBase):
@@ -259,6 +289,12 @@ class FusedAdam(_FusedBase):
                                              self.epsilon, _ptr(init), _ptr(ws), ws.numel(), None,
                                              _stream_ptr(table.device)))
 
+  def _apply_table_sparse(self, table, h, gout, init, ws):
+    _lib.check(_lib.lib().det_apply_adam_sparse(table.handle, _ptr(h.ids), _ptr(h.segment_ids), _ptr(h.weights),
+                                                h.ids.numel(), h.batch, _lib.COMBINERS[h.combiner], _ptr(gout),
+                                                self.alpha(), self.beta_1, self.beta_2, self.epsilon, _ptr(init), _ptr(ws),
+                                                ws.numel(), None, _stream_ptr(table.device)))
+
 
 class FusedSGD(_FusedBase):
   """SGD and momentum on dynamic-embedding rows (TF1 GradientDescent / MomentumOptimizer; torch SGD(momentum,
@@ -290,6 +326,12 @@ class FusedSGD(_FusedBase):
     _lib.check(_lib.lib().det_apply_sgd_dup(table.handle, _ptr(ids), _ptr(grads), n, self.learning_rate, self.momentum,
                                             int(self.nesterov), _ptr(init), _ptr(ws), ws.numel(), None,
                                             _stream_ptr(table.device)))
+
+  def _apply_table_sparse(self, table, h, gout, init, ws):
+    _lib.check(_lib.lib().det_apply_sgd_sparse(table.handle, _ptr(h.ids), _ptr(h.segment_ids), _ptr(h.weights),
+                                               h.ids.numel(), h.batch, _lib.COMBINERS[h.combiner], _ptr(gout),
+                                               self.learning_rate, self.momentum, int(self.nesterov), _ptr(init), _ptr(ws),
+                                               ws.numel(), None, _stream_ptr(table.device)))
 
 
 class FusedFtrl(_FusedBase):
@@ -336,6 +378,13 @@ class FusedFtrl(_FusedBase):
     _lib.check(_lib.lib().det_apply_ftrl_dup(table.handle, _ptr(ids), _ptr(grads), n, self.learning_rate, self.l1,
                                              self.l2, self.l2_shrinkage, _ptr(init), self.initial_accumulator_value,
                                              _ptr(ws), ws.numel(), None, _stream_ptr(table.device)))
+
+  def _apply_table_sparse(self, table, h, gout, init, ws):
+    _lib.check(_lib.lib().det_apply_ftrl_sparse(table.handle, _ptr(h.ids), _ptr(h.segment_ids), _ptr(h.weights),
+                                                h.ids.numel(), h.batch, _lib.COMBINERS[h.combiner], _ptr(gout),
+                                                self.learning_rate, self.l1, self.l2, self.l2_shrinkage, _ptr(init),
+                                                self.initial_accumulator_value, _ptr(ws), ws.numel(), None,
+                                                _stream_ptr(table.device)))
 
 
 class ComposedOptimizer(object):
@@ -427,9 +476,15 @@ class ComposedOptimizer(object):
     return opt.state.get(p, {})
 
   def apply_gradients(self, grads_and_vars):
-    """grads_and_vars: iterable of (grad [n, dim], TrainableWrapper) or (grad, (Variable, unique ids))."""
+    """grads_and_vars: iterable of (grad [n, dim], TrainableWrapper), (grad, (Variable, unique ids)) or
+    (dL/dout [batch, dim], SparseLookupTrainable) -- the last through det_lookup_sparse_grad, then one step."""
+    from .ops import SparseLookupTrainable
     self.iterations += 1
     for grad, var in grads_and_vars:
+      if isinstance(var, SparseLookupTrainable):
+        uniq, g = var.grad_rows(grad)
+        self.apply_sparse(var.params, uniq, g)
+        continue
       tw = var if isinstance(var, TrainableWrapper) else TrainableWrapper(var[0], var[1])
       self._apply_one(tw, grad)
 

@@ -1,0 +1,229 @@
+"""Training through the fused embedding_lookup_sparse: the new public path against the ones it replaces, on one GPU at
+dim 64, on a variable holding --resident rows with one Adagrad plane, timed in one process.
+
+  (1) multi-hot public training step: 65536 bags x 20 Zipf ids, with weights, combiner "mean": forward, backward of a
+      fixed stand-in loss gradient, apply_gradients(FusedAdagrad).  embedding_lookup_sparse(return_trainable=True)
+      (unique with a host synchronisation, find into a [U, dim] scratch, det_sparse_segment_sum; its backward
+      materialises the [nnz, dim] rows) against trainable_embedding_lookup_sparse (fused forward; det_apply_adagrad_sparse);
+  (2) one id per row (26 x 65536 ids, no weights, "sum") through both public paths, next to the floor of a hand-written
+      step: lookup_sparse_fused + apply_sparse_duplicate_indices on the [nnz, dim] output gradient;
+  (3) the backward alone at shape (1): det_apply_adagrad_sparse against torch's gout[seg] * c materialisation followed by
+      det_apply_adagrad_dup.
+CUDA events, median of --rounds rounds that alternate the order of the arms.  A sample of every arm's result is checked
+against the oracle: the sampled ids' rows after one step of each arm (the fused arms bit for bit against
+tests/sparse_grad_oracle.py + oracle.sparse_adagrad_step; the composed arm, whose weighted denominators are summed by
+atomics, to 1e-4 relative).  The card name, power limit and max SM clock are read in the same run.  Prints one JSON line.
+
+  python scripts/sparse_train_microbench.py [--resident 40000000] [--rounds 5] [--calls 5]
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+import numpy as np
+import torch
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+DIM = 64
+BAGS, PER_BAG = 65536, 20
+FEATURES = 26
+LR, INIT_ACCUM = 0.05, 0.1
+
+
+def card():
+  q = "name,power.limit,clocks.max.sm"
+  try:
+    out = subprocess.run(["nvidia-smi", "-i", str(torch.cuda.current_device()), "--query-gpu=" + q,
+                          "--format=csv,noheader"], capture_output=True, text=True, timeout=30).stdout.strip()
+    name, pl, clk = [s.strip() for s in out.split(",")]
+    return {"name": name, "power_limit": pl, "max_sm_clock": clk}
+  except Exception as ex:   # noqa: BLE001
+    return {"name": torch.cuda.get_device_name(0), "error": repr(ex)}
+
+
+def timed(fn, calls):
+  a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+  torch.cuda.synchronize()
+  a.record()
+  for _ in range(calls):
+    fn()
+  b.record()
+  b.synchronize()
+  return a.elapsed_time(b) / calls
+
+
+def medians(rounds, calls, fns):
+  ts = [[] for _ in fns]
+  order = list(range(len(fns)))
+  for r in range(rounds):
+    for i in (order if r % 2 == 0 else order[::-1]):
+      ts[i].append(timed(fns[i], calls))
+  return [round(float(np.median(t)), 4) for t in ts]
+
+
+def main():
+  ap = argparse.ArgumentParser()
+  ap.add_argument("--resident", type=int, default=40_000_000)
+  ap.add_argument("--rounds", type=int, default=5)
+  ap.add_argument("--calls", type=int, default=5)
+  ap.add_argument("--sample", type=int, default=2000)
+  args = ap.parse_args()
+  if not torch.cuda.is_available():
+    raise SystemExit("sparse_train_microbench.py needs a GPU")
+  from oracle import oracle as O
+  from recommenders_addons_b200 import _lib
+  from recommenders_addons_b200 import dynamic_embedding as de
+  from recommenders_addons_b200.dynamic_embedding.ops import lookup_sparse_fused
+  from recommenders_addons_b200.dynamic_embedding.table import _ptr, _stream_ptr
+  from tests import sparse_grad_oracle as SG
+  lib = _lib.lib()
+  dev = torch.device("cuda", torch.cuda.current_device())
+  rng = np.random.default_rng(0)
+  result = {"metric": "sparse training step microbenchmark", "dim": DIM, "resident": args.resident, "card": card(),
+            "unit": "ms"}
+
+  v = de.Variable(dim=DIM, initializer=0.0, num_slot_planes=1, devices=[str(dev)], name="sparse_train_bench",
+                  init_size=2 * args.resident)
+  step = 1 << 22
+  for b in range(0, args.resident, step):
+    k = torch.arange(b, min(b + step, args.resident), dtype=torch.int64, device=dev)
+    v.upsert(k, torch.randn(k.numel(), DIM, device=dev) * 0.05)
+  opt = de.FusedAdagrad(LR, INIT_ACCUM)
+  t = v.tables[0]
+
+  def zipf_ids(n, fields):
+    """position p draws from field p % fields: Zipf(1.05) ranks over the field's resident/fields keys (redrawn beyond
+    them), key = rank * fields + field -- the per-feature vocabularies of bench.py's configs[2], so a head key holds
+    thousands of rows, not a fixed share of the whole batch"""
+    per = args.resident // fields
+    r = np.empty(0, np.int64)
+    while r.shape[0] < n:
+      d = rng.zipf(1.05, 2 * n)
+      r = np.concatenate([r, d[d <= per] - 1])
+    return torch.as_tensor(r[:n] * fields + np.arange(n) % fields, device=dev)
+
+  # ---- (1) multi-hot ----
+  nnz = BAGS * PER_BAG
+  seg = torch.arange(BAGS, device=dev).repeat_interleave(PER_BAG)
+  ind = torch.stack([seg, torch.arange(PER_BAG, device=dev).repeat(BAGS)], 1)
+  ids = zipf_ids(nnz, PER_BAG)
+  wv = torch.as_tensor(rng.uniform(0.5, 2.0, nnz).astype(np.float32), device=dev)
+  sp, sw = de.SparseIds(ind, ids, (BAGS, PER_BAG)), de.SparseIds(ind, wv, (BAGS, PER_BAG))
+  gout = torch.randn(BAGS, DIM, device=dev) * 1e-3
+
+  def composed():
+    out, tw = de.embedding_lookup_sparse(v, sp, sw, combiner="mean", return_trainable=True)
+    out.backward(gout)
+    opt.apply_gradients([(tw.values.grad, tw)])
+
+  def fused():
+    out, h = de.trainable_embedding_lookup_sparse(v, sp, sw, combiner="mean")
+    out.backward(gout)
+    opt.apply_gradients([(out.grad, h)])
+
+  # correctness of one step of each arm on a sample of the ids
+  ids_np, seg_np, w_np, g_np = ids.cpu().numpy(), seg.cpu().numpy().astype(np.int32), wv.cpu().numpy(), gout.cpu().numpy()
+  uniq = np.unique(ids_np)
+  pick = np.unique(np.concatenate([uniq[:50], rng.choice(uniq, min(args.sample, uniq.shape[0]), replace=False)]))
+  g_pick = SG.lookup_sparse_grad_of(ids_np, seg_np, w_np, BAGS, "mean", g_np, pick)
+  checks = {}
+  for name, fn, exact in (("multi_hot_composed", composed, False), ("multi_hot_fused", fused, True)):
+    p0 = v.lookup(torch.as_tensor(pick, device=dev)).cpu().numpy()
+    pt, pa = O.PortTable(DIM), O.PortTable(DIM)
+    k_all, a_all = t.export(plane=1)
+    sel = torch.isin(k_all, torch.as_tensor(pick, device=dev))
+    ka, va = k_all[sel].cpu().numpy(), a_all[sel].cpu().numpy()
+    # before the table's first Adagrad step its plane 1 exports 0 for keys without slot state (the step starts them
+    # from the initial accumulator); a stepped key's accumulator is never 0
+    stepped = (va != 0).any(1)
+    pt.insert(pick[pick < args.resident], p0[pick < args.resident])
+    pa.insert(ka[stepped], va[stepped])
+    fn()
+    torch.cuda.synchronize()
+    exp_p, _ = O.sparse_adagrad_step(pt, pa, pick, g_pick, LR, np.zeros(DIM, np.float32), np.full(DIM, INIT_ACCUM, np.float32))
+    got = v.lookup(torch.as_tensor(pick, device=dev)).cpu().numpy()
+    checks[name] = bool(np.array_equal(got.view(np.uint32), exp_p.view(np.uint32))) if exact else \
+        bool(np.allclose(got, exp_p, rtol=1e-4, atol=1e-6))
+    del k_all, a_all, sel
+  for _ in range(2):
+    composed()
+    fused()
+  result["multi_hot"] = dict(zip(("composed_public", "fused_public"), medians(args.rounds, args.calls, [composed, fused])))
+
+  # ---- (3) the backward alone at shape (1) ----
+  ws_bytes = int(lib.det_apply_sparse_workspace_bytes(nnz, BAGS, DIM))
+  ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+  seg32 = seg.to(torch.int32)
+  init = torch.zeros(DIM, device=dev)
+
+  def bwd_fused():
+    _lib.check(lib.det_apply_adagrad_sparse(t.handle, _ptr(ids), _ptr(seg32), _ptr(wv), nnz, BAGS, 1, _ptr(gout), LR, 0.0,
+                                            _ptr(init), INIT_ACCUM, _ptr(ws), ws_bytes, None, _stream_ptr(dev)))
+
+  def bwd_materialised():
+    den = torch.zeros(BAGS, device=dev).index_add_(0, seg, wv)
+    rows = (gout[seg] * (wv / den[seg])[:, None]).contiguous()
+    opt.apply_sparse_duplicate_indices(v, ids, rows)
+
+  for _ in range(2):
+    bwd_fused()
+    bwd_materialised()
+  result["backward_only"] = dict(zip(("fused_sparse", "materialised_dup"),
+                                     medians(args.rounds, args.calls, [bwd_fused, bwd_materialised])))
+  del ws
+
+  # ---- (2) one id per row ----
+  n1 = FEATURES * BAGS
+  ids1 = zipf_ids(n1, FEATURES)
+  ind1 = torch.stack([torch.arange(n1, device=dev), torch.zeros(n1, dtype=torch.int64, device=dev)], 1)
+  sp1 = de.SparseIds(ind1, ids1, (n1, 1))
+  seg1 = torch.arange(n1, dtype=torch.int32, device=dev)
+  gout1 = torch.randn(n1, DIM, device=dev) * 1e-3
+
+  def c3_composed():
+    out, tw = de.embedding_lookup_sparse(v, sp1, None, combiner="sum", return_trainable=True)
+    out.backward(gout1)
+    opt.apply_gradients([(tw.values.grad, tw)])
+
+  def c3_fused():
+    out, h = de.trainable_embedding_lookup_sparse(v, sp1, None, combiner="sum")
+    out.backward(gout1)
+    opt.apply_gradients([(out.grad, h)])
+
+  def c3_floor():
+    lookup_sparse_fused(v, ids1, seg1, None, n1, "sum")
+    opt.apply_sparse_duplicate_indices(v, ids1, gout1)
+
+  ids1_np = ids1.cpu().numpy()
+  u1 = np.unique(ids1_np)
+  pick1 = np.unique(np.concatenate([u1[:50], rng.choice(u1, min(args.sample, u1.shape[0]), replace=False)]))
+  g1 = SG.lookup_sparse_grad_of(ids1_np, np.arange(n1, dtype=np.int32), None, n1, "sum", gout1.cpu().numpy(), pick1)
+  for name, fn in (("one_per_row_composed", c3_composed), ("one_per_row_fused", c3_fused), ("one_per_row_floor", c3_floor)):
+    p0 = v.lookup(torch.as_tensor(pick1, device=dev)).cpu().numpy()
+    k_all, a_all = t.export(plane=1)
+    sel = torch.isin(k_all, torch.as_tensor(pick1, device=dev))
+    pt, pa = O.PortTable(DIM), O.PortTable(DIM)
+    pt.insert(pick1, p0)
+    pa.insert(k_all[sel].cpu().numpy(), a_all[sel].cpu().numpy())
+    fn()
+    torch.cuda.synchronize()
+    exp_p, _ = O.sparse_adagrad_step(pt, pa, pick1, g1, LR, np.zeros(DIM, np.float32), np.full(DIM, INIT_ACCUM, np.float32))
+    got = v.lookup(torch.as_tensor(pick1, device=dev)).cpu().numpy()
+    checks[name] = bool(np.array_equal(got.view(np.uint32), exp_p.view(np.uint32)))
+    del k_all, a_all, sel
+  for _ in range(2):
+    c3_composed()
+    c3_fused()
+    c3_floor()
+  result["one_per_row"] = dict(zip(("composed_public", "fused_public", "harness_floor"),
+                                   medians(args.rounds, args.calls, [c3_composed, c3_fused, c3_floor])))
+  result["checks"] = checks
+  result["ok"] = all(checks.values())
+  print(json.dumps(result))
+
+
+if __name__ == "__main__":
+  main()
