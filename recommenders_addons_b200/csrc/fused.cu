@@ -769,31 +769,42 @@ segment_sum_wide_kernel(TableView t, const long long* __restrict__ slots, const 
 // ------------------------------------------------------------------------------------------------
 // K7: fused find-or-insert + optimizer update
 // ------------------------------------------------------------------------------------------------
-// The optimizer of a K7 launch (template parameter OPT) and its hyper-parameters.  The fields mean, per optimizer:
-//   OPT 0 Adagrad : lr,    eps = epsilon,                             init_slot = initial accumulator
-//   OPT 1 Adam    : lr = alpha, eps = epsilon, beta1, beta2
-//   OPT 2 SGD     : lr
-//   OPT 3 Momentum: lr,    eps = 1 for nesterov (else 0), beta1 = momentum
-//   OPT 4 FTRL    : lr,    eps = l1, beta1 = 2*l2, beta2 = 2*l2_shrinkage, init_slot = initial accumulator
-struct OptHyper {
-  float lr;       // adagrad lr | adam alpha | sgd, momentum and ftrl lr
-  float eps;      // adagrad / adam epsilon | momentum: nesterov flag | ftrl l1
-  float beta1, beta2;
-  float init_slot;  // adagrad / ftrl initial accumulator
-};
+// The optimizer of a K7 launch is its template parameter OPT (kAdagrad .. kFtrl, host.h) with an OptHyper.
 
-// slot planes an optimizer reads and writes (planes 1 .. opt_slots(OPT)): momentum = plane 1; FTRL accumulator n =
-// plane 1, linear z = plane 2
-__host__ __device__ constexpr int opt_slots(int opt) { return opt == 1 || opt == 4 ? 2 : opt == 2 ? 0 : 1; }
+// slot planes an optimizer reads and writes (planes 1 .. opt_slots(OPT)): Adagrad accumulator = plane 1; Adam m =
+// plane 1, v = plane 2; momentum = plane 1; FTRL accumulator n = plane 1, linear z = plane 2
+__host__ __device__ constexpr int opt_slots(int opt) { return opt == kAdam || opt == kFtrl ? 2 : opt == kSgd ? 0 : 1; }
 
-// SGD, momentum and FTRL on one fp32 element, one IEEE operation per operation in the order written (the library is
-// built with --fmad=false): p param, a slot 1, b slot 2, updated in place.  These restate TF's sparse CPU kernels
-// (ResourceSparseApplyMomentum, ResourceSparseApplyFtrl(V2) with learning_rate_power = -0.5).
+// The slot values a key without slot state starts from: a slot 1, b slot 2.
+template <int OPT, int VF>
+__device__ __forceinline__ void opt_fresh(const OptHyper& h, FVec<VF>& a, FVec<VF>& b) {
+  if constexpr (OPT == kAdagrad) {
+    a.fill(h.init_slot);
+  } else if constexpr (OPT == kAdam) {
+    a.zero();
+    b.zero();
+  } else if constexpr (OPT == kMomentum) {
+    a.zero();
+  } else if constexpr (OPT == kFtrl) {
+    a.fill(h.init_slot);
+    b.zero();
+  }
+}
+
+// One step of the optimizer, one IEEE fp32 operation per operation in the order written (the library is built with
+// --fmad=false): g gradient, p param, a slot 1, b slot 2, updated in place.  SGD, momentum and FTRL restate TF's sparse
+// CPU kernels (ResourceSparseApplyMomentum, ResourceSparseApplyFtrl(V2) with learning_rate_power = -0.5).
+// The hyper-parameters, as the builders fill them:
+//   Adagrad : lr, eps = epsilon, init_slot = initial accumulator
+//   Adam    : lr = alpha, eps = epsilon, beta1, beta2
+//   SGD     : lr
+//   Momentum: lr, eps = 1 for nesterov (else 0), beta1 = momentum
+//   FTRL    : lr, eps = l1, beta1 = 2*l2, beta2 = 2*l2_shrinkage, init_slot = initial accumulator
 template <int OPT>
 __device__ __forceinline__ void opt_elem(const OptHyper& h, float g, float& p, float& a, float& b) {
-  if (OPT == 2) {
+  if (OPT == kSgd) {
     p = p - h.lr * g;
-  } else if (OPT == 3) {
+  } else if (OPT == kMomentum) {
     a = a * h.beta1 + g;
     if (h.eps != 0.f) p = p - ((g * h.lr) + ((a * h.beta1) * h.lr));   // nesterov
     else p = p - a * h.lr;
@@ -813,20 +824,36 @@ __device__ __forceinline__ void opt_elem(const OptHyper& h, float g, float& p, f
 }
 template <int OPT, int VF>
 __device__ __forceinline__ void opt_step(const OptHyper& h, const FVec<VF>& g, FVec<VF>& p, FVec<VF>& a, FVec<VF>& b) {
-  const float* gv = reinterpret_cast<const float*>(&g.v);
-  float* pv = reinterpret_cast<float*>(&p.v);
-  float* av = reinterpret_cast<float*>(&a.v);
-  float* bv = reinterpret_cast<float*>(&b.v);
+  if constexpr (OPT == kAdagrad) {
+    // accum += g*g ; var -= lr*g / (sqrt(accum) + eps)
+    a.zip(g, [](float& av, float gv) { av = av + gv * gv; });
+    FVec<VF> upd = g;
+    upd.zip(a, [&h](float& x, float av) { x = (h.lr * x) / (sqrtf(av) + h.eps); });
+    p.zip(upd, [](float& pv, float x) { pv = pv - x; });
+  } else if constexpr (OPT == kAdam) {
+    // m += (g-m)(1-b1) ; v += (g*g-v)(1-b2) ; var -= (m*alpha)/(sqrt(v)+eps)
+    const float omb1 = 1.f - h.beta1, omb2 = 1.f - h.beta2;
+    a.zip(g, [omb1](float& mv, float gv) { mv = mv + (gv - mv) * omb1; });
+    b.zip(g, [omb2](float& vv, float gv) { vv = vv + (gv * gv - vv) * omb2; });
+    FVec<VF> upd = a;
+    upd.zip(b, [&h](float& x, float vv) { x = (x * h.lr) / (sqrtf(vv) + h.eps); });
+    p.zip(upd, [](float& pv, float x) { pv = pv - x; });
+  } else {
+    const float* gv = reinterpret_cast<const float*>(&g.v);
+    float* pv = reinterpret_cast<float*>(&p.v);
+    float* av = reinterpret_cast<float*>(&a.v);
+    float* bv = reinterpret_cast<float*>(&b.v);
 #pragma unroll
-  for (int e = 0; e < VF; ++e) opt_elem<OPT>(h, gv[e], pv[e], av[e], bv[e]);
+    for (int e = 0; e < VF; ++e) opt_elem<OPT>(h, gv[e], pv[e], av[e], bv[e]);
+  }
 }
 
 // The slot-plane count of the table, for the optimizers that mark the slot planes they do not write (SGD, momentum,
 // FTRL): a key such a step creates gets kSlotUninit in the first word of its row in every other slot plane, as insert
 // gives it (table.cu insert_step).  An EMPTY trailing parameter for Adagrad and Adam keeps their kernels unchanged.
 template <int OPT> struct SlotPlanes { int n; };
-template <> struct SlotPlanes<0> {};
-template <> struct SlotPlanes<1> {};
+template <> struct SlotPlanes<kAdagrad> {};
+template <> struct SlotPlanes<kAdam> {};
 template <int OPT>
 __device__ __forceinline__ void mark_unwritten(const TableView& t, const SlotPlanes<OPT>& sp, long long slot) {
   // unrolled: a plane index known at compile time keeps the TableView parameter out of local memory
@@ -834,11 +861,10 @@ __device__ __forceinline__ void mark_unwritten(const TableView& t, const SlotPla
   for (int p = 1 + opt_slots(OPT); p < kMaxPlanes; ++p)
     if (p <= sp.n) *reinterpret_cast<unsigned*>(t.planes[p] + (size_t)slot * t.dim * 4u) = kSlotUninit;
 }
-constexpr int kNumOpts = 5;   // OPT 0 .. 4
 template <int OPT>
 static SlotPlanes<OPT> slot_planes_arg(const det_table* t) {
   SlotPlanes<OPT> sp;
-  if constexpr (OPT >= 2) sp.n = t->cfg.num_slot_planes;
+  if constexpr (OPT >= kSgd) sp.n = t->cfg.num_slot_planes;
   return sp;
 }
 
@@ -849,7 +875,7 @@ static SlotPlanes<OPT> slot_planes_arg(const det_table* t) {
 // FTRL's two square roots and three divisions per element: left to its own heuristics ptxas spills the probe's
 // first-bucket loads to reach 4 CTAs per SM; asking for 3 (the register-held Adagrad / Adam kernels' occupancy) keeps
 // them in registers.  0 = no minimum, the other optimizers' kernels as before.
-template <int OPT> constexpr int kApplyMinBlocks = OPT == 4 ? 3 : 0;
+template <int OPT> constexpr int kApplyMinBlocks = OPT == kFtrl ? 3 : 0;
 
 // KEYED: a new key's param starts from its row of the table's keyed initializer (init_param is NULL).
 // (keyed: 2 CTAs per SM, the register budget the generator's calls need without spilling, as segment_sum_kernel)
@@ -874,7 +900,6 @@ apply_kernel(TableView t, const long long* __restrict__ keys, const float* __res
   T* P = (T*)t.planes[0];
   float* S1 = (float*)t.planes[1];
   float* S2 = (float*)t.planes[2];
-  const float omb1 = 1.f - h.beta1, omb2 = 1.f - h.beta2;
   KeyTiles kt;
   kt.init(s_keys, s_bar, keys, n, use_tma != 0);
   for (; kt.valid(); kt.next()) {
@@ -910,7 +935,7 @@ apply_kernel(TableView t, const long long* __restrict__ keys, const float* __res
         // slot state absent: key created in this launch, or created by insert/accum and never stepped.
         // Every lane reads the marker word BEFORE any lane of the row's group overwrites it.
         mark[u] = ok[u] && opt_slots(OPT) > 0 ? __float_as_uint(S1[ro[u]]) : 0u;
-        if constexpr (OPT >= 2) {
+        if constexpr (OPT >= kSgd) {
           if (ok[u] && nwv[u] && c0 == 0) mark_unwritten(t, sp, s);
         }
       }
@@ -931,43 +956,20 @@ apply_kernel(TableView t, const long long* __restrict__ keys, const float* __res
             if (nwv[u]) p[u].load((full_init ? init_param + gi[u] * dim : init_param) + o);
             else p[u].load(P + ro[u] + o);
           }
-          if (OPT == 0) {
-            if (fresh[u]) a[u].fill(h.init_slot); else a[u].load(S1 + ro[u] + o);
-          } else if (OPT == 1) {
-            if (fresh[u]) { a[u].zero(); b[u].zero(); } else { a[u].load(S1 + ro[u] + o); b[u].load(S2 + ro[u] + o); }
-          } else if (OPT == 3) {
-            if (fresh[u]) a[u].zero(); else a[u].load(S1 + ro[u] + o);
-          } else if (OPT == 4) {
-            if (fresh[u]) { a[u].fill(h.init_slot); b[u].zero(); } else { a[u].load(S1 + ro[u] + o); b[u].load(S2 + ro[u] + o); }
+          if (fresh[u]) {
+            opt_fresh<OPT>(h, a[u], b[u]);
+          } else {
+            if (opt_slots(OPT) > 0) a[u].load(S1 + ro[u] + o);
+            if (opt_slots(OPT) > 1) b[u].load(S2 + ro[u] + o);
           }
         }
 #pragma unroll
         for (int u = 0; u < RU; ++u) {
           if (!ok[u]) continue;
-          if (OPT == 0) {
-            // accum += g*g ; var -= lr*g / (sqrt(accum) + eps)
-            a[u].zip(g[u], [](float& av, float gv) { av = av + gv * gv; });
-            FVec<VF> upd = g[u];
-            upd.zip(a[u], [&h](float& x, float av) { x = (h.lr * x) / (sqrtf(av) + h.eps); });
-            p[u].zip(upd, [](float& pv, float x) { pv = pv - x; });
-            a[u].store(S1 + ro[u] + o);
-            p[u].store(P + ro[u] + o);
-          } else if (OPT == 1) {
-            // m += (g-m)(1-b1) ; v += (g*g-v)(1-b2) ; var -= (m*alpha)/(sqrt(v)+eps)
-            a[u].zip(g[u], [omb1](float& mv, float gv) { mv = mv + (gv - mv) * omb1; });
-            b[u].zip(g[u], [omb2](float& vv, float gv) { vv = vv + (gv * gv - vv) * omb2; });
-            FVec<VF> upd = a[u];
-            upd.zip(b[u], [&h](float& x, float vv) { x = (x * h.lr) / (sqrtf(vv) + h.eps); });
-            p[u].zip(upd, [](float& pv, float x) { pv = pv - x; });
-            a[u].store(S1 + ro[u] + o);
-            b[u].store(S2 + ro[u] + o);
-            p[u].store(P + ro[u] + o);
-          } else {
-            opt_step<OPT>(h, g[u], p[u], a[u], b[u]);
-            if (opt_slots(OPT) > 0) a[u].store(S1 + ro[u] + o);
-            if (opt_slots(OPT) > 1) b[u].store(S2 + ro[u] + o);
-            p[u].store(P + ro[u] + o);
-          }
+          opt_step<OPT>(h, g[u], p[u], a[u], b[u]);
+          if (opt_slots(OPT) > 0) a[u].store(S1 + ro[u] + o);
+          if (opt_slots(OPT) > 1) b[u].store(S2 + ro[u] + o);
+          p[u].store(P + ro[u] + o);
         }
       }
     }
@@ -1032,7 +1034,6 @@ apply_staged_kernel(TableView t, const long long* __restrict__ keys, const float
   T* P = (T*)t.planes[0];
   float* S1 = (float*)t.planes[1];
   float* S2 = (float*)t.planes[2];
-  const float omb1 = 1.f - h.beta1, omb2 = 1.f - h.beta2;
   // per warp: 2 stages x kStageSteps steps x NS streams x 32 lanes x 16 B
   float4* wbuf = reinterpret_cast<float4*>(dyn_smem) + (size_t)warp * (2 * kStageSteps * NS * 32);
   auto sm = [&](int stage, int step, int stream) -> float4* { return wbuf + ((stage * kStageSteps + step) * NS + stream) * 32 + lane; };
@@ -1120,37 +1121,18 @@ apply_staged_kernel(TableView t, const long long* __restrict__ keys, const float
             else if (nw) p.v = *sm(stage, st, 1);
             else p.load(reinterpret_cast<const T*>(sm(stage, st, 1)));
           }
-          if (OPT == 0) {
-            if (fresh) a.fill(h.init_slot); else a.v = *sm(stage, st, 2);
-            a.zip(g, [](float& av, float gv) { av = av + gv * gv; });
-            FVec<4> upd = g;
-            upd.zip(a, [&h](float& x, float av) { x = (h.lr * x) / (sqrtf(av) + h.eps); });
-            p.zip(upd, [](float& pv, float x) { pv = pv - x; });
-            a.store(S1 + ro);
-            p.store(P + ro);
-          } else if (OPT == 1) {
-            if (fresh) { a.zero(); b2.zero(); } else { a.v = *sm(stage, st, 2); b2.v = *sm(stage, st, 3); }
-            a.zip(g, [omb1](float& mv, float gv) { mv = mv + (gv - mv) * omb1; });
-            b2.zip(g, [omb2](float& vv, float gv) { vv = vv + (gv * gv - vv) * omb2; });
-            FVec<4> upd = a;
-            upd.zip(b2, [&h](float& x, float vv) { x = (x * h.lr) / (sqrtf(vv) + h.eps); });
-            p.zip(upd, [](float& pv, float x) { pv = pv - x; });
-            a.store(S1 + ro);
-            b2.store(S2 + ro);
-            p.store(P + ro);
+          if (fresh) {
+            opt_fresh<OPT>(h, a, b2);
           } else {
-            if (OPT == 3) {
-              if (fresh) a.zero(); else a.v = *sm(stage, st, 2);
-            } else if (OPT == 4) {
-              if (fresh) { a.fill(h.init_slot); b2.zero(); } else { a.v = *sm(stage, st, 2); b2.v = *sm(stage, st, 3); }
-            }
-            opt_step<OPT>(h, g, p, a, b2);
-            if (opt_slots(OPT) > 0) a.store(S1 + ro);
-            if (opt_slots(OPT) > 1) b2.store(S2 + ro);
-            p.store(P + ro);
-            if constexpr (OPT >= 2) {
-              if (nw && c0 == 0) mark_unwritten(t, sp, sl);
-            }
+            if (NS > 2) a.v = *sm(stage, st, 2);
+            if (NS > 3) b2.v = *sm(stage, st, 3);
+          }
+          opt_step<OPT>(h, g, p, a, b2);
+          if (opt_slots(OPT) > 0) a.store(S1 + ro);
+          if (opt_slots(OPT) > 1) b2.store(S2 + ro);
+          p.store(P + ro);
+          if constexpr (OPT >= kSgd) {
+            if (nw && c0 == 0) mark_unwritten(t, sp, sl);
           }
         }
       }
@@ -1793,89 +1775,105 @@ static size_t seg_reduce_layout(size_t n, size_t n_groups, unsigned char* base, 
   return c.off;
 }
 
+// The trailing initializer argument of a launch: with KEYED, the table's keyed initializer (and the ids of a lookup,
+// whose segment-sum kernels see only slots); empty otherwise.
+template <bool KEYED>
+static InitArg<KEYED> init_arg(const det_table* t, const long long* ids = nullptr) {
+  InitArg<KEYED> ki{};
+  if constexpr (KEYED) {
+    static_cast<KeyedInit&>(ki) = t->init;
+    ki.ids = ids;
+  }
+  return ki;
+}
+
 // K6 one-id-per-row kernel of a table whose rows are T: float, or __half / __nv_bfloat16 rows it widens to fp32
-using IdentityKernel = void (*)(TableView, const long long*, const int*, size_t, const unsigned char*, unsigned char*,
-                                RowGeom, int, unsigned*, unsigned, InitArg<false>);
-template <typename T, int V> static IdentityKernel identity_kernel() {
+template <typename T, int V, bool KEYED> static auto identity_kernel() {
   if constexpr (std::is_same<T, float>::value)
-    return lookup_identity_kernel<V>;
+    return lookup_identity_kernel<V, KEYED>;
   else
-    return lookup_identity_widen_kernel<T, V>;
+    return lookup_identity_widen_kernel<T, V, KEYED>;
 }
 
 // K6 phase B: the weighted segment sum of rows of type T gathered through `slots` from the view's plane 0 -- the looked-up
 // table rows of det_lookup_sparse, or the dense matrix of det_sparse_segment_sum.  sms: SM count the grid is sized for.
-// A clipping launch (CLIP) needs rows of at most 32 vectors (vpr <= lpr).
-template <typename T, bool CLIP>
+// A clipping launch (CLIP) needs rows of at most 32 vectors (vpr <= lpr).  KEYED: a table with a keyed initializer and
+// no default row (NULL): the kernels generate missing ids' rows.
+template <typename T, bool CLIP, bool KEYED>
 static void launch_segment_sum(const TableView& v, int sms, const long long* slots, const long long* seg_start,
                                const float* weights, size_t batch, int combiner, const float* default_row, float* out,
                                bool vec4, unsigned vpr, unsigned lpr, unsigned sh, const ClipArg<CLIP>& clip,
-                               const unsigned* gate, unsigned epoch, cudaStream_t s) {
+                               const unsigned* gate, unsigned epoch, const InitArg<KEYED>& ki, cudaStream_t s) {
   const unsigned gpw = 32u >> sh;
   if (vpr <= lpr) {
-    const auto k4 = segment_sum_kernel<4, CLIP, T>;
-    const auto k1 = segment_sum_kernel<1, CLIP, T>;
+    const auto k4 = segment_sum_kernel<4, CLIP, T, KEYED>;
+    const auto k1 = segment_sum_kernel<1, CLIP, T, KEYED>;
     const int occ = vec4 ? occupancy_of(k4, kThreadsF) : occupancy_of(k1, kThreadsF);
     const int grid = grid_for(batch, (int)(gpw * kSegPerGroup * (kThreadsF / 32)), sms, occ);
     if (vec4)
-      DET_LAUNCH(k4, grid, kThreadsF, 0, s, v, slots, seg_start, weights, batch, combiner, default_row, out, vpr, lpr, sh, clip, gate, epoch,
-                 InitArg<false>());
+      DET_LAUNCH(k4, grid, kThreadsF, 0, s, v, slots, seg_start, weights, batch, combiner, default_row, out, vpr, lpr, sh, clip, gate, epoch, ki);
     else
-      DET_LAUNCH(k1, grid, kThreadsF, 0, s, v, slots, seg_start, weights, batch, combiner, default_row, out, vpr, lpr, sh, clip, gate, epoch,
-                 InitArg<false>());
+      DET_LAUNCH(k1, grid, kThreadsF, 0, s, v, slots, seg_start, weights, batch, combiner, default_row, out, vpr, lpr, sh, clip, gate, epoch, ki);
   } else {
     // rows wider than kMaxVecPerLane vectors per lane are swept in column chunks by the same kernel
     const int grid = grid_for(batch, (int)(gpw * (kThreadsF / 32)), sms, 8);
     if (vec4)
-      DET_LAUNCH((segment_sum_wide_kernel<4, T>), grid, kThreadsF, 0, s, v, slots, seg_start, weights, batch, combiner, default_row, out, vpr, lpr, sh);
+      DET_LAUNCH((segment_sum_wide_kernel<4, T, KEYED>), grid, kThreadsF, 0, s, v, slots, seg_start, weights, batch, combiner, default_row, out, vpr, lpr, sh, ki);
     else
-      DET_LAUNCH((segment_sum_wide_kernel<1, T>), grid, kThreadsF, 0, s, v, slots, seg_start, weights, batch, combiner, default_row, out, vpr, lpr, sh);
+      DET_LAUNCH((segment_sum_wide_kernel<1, T, KEYED>), grid, kThreadsF, 0, s, v, slots, seg_start, weights, batch, combiner, default_row, out, vpr, lpr, sh, ki);
   }
 }
 
-// launch_segment_sum of a table with a keyed initializer and no default row: the kernels generate missing ids' rows
-template <typename T, bool CLIP>
-static void launch_segment_sum_keyed(const TableView& v, int sms, const long long* slots, const long long* seg_start,
-                                     const float* weights, size_t batch, int combiner, float* out, bool vec4, unsigned vpr,
-                                     unsigned lpr, unsigned sh, const ClipArg<CLIP>& clip, const unsigned* gate,
-                                     unsigned epoch, const InitArg<true>& ki, cudaStream_t s) {
-  const unsigned gpw = 32u >> sh;
-  const float* nodef = nullptr;
-  if (vpr <= lpr) {
-    const auto k4 = segment_sum_kernel<4, CLIP, T, true>;
-    const auto k1 = segment_sum_kernel<1, CLIP, T, true>;
-    const int occ = vec4 ? occupancy_of(k4, kThreadsF) : occupancy_of(k1, kThreadsF);
-    const int grid = grid_for(batch, (int)(gpw * kSegPerGroup * (kThreadsF / 32)), sms, occ);
-    if (vec4)
-      DET_LAUNCH(k4, grid, kThreadsF, 0, s, v, slots, seg_start, weights, batch, combiner, nodef, out, vpr, lpr, sh, clip, gate, epoch, ki);
-    else
-      DET_LAUNCH(k1, grid, kThreadsF, 0, s, v, slots, seg_start, weights, batch, combiner, nodef, out, vpr, lpr, sh, clip, gate, epoch, ki);
-  } else {
-    const int grid = grid_for(batch, (int)(gpw * (kThreadsF / 32)), sms, 8);
-    if (vec4)
-      DET_LAUNCH((segment_sum_wide_kernel<4, T, true>), grid, kThreadsF, 0, s, v, slots, seg_start, weights, batch, combiner, nodef, out, vpr, lpr, sh, ki);
-    else
-      DET_LAUNCH((segment_sum_wide_kernel<1, T, true>), grid, kThreadsF, 0, s, v, slots, seg_start, weights, batch, combiner, nodef, out, vpr, lpr, sh, ki);
-  }
-}
-
-using IdentityKernelKeyed = void (*)(TableView, const long long*, const int*, size_t, const unsigned char*, unsigned char*,
-                                     RowGeom, int, unsigned*, unsigned, InitArg<true>);
-template <typename T, int V> static IdentityKernelKeyed identity_kernel_keyed() {
-  if constexpr (std::is_same<T, float>::value)
-    return lookup_identity_kernel<V, true>;
-  else
-    return lookup_identity_widen_kernel<T, V, true>;
-}
-
-// K7: f(row) with decltype(row)::type the param row storage type of a float32, float16 or bfloat16 table (the caller
+// f(row) with decltype(row)::type the param row storage type of a float32, float16 or bfloat16 table (the caller
 // has refused every other dtype)
 template <typename T> struct RowType { using type = T; };
 template <typename F>
 static det_status dispatch_row_type(int value_dtype, F&& f) {
+  if (value_dtype == DET_FLOAT32) return f(RowType<float>());
   if (value_dtype == DET_FLOAT16) return f(RowType<__half>());
-  if (value_dtype == DET_BFLOAT16) return f(RowType<__nv_bfloat16>());
-  return f(RowType<float>());
+  return f(RowType<__nv_bfloat16>());
+}
+
+// K7 hyper-parameters, one builder per optimizer: validate, fill OptHyper (its fields per optimizer: opt_step), set *opt
+det_status adagrad_hyper(float lr, float epsilon, float init_accum, OptHyper* h, int* opt) {
+  h->lr = lr; h->eps = epsilon; h->beta1 = 0.f; h->beta2 = 0.f; h->init_slot = init_accum;
+  *opt = kAdagrad;
+  return DET_OK;
+}
+
+det_status adam_hyper(float alpha, float beta1, float beta2, float epsilon, OptHyper* h, int* opt) {
+  h->lr = alpha; h->eps = epsilon; h->beta1 = beta1; h->beta2 = beta2; h->init_slot = 0.f;
+  *opt = kAdam;
+  return DET_OK;
+}
+
+// SGD (momentum == 0) or momentum
+static det_status sgd_hyper(float lr, float momentum, int nesterov, OptHyper* h, int* opt) {
+  if (nesterov && momentum == 0.f) return fail(DET_INVALID_ARGUMENT, "det_apply_sgd: nesterov needs a momentum");
+  h->lr = lr; h->eps = nesterov ? 1.f : 0.f; h->beta1 = momentum; h->beta2 = 0.f; h->init_slot = 0.f;
+  *opt = momentum == 0.f ? kSgd : kMomentum;
+  return DET_OK;
+}
+
+// FTRL: lr > 0 and l1, l2, l2_shrinkage, init_accum >= 0 as TF's ApplyFtrl checks them; 2*l2 and 2*l2_shrinkage are
+// exact in fp32
+static det_status ftrl_hyper(float lr, float l1, float l2, float l2_shrinkage, float init_accum, OptHyper* h, int* opt) {
+  if (!(lr > 0.f)) return fail(DET_INVALID_ARGUMENT, "det_apply_ftrl: lr must be positive");
+  if (!(l1 >= 0.f) || !(l2 >= 0.f) || !(l2_shrinkage >= 0.f) || !(init_accum >= 0.f))
+    return fail(DET_INVALID_ARGUMENT, "det_apply_ftrl: l1, l2, l2_shrinkage and init_accum must be >= 0");
+  h->lr = lr; h->eps = l1; h->beta1 = 2.f * l2; h->beta2 = 2.f * l2_shrinkage; h->init_slot = init_accum;
+  *opt = kFtrl;
+  return DET_OK;
+}
+
+// det_table::slot_init, the slot values of a key created by insert / accum and never stepped: the initial accumulator
+// of Adagrad and FTRL (FTRL's z: 0), 0 for momentum; Adam and plain SGD leave them as they are.  Every optimizer entry
+// point records them before it takes the table lock.
+static void record_slot_init(det_table* t, int opt, const OptHyper& h) {
+  if (!t) return;
+  if (opt == kAdagrad || opt == kFtrl) t->slot_init[1] = h.init_slot;
+  if (opt == kMomentum) t->slot_init[1] = 0.f;
+  if (opt == kFtrl) t->slot_init[2] = 0.f;
 }
 
 }  // namespace det
@@ -1937,9 +1935,6 @@ static det_status lookup_sparse_impl(det_table* t, const int64_t* ids, const int
   const bool keyed = default_row == nullptr;
   if (keyed && !t->keyed)
     return fail(DET_INVALID_ARGUMENT, "det_lookup_sparse: null default_row (the table has no keyed initializer)");
-  InitArg<true> ki{};
-  static_cast<KeyedInit&>(ki) = t->init;
-  ki.ids = (const long long*)ids;
   cudaStream_t s = (cudaStream_t)stream;
   det::DevGuard _dg(t->cfg.device);
   long long* seg_start = nullptr;
@@ -1982,61 +1977,42 @@ static det_status lookup_sparse_impl(det_table* t, const int64_t* ids, const int
     unsigned char* o = (unsigned char*)out;
     dispatch_vec<4>(out_row_bytes, {{default_row, "det_lookup_sparse: default_row"}, {out, "det_lookup_sparse: out"}},
                     [&](auto V, const RowGeom& g) -> det_status {
-      constexpr int VV = decltype(V)::value;
-      if (keyed) {
-        const IdentityKernelKeyed kern = vt == DET_FLOAT32   ? identity_kernel_keyed<float, VV>()
-                                         : vt == DET_FLOAT16 ? identity_kernel_keyed<__half, VV>()
-                                                             : identity_kernel_keyed<__nv_bfloat16, VV>();
-        const int grid = grid_for(nnz, kTileKeys, t->sm_count, occupancy_of(kern, kThreadsF));
-        DET_LAUNCH(kern, grid, kThreadsF, 0, s, t->view, k, segment_ids, nnz, d, o, g, tma, not_identity, epoch, ki);
-        return DET_OK;
-      }
-      const IdentityKernel kern = vt == DET_FLOAT32   ? identity_kernel<float, VV>()
-                                  : vt == DET_FLOAT16 ? identity_kernel<__half, VV>()
-                                                      : identity_kernel<__nv_bfloat16, VV>();
-      const int grid = grid_for(nnz, kTileKeys, t->sm_count, occupancy_of(kern, kThreadsF));
-      DET_LAUNCH(kern, grid, kThreadsF, 0, s, t->view, k, segment_ids, nnz, d, o, g, tma, not_identity, epoch, InitArg<false>());
-      return DET_OK;
+      return dispatch_bit(keyed, [&](auto KEYED) -> det_status {
+        return dispatch_row_type(vt, [&](auto row) -> det_status {
+          constexpr bool kKeyed = decltype(KEYED)::value;
+          const auto kern = identity_kernel<typename decltype(row)::type, decltype(V)::value, kKeyed>();
+          const int grid = grid_for(nnz, kTileKeys, t->sm_count, occupancy_of(kern, kThreadsF));
+          DET_LAUNCH(kern, grid, kThreadsF, 0, s, t->view, k, segment_ids, nnz, d, o, g, tma, not_identity, epoch,
+                     init_arg<kKeyed>(t, k));
+          return DET_OK;
+        });
+      });
     });
   }
   DET_LAUNCH(segment_offsets_kernel, (int)((nnz + 1 + 255) / 256), 256, 0, s, segment_ids, nnz, batch, seg_start, t->view.st, gate, epoch);
   if (nnz)
     DET_LAUNCH(resolve_slots_kernel, grid_for(nnz, kTileKeys, t->sm_count, occupancy_of(resolve_slots_kernel, kThreadsF)), kThreadsF, 0, s, t->view, (const long long*)ids, nnz, slots, (((uintptr_t)ids & 15u) == 0) ? 1 : 0, gate, epoch);
   det_status rc = DET_OK;
-  const ClipArg<false> noclip;
-  if (keyed && !(max_norm > 0.f && !(vpr <= lpr))) {
-    if (max_norm > 0.f) {
-      ClipArg<true> clip;
-      clip.max_norm = max_norm;
-      launch_segment_sum_keyed<float>(t->view, t->sm_count, slots, seg_start, weights, batch, combiner, out, vec4, vpr, lpr,
-                                      sh, clip, gate, epoch, ki, s);
-    } else if (vt == DET_FLOAT32) {
-      launch_segment_sum_keyed<float>(t->view, t->sm_count, slots, seg_start, weights, batch, combiner, out, vec4, vpr, lpr,
-                                      sh, noclip, gate, epoch, ki, s);
-    } else if (vt == DET_FLOAT16) {
-      launch_segment_sum_keyed<__half>(t->view, t->sm_count, slots, seg_start, weights, batch, combiner, out, vec4, vpr, lpr,
-                                       sh, noclip, gate, epoch, ki, s);
-    } else {
-      launch_segment_sum_keyed<__nv_bfloat16>(t->view, t->sm_count, slots, seg_start, weights, batch, combiner, out, vec4,
-                                              vpr, lpr, sh, noclip, gate, epoch, ki, s);
-    }
-  } else if (vpr <= lpr && max_norm > 0.f) {
-    ClipArg<true> clip;
-    clip.max_norm = max_norm;
-    launch_segment_sum<float>(t->view, t->sm_count, slots, seg_start, weights, batch, combiner, default_row, out, vec4, vpr,
-                              lpr, sh, clip, gate, epoch, s);
-  } else if (max_norm > 0.f) {
+  if (max_norm > 0.f && !(vpr <= lpr)) {
     rc = fail(DET_UNIMPLEMENTED, "det_lookup_sparse_clip: max_norm is fused for rows of at most 32 vectors (dim <= 128 when "
                                  "dim % 4 == 0, else dim <= 32); use the composed path for wider rows");
-  } else if (vt == DET_FLOAT32) {
-    launch_segment_sum<float>(t->view, t->sm_count, slots, seg_start, weights, batch, combiner, default_row, out, vec4, vpr,
-                              lpr, sh, noclip, gate, epoch, s);
-  } else if (vt == DET_FLOAT16) {
-    launch_segment_sum<__half>(t->view, t->sm_count, slots, seg_start, weights, batch, combiner, default_row, out, vec4, vpr,
-                               lpr, sh, noclip, gate, epoch, s);
   } else {
-    launch_segment_sum<__nv_bfloat16>(t->view, t->sm_count, slots, seg_start, weights, batch, combiner, default_row, out,
-                                      vec4, vpr, lpr, sh, noclip, gate, epoch, s);
+    // a keyed launch has no default row: default_row is NULL
+    dispatch_bit(keyed, [&](auto KEYED) -> det_status {
+      constexpr bool kKeyed = decltype(KEYED)::value;
+      const InitArg<kKeyed> ki = init_arg<kKeyed>(t, (const long long*)ids);
+      auto sum = [&](auto row, const auto& clip) -> det_status {
+        launch_segment_sum<typename decltype(row)::type>(t->view, t->sm_count, slots, seg_start, weights, batch, combiner,
+                                                         default_row, out, vec4, vpr, lpr, sh, clip, gate, epoch, ki, s);
+        return DET_OK;
+      };
+      if (max_norm > 0.f) {   // float32 tables only (refused above otherwise)
+        ClipArg<true> clip;
+        clip.max_norm = max_norm;
+        return sum(RowType<float>(), clip);
+      }
+      return dispatch_row_type(vt, [&](auto row) -> det_status { return sum(row, ClipArg<false>()); });
+    });
   }
   if (rc == DET_OK && cudaGetLastError() != cudaSuccess) rc = fail(DET_CUDA_ERROR, "det_lookup_sparse: launch failed");
   return rc;
@@ -2073,9 +2049,6 @@ static det_status apply_common(det_table* t, const int64_t* keys, const float* g
   if (keyed && !t->keyed) return fail(DET_INVALID_ARGUMENT, "det_apply: null init_param (the table has no keyed initializer)");
   if (keyed && full_init)
     return fail(DET_INVALID_ARGUMENT, "det_apply: full_size_init needs init_param rows (NULL generates them)");
-  InitArg<true> ki{};
-  static_cast<KeyedInit&>(ki) = t->init;
-  ki.ids = nullptr;
   det::DevGuard _dg(t->cfg.device);
   const unsigned dim = (unsigned)t->cfg.dim;
   const bool vec4 = (dim % 4 == 0) && ((((uintptr_t)grads | (uintptr_t)init_param) & 15u) == 0);
@@ -2094,29 +2067,22 @@ static det_status apply_common(det_table* t, const int64_t* keys, const float* g
     const int tma = (((uintptr_t)keys & 15u) == 0) ? 1 : 0;
     st = dispatch_row_type(vt, [&](auto row) -> det_status {
       return dispatch_bit(t->ev != nullptr, [&](auto SCORED) -> det_status {
-        return dispatch_int<kNumOpts>(opt, [&](auto OPT) -> det_status {
-          constexpr bool kScored = decltype(SCORED)::value;
-          ScoreArg<kScored> sa;
-          if constexpr (kScored) {
-            sa.sc = evict_scores(t);
-            sa.rule = evict_rule(t);
-          }
-          if (keyed) {
-            const auto kern = apply_staged_kernel<decltype(OPT)::value, kScored, typename decltype(row)::type, true>;
+        return dispatch_bit(keyed, [&](auto KEYED) -> det_status {
+          return dispatch_int<kNumOpts>(opt, [&](auto OPT) -> det_status {
+            constexpr bool kScored = decltype(SCORED)::value, kKeyed = decltype(KEYED)::value;
+            ScoreArg<kScored> sa;
+            if constexpr (kScored) {
+              sa.sc = evict_scores(t);
+              sa.rule = evict_rule(t);
+            }
+            const auto kern = apply_staged_kernel<decltype(OPT)::value, kScored, typename decltype(row)::type, kKeyed>;
             CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
             int occ = 1;
             if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, kThreadsF, smem) != cudaSuccess || occ < 1) occ = 1;
             DET_LAUNCH(kern, grid_for(n, kTileKeys, t->sm_count, occ), kThreadsF, smem, s, v, k, grads, n, h, init_param,
-                       0, vpr, lpr, sh, tma, sa, n_dev, slot_planes_arg<decltype(OPT)::value>(t), ki);
+                       full_init, vpr, lpr, sh, tma, sa, n_dev, slot_planes_arg<decltype(OPT)::value>(t), init_arg<kKeyed>(t));
             return DET_OK;
-          }
-          const auto kern = apply_staged_kernel<decltype(OPT)::value, kScored, typename decltype(row)::type>;
-          CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-          int occ = 1;
-          if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, kThreadsF, smem) != cudaSuccess || occ < 1) occ = 1;
-          DET_LAUNCH(kern, grid_for(n, kTileKeys, t->sm_count, occ), kThreadsF, smem, s, v, k, grads, n, h, init_param,
-                     full_init, vpr, lpr, sh, tma, sa, n_dev, slot_planes_arg<decltype(OPT)::value>(t), InitArg<false>());
-          return DET_OK;
+          });
         });
       });
     });
@@ -2128,18 +2094,14 @@ static det_status apply_common(det_table* t, const int64_t* keys, const float* g
   dispatch_row_type(vt, [&](auto row) -> det_status {
     return dispatch_int<kNumOpts>(opt, [&](auto OPT) -> det_status {
       return dispatch_bit(vec4, [&](auto VEC4) -> det_status {
-        if (keyed) {
-          const auto kern = apply_kernel<decltype(VEC4)::value ? 4 : 1, decltype(OPT)::value, typename decltype(row)::type, true>;
+        return dispatch_bit(keyed, [&](auto KEYED) -> det_status {
+          constexpr bool kKeyed = decltype(KEYED)::value;
+          const auto kern = apply_kernel<decltype(VEC4)::value ? 4 : 1, decltype(OPT)::value, typename decltype(row)::type, kKeyed>;
           const int grid = grid_for(n, kTileKeys, t->sm_count, occupancy_of(kern, kThreadsF));
-          DET_LAUNCH(kern, grid, kThreadsF, 0, s, v, k, grads, n, h, init_param, 0, vpr, lpr, sh,
-                     (((uintptr_t)keys & 15u) == 0) ? 1 : 0, slot_planes_arg<decltype(OPT)::value>(t), ki);
+          DET_LAUNCH(kern, grid, kThreadsF, 0, s, v, k, grads, n, h, init_param, full_init, vpr, lpr, sh,
+                     (((uintptr_t)keys & 15u) == 0) ? 1 : 0, slot_planes_arg<decltype(OPT)::value>(t), init_arg<kKeyed>(t));
           return DET_OK;
-        }
-        const auto kern = apply_kernel<decltype(VEC4)::value ? 4 : 1, decltype(OPT)::value, typename decltype(row)::type>;
-        const int grid = grid_for(n, kTileKeys, t->sm_count, occupancy_of(kern, kThreadsF));
-        DET_LAUNCH(kern, grid, kThreadsF, 0, s, v, k, grads, n, h, init_param, full_init, vpr, lpr, sh,
-                   (((uintptr_t)keys & 15u) == 0) ? 1 : 0, slot_planes_arg<decltype(OPT)::value>(t), InitArg<false>());
-        return DET_OK;
+        });
       });
     });
   });
@@ -2152,49 +2114,28 @@ static det_status apply_common(det_table* t, const int64_t* keys, const float* g
 det_status det_apply_adagrad(det_table* t, const int64_t* keys, const float* grads, size_t n, float lr, float epsilon,
                              const float* init_param, int full_size_init, float init_accum, det_stream_t stream) {
   OptHyper h;
-  h.lr = lr; h.eps = epsilon; h.beta1 = 0.f; h.beta2 = 0.f; h.init_slot = init_accum;
-  if (t) t->slot_init[1] = init_accum;
-  return apply_common(t, keys, grads, n, h, init_param, full_size_init, 0, (cudaStream_t)stream);
+  int opt;
+  if (det_status st = adagrad_hyper(lr, epsilon, init_accum, &h, &opt)) return st;
+  record_slot_init(t, opt, h);
+  return apply_common(t, keys, grads, n, h, init_param, full_size_init, opt, (cudaStream_t)stream);
 }
 
 det_status det_apply_adam(det_table* t, const int64_t* keys, const float* grads, size_t n, float alpha, float beta1,
                           float beta2, float epsilon, const float* init_param, int full_size_init,
                           det_stream_t stream) {
   OptHyper h;
-  h.lr = alpha; h.eps = epsilon; h.beta1 = beta1; h.beta2 = beta2; h.init_slot = 0.f;
-  return apply_common(t, keys, grads, n, h, init_param, full_size_init, 1, (cudaStream_t)stream);
-}
-
-// SGD (momentum == 0, OPT 2) or momentum (OPT 3); sets *opt.  A momentum table's unstepped keys export 0.
-static det_status sgd_hyper(det_table* t, float lr, float momentum, int nesterov, OptHyper* h, int* opt) {
-  if (nesterov && momentum == 0.f) return fail(DET_INVALID_ARGUMENT, "det_apply_sgd: nesterov needs a momentum");
-  h->lr = lr; h->eps = nesterov ? 1.f : 0.f; h->beta1 = momentum; h->beta2 = 0.f; h->init_slot = 0.f;
-  *opt = momentum == 0.f ? 2 : 3;
-  if (t && *opt == 3) t->slot_init[1] = 0.f;
-  return DET_OK;
-}
-
-// FTRL (OPT 4): lr > 0 and l1, l2, l2_shrinkage, init_accum >= 0 as TF's ApplyFtrl checks them; 2*l2 and
-// 2*l2_shrinkage are exact in fp32
-static det_status ftrl_hyper(det_table* t, float lr, float l1, float l2, float l2_shrinkage, float init_accum,
-                             OptHyper* h) {
-  if (!(lr > 0.f)) return fail(DET_INVALID_ARGUMENT, "det_apply_ftrl: lr must be positive");
-  if (!(l1 >= 0.f) || !(l2 >= 0.f) || !(l2_shrinkage >= 0.f) || !(init_accum >= 0.f))
-    return fail(DET_INVALID_ARGUMENT, "det_apply_ftrl: l1, l2, l2_shrinkage and init_accum must be >= 0");
-  h->lr = lr; h->eps = l1; h->beta1 = 2.f * l2; h->beta2 = 2.f * l2_shrinkage; h->init_slot = init_accum;
-  if (t) {
-    t->slot_init[1] = init_accum;
-    t->slot_init[2] = 0.f;
-  }
-  return DET_OK;
+  int opt;
+  if (det_status st = adam_hyper(alpha, beta1, beta2, epsilon, &h, &opt)) return st;
+  record_slot_init(t, opt, h);
+  return apply_common(t, keys, grads, n, h, init_param, full_size_init, opt, (cudaStream_t)stream);
 }
 
 det_status det_apply_sgd(det_table* t, const int64_t* keys, const float* grads, size_t n, float lr, float momentum,
                          int nesterov, const float* init_param, int full_size_init, det_stream_t stream) {
   OptHyper h;
-  int opt = 2;
-  const det_status st = sgd_hyper(t, lr, momentum, nesterov, &h, &opt);
-  if (st != DET_OK) return st;
+  int opt;
+  if (det_status st = sgd_hyper(lr, momentum, nesterov, &h, &opt)) return st;
+  record_slot_init(t, opt, h);
   return apply_common(t, keys, grads, n, h, init_param, full_size_init, opt, (cudaStream_t)stream);
 }
 
@@ -2202,9 +2143,10 @@ det_status det_apply_ftrl(det_table* t, const int64_t* keys, const float* grads,
                           float l2_shrinkage, const float* init_param, int full_size_init, float init_accum,
                           det_stream_t stream) {
   OptHyper h;
-  const det_status st = ftrl_hyper(t, lr, l1, l2, l2_shrinkage, init_accum, &h);
-  if (st != DET_OK) return st;
-  return apply_common(t, keys, grads, n, h, init_param, full_size_init, 4, (cudaStream_t)stream);
+  int opt;
+  if (det_status st = ftrl_hyper(lr, l1, l2, l2_shrinkage, init_accum, &h, &opt)) return st;
+  record_slot_init(t, opt, h);
+  return apply_common(t, keys, grads, n, h, init_param, full_size_init, opt, (cudaStream_t)stream);
 }
 
 size_t det_partition_workspace_bytes(size_t n, int num_shards) {
@@ -2299,7 +2241,7 @@ det_status det_sparse_segment_sum(const float* rows, size_t dim, const int64_t* 
   unsigned vpr, lpr, sh;
   fgeom((unsigned)dim, vec4, 1, &vpr, &lpr, &sh);
   launch_segment_sum<float>(v, sms, slots, seg_start, weights, batch, combiner, default_row, out, vec4, vpr, lpr, sh,
-                            ClipArg<false>(), nullptr, 0u, s);
+                            ClipArg<false>(), nullptr, 0u, InitArg<false>(), s);
   CUDA_TRY(cudaGetLastError());
   return DET_OK;
 }
@@ -2548,26 +2490,29 @@ det_status det_apply_adagrad_dup(det_table* t, const int64_t* ids, const float* 
                                  const float* init_param, float init_accum, void* workspace, size_t workspace_bytes,
                                  int64_t* n_unique_dev_out, det_stream_t stream) {
   OptHyper h;
-  h.lr = lr; h.eps = epsilon; h.beta1 = 0.f; h.beta2 = 0.f; h.init_slot = init_accum;
-  if (t) t->slot_init[1] = init_accum;
-  return apply_dup(t, ids, grads, n, h, init_param, 0, workspace, workspace_bytes, n_unique_dev_out, (cudaStream_t)stream);
+  int opt;
+  if (det_status st = adagrad_hyper(lr, epsilon, init_accum, &h, &opt)) return st;
+  record_slot_init(t, opt, h);
+  return apply_dup(t, ids, grads, n, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out, (cudaStream_t)stream);
 }
 
 det_status det_apply_adam_dup(det_table* t, const int64_t* ids, const float* grads, size_t n, float alpha, float beta1,
                               float beta2, float epsilon, const float* init_param, void* workspace, size_t workspace_bytes,
                               int64_t* n_unique_dev_out, det_stream_t stream) {
   OptHyper h;
-  h.lr = alpha; h.eps = epsilon; h.beta1 = beta1; h.beta2 = beta2; h.init_slot = 0.f;
-  return apply_dup(t, ids, grads, n, h, init_param, 1, workspace, workspace_bytes, n_unique_dev_out, (cudaStream_t)stream);
+  int opt;
+  if (det_status st = adam_hyper(alpha, beta1, beta2, epsilon, &h, &opt)) return st;
+  record_slot_init(t, opt, h);
+  return apply_dup(t, ids, grads, n, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out, (cudaStream_t)stream);
 }
 
 det_status det_apply_sgd_dup(det_table* t, const int64_t* ids, const float* grads, size_t n, float lr, float momentum,
                              int nesterov, const float* init_param, void* workspace, size_t workspace_bytes,
                              int64_t* n_unique_dev_out, det_stream_t stream) {
   OptHyper h;
-  int opt = 2;
-  const det_status st = sgd_hyper(t, lr, momentum, nesterov, &h, &opt);
-  if (st != DET_OK) return st;
+  int opt;
+  if (det_status st = sgd_hyper(lr, momentum, nesterov, &h, &opt)) return st;
+  record_slot_init(t, opt, h);
   return apply_dup(t, ids, grads, n, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out, (cudaStream_t)stream);
 }
 
@@ -2575,9 +2520,10 @@ det_status det_apply_ftrl_dup(det_table* t, const int64_t* ids, const float* gra
                               float l2_shrinkage, const float* init_param, float init_accum, void* workspace,
                               size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream) {
   OptHyper h;
-  const det_status st = ftrl_hyper(t, lr, l1, l2, l2_shrinkage, init_accum, &h);
-  if (st != DET_OK) return st;
-  return apply_dup(t, ids, grads, n, h, init_param, 4, workspace, workspace_bytes, n_unique_dev_out, (cudaStream_t)stream);
+  int opt;
+  if (det_status st = ftrl_hyper(lr, l1, l2, l2_shrinkage, init_accum, &h, &opt)) return st;
+  record_slot_init(t, opt, h);
+  return apply_dup(t, ids, grads, n, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out, (cudaStream_t)stream);
 }
 
 det_status det_apply_adagrad_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
@@ -2585,11 +2531,12 @@ det_status det_apply_adagrad_sparse(det_table* t, const int64_t* ids, const int3
                                     const float* init_param, float init_accum, void* workspace, size_t workspace_bytes,
                                     int64_t* n_unique_dev_out, det_stream_t stream) {
   OptHyper h;
-  h.lr = lr; h.eps = epsilon; h.beta1 = 0.f; h.beta2 = 0.f; h.init_slot = init_accum;
-  if (t) t->slot_init[1] = init_accum;
+  int opt;
+  if (det_status st = adagrad_hyper(lr, epsilon, init_accum, &h, &opt)) return st;
+  record_slot_init(t, opt, h);
   const SparseSrc sp{segment_ids, weights, batch, combiner};
-  return apply_dup(t, ids, gout, nnz, h, init_param, 0, workspace, workspace_bytes, n_unique_dev_out, (cudaStream_t)stream,
-                   nullptr, &sp);
+  return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
+                   (cudaStream_t)stream, nullptr, &sp);
 }
 
 det_status det_apply_adam_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
@@ -2597,10 +2544,12 @@ det_status det_apply_adam_sparse(det_table* t, const int64_t* ids, const int32_t
                                  float beta2, float epsilon, const float* init_param, void* workspace,
                                  size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream) {
   OptHyper h;
-  h.lr = alpha; h.eps = epsilon; h.beta1 = beta1; h.beta2 = beta2; h.init_slot = 0.f;
+  int opt;
+  if (det_status st = adam_hyper(alpha, beta1, beta2, epsilon, &h, &opt)) return st;
+  record_slot_init(t, opt, h);
   const SparseSrc sp{segment_ids, weights, batch, combiner};
-  return apply_dup(t, ids, gout, nnz, h, init_param, 1, workspace, workspace_bytes, n_unique_dev_out, (cudaStream_t)stream,
-                   nullptr, &sp);
+  return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
+                   (cudaStream_t)stream, nullptr, &sp);
 }
 
 det_status det_apply_sgd_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
@@ -2608,9 +2557,9 @@ det_status det_apply_sgd_sparse(det_table* t, const int64_t* ids, const int32_t*
                                 int nesterov, const float* init_param, void* workspace, size_t workspace_bytes,
                                 int64_t* n_unique_dev_out, det_stream_t stream) {
   OptHyper h;
-  int opt = 2;
-  const det_status st = sgd_hyper(t, lr, momentum, nesterov, &h, &opt);
-  if (st != DET_OK) return st;
+  int opt;
+  if (det_status st = sgd_hyper(lr, momentum, nesterov, &h, &opt)) return st;
+  record_slot_init(t, opt, h);
   const SparseSrc sp{segment_ids, weights, batch, combiner};
   return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
                    (cudaStream_t)stream, nullptr, &sp);
@@ -2621,25 +2570,23 @@ det_status det_apply_ftrl_sparse(det_table* t, const int64_t* ids, const int32_t
                                  float l2_shrinkage, const float* init_param, float init_accum, void* workspace,
                                  size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream) {
   OptHyper h;
-  const det_status st = ftrl_hyper(t, lr, l1, l2, l2_shrinkage, init_accum, &h);
-  if (st != DET_OK) return st;
+  int opt;
+  if (det_status st = ftrl_hyper(lr, l1, l2, l2_shrinkage, init_accum, &h, &opt)) return st;
+  record_slot_init(t, opt, h);
   const SparseSrc sp{segment_ids, weights, batch, combiner};
-  return apply_dup(t, ids, gout, nnz, h, init_param, 4, workspace, workspace_bytes, n_unique_dev_out, (cudaStream_t)stream,
-                   nullptr, &sp);
+  return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
+                   (cudaStream_t)stream, nullptr, &sp);
 }
 
 }  // extern "C"
 
 namespace det {
 // owner side of the sharded backward (sharded.cu): ids / grads were compacted out of the inbox segments by a kernel,
-// their count lives in *n_items_dev; opt 0 = Adagrad (lr, eps, init_slot), 1 = Adam (lr = alpha, eps, beta1, beta2)
+// their count lives in *n_items_dev; h and opt come from adagrad_hyper or adam_hyper
 det_status apply_dup_on_device_count(det_table* t, const int64_t* ids, const float* grads, size_t n_bound,
-                                     const long long* n_items_dev, int opt, float lr, float eps, float beta1, float beta2,
-                                     float init_slot, const float* init_param, void* workspace, size_t workspace_bytes,
-                                     cudaStream_t s) {
-  OptHyper h;
-  h.lr = lr; h.eps = eps; h.beta1 = beta1; h.beta2 = beta2; h.init_slot = init_slot;
-  if (t && opt == 0) t->slot_init[1] = init_slot;
+                                     const long long* n_items_dev, const OptHyper& h, int opt, const float* init_param,
+                                     void* workspace, size_t workspace_bytes, cudaStream_t s) {
+  record_slot_init(t, opt, h);
   // the owner side does not generate rows: the exchange always passes the initial param row
   if (!init_param) return fail(DET_INVALID_ARGUMENT, "det_peer_xchg_apply: null init_param");
   return apply_dup(t, ids, grads, n_bound, h, init_param, opt, workspace, workspace_bytes, nullptr, s, n_items_dev);

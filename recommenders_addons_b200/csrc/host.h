@@ -276,11 +276,23 @@ det_status table_clear_async(det_table* t, cudaStream_t s);
 det_status table_scratch(det_table* t, size_t bytes, void** out);
 void host_pipe_free(det_table* t);
 det_status rehash_to(det_table* t, uint64_t new_nb, cudaStream_t s);
-// fused.cu: unique -> position-order gradient sum -> fused optimizer step with the id count on the device (sharded.cu)
+// fused.cu: the optimizers of the fused find-or-insert step (K7, its template parameter OPT) and their
+// hyper-parameters.  What each OptHyper field holds depends on the optimizer (listed at opt_step); only the builders
+// (adagrad_hyper, adam_hyper, sgd_hyper, ftrl_hyper) fill them.
+enum : int { kAdagrad, kAdam, kSgd, kMomentum, kFtrl, kNumOpts };
+struct OptHyper {
+  float lr;
+  float eps;
+  float beta1, beta2;
+  float init_slot;
+};
+// validate the hyper-parameters, fill *h and set *opt
+det_status adagrad_hyper(float lr, float epsilon, float init_accum, OptHyper* h, int* opt);
+det_status adam_hyper(float alpha, float beta1, float beta2, float epsilon, OptHyper* h, int* opt);
+// unique -> position-order gradient sum -> fused optimizer step with the id count on the device (sharded.cu)
 det_status apply_dup_on_device_count(det_table* t, const int64_t* ids, const float* grads, size_t n_bound,
-                                     const long long* n_items_dev, int opt, float lr, float eps, float beta1, float beta2,
-                                     float init_slot, const float* init_param, void* workspace, size_t workspace_bytes,
-                                     cudaStream_t s);
+                                     const long long* n_items_dev, const OptHyper& h, int opt, const float* init_param,
+                                     void* workspace, size_t workspace_bytes, cudaStream_t s);
 // evict.cu (all called with t->mu held, except evict_insert which takes it)
 det_status evict_attach(det_table* t, int strategy);
 void evict_free(det_table* t);

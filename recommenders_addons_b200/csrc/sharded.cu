@@ -1215,9 +1215,8 @@ size_t det_peer_xchg_apply_workspace_bytes(det_peer_group* g) {
   return xchg_apply_layout(g, nullptr, nullptr, nullptr, nullptr);
 }
 
-static det_status xchg_apply(det_peer_group* g, const int64_t* keys, const float* grads, size_t n, int opt, float lr,
-                             float eps, float beta1, float beta2, float init_slot, const float* init_param,
-                             void* workspace, size_t workspace_bytes, cudaStream_t s) {
+static det_status xchg_apply(det_peer_group* g, const int64_t* keys, const float* grads, size_t n, const OptHyper& h,
+                             int opt, const float* init_param, void* workspace, size_t workspace_bytes, cudaStream_t s) {
   if (!g || !g->xchg) return fail(DET_INVALID_ARGUMENT, "det_peer_xchg_apply: no exchange mailbox attached");
   if (g->local->cfg.value_dtype != DET_FLOAT32) return fail(DET_UNIMPLEMENTED, "det_peer_xchg_apply: float32 tables only");
   if (n > g->xv.cap) return fail(DET_INVALID_ARGUMENT, "det_peer_xchg_apply: batch larger than the mailbox (max_items)");
@@ -1237,8 +1236,8 @@ static det_status xchg_apply(det_peer_group* g, const int64_t* keys, const float
   if (rc != DET_OK) return rc;
   CUDA_TRY(cudaGetLastError());
   const size_t bound = (size_t)g->pv.world * g->xv.cap;
-  rc = det::apply_dup_on_device_count(g->local, (const int64_t*)in.keys, (const float*)in.rows, bound, in.n_dev, opt, lr,
-                                      eps, beta1, beta2, init_slot, init_param, dup, dup_bytes, s);
+  rc = det::apply_dup_on_device_count(g->local, (const int64_t*)in.keys, (const float*)in.rows, bound, in.n_dev, h, opt,
+                                      init_param, dup, dup_bytes, s);
   if (rc != DET_OK) return rc;
   peer_snapshot(g, s);
   return DET_OK;
@@ -1247,15 +1246,19 @@ static det_status xchg_apply(det_peer_group* g, const int64_t* keys, const float
 det_status det_peer_xchg_apply_adagrad(det_peer_group* g, const int64_t* keys, const float* grads, size_t n, float lr,
                                        float epsilon, const float* init_param, float init_accum, void* workspace,
                                        size_t workspace_bytes, det_stream_t stream) {
-  return xchg_apply(g, keys, grads, n, 0, lr, epsilon, 0.f, 0.f, init_accum, init_param, workspace, workspace_bytes,
-                    (cudaStream_t)stream);
+  OptHyper h;
+  int opt;
+  if (det_status st = det::adagrad_hyper(lr, epsilon, init_accum, &h, &opt)) return st;
+  return xchg_apply(g, keys, grads, n, h, opt, init_param, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 det_status det_peer_xchg_apply_adam(det_peer_group* g, const int64_t* keys, const float* grads, size_t n, float alpha,
                                     float beta1, float beta2, float epsilon, const float* init_param, void* workspace,
                                     size_t workspace_bytes, det_stream_t stream) {
-  return xchg_apply(g, keys, grads, n, 1, alpha, epsilon, beta1, beta2, 0.f, init_param, workspace, workspace_bytes,
-                    (cudaStream_t)stream);
+  OptHyper h;
+  int opt;
+  if (det_status st = det::adam_hyper(alpha, beta1, beta2, epsilon, &h, &opt)) return st;
+  return xchg_apply(g, keys, grads, n, h, opt, init_param, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 det_status det_peer_find(det_peer_group* g, const int64_t* keys, size_t n, const void* defaults,
