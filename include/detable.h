@@ -310,6 +310,22 @@ det_status det_apply_sgd(det_table* t, const int64_t* keys, const float* grads, 
 det_status det_apply_ftrl(det_table* t, const int64_t* keys, const float* grads, size_t n, float lr, float l1, float l2,
                           float l2_shrinkage, const float* init_param, int full_size_init, float init_accum,
                           det_stream_t stream);
+/* The same step for RMSprop and Adadelta; r = 1 - rho, computed once in fp32.  Correctly rounded square roots and one
+ * division where TF's CPU kernels multiply by rsqrt (not bit-identical to TF, see DESIGN.md section 4).
+ * RMSprop: ms = ms*rho + (g*g)*r;  centered: mg = mg*rho + g*r, d = ms - mg*mg;  else d = ms;
+ *   momentum > 0:  mom = mom*momentum + (lr*g) / sqrt(d + eps);  p = p - mom;
+ *   momentum == 0: p = p - (lr*g) / (eps_in_sqrt ? sqrt(d + eps) : sqrt(d) + eps).
+ *   Planes: 1 = rms (initial init_ms), then mg if centered, then mom if momentum > 0 (initial 0); 1 to 3 planes.
+ *   Keras RMSprop: eps_in_sqrt = (momentum > 0), init_ms = 0;  TF1 RMSPropOptimizer: eps_in_sqrt = 1, init_ms = 1.
+ *   A negative or NaN momentum, or momentum > 0 with eps_in_sqrt == 0: DET_INVALID_ARGUMENT.
+ * Adadelta (TF1 AdadeltaOptimizer, Keras Adadelta): acc = acc*rho + (g*g)*r;  u = (sqrt(au + eps) / sqrt(acc + eps))*g;
+ *   p = p - u*lr;  au = au*rho + (u*u)*r.  Plane 1 = accum_grad acc, plane 2 = accum_var au (both initial 0).
+ * Additive to ABI 8. */
+det_status det_apply_rmsprop(det_table* t, const int64_t* keys, const float* grads, size_t n, float lr, float rho,
+                             float momentum, float epsilon, int centered, int eps_in_sqrt, const float* init_param,
+                             int full_size_init, float init_ms, det_stream_t stream);
+det_status det_apply_adadelta(det_table* t, const int64_t* keys, const float* grads, size_t n, float lr, float rho,
+                              float epsilon, const float* init_param, int full_size_init, det_stream_t stream);
 
 /* ---- HOST-buffer entry points (the op placed on host tensors; used for end-to-end timing):
  * pinned or pageable HOST pointers; chunked H2D -> kernel -> D2H pipeline on internal streams;
@@ -353,6 +369,13 @@ det_status det_apply_sgd_dup(det_table* t, const int64_t* ids, const float* grad
 det_status det_apply_ftrl_dup(det_table* t, const int64_t* ids, const float* grads, size_t n, float lr, float l1,
                               float l2, float l2_shrinkage, const float* init_param, float init_accum, void* workspace,
                               size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_rmsprop_dup(det_table* t, const int64_t* ids, const float* grads, size_t n, float lr, float rho,
+                                 float momentum, float epsilon, int centered, int eps_in_sqrt, const float* init_param,
+                                 float init_ms, void* workspace, size_t workspace_bytes, int64_t* n_unique_dev_out,
+                                 det_stream_t stream);
+det_status det_apply_adadelta_dup(det_table* t, const int64_t* ids, const float* grads, size_t n, float lr, float rho,
+                                  float epsilon, const float* init_param, void* workspace, size_t workspace_bytes,
+                                  int64_t* n_unique_dev_out, det_stream_t stream);
 
 /* The backward of det_lookup_sparse, fused: per-unique-id gradients straight from the output gradient (ABI >= 8).
  * Inputs are the forward's ids int64[nnz], segment_ids int32[nnz] (ascending, in [0, batch)), weights f32[nnz] or NULL
@@ -396,6 +419,15 @@ det_status det_apply_ftrl_sparse(det_table* t, const int64_t* ids, const int32_t
                                  size_t nnz, size_t batch, int combiner, const float* gout, float lr, float l1, float l2,
                                  float l2_shrinkage, const float* init_param, float init_accum, void* workspace,
                                  size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_rmsprop_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
+                                    size_t nnz, size_t batch, int combiner, const float* gout, float lr, float rho,
+                                    float momentum, float epsilon, int centered, int eps_in_sqrt,
+                                    const float* init_param, float init_ms, void* workspace, size_t workspace_bytes,
+                                    int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_adadelta_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
+                                     size_t nnz, size_t batch, int combiner, const float* gout, float lr, float rho,
+                                     float epsilon, const float* init_param, void* workspace, size_t workspace_bytes,
+                                     int64_t* n_unique_dev_out, det_stream_t stream);
 
 /* ---- key-hash sharding across GPUs (python/ops/dynamic_embedding_variable.py:165-197 default_partition_fn,
  * python/ops/shadow_embedding_ops.py:397-447 alltoall exchange) ----

@@ -109,6 +109,53 @@ REGISTER_OP("TFRA>DetApplyFtrlDuplicateIndices")
     .Attr("l2_shrinkage: float = 0.0")
     .Attr("initial_accumulator_value: float = 0.1");
 
+// RMSprop (ResourceSparseApply(Centered)RMSProp; Keras' momentum-free form with epsilon_in_sqrt = 0) and Adadelta
+// (ResourceSparseApplyAdadelta), as det_apply_rmsprop / det_apply_adadelta.  TF1 RMSPropOptimizer is
+// epsilon_in_sqrt = 1, initial_accumulator_value = 1.0.
+REGISTER_OP("TFRA>DetApplyRmsprop")
+    .Input("table_handle: resource")
+    .Input("keys: int64")          // [n] unique
+    .Input("grads: float")         // [n, dim]
+    .Input("lr: float")
+    .Input("init_param: float")    // [dim] or [n, dim]
+    .Attr("rho: float = 0.9")
+    .Attr("momentum: float = 0.0")
+    .Attr("epsilon: float = 1e-7")
+    .Attr("centered: int = 0")
+    .Attr("epsilon_in_sqrt: int = 0")   // must be 1 with momentum > 0
+    .Attr("initial_accumulator_value: float = 0.0");
+
+REGISTER_OP("TFRA>DetApplyAdadelta")
+    .Input("table_handle: resource")
+    .Input("keys: int64")
+    .Input("grads: float")
+    .Input("lr: float")
+    .Input("init_param: float")
+    .Attr("rho: float = 0.95")
+    .Attr("epsilon: float = 1e-7");
+
+REGISTER_OP("TFRA>DetApplyRmspropDuplicateIndices")
+    .Input("table_handle: resource")
+    .Input("ids: int64")
+    .Input("grads: float")
+    .Input("lr: float")
+    .Input("init_param: float")    // [dim]
+    .Attr("rho: float = 0.9")
+    .Attr("momentum: float = 0.0")
+    .Attr("epsilon: float = 1e-7")
+    .Attr("centered: int = 0")
+    .Attr("epsilon_in_sqrt: int = 0")
+    .Attr("initial_accumulator_value: float = 0.0");
+
+REGISTER_OP("TFRA>DetApplyAdadeltaDuplicateIndices")
+    .Input("table_handle: resource")
+    .Input("ids: int64")
+    .Input("grads: float")
+    .Input("lr: float")
+    .Input("init_param: float")    // [dim]
+    .Attr("rho: float = 0.95")
+    .Attr("epsilon: float = 1e-7");
+
 // The gradient dedupe in front of the sparse optimizer step: unsorted_segment_sum(values, idx, num_segments) as
 // _deduplicate_indexed_slices calls it before _resource_apply_sparse_duplicate_indices
 // (python/ops/dynamic_embedding_optimizer.py:150,184), with the rows of one segment added in position order
@@ -356,6 +403,72 @@ class DetApplySgdFtrlOp : public OpKernel {
   int nesterov_ = 0;
 };
 
+// RMSprop (OPT 0) and Adadelta (OPT 1), unique keys (DUP false) or repeated ids in one call (DUP true)
+template <int OPT, bool DUP>
+class DetApplyRmspropAdadeltaOp : public OpKernel {
+ public:
+  explicit DetApplyRmspropAdadeltaOp(OpKernelConstruction* ctx) : OpKernel(ctx) {
+    OP_REQUIRES_OK(ctx, ctx->GetAttr("rho", &rho_));
+    OP_REQUIRES_OK(ctx, ctx->GetAttr("epsilon", &epsilon_));
+    if (OPT == 0) {
+      OP_REQUIRES_OK(ctx, ctx->GetAttr("momentum", &momentum_));
+      OP_REQUIRES_OK(ctx, ctx->GetAttr("centered", &centered_));
+      OP_REQUIRES_OK(ctx, ctx->GetAttr("epsilon_in_sqrt", &eps_in_sqrt_));
+      OP_REQUIRES_OK(ctx, ctx->GetAttr("initial_accumulator_value", &init_ms_));
+    }
+  }
+  void Compute(OpKernelContext* ctx) override {
+    tensorflow::lookup::LookupInterface* table = nullptr;
+    OP_REQUIRES_OK(ctx, GetLookupTable("table_handle", ctx, &table));
+    core::ScopedUnref unref_me(table);
+    det_table* handle = FusedHandle(table);
+    OP_REQUIRES(ctx, handle != nullptr,
+                errors::InvalidArgument(string(OPT == 0 ? "DetApplyRmsprop" : "DetApplyAdadelta") +
+                                        ": the table's value dtype must be float, half or bfloat16"));
+    const Tensor& keys = ctx->input(1);
+    const Tensor& grads = ctx->input(2);
+    const Tensor& lr = ctx->input(3);
+    const Tensor& init = ctx->input(4);
+    const int64 n = keys.NumElements(), dim = table->value_shape().dim_size(0);
+    OP_REQUIRES(ctx, grads.NumElements() == n * dim, errors::InvalidArgument("grads must have shape [n, dim]"));
+    OP_REQUIRES(ctx, init.NumElements() == dim || (!DUP && init.NumElements() == n * dim),
+                errors::InvalidArgument(DUP ? "init_param must have shape [dim]" : "init_param must have shape [dim] or [n, dim]"));
+    const int64_t* k = reinterpret_cast<const int64_t*>(keys.flat<int64>().data());
+    const float* g = grads.flat<float>().data();
+    const float* ip = init.flat<float>().data();
+    const float step = lr.scalar<float>()();
+    const size_t nn = static_cast<size_t>(n);
+    if (!DUP) {
+      const int full = init.NumElements() == dim ? 0 : 1;
+      if (OPT == 0) {
+        OP_REQUIRES_OK(ctx, ToStatus(det_apply_rmsprop(handle, k, g, nn, step, rho_, momentum_, epsilon_, centered_,
+                                                       eps_in_sqrt_, ip, full, init_ms_, StreamOf(ctx))));
+      } else {
+        OP_REQUIRES_OK(ctx, ToStatus(det_apply_adadelta(handle, k, g, nn, step, rho_, epsilon_, ip, full, StreamOf(ctx))));
+      }
+      return;
+    }
+    if (n == 0) return;
+    const size_t ws_bytes = det_apply_dup_workspace_bytes(nn, static_cast<size_t>(dim));
+    Tensor ws;
+    OP_REQUIRES_OK(ctx, ctx->allocate_temp(DT_INT8, TensorShape({static_cast<int64>(ws_bytes + 256)}), &ws));
+    int8* raw = ws.flat<int8>().data();
+    void* aligned = raw + ((256 - (reinterpret_cast<uintptr_t>(raw) & 255u)) & 255u);
+    if (OPT == 0) {
+      OP_REQUIRES_OK(ctx, ToStatus(det_apply_rmsprop_dup(handle, k, g, nn, step, rho_, momentum_, epsilon_, centered_,
+                                                         eps_in_sqrt_, ip, init_ms_, aligned, ws_bytes, nullptr,
+                                                         StreamOf(ctx))));
+    } else {
+      OP_REQUIRES_OK(ctx, ToStatus(det_apply_adadelta_dup(handle, k, g, nn, step, rho_, epsilon_, ip, aligned, ws_bytes,
+                                                          nullptr, StreamOf(ctx))));
+    }
+  }
+
+ private:
+  float rho_ = 0.9f, momentum_ = 0.f, epsilon_ = 1e-7f, init_ms_ = 0.f;
+  int centered_ = 0, eps_in_sqrt_ = 0;
+};
+
 class DetSegmentReduceOp : public OpKernel {
  public:
   explicit DetSegmentReduceOp(OpKernelConstruction* ctx) : OpKernel(ctx) {}
@@ -394,6 +507,14 @@ REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplySgdDuplicateIndices").Device(DEVICE_G
                         DetApplySgdFtrlOp<0, true>);
 REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplyFtrlDuplicateIndices").Device(DEVICE_GPU).HostMemory("lr"),
                         DetApplySgdFtrlOp<1, true>);
+REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplyRmsprop").Device(DEVICE_GPU).HostMemory("lr"),
+                        DetApplyRmspropAdadeltaOp<0, false>);
+REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplyAdadelta").Device(DEVICE_GPU).HostMemory("lr"),
+                        DetApplyRmspropAdadeltaOp<1, false>);
+REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplyRmspropDuplicateIndices").Device(DEVICE_GPU).HostMemory("lr"),
+                        DetApplyRmspropAdadeltaOp<0, true>);
+REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplyAdadeltaDuplicateIndices").Device(DEVICE_GPU).HostMemory("lr"),
+                        DetApplyRmspropAdadeltaOp<1, true>);
 
 }  // namespace det_shim
 }  // namespace lookup

@@ -84,6 +84,13 @@ SIGNATURES = {
     "det_apply_sgd_dup": (_i, [_vp, _vp, _vp, _sz, ctypes.c_float, ctypes.c_float, _i, _vp, _vp, _sz, _vp, _vp]),
     "det_apply_ftrl_dup": (_i, [_vp, _vp, _vp, _sz, ctypes.c_float, ctypes.c_float, ctypes.c_float, ctypes.c_float, _vp,
                                 ctypes.c_float, _vp, _sz, _vp, _vp]),
+    "det_apply_rmsprop": (_i, [_vp, _vp, _vp, _sz, ctypes.c_float, ctypes.c_float, ctypes.c_float, ctypes.c_float, _i, _i,
+                               _vp, _i, ctypes.c_float, _vp]),
+    "det_apply_adadelta": (_i, [_vp, _vp, _vp, _sz, ctypes.c_float, ctypes.c_float, ctypes.c_float, _vp, _i, _vp]),
+    "det_apply_rmsprop_dup": (_i, [_vp, _vp, _vp, _sz, ctypes.c_float, ctypes.c_float, ctypes.c_float, ctypes.c_float, _i,
+                                   _i, _vp, ctypes.c_float, _vp, _sz, _vp, _vp]),
+    "det_apply_adadelta_dup": (_i, [_vp, _vp, _vp, _sz, ctypes.c_float, ctypes.c_float, ctypes.c_float, _vp, _vp, _sz, _vp,
+                                    _vp]),
     "det_lookup_sparse_grad_workspace_bytes": (_sz, [_sz, _sz, _sz]),
     "det_lookup_sparse_grad": (_i, [_vp, _vp, _vp, _sz, _sz, _i, _vp, _sz, _vp, _vp, _vp, _vp, _sz, _vp]),
     "det_apply_sparse_workspace_bytes": (_sz, [_sz, _sz, _sz]),
@@ -95,6 +102,10 @@ SIGNATURES = {
                                   _vp, _vp]),
     "det_apply_ftrl_sparse": (_i, [_vp, _vp, _vp, _vp, _sz, _sz, _i, _vp, ctypes.c_float, ctypes.c_float, ctypes.c_float,
                                    ctypes.c_float, _vp, ctypes.c_float, _vp, _sz, _vp, _vp]),
+    "det_apply_rmsprop_sparse": (_i, [_vp, _vp, _vp, _vp, _sz, _sz, _i, _vp, ctypes.c_float, ctypes.c_float,
+                                      ctypes.c_float, ctypes.c_float, _i, _i, _vp, ctypes.c_float, _vp, _sz, _vp, _vp]),
+    "det_apply_adadelta_sparse": (_i, [_vp, _vp, _vp, _vp, _sz, _sz, _i, _vp, ctypes.c_float, ctypes.c_float,
+                                       ctypes.c_float, _vp, _vp, _sz, _vp, _vp]),
     "det_find_host": (_i, [_vp, _vp, _sz, _vp, _i, _vp, _vp]),
     "det_insert_host": (_i, [_vp, _vp, _vp, _sz]),
     "det_find_host_async": (_i, [_vp, _vp, _sz, _vp, _i, _vp, _vp]),

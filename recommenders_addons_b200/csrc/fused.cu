@@ -769,16 +769,29 @@ segment_sum_wide_kernel(TableView t, const long long* __restrict__ slots, const 
 // ------------------------------------------------------------------------------------------------
 // K7: fused find-or-insert + optimizer update
 // ------------------------------------------------------------------------------------------------
-// The optimizer of a K7 launch is its template parameter OPT (kAdagrad .. kFtrl, host.h) with an OptHyper.
+// The optimizer of a K7 launch is its template parameter OPT (kAdagrad .. kAdadelta, host.h) with an OptHyper.
 
 // slot planes an optimizer reads and writes (planes 1 .. opt_slots(OPT)): Adagrad accumulator = plane 1; Adam m =
-// plane 1, v = plane 2; momentum = plane 1; FTRL accumulator n = plane 1, linear z = plane 2
-__host__ __device__ constexpr int opt_slots(int opt) { return opt == kAdam || opt == kFtrl ? 2 : opt == kSgd ? 0 : 1; }
+// plane 1, v = plane 2; momentum = plane 1; FTRL accumulator n = plane 1, linear z = plane 2; RMSprop rms = plane 1,
+// then mg if centered, then momentum if momentum > 0 (kRmsprop1 .. kRmsprop3); Adadelta accum_grad = plane 1,
+// accum_var = plane 2
+__host__ __device__ constexpr int opt_slots(int opt) {
+  return opt == kRmsprop3 ? 3
+         : opt == kAdam || opt == kFtrl || opt == kRmsprop2 || opt == kAdadelta ? 2
+         : opt == kSgd ? 0 : 1;
+}
 
-// The slot values a key without slot state starts from: a slot 1, b slot 2.
+// The slot values a key without slot state starts from: a slot 1, b slot 2, c slot 3.
 template <int OPT, int VF>
-__device__ __forceinline__ void opt_fresh(const OptHyper& h, FVec<VF>& a, FVec<VF>& b) {
-  if constexpr (OPT == kAdagrad) {
+__device__ __forceinline__ void opt_fresh(const OptHyper& h, FVec<VF>& a, FVec<VF>& b, FVec<VF>& c) {
+  if constexpr (OPT >= kRmsprop1 && OPT <= kRmsprop3) {
+    a.fill(h.init_slot);
+    if constexpr (opt_slots(OPT) > 1) b.zero();
+    if constexpr (opt_slots(OPT) > 2) c.zero();
+  } else if constexpr (OPT == kAdadelta) {
+    a.zero();
+    b.zero();
+  } else if constexpr (OPT == kAdagrad) {
     a.fill(h.init_slot);
   } else if constexpr (OPT == kAdam) {
     a.zero();
@@ -792,17 +805,45 @@ __device__ __forceinline__ void opt_fresh(const OptHyper& h, FVec<VF>& a, FVec<V
 }
 
 // One step of the optimizer, one IEEE fp32 operation per operation in the order written (the library is built with
-// --fmad=false): g gradient, p param, a slot 1, b slot 2, updated in place.  SGD, momentum and FTRL restate TF's sparse
-// CPU kernels (ResourceSparseApplyMomentum, ResourceSparseApplyFtrl(V2) with learning_rate_power = -0.5).
+// --fmad=false): g gradient, p param, a slot 1, b slot 2, c3 slot 3, updated in place.  SGD, momentum and FTRL restate
+// TF's sparse CPU kernels (ResourceSparseApplyMomentum, ResourceSparseApplyFtrl(V2) with learning_rate_power = -0.5);
+// RMSprop and Adadelta restate ResourceSparseApply(Centered)RMSProp and ResourceSparseApplyAdadelta with correctly
+// rounded square roots and one division where TF's CPU kernels multiply by an Eigen rsqrt (DESIGN.md section 4).
 // The hyper-parameters, as the builders fill them:
 //   Adagrad : lr, eps = epsilon, init_slot = initial accumulator
 //   Adam    : lr = alpha, eps = epsilon, beta1, beta2
 //   SGD     : lr
 //   Momentum: lr, eps = 1 for nesterov (else 0), beta1 = momentum
 //   FTRL    : lr, eps = l1, beta1 = 2*l2, beta2 = 2*l2_shrinkage, init_slot = initial accumulator
+//   RMSprop : lr, eps = epsilon, beta1 = rho, beta2 = momentum, init_slot = initial rms, flags = kEpsInSqrt | kCentered
+//   Adadelta: lr, eps = epsilon, beta1 = rho
+// r = 1 - beta1 (RMSprop and Adadelta), computed once per step in fp32.
 template <int OPT>
-__device__ __forceinline__ void opt_elem(const OptHyper& h, float g, float& p, float& a, float& b) {
-  if (OPT == kSgd) {
+__device__ __forceinline__ void opt_elem(const OptHyper& h, float r, float g, float& p, float& a, float& b, float& c3) {
+  if (OPT >= kRmsprop1 && OPT <= kRmsprop3) {
+    // a = rms; kRmsprop2: b = mg (centered) or momentum; kRmsprop3: b = mg, c3 = momentum
+    const bool centered = OPT == kRmsprop3 || (OPT == kRmsprop2 && (h.flags & kCentered));
+    const bool mom = OPT == kRmsprop3 || (OPT == kRmsprop2 && !(h.flags & kCentered));
+    float& m = OPT == kRmsprop3 ? c3 : b;
+    a = a * h.beta1 + (g * g) * r;
+    float d = a;
+    if (centered) {
+      b = b * h.beta1 + g * r;
+      d = a - b * b;
+    }
+    if (mom) {
+      m = m * h.beta2 + (h.lr * g) / sqrtf(d + h.eps);
+      p = p - m;
+    } else {
+      p = p - (h.lr * g) / ((h.flags & kEpsInSqrt) ? sqrtf(d + h.eps) : sqrtf(d) + h.eps);
+    }
+  } else if (OPT == kAdadelta) {
+    // a = accum_grad, b = accum_var
+    a = a * h.beta1 + (g * g) * r;
+    const float u = (sqrtf(b + h.eps) / sqrtf(a + h.eps)) * g;
+    p = p - u * h.lr;
+    b = b * h.beta1 + (u * u) * r;
+  } else if (OPT == kSgd) {
     p = p - h.lr * g;
   } else if (OPT == kMomentum) {
     a = a * h.beta1 + g;
@@ -823,7 +864,8 @@ __device__ __forceinline__ void opt_elem(const OptHyper& h, float g, float& p, f
   }
 }
 template <int OPT, int VF>
-__device__ __forceinline__ void opt_step(const OptHyper& h, const FVec<VF>& g, FVec<VF>& p, FVec<VF>& a, FVec<VF>& b) {
+__device__ __forceinline__ void opt_step(const OptHyper& h, const FVec<VF>& g, FVec<VF>& p, FVec<VF>& a, FVec<VF>& b,
+                                         FVec<VF>& c) {
   if constexpr (OPT == kAdagrad) {
     // accum += g*g ; var -= lr*g / (sqrt(accum) + eps)
     a.zip(g, [](float& av, float gv) { av = av + gv * gv; });
@@ -843,14 +885,16 @@ __device__ __forceinline__ void opt_step(const OptHyper& h, const FVec<VF>& g, F
     float* pv = reinterpret_cast<float*>(&p.v);
     float* av = reinterpret_cast<float*>(&a.v);
     float* bv = reinterpret_cast<float*>(&b.v);
+    float* cv = reinterpret_cast<float*>(&c.v);
+    const float r = 1.f - h.beta1;
 #pragma unroll
-    for (int e = 0; e < VF; ++e) opt_elem<OPT>(h, gv[e], pv[e], av[e], bv[e]);
+    for (int e = 0; e < VF; ++e) opt_elem<OPT>(h, r, gv[e], pv[e], av[e], bv[e], cv[e]);
   }
 }
 
-// The slot-plane count of the table, for the optimizers that mark the slot planes they do not write (SGD, momentum,
-// FTRL): a key such a step creates gets kSlotUninit in the first word of its row in every other slot plane, as insert
-// gives it (table.cu insert_step).  An EMPTY trailing parameter for Adagrad and Adam keeps their kernels unchanged.
+// The slot-plane count of the table, for the optimizers that mark the slot planes they do not write (all but Adagrad
+// and Adam): a key such a step creates gets kSlotUninit in the first word of its row in every other slot plane, as
+// insert gives it (table.cu insert_step).  An EMPTY trailing parameter for Adagrad and Adam keeps their kernels unchanged.
 template <int OPT> struct SlotPlanes { int n; };
 template <> struct SlotPlanes<kAdagrad> {};
 template <> struct SlotPlanes<kAdam> {};
@@ -874,8 +918,9 @@ static SlotPlanes<OPT> slot_planes_arg(const det_table* t) {
 // once, at its store.
 // FTRL's two square roots and three divisions per element: left to its own heuristics ptxas spills the probe's
 // first-bucket loads to reach 4 CTAs per SM; asking for 3 (the register-held Adagrad / Adam kernels' occupancy) keeps
-// them in registers.  0 = no minimum, the other optimizers' kernels as before.
-template <int OPT> constexpr int kApplyMinBlocks = OPT == kFtrl ? 3 : 0;
+// them in registers.  RMSprop spills the same way: its 1-plane kernel keeps 3 CTAs per SM, the 3-plane one (three slot
+// vectors in flight) 2.  0 = no minimum, the other optimizers' kernels as before.
+template <int OPT> constexpr int kApplyMinBlocks = OPT == kFtrl || OPT == kRmsprop1 ? 3 : OPT == kRmsprop3 ? 2 : 0;
 
 // KEYED: a new key's param starts from its row of the table's keyed initializer (init_param is NULL).
 // (keyed: 2 CTAs per SM, the register budget the generator's calls need without spilling, as segment_sum_kernel)
@@ -944,7 +989,7 @@ apply_kernel(TableView t, const long long* __restrict__ keys, const float* __res
       for (int u = 0; u < RU; ++u) fresh[u] = nwv[u] || (mark[u] == kSlotUninit);
       for (unsigned c = c0; c < vpr; c += lpr) {
         const size_t o = (size_t)c * VF;
-        FVec<VF> g[RU], p[RU], a[RU], b[RU];
+        FVec<VF> g[RU], p[RU], a[RU], b[RU], c3[RU];
 #pragma unroll
         for (int u = 0; u < RU; ++u) {
           if (!ok[u]) continue;
@@ -957,18 +1002,20 @@ apply_kernel(TableView t, const long long* __restrict__ keys, const float* __res
             else p[u].load(P + ro[u] + o);
           }
           if (fresh[u]) {
-            opt_fresh<OPT>(h, a[u], b[u]);
+            opt_fresh<OPT>(h, a[u], b[u], c3[u]);
           } else {
             if (opt_slots(OPT) > 0) a[u].load(S1 + ro[u] + o);
             if (opt_slots(OPT) > 1) b[u].load(S2 + ro[u] + o);
+            if constexpr (opt_slots(OPT) > 2) c3[u].load((const float*)t.planes[3] + ro[u] + o);
           }
         }
 #pragma unroll
         for (int u = 0; u < RU; ++u) {
           if (!ok[u]) continue;
-          opt_step<OPT>(h, g[u], p[u], a[u], b[u]);
+          opt_step<OPT>(h, g[u], p[u], a[u], b[u], c3[u]);
           if (opt_slots(OPT) > 0) a[u].store(S1 + ro[u] + o);
           if (opt_slots(OPT) > 1) b[u].store(S2 + ro[u] + o);
+          if constexpr (opt_slots(OPT) > 2) c3[u].store((float*)t.planes[3] + ro[u] + o);
           p[u].store(P + ro[u] + o);
         }
       }
@@ -1015,7 +1062,7 @@ apply_staged_kernel(TableView t, const long long* __restrict__ keys, const float
                     unsigned lpr_shift, int use_tma, ScoreArg<SCORED> sa, const long long* __restrict__ n_dev,
                     SlotPlanes<OPT> sp, InitArg<KEYED> ki = InitArg<KEYED>()) {
   if (n_dev) n = (size_t)*n_dev;        // key count produced on the device (det_apply_*_dup); the grid covers the bound
-  constexpr int NS = 2 + opt_slots(OPT);  // streams per row: grad, param (, slot1 (, slot2))
+  constexpr int NS = 2 + opt_slots(OPT);  // streams per row: grad, param (, slot1 (, slot2 (, slot3)))
   DET_DYN_SHARED(dyn_smem);
   __shared__ __align__(128) long long s_keys[kStages][kTileKeys];
   __shared__ __align__(8) unsigned long long s_bar[kStages];
@@ -1082,6 +1129,7 @@ apply_staged_kernel(TableView t, const long long* __restrict__ keys, const float
           if (!nw && NS > 2) {
             cp_async16(sm(stage, st, 2), S1 + ro);
             if (NS > 3) cp_async16(sm(stage, st, 3), S2 + ro);
+            if constexpr (NS > 4) cp_async16(sm(stage, st, 4), (const float*)t.planes[3] + ro);
           }
         }
       }
@@ -1110,7 +1158,7 @@ apply_staged_kernel(TableView t, const long long* __restrict__ keys, const float
         const bool fresh = nw || (NS > 2 && row_ok && __float_as_uint(*sm_mark(stage, st)) == kSlotUninit);
         if (row_ok && lane_on) {
           const size_t ro = (size_t)sl * dim + (size_t)c0 * 4;
-          FVec<4> g, p, a, b2;
+          FVec<4> g, p, a, b2, c3;
           g.v = *sm(stage, st, 0);
           if constexpr (KEYED) {
             if (nw) p.keyed(ki, kj, c0 * 4u);
@@ -1122,14 +1170,16 @@ apply_staged_kernel(TableView t, const long long* __restrict__ keys, const float
             else p.load(reinterpret_cast<const T*>(sm(stage, st, 1)));
           }
           if (fresh) {
-            opt_fresh<OPT>(h, a, b2);
+            opt_fresh<OPT>(h, a, b2, c3);
           } else {
             if (NS > 2) a.v = *sm(stage, st, 2);
             if (NS > 3) b2.v = *sm(stage, st, 3);
+            if constexpr (NS > 4) c3.v = *sm(stage, st, 4);
           }
-          opt_step<OPT>(h, g, p, a, b2);
+          opt_step<OPT>(h, g, p, a, b2, c3);
           if (opt_slots(OPT) > 0) a.store(S1 + ro);
           if (opt_slots(OPT) > 1) b2.store(S2 + ro);
+          if constexpr (opt_slots(OPT) > 2) c3.store((float*)t.planes[3] + ro);
           p.store(P + ro);
           if constexpr (OPT >= kSgd) {
             if (nw && c0 == 0) mark_unwritten(t, sp, sl);
@@ -1866,14 +1916,35 @@ static det_status ftrl_hyper(float lr, float l1, float l2, float l2_shrinkage, f
   return DET_OK;
 }
 
+// RMSprop: momentum >= 0 (not NaN); epsilon outside the square root only without momentum (Keras' composed branch).
+// The slot-plane count picks the instantiation: rms, then mg if centered, then the momentum if momentum > 0.
+static det_status rmsprop_hyper(float lr, float rho, float momentum, float epsilon, int centered, int eps_in_sqrt,
+                                float init_ms, OptHyper* h, int* opt) {
+  if (!(momentum >= 0.f)) return fail(DET_INVALID_ARGUMENT, "det_apply_rmsprop: momentum must be >= 0");
+  if (momentum > 0.f && !eps_in_sqrt)
+    return fail(DET_INVALID_ARGUMENT, "det_apply_rmsprop: a momentum needs epsilon inside the square root");
+  h->lr = lr; h->eps = epsilon; h->beta1 = rho; h->beta2 = momentum; h->init_slot = init_ms;
+  h->flags = (eps_in_sqrt ? kEpsInSqrt : 0u) | (centered ? kCentered : 0u);
+  *opt = kRmsprop1 + (centered ? 1 : 0) + (momentum > 0.f ? 1 : 0);
+  return DET_OK;
+}
+
+static det_status adadelta_hyper(float lr, float rho, float epsilon, OptHyper* h, int* opt) {
+  h->lr = lr; h->eps = epsilon; h->beta1 = rho; h->beta2 = 0.f; h->init_slot = 0.f;
+  *opt = kAdadelta;
+  return DET_OK;
+}
+
 // det_table::slot_init, the slot values of a key created by insert / accum and never stepped: the initial accumulator
-// of Adagrad and FTRL (FTRL's z: 0), 0 for momentum; Adam and plain SGD leave them as they are.  Every optimizer entry
-// point records them before it takes the table lock.
+// of Adagrad and FTRL (FTRL's z: 0), 0 for momentum, RMSprop's initial rms (its mg and momentum: 0), 0 for both Adadelta
+// planes; Adam and plain SGD leave them as they are.  Every optimizer entry point records them before it takes the
+// table lock.
 static void record_slot_init(det_table* t, int opt, const OptHyper& h) {
   if (!t) return;
-  if (opt == kAdagrad || opt == kFtrl) t->slot_init[1] = h.init_slot;
-  if (opt == kMomentum) t->slot_init[1] = 0.f;
-  if (opt == kFtrl) t->slot_init[2] = 0.f;
+  if (opt == kAdagrad || opt == kFtrl || (opt >= kRmsprop1 && opt <= kRmsprop3)) t->slot_init[1] = h.init_slot;
+  if (opt == kMomentum || opt == kAdadelta) t->slot_init[1] = 0.f;
+  if (opt == kFtrl || opt == kRmsprop2 || opt == kAdadelta) t->slot_init[2] = 0.f;
+  if (opt == kRmsprop3) t->slot_init[2] = t->slot_init[3] = 0.f;
 }
 
 }  // namespace det
@@ -2145,6 +2216,25 @@ det_status det_apply_ftrl(det_table* t, const int64_t* keys, const float* grads,
   OptHyper h;
   int opt;
   if (det_status st = ftrl_hyper(lr, l1, l2, l2_shrinkage, init_accum, &h, &opt)) return st;
+  record_slot_init(t, opt, h);
+  return apply_common(t, keys, grads, n, h, init_param, full_size_init, opt, (cudaStream_t)stream);
+}
+
+det_status det_apply_rmsprop(det_table* t, const int64_t* keys, const float* grads, size_t n, float lr, float rho,
+                             float momentum, float epsilon, int centered, int eps_in_sqrt, const float* init_param,
+                             int full_size_init, float init_ms, det_stream_t stream) {
+  OptHyper h;
+  int opt;
+  if (det_status st = rmsprop_hyper(lr, rho, momentum, epsilon, centered, eps_in_sqrt, init_ms, &h, &opt)) return st;
+  record_slot_init(t, opt, h);
+  return apply_common(t, keys, grads, n, h, init_param, full_size_init, opt, (cudaStream_t)stream);
+}
+
+det_status det_apply_adadelta(det_table* t, const int64_t* keys, const float* grads, size_t n, float lr, float rho,
+                              float epsilon, const float* init_param, int full_size_init, det_stream_t stream) {
+  OptHyper h;
+  int opt;
+  if (det_status st = adadelta_hyper(lr, rho, epsilon, &h, &opt)) return st;
   record_slot_init(t, opt, h);
   return apply_common(t, keys, grads, n, h, init_param, full_size_init, opt, (cudaStream_t)stream);
 }
@@ -2526,6 +2616,27 @@ det_status det_apply_ftrl_dup(det_table* t, const int64_t* ids, const float* gra
   return apply_dup(t, ids, grads, n, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out, (cudaStream_t)stream);
 }
 
+det_status det_apply_rmsprop_dup(det_table* t, const int64_t* ids, const float* grads, size_t n, float lr, float rho,
+                                 float momentum, float epsilon, int centered, int eps_in_sqrt, const float* init_param,
+                                 float init_ms, void* workspace, size_t workspace_bytes, int64_t* n_unique_dev_out,
+                                 det_stream_t stream) {
+  OptHyper h;
+  int opt;
+  if (det_status st = rmsprop_hyper(lr, rho, momentum, epsilon, centered, eps_in_sqrt, init_ms, &h, &opt)) return st;
+  record_slot_init(t, opt, h);
+  return apply_dup(t, ids, grads, n, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out, (cudaStream_t)stream);
+}
+
+det_status det_apply_adadelta_dup(det_table* t, const int64_t* ids, const float* grads, size_t n, float lr, float rho,
+                                  float epsilon, const float* init_param, void* workspace, size_t workspace_bytes,
+                                  int64_t* n_unique_dev_out, det_stream_t stream) {
+  OptHyper h;
+  int opt;
+  if (det_status st = adadelta_hyper(lr, rho, epsilon, &h, &opt)) return st;
+  record_slot_init(t, opt, h);
+  return apply_dup(t, ids, grads, n, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out, (cudaStream_t)stream);
+}
+
 det_status det_apply_adagrad_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
                                     size_t nnz, size_t batch, int combiner, const float* gout, float lr, float epsilon,
                                     const float* init_param, float init_accum, void* workspace, size_t workspace_bytes,
@@ -2572,6 +2683,33 @@ det_status det_apply_ftrl_sparse(det_table* t, const int64_t* ids, const int32_t
   OptHyper h;
   int opt;
   if (det_status st = ftrl_hyper(lr, l1, l2, l2_shrinkage, init_accum, &h, &opt)) return st;
+  record_slot_init(t, opt, h);
+  const SparseSrc sp{segment_ids, weights, batch, combiner};
+  return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
+                   (cudaStream_t)stream, nullptr, &sp);
+}
+
+det_status det_apply_rmsprop_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
+                                    size_t nnz, size_t batch, int combiner, const float* gout, float lr, float rho,
+                                    float momentum, float epsilon, int centered, int eps_in_sqrt,
+                                    const float* init_param, float init_ms, void* workspace, size_t workspace_bytes,
+                                    int64_t* n_unique_dev_out, det_stream_t stream) {
+  OptHyper h;
+  int opt;
+  if (det_status st = rmsprop_hyper(lr, rho, momentum, epsilon, centered, eps_in_sqrt, init_ms, &h, &opt)) return st;
+  record_slot_init(t, opt, h);
+  const SparseSrc sp{segment_ids, weights, batch, combiner};
+  return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
+                   (cudaStream_t)stream, nullptr, &sp);
+}
+
+det_status det_apply_adadelta_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
+                                     size_t nnz, size_t batch, int combiner, const float* gout, float lr, float rho,
+                                     float epsilon, const float* init_param, void* workspace, size_t workspace_bytes,
+                                     int64_t* n_unique_dev_out, det_stream_t stream) {
+  OptHyper h;
+  int opt;
+  if (det_status st = adadelta_hyper(lr, rho, epsilon, &h, &opt)) return st;
   record_slot_init(t, opt, h);
   const SparseSrc sp{segment_ids, weights, batch, combiner};
   return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,

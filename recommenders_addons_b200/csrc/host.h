@@ -278,13 +278,17 @@ void host_pipe_free(det_table* t);
 det_status rehash_to(det_table* t, uint64_t new_nb, cudaStream_t s);
 // fused.cu: the optimizers of the fused find-or-insert step (K7, its template parameter OPT) and their
 // hyper-parameters.  What each OptHyper field holds depends on the optimizer (listed at opt_step); only the builders
-// (adagrad_hyper, adam_hyper, sgd_hyper, ftrl_hyper) fill them.
-enum : int { kAdagrad, kAdam, kSgd, kMomentum, kFtrl, kNumOpts };
+// (adagrad_hyper, adam_hyper, sgd_hyper, ftrl_hyper, rmsprop_hyper, adadelta_hyper) fill them.  RMSprop has one id
+// per slot-plane count (kRmsprop1 .. kRmsprop3): the count is a compile-time property of a K7 instantiation.
+enum : int { kAdagrad, kAdam, kSgd, kMomentum, kFtrl, kRmsprop1, kRmsprop2, kRmsprop3, kAdadelta, kNumOpts };
+// OptHyper::flags (RMSprop only; 0 for the other optimizers)
+enum : unsigned { kEpsInSqrt = 1u, kCentered = 2u };
 struct OptHyper {
   float lr;
   float eps;
   float beta1, beta2;
   float init_slot;
+  unsigned flags = 0;   // fills what was the struct's tail padding before an 8-byte kernel parameter
 };
 // validate the hyper-parameters, fill *h and set *opt
 det_status adagrad_hyper(float lr, float epsilon, float init_accum, OptHyper* h, int* opt);

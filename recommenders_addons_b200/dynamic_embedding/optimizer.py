@@ -387,6 +387,88 @@ class FusedFtrl(_FusedBase):
                                                 _stream_ptr(table.device)))
 
 
+class FusedRMSprop(_FusedBase):
+  """RMSprop on dynamic-embedding rows, with Keras' signature (tf.keras.optimizers.RMSprop):
+  ms = ms*rho + (g*g)*(1-rho); centered: mg = mg*rho + g*(1-rho), d = ms - mg*mg, else d = ms;
+  momentum > 0: mom = mom*momentum + (lr*g)/sqrt(d + eps), var -= mom;
+  momentum == 0: var -= (lr*g) / (sqrt(d + eps) if epsilon_in_sqrt else sqrt(d) + eps).
+  epsilon_in_sqrt=None is Keras' choice (momentum > 0); TF1 RMSPropOptimizer is initial_accumulator_value=1.0,
+  epsilon_in_sqrt=True.  Slots: "rms" (starts at initial_accumulator_value), then "mg" if centered, then "momentum" if
+  momentum > 0 (both start at 0)."""
+  opt_name = "RMSprop"
+
+  def __init__(self, learning_rate=0.001, rho=0.9, momentum=0.0, epsilon=1e-7, centered=False,
+               initial_accumulator_value=0.0, epsilon_in_sqrt=None):
+    super().__init__()
+    if not momentum >= 0:
+      raise ValueError("momentum must be >= 0, got %r" % (momentum,))
+    if epsilon_in_sqrt is None:
+      epsilon_in_sqrt = momentum > 0
+    if momentum > 0 and not epsilon_in_sqrt:
+      raise ValueError("a momentum needs epsilon inside the square root (epsilon_in_sqrt=True)")
+    self.learning_rate = float(learning_rate)
+    self.rho = float(rho)
+    self.momentum = float(momentum)
+    self.epsilon = float(epsilon)
+    self.centered = bool(centered)
+    self.initial_accumulator_value = float(initial_accumulator_value)
+    self.epsilon_in_sqrt = bool(epsilon_in_sqrt)
+    self.slot_plane_names = ("rms",) + (("mg",) if self.centered else ()) + (("momentum",) if self.momentum > 0 else ())
+    self.n_slots = len(self.slot_plane_names)
+
+  def _hyper(self):
+    return (self.learning_rate, self.rho, self.momentum, self.epsilon, int(self.centered), int(self.epsilon_in_sqrt))
+
+  def _apply_table(self, params, table, keys, grads):
+    n = keys.numel()
+    init, full = _init_rows(params, n, table.device)
+    _lib.check(_lib.lib().det_apply_rmsprop(table.handle, _ptr(keys), _ptr(grads), n, *self._hyper(), _ptr(init), full,
+                                            self.initial_accumulator_value, _stream_ptr(table.device)))
+
+  def _apply_table_dup(self, table, ids, grads, n, init, ws):
+    _lib.check(_lib.lib().det_apply_rmsprop_dup(table.handle, _ptr(ids), _ptr(grads), n, *self._hyper(), _ptr(init),
+                                                self.initial_accumulator_value, _ptr(ws), ws.numel(), None,
+                                                _stream_ptr(table.device)))
+
+  def _apply_table_sparse(self, table, h, gout, init, ws):
+    _lib.check(_lib.lib().det_apply_rmsprop_sparse(table.handle, _ptr(h.ids), _ptr(h.segment_ids), _ptr(h.weights),
+                                                   h.ids.numel(), h.batch, _lib.COMBINERS[h.combiner], _ptr(gout),
+                                                   *self._hyper(), _ptr(init), self.initial_accumulator_value, _ptr(ws),
+                                                   ws.numel(), None, _stream_ptr(table.device)))
+
+
+class FusedAdadelta(_FusedBase):
+  """Adadelta on dynamic-embedding rows (TF1 AdadeltaOptimizer and Keras Adadelta run the same kernel):
+  acc = acc*rho + (g*g)*(1-rho); u = (sqrt(au + eps) / sqrt(acc + eps))*g; var -= u*lr; au = au*rho + (u*u)*(1-rho).
+  Slots: "accum_grad" and "accum_var", both starting at 0."""
+  n_slots = 2
+  opt_name = "Adadelta"
+  slot_plane_names = ("accum_grad", "accum_var")
+
+  def __init__(self, learning_rate=0.001, rho=0.95, epsilon=1e-7):
+    super().__init__()
+    self.learning_rate = float(learning_rate)
+    self.rho = float(rho)
+    self.epsilon = float(epsilon)
+
+  def _apply_table(self, params, table, keys, grads):
+    n = keys.numel()
+    init, full = _init_rows(params, n, table.device)
+    _lib.check(_lib.lib().det_apply_adadelta(table.handle, _ptr(keys), _ptr(grads), n, self.learning_rate, self.rho,
+                                             self.epsilon, _ptr(init), full, _stream_ptr(table.device)))
+
+  def _apply_table_dup(self, table, ids, grads, n, init, ws):
+    _lib.check(_lib.lib().det_apply_adadelta_dup(table.handle, _ptr(ids), _ptr(grads), n, self.learning_rate, self.rho,
+                                                 self.epsilon, _ptr(init), _ptr(ws), ws.numel(), None,
+                                                 _stream_ptr(table.device)))
+
+  def _apply_table_sparse(self, table, h, gout, init, ws):
+    _lib.check(_lib.lib().det_apply_adadelta_sparse(table.handle, _ptr(h.ids), _ptr(h.segment_ids), _ptr(h.weights),
+                                                    h.ids.numel(), h.batch, _lib.COMBINERS[h.combiner], _ptr(gout),
+                                                    self.learning_rate, self.rho, self.epsilon, _ptr(init), _ptr(ws),
+                                                    ws.numel(), None, _stream_ptr(table.device)))
+
+
 class ComposedOptimizer(object):
   """ANY torch.optim optimizer on dynamic-embedding rows, the way the reference patches a stock optimizer
   (dynamic_embedding_optimizer.py:137-204 `apply_grad_to_update_var`, :870-958 `create_slots`): per step and per
@@ -394,8 +476,9 @@ class ComposedOptimizer(object):
   named `<var>/<Optimizer>/<slot>` like the reference's slot tables), run the stock dense rule on the [U, dim] scratch,
   write param and slots back (`TrainableWrapper.update_op`, embedding_weights.py:434-444).  Table passes per step:
   (1 + slots) finds + (1 + slots) upserts, all through the validated table kernels; Adagrad / Adam have the fused
-  single-kernel path (FusedAdagrad / FusedAdam), which DynamicEmbeddingOptimizer picks by default.  SGD, momentum and
-  FTRL have fused steps too (FusedSGD / FusedFtrl), used when passed explicitly.
+  single-kernel path (FusedAdagrad / FusedAdam), which DynamicEmbeddingOptimizer picks by default.  SGD, momentum,
+  FTRL, RMSprop and Adadelta have fused steps too (FusedSGD / FusedFtrl / FusedRMSprop / FusedAdadelta), used when
+  passed explicitly.
 
   A key without slot state starts from the state a fresh torch optimizer gives a new parameter (zeros; Adagrad's
   `sum` from initial_accumulator_value) -- the reference's slot initializers.  State that is not per row (`step`,

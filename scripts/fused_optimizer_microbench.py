@@ -6,9 +6,14 @@ rows.  Timed with CUDA events, in rounds that alternate the dtype order, median 
   * sgd, momentum (0.9), ftrl, adagrad, adam -- det_apply_* on 2^20 unique resident keys;
   * sgd_dup (momentum 0.9), ftrl_dup        -- det_apply_*_dup at the c3 backward shape (26 x 65536 Zipf ids);
   * composed_momentum -- ComposedOptimizer(torch.optim.SGD(momentum=0.9)): unique ids, finds of the param and slot
-    rows, torch's dense rule, upserts -- on an fp32 variable of --composed-resident rows, next to FusedSGD(0.9) on it.
+    rows, torch's dense rule, upserts -- on an fp32 variable of --composed-resident rows, next to FusedSGD(0.9) on it;
+  * rmsprop (1 slot plane), rmsprop_c (centered), rmsprop_m (momentum 0.9), rmsprop_cm (centered + momentum, 3 slot
+    planes), adadelta -- det_apply_rmsprop / det_apply_adadelta on 2^20 unique resident keys of two more variables
+    (fp32, bf16) with three slot planes and 2/3 of --resident rows, made after the variables above are released, and the composed torch.optim.RMSprop / Adadelta next to FusedRMSprop /
+    FusedAdadelta on one more fp32 variable of --composed-resident rows.
 Before the timing, the first step of each new optimizer on a sample of its keys (rows written by insert, no slot state
-yet) is checked bit for bit against tests/optimizer_oracle.py: params of both dtypes (bf16: the fp32 result rounded).
+yet) is checked bit for bit against tests/optimizer_oracle.py (RMSprop and Adadelta: tests/rmsprop_adadelta_oracle.py):
+params of both dtypes (bf16: the fp32 result rounded).
 
 Bytes per key are what the unique-key step must move at dim 64: key 8 + probed bucket 64 + fp32 gradient 256 + param
 row read and write + fp32 slot rows read and write.  The rate is against the H100 SXM data-sheet HBM3 bandwidth of
@@ -34,7 +39,9 @@ BUCKET_BYTES = 64          # one probed 8-slot bucket of int64 keys
 N_UNIQUE = 1 << 20
 N_DUP = 26 * 65536
 N_SAMPLE = 1 << 16
-SLOTS = {"sgd": 0, "momentum": 1, "ftrl": 2, "adagrad": 1, "adam": 2}
+SLOTS = {"sgd": 0, "momentum": 1, "ftrl": 2, "adagrad": 1, "adam": 2,
+         "rmsprop": 1, "rmsprop_c": 2, "rmsprop_m": 2, "rmsprop_cm": 3, "adadelta": 2}
+RMS = {"rmsprop": (0.0, 0), "rmsprop_c": (0.0, 1), "rmsprop_m": (0.9, 0), "rmsprop_cm": (0.9, 1)}   # momentum, centered
 FTRL = dict(lr=0.05, l1=0.001, l2=0.01, l2_shrinkage=0.0)
 
 
@@ -190,9 +197,96 @@ def main():
   res["composed_vs_fused_fp32_momentum"] = {"resident": Rc, "keys": N_UNIQUE, "composed_is": type(comp).__name__,
                                             "composed_ms": round(float(np.median(ms_comp)), 4),
                                             "fused_ms": round(float(np.median(ms_fused_small)), 4)}
+  # the tables above are released first: the three-plane variables do not fit beside them
+  for v in list(vars_.values()) + [small]:
+    for t in v.tables:
+      t.close()
+  del vars_, small, comp, fused_small
+  torch.cuda.empty_cache()
+  res.update(rmsprop_adadelta_arms(args, lib, de, P, dev, gen, dts, fill, timed, mismatches))
   print(json.dumps({"metric": "fused optimizer step ms per call (median of rounds, CUDA events)", "card": info,
                     "resident": R, "dim": DIM, "rounds": args.rounds, "calls": args.calls,
                     "datasheet_hbm_TB_s": DATASHEET_HBM_BPS / 1e12, "oracle_mismatches": mismatches, "shapes": res}))
+
+
+def rmsprop_adadelta_arms(args, lib, de, P, dev, gen, dts, fill, timed, mismatches):
+  """the RMSprop layouts and Adadelta, on their own three-plane variables (the arms above keep their two-plane ones)"""
+  from recommenders_addons_b200 import _lib
+  from tests import rmsprop_adadelta_oracle as RO
+  R = max(args.resident * 2 // 3, 6 * N_UNIQUE)   # room for a 2^20-key range per arm
+  v3 = {n: de.Variable(value_dtype=dt, dim=DIM, init_size=2 * R, initializer=0.0, name="fob3_" + n, num_slot_planes=3)
+        for n, dt in dts.items()}
+  fill(list(v3.values()), R)
+  part = R // 6
+  shapes = tuple(RMS) + ("adadelta",)
+  keys = {o: mix_keys(i * part + torch.randperm(part, device=dev, generator=gen)[:N_UNIQUE]) for i, o in enumerate(shapes)}
+  g_uni = torch.randn(N_UNIQUE, DIM, device=dev, generator=gen) * 0.01
+  init = torch.zeros(DIM, device=dev)
+
+  def step(name, shape, k=None, g=None, n=N_UNIQUE):
+    h = v3[name].tables[0].handle
+    k = keys[shape] if k is None else k
+    g = g_uni if g is None else g
+    if shape == "adadelta":
+      st = lib.det_apply_adadelta(h, P(k), P(g), n, 1.0, 0.95, 1e-7, P(init), 0, None)
+    else:
+      m, c = RMS[shape]
+      st = lib.det_apply_rmsprop(h, P(k), P(g), n, 0.001, 0.9, m, 1e-7, c, int(m > 0), P(init), 0, 0.0, None)
+    _lib.check(st)
+
+  for shape in shapes:
+    k = keys[shape][:N_SAMPLE].contiguous()
+    g = g_uni[:N_SAMPLE].contiguous()
+    bad = 0
+    for name, dt in dts.items():
+      p0 = v3[name].lookup(k).float().cpu().numpy()
+      step(name, shape, k, g, N_SAMPLE)
+      got = v3[name].lookup(k).float().cpu().numpy()
+      gn, z = g.cpu().numpy(), np.zeros_like(p0)
+      if shape == "adadelta":
+        exp = RO.adadelta_dense(p0, z, z, gn, 1.0, 0.95, 1e-7)[0]
+      else:
+        m, c = RMS[shape]
+        exp = RO.rmsprop_dense(p0, z, z, z, gn, 0.001, 0.9, m, 1e-7, bool(c), m > 0)[0]
+      exp = torch.from_numpy(exp).to(dt).float().numpy()
+      bad += int((got.view(np.uint32) != exp.view(np.uint32)).sum())
+    mismatches[shape] = bad
+
+  Rc = args.composed_resident
+  small = de.Variable(dim=DIM, init_size=2 * Rc, initializer=0.0, name="fob3_small", num_slot_planes=3)
+  fill([small], Rc)
+  keys_small = mix_keys(torch.randperm(Rc, device=dev, generator=gen)[:N_UNIQUE])
+  dummy = [torch.nn.Parameter(torch.zeros(1))]
+  pairs = {"rmsprop": (de.DynamicEmbeddingOptimizer(torch.optim.RMSprop(dummy, lr=0.001, alpha=0.9, eps=1e-7)),
+                       de.FusedRMSprop(0.001, 0.9, epsilon=1e-7)),
+           "adadelta": (de.DynamicEmbeddingOptimizer(torch.optim.Adadelta(dummy, lr=1.0, rho=0.95, eps=1e-7)),
+                        de.FusedAdadelta(1.0, 0.95, 1e-7))}
+  ms = {(n, s): [] for n in dts for s in shapes}
+  mc = {(o, kind): [] for o in pairs for kind in ("composed", "fused")}
+  for r in range(args.rounds):
+    order = list(dts) if r % 2 == 0 else list(reversed(list(dts)))
+    for shape in shapes:
+      for n in order:
+        ms[(n, shape)].append(timed(lambda: step(n, shape), args.calls))
+    for o, (comp, fused) in pairs.items():
+      mc[(o, "composed")].append(timed(lambda: comp.apply_sparse(small, keys_small, g_uni), max(2, args.calls // 2)))
+      mc[(o, "fused")].append(timed(lambda: fused.apply_sparse(small, keys_small, g_uni), args.calls))
+  res = {}
+  for shape in shapes:
+    row = {}
+    for n, dt in dts.items():
+      t = float(np.median(ms[(n, shape)]))
+      bpk = bytes_per_key(shape, torch.empty(0, dtype=dt).element_size())
+      row[n] = {"ms": round(t, 4), "ms_spread": [round(min(ms[(n, shape)]), 4), round(max(ms[(n, shape)]), 4)],
+                "bytes_per_key": bpk, "GB_s": round(bpk * N_UNIQUE / t / 1e6, 1),
+                "of_datasheet_hbm": round(bpk * N_UNIQUE / (t * 1e-3) / DATASHEET_HBM_BPS, 3)}
+    row["ids"] = N_UNIQUE
+    res[shape] = row
+  for o, (comp, _) in pairs.items():
+    res["composed_vs_fused_fp32_" + o] = {"resident": Rc, "keys": N_UNIQUE, "composed_is": type(comp).__name__,
+                                          "composed_ms": round(float(np.median(mc[(o, "composed")])), 4),
+                                          "fused_ms": round(float(np.median(mc[(o, "fused")])), 4)}
+  return res
 
 
 if __name__ == "__main__":
