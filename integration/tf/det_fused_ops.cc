@@ -221,252 +221,172 @@ class DetLookupSparseOp : public OpKernel {
   float max_norm_ = 0.f;
 };
 
-class DetApplyAdagradOp : public OpKernel {
- public:
-  explicit DetApplyAdagradOp(OpKernelConstruction* ctx) : OpKernel(ctx) {
-    OP_REQUIRES_OK(ctx, ctx->GetAttr("epsilon", &epsilon_));
-    OP_REQUIRES_OK(ctx, ctx->GetAttr("initial_accumulator_value", &init_accum_));
-  }
-  void Compute(OpKernelContext* ctx) override {
-    tensorflow::lookup::LookupInterface* table = nullptr;
-    OP_REQUIRES_OK(ctx, GetLookupTable("table_handle", ctx, &table));
-    core::ScopedUnref unref_me(table);
-    det_table* handle = FusedHandle(table);
-    OP_REQUIRES(ctx, handle != nullptr,
-                errors::InvalidArgument("DetApplyAdagrad: the table's value dtype must be float, half or bfloat16"));
-    const Tensor& keys = ctx->input(1);
-    const Tensor& grads = ctx->input(2);
-    const Tensor& lr = ctx->input(3);
-    const Tensor& init = ctx->input(4);
-    const int64 n = keys.NumElements(), dim = table->value_shape().dim_size(0);
-    OP_REQUIRES(ctx, grads.NumElements() == n * dim, errors::InvalidArgument("grads must have shape [n, dim]"));
-    OP_REQUIRES(ctx, init.NumElements() == dim || init.NumElements() == n * dim,
-                errors::InvalidArgument("init_param must have shape [dim] or [n, dim]"));
-    OP_REQUIRES_OK(ctx, ToStatus(det_apply_adagrad(
-                            handle, reinterpret_cast<const int64_t*>(keys.flat<int64>().data()),
-                            grads.flat<float>().data(), static_cast<size_t>(n), lr.scalar<float>()(), epsilon_,
-                            init.flat<float>().data(), init.NumElements() == dim ? 0 : 1,
-                            init_accum_, StreamOf(ctx))));
-  }
-
- private:
-  float epsilon_ = 0.f, init_accum_ = 0.1f;
+// What a TFRA>DetApply* op hands the library.  `step` is input 3: lr, or alpha for Adam.  `full` is 1 when init_param
+// holds one row per key (unique-key forms only); `ws` / `ws_bytes` are the duplicate-id forms' workspace.
+struct ApplyArgs {
+  det_table* table;
+  const int64_t* keys;
+  const float* grads;
+  size_t n;
+  float step;
+  const float* init;
+  int full;
+  void* ws;
+  size_t ws_bytes;
+  det_stream_t stream;
 };
 
-class DetApplyAdamOp : public OpKernel {
- public:
-  explicit DetApplyAdamOp(OpKernelConstruction* ctx) : OpKernel(ctx) {
-    OP_REQUIRES_OK(ctx, ctx->GetAttr("beta1", &beta1_));
-    OP_REQUIRES_OK(ctx, ctx->GetAttr("beta2", &beta2_));
-    OP_REQUIRES_OK(ctx, ctx->GetAttr("epsilon", &epsilon_));
+// One rule per optimizer: its attributes, read once at kernel construction, and its unique-key and duplicate-id calls.
+struct AdagradRule {
+  static constexpr const char* kName = "DetApplyAdagrad";
+  float epsilon = 0.f, init_accum = 0.1f;
+  explicit AdagradRule(OpKernelConstruction* ctx) {
+    OP_REQUIRES_OK(ctx, ctx->GetAttr("epsilon", &epsilon));
+    OP_REQUIRES_OK(ctx, ctx->GetAttr("initial_accumulator_value", &init_accum));
   }
-  void Compute(OpKernelContext* ctx) override {
-    tensorflow::lookup::LookupInterface* table = nullptr;
-    OP_REQUIRES_OK(ctx, GetLookupTable("table_handle", ctx, &table));
-    core::ScopedUnref unref_me(table);
-    det_table* handle = FusedHandle(table);
-    OP_REQUIRES(ctx, handle != nullptr,
-                errors::InvalidArgument("DetApplyAdam: the table's value dtype must be float, half or bfloat16"));
-    const Tensor& keys = ctx->input(1);
-    const Tensor& grads = ctx->input(2);
-    const Tensor& alpha = ctx->input(3);
-    const Tensor& init = ctx->input(4);
-    const int64 n = keys.NumElements(), dim = table->value_shape().dim_size(0);
-    OP_REQUIRES(ctx, grads.NumElements() == n * dim, errors::InvalidArgument("grads must have shape [n, dim]"));
-    OP_REQUIRES(ctx, init.NumElements() == dim || init.NumElements() == n * dim,
-                errors::InvalidArgument("init_param must have shape [dim] or [n, dim]"));
-    OP_REQUIRES_OK(ctx, ToStatus(det_apply_adam(
-                            handle, reinterpret_cast<const int64_t*>(keys.flat<int64>().data()),
-                            grads.flat<float>().data(), static_cast<size_t>(n), alpha.scalar<float>()(), beta1_,
-                            beta2_, epsilon_, init.flat<float>().data(), init.NumElements() == dim ? 0 : 1,
-                            StreamOf(ctx))));
+  det_status Unique(const ApplyArgs& a) const {
+    return det_apply_adagrad(a.table, a.keys, a.grads, a.n, a.step, epsilon, a.init, a.full, init_accum, a.stream);
   }
-
- private:
-  float beta1_ = 0.9f, beta2_ = 0.999f, epsilon_ = 1e-8f;
+  det_status Dup(const ApplyArgs& a) const {
+    return det_apply_adagrad_dup(a.table, a.keys, a.grads, a.n, a.step, epsilon, a.init, init_accum, a.ws, a.ws_bytes,
+                                 nullptr, a.stream);
+  }
 };
 
-// OPT 0 = Adagrad (input 3 = lr), 1 = Adam (input 3 = alpha)
-template <int OPT>
-class DetApplyDuplicateIndicesOp : public OpKernel {
- public:
-  explicit DetApplyDuplicateIndicesOp(OpKernelConstruction* ctx) : OpKernel(ctx) {
-    OP_REQUIRES_OK(ctx, ctx->GetAttr("epsilon", &epsilon_));
-    if (OPT == 0) {
-      OP_REQUIRES_OK(ctx, ctx->GetAttr("initial_accumulator_value", &init_accum_));
-    } else {
-      OP_REQUIRES_OK(ctx, ctx->GetAttr("beta1", &beta1_));
-      OP_REQUIRES_OK(ctx, ctx->GetAttr("beta2", &beta2_));
-    }
+struct AdamRule {
+  static constexpr const char* kName = "DetApplyAdam";
+  float beta1 = 0.9f, beta2 = 0.999f, epsilon = 1e-8f;
+  explicit AdamRule(OpKernelConstruction* ctx) {
+    OP_REQUIRES_OK(ctx, ctx->GetAttr("beta1", &beta1));
+    OP_REQUIRES_OK(ctx, ctx->GetAttr("beta2", &beta2));
+    OP_REQUIRES_OK(ctx, ctx->GetAttr("epsilon", &epsilon));
   }
-  void Compute(OpKernelContext* ctx) override {
-    tensorflow::lookup::LookupInterface* table = nullptr;
-    OP_REQUIRES_OK(ctx, GetLookupTable("table_handle", ctx, &table));
-    core::ScopedUnref unref_me(table);
-    det_table* handle = FusedHandle(table);
-    OP_REQUIRES(ctx, handle != nullptr,
-                errors::InvalidArgument("DetApply*DuplicateIndices: the table's value dtype must be float, half or bfloat16"));
-    const Tensor& ids = ctx->input(1);
-    const Tensor& grads = ctx->input(2);
-    const Tensor& step = ctx->input(3);
-    const Tensor& init = ctx->input(4);
-    const int64 n = ids.NumElements(), dim = table->value_shape().dim_size(0);
-    OP_REQUIRES(ctx, grads.NumElements() == n * dim, errors::InvalidArgument("grads must have shape [n, dim]"));
-    OP_REQUIRES(ctx, init.NumElements() == dim, errors::InvalidArgument("init_param must have shape [dim]"));
-    if (n == 0) return;
-    // stream-ordered scratch from TF's allocator, aligned up to the 256 B the library asks for
-    const size_t ws_bytes = det_apply_dup_workspace_bytes(static_cast<size_t>(n), static_cast<size_t>(dim));
-    Tensor ws;
-    OP_REQUIRES_OK(ctx, ctx->allocate_temp(DT_INT8, TensorShape({static_cast<int64>(ws_bytes + 256)}), &ws));
-    int8* raw = ws.flat<int8>().data();
-    void* aligned = raw + ((256 - (reinterpret_cast<uintptr_t>(raw) & 255u)) & 255u);
-    const int64_t* k = reinterpret_cast<const int64_t*>(ids.flat<int64>().data());
-    const float* g = grads.flat<float>().data();
-    if (OPT == 0) {
-      OP_REQUIRES_OK(ctx, ToStatus(det_apply_adagrad_dup(handle, k, g, static_cast<size_t>(n), step.scalar<float>()(),
-                                                         epsilon_, init.flat<float>().data(), init_accum_, aligned,
-                                                         ws_bytes, nullptr, StreamOf(ctx))));
-    } else {
-      OP_REQUIRES_OK(ctx, ToStatus(det_apply_adam_dup(handle, k, g, static_cast<size_t>(n), step.scalar<float>()(),
-                                                      beta1_, beta2_, epsilon_, init.flat<float>().data(), aligned,
-                                                      ws_bytes, nullptr, StreamOf(ctx))));
-    }
+  det_status Unique(const ApplyArgs& a) const {
+    return det_apply_adam(a.table, a.keys, a.grads, a.n, a.step, beta1, beta2, epsilon, a.init, a.full, a.stream);
   }
-
- private:
-  float epsilon_ = 0.f, init_accum_ = 0.1f, beta1_ = 0.9f, beta2_ = 0.999f;
+  det_status Dup(const ApplyArgs& a) const {
+    return det_apply_adam_dup(a.table, a.keys, a.grads, a.n, a.step, beta1, beta2, epsilon, a.init, a.ws, a.ws_bytes,
+                              nullptr, a.stream);
+  }
 };
 
-// SGD / momentum (OPT 0) and FTRL (OPT 1), unique keys (DUP false) or repeated ids in one call (DUP true)
-template <int OPT, bool DUP>
-class DetApplySgdFtrlOp : public OpKernel {
- public:
-  explicit DetApplySgdFtrlOp(OpKernelConstruction* ctx) : OpKernel(ctx) {
-    if (OPT == 0) {
-      OP_REQUIRES_OK(ctx, ctx->GetAttr("momentum", &momentum_));
-      OP_REQUIRES_OK(ctx, ctx->GetAttr("nesterov", &nesterov_));
-    } else {
-      OP_REQUIRES_OK(ctx, ctx->GetAttr("l1", &l1_));
-      OP_REQUIRES_OK(ctx, ctx->GetAttr("l2", &l2_));
-      OP_REQUIRES_OK(ctx, ctx->GetAttr("l2_shrinkage", &l2_shrinkage_));
-      OP_REQUIRES_OK(ctx, ctx->GetAttr("initial_accumulator_value", &init_accum_));
-    }
+struct SgdRule {
+  static constexpr const char* kName = "DetApplySgd";
+  float momentum = 0.f;
+  int nesterov = 0;
+  explicit SgdRule(OpKernelConstruction* ctx) {
+    OP_REQUIRES_OK(ctx, ctx->GetAttr("momentum", &momentum));
+    OP_REQUIRES_OK(ctx, ctx->GetAttr("nesterov", &nesterov));
   }
+  det_status Unique(const ApplyArgs& a) const {
+    return det_apply_sgd(a.table, a.keys, a.grads, a.n, a.step, momentum, nesterov, a.init, a.full, a.stream);
+  }
+  det_status Dup(const ApplyArgs& a) const {
+    return det_apply_sgd_dup(a.table, a.keys, a.grads, a.n, a.step, momentum, nesterov, a.init, a.ws, a.ws_bytes,
+                             nullptr, a.stream);
+  }
+};
+
+struct FtrlRule {
+  static constexpr const char* kName = "DetApplyFtrl";
+  float l1 = 0.f, l2 = 0.f, l2_shrinkage = 0.f, init_accum = 0.1f;
+  explicit FtrlRule(OpKernelConstruction* ctx) {
+    OP_REQUIRES_OK(ctx, ctx->GetAttr("l1", &l1));
+    OP_REQUIRES_OK(ctx, ctx->GetAttr("l2", &l2));
+    OP_REQUIRES_OK(ctx, ctx->GetAttr("l2_shrinkage", &l2_shrinkage));
+    OP_REQUIRES_OK(ctx, ctx->GetAttr("initial_accumulator_value", &init_accum));
+  }
+  det_status Unique(const ApplyArgs& a) const {
+    return det_apply_ftrl(a.table, a.keys, a.grads, a.n, a.step, l1, l2, l2_shrinkage, a.init, a.full, init_accum,
+                          a.stream);
+  }
+  det_status Dup(const ApplyArgs& a) const {
+    return det_apply_ftrl_dup(a.table, a.keys, a.grads, a.n, a.step, l1, l2, l2_shrinkage, a.init, init_accum, a.ws,
+                              a.ws_bytes, nullptr, a.stream);
+  }
+};
+
+struct RmspropRule {
+  static constexpr const char* kName = "DetApplyRmsprop";
+  float rho = 0.9f, epsilon = 1e-7f, momentum = 0.f, init_ms = 0.f;
+  int centered = 0, eps_in_sqrt = 0;
+  explicit RmspropRule(OpKernelConstruction* ctx) {
+    OP_REQUIRES_OK(ctx, ctx->GetAttr("rho", &rho));
+    OP_REQUIRES_OK(ctx, ctx->GetAttr("epsilon", &epsilon));
+    OP_REQUIRES_OK(ctx, ctx->GetAttr("momentum", &momentum));
+    OP_REQUIRES_OK(ctx, ctx->GetAttr("centered", &centered));
+    OP_REQUIRES_OK(ctx, ctx->GetAttr("epsilon_in_sqrt", &eps_in_sqrt));
+    OP_REQUIRES_OK(ctx, ctx->GetAttr("initial_accumulator_value", &init_ms));
+  }
+  det_status Unique(const ApplyArgs& a) const {
+    return det_apply_rmsprop(a.table, a.keys, a.grads, a.n, a.step, rho, momentum, epsilon, centered, eps_in_sqrt,
+                             a.init, a.full, init_ms, a.stream);
+  }
+  det_status Dup(const ApplyArgs& a) const {
+    return det_apply_rmsprop_dup(a.table, a.keys, a.grads, a.n, a.step, rho, momentum, epsilon, centered, eps_in_sqrt,
+                                 a.init, init_ms, a.ws, a.ws_bytes, nullptr, a.stream);
+  }
+};
+
+struct AdadeltaRule {
+  static constexpr const char* kName = "DetApplyAdadelta";
+  float rho = 0.9f, epsilon = 1e-7f;
+  explicit AdadeltaRule(OpKernelConstruction* ctx) {
+    OP_REQUIRES_OK(ctx, ctx->GetAttr("rho", &rho));
+    OP_REQUIRES_OK(ctx, ctx->GetAttr("epsilon", &epsilon));
+  }
+  det_status Unique(const ApplyArgs& a) const {
+    return det_apply_adadelta(a.table, a.keys, a.grads, a.n, a.step, rho, epsilon, a.init, a.full, a.stream);
+  }
+  det_status Dup(const ApplyArgs& a) const {
+    return det_apply_adadelta_dup(a.table, a.keys, a.grads, a.n, a.step, rho, epsilon, a.init, a.ws, a.ws_bytes,
+                                  nullptr, a.stream);
+  }
+};
+
+// TFRA>DetApply<Rule> (DUP false: unique keys, init_param [dim] or [n, dim]) and TFRA>DetApply<Rule>DuplicateIndices
+// (DUP true: ids with repeats, init_param [dim], a 256 B aligned workspace)
+template <class Rule, bool DUP>
+class DetApplyOp : public OpKernel {
+ public:
+  explicit DetApplyOp(OpKernelConstruction* ctx) : OpKernel(ctx), rule_(ctx) {}
   void Compute(OpKernelContext* ctx) override {
     tensorflow::lookup::LookupInterface* table = nullptr;
     OP_REQUIRES_OK(ctx, GetLookupTable("table_handle", ctx, &table));
     core::ScopedUnref unref_me(table);
-    det_table* handle = FusedHandle(table);
-    OP_REQUIRES(ctx, handle != nullptr,
-                errors::InvalidArgument(string(OPT == 0 ? "DetApplySgd" : "DetApplyFtrl") +
+    ApplyArgs a{};
+    a.table = FusedHandle(table);
+    OP_REQUIRES(ctx, a.table != nullptr,
+                errors::InvalidArgument(string(Rule::kName) + (DUP ? "DuplicateIndices" : "") +
                                         ": the table's value dtype must be float, half or bfloat16"));
     const Tensor& keys = ctx->input(1);
     const Tensor& grads = ctx->input(2);
-    const Tensor& lr = ctx->input(3);
     const Tensor& init = ctx->input(4);
     const int64 n = keys.NumElements(), dim = table->value_shape().dim_size(0);
     OP_REQUIRES(ctx, grads.NumElements() == n * dim, errors::InvalidArgument("grads must have shape [n, dim]"));
     OP_REQUIRES(ctx, init.NumElements() == dim || (!DUP && init.NumElements() == n * dim),
                 errors::InvalidArgument(DUP ? "init_param must have shape [dim]" : "init_param must have shape [dim] or [n, dim]"));
-    const int64_t* k = reinterpret_cast<const int64_t*>(keys.flat<int64>().data());
-    const float* g = grads.flat<float>().data();
-    const float* ip = init.flat<float>().data();
-    const float step = lr.scalar<float>()();
-    if (!DUP) {
-      const int full = init.NumElements() == dim ? 0 : 1;
-      if (OPT == 0) {
-        OP_REQUIRES_OK(ctx, ToStatus(det_apply_sgd(handle, k, g, static_cast<size_t>(n), step, momentum_, nesterov_,
-                                                   ip, full, StreamOf(ctx))));
-      } else {
-        OP_REQUIRES_OK(ctx, ToStatus(det_apply_ftrl(handle, k, g, static_cast<size_t>(n), step, l1_, l2_, l2_shrinkage_, ip,
-                                                    full, init_accum_, StreamOf(ctx))));
-      }
-      return;
-    }
-    if (n == 0) return;
-    const size_t ws_bytes = det_apply_dup_workspace_bytes(static_cast<size_t>(n), static_cast<size_t>(dim));
     Tensor ws;
-    OP_REQUIRES_OK(ctx, ctx->allocate_temp(DT_INT8, TensorShape({static_cast<int64>(ws_bytes + 256)}), &ws));
-    int8* raw = ws.flat<int8>().data();
-    void* aligned = raw + ((256 - (reinterpret_cast<uintptr_t>(raw) & 255u)) & 255u);
-    if (OPT == 0) {
-      OP_REQUIRES_OK(ctx, ToStatus(det_apply_sgd_dup(handle, k, g, static_cast<size_t>(n), step, momentum_, nesterov_,
-                                                     ip, aligned, ws_bytes, nullptr, StreamOf(ctx))));
-    } else {
-      OP_REQUIRES_OK(ctx, ToStatus(det_apply_ftrl_dup(handle, k, g, static_cast<size_t>(n), step, l1_, l2_, l2_shrinkage_,
-                                                      ip, init_accum_, aligned, ws_bytes, nullptr, StreamOf(ctx))));
+    if (DUP) {
+      if (n == 0) return;
+      // stream-ordered scratch from TF's allocator, aligned up to the 256 B the library asks for
+      a.ws_bytes = det_apply_dup_workspace_bytes(static_cast<size_t>(n), static_cast<size_t>(dim));
+      OP_REQUIRES_OK(ctx, ctx->allocate_temp(DT_INT8, TensorShape({static_cast<int64>(a.ws_bytes + 256)}), &ws));
+      int8* raw = ws.flat<int8>().data();
+      a.ws = raw + ((256 - (reinterpret_cast<uintptr_t>(raw) & 255u)) & 255u);
     }
+    a.keys = reinterpret_cast<const int64_t*>(keys.flat<int64>().data());
+    a.grads = grads.flat<float>().data();
+    a.n = static_cast<size_t>(n);
+    a.step = ctx->input(3).scalar<float>()();
+    a.init = init.flat<float>().data();
+    a.full = init.NumElements() == dim ? 0 : 1;
+    a.stream = StreamOf(ctx);
+    OP_REQUIRES_OK(ctx, ToStatus(DUP ? rule_.Dup(a) : rule_.Unique(a)));
   }
 
  private:
-  float momentum_ = 0.f, l1_ = 0.f, l2_ = 0.f, l2_shrinkage_ = 0.f, init_accum_ = 0.1f;
-  int nesterov_ = 0;
-};
-
-// RMSprop (OPT 0) and Adadelta (OPT 1), unique keys (DUP false) or repeated ids in one call (DUP true)
-template <int OPT, bool DUP>
-class DetApplyRmspropAdadeltaOp : public OpKernel {
- public:
-  explicit DetApplyRmspropAdadeltaOp(OpKernelConstruction* ctx) : OpKernel(ctx) {
-    OP_REQUIRES_OK(ctx, ctx->GetAttr("rho", &rho_));
-    OP_REQUIRES_OK(ctx, ctx->GetAttr("epsilon", &epsilon_));
-    if (OPT == 0) {
-      OP_REQUIRES_OK(ctx, ctx->GetAttr("momentum", &momentum_));
-      OP_REQUIRES_OK(ctx, ctx->GetAttr("centered", &centered_));
-      OP_REQUIRES_OK(ctx, ctx->GetAttr("epsilon_in_sqrt", &eps_in_sqrt_));
-      OP_REQUIRES_OK(ctx, ctx->GetAttr("initial_accumulator_value", &init_ms_));
-    }
-  }
-  void Compute(OpKernelContext* ctx) override {
-    tensorflow::lookup::LookupInterface* table = nullptr;
-    OP_REQUIRES_OK(ctx, GetLookupTable("table_handle", ctx, &table));
-    core::ScopedUnref unref_me(table);
-    det_table* handle = FusedHandle(table);
-    OP_REQUIRES(ctx, handle != nullptr,
-                errors::InvalidArgument(string(OPT == 0 ? "DetApplyRmsprop" : "DetApplyAdadelta") +
-                                        ": the table's value dtype must be float, half or bfloat16"));
-    const Tensor& keys = ctx->input(1);
-    const Tensor& grads = ctx->input(2);
-    const Tensor& lr = ctx->input(3);
-    const Tensor& init = ctx->input(4);
-    const int64 n = keys.NumElements(), dim = table->value_shape().dim_size(0);
-    OP_REQUIRES(ctx, grads.NumElements() == n * dim, errors::InvalidArgument("grads must have shape [n, dim]"));
-    OP_REQUIRES(ctx, init.NumElements() == dim || (!DUP && init.NumElements() == n * dim),
-                errors::InvalidArgument(DUP ? "init_param must have shape [dim]" : "init_param must have shape [dim] or [n, dim]"));
-    const int64_t* k = reinterpret_cast<const int64_t*>(keys.flat<int64>().data());
-    const float* g = grads.flat<float>().data();
-    const float* ip = init.flat<float>().data();
-    const float step = lr.scalar<float>()();
-    const size_t nn = static_cast<size_t>(n);
-    if (!DUP) {
-      const int full = init.NumElements() == dim ? 0 : 1;
-      if (OPT == 0) {
-        OP_REQUIRES_OK(ctx, ToStatus(det_apply_rmsprop(handle, k, g, nn, step, rho_, momentum_, epsilon_, centered_,
-                                                       eps_in_sqrt_, ip, full, init_ms_, StreamOf(ctx))));
-      } else {
-        OP_REQUIRES_OK(ctx, ToStatus(det_apply_adadelta(handle, k, g, nn, step, rho_, epsilon_, ip, full, StreamOf(ctx))));
-      }
-      return;
-    }
-    if (n == 0) return;
-    const size_t ws_bytes = det_apply_dup_workspace_bytes(nn, static_cast<size_t>(dim));
-    Tensor ws;
-    OP_REQUIRES_OK(ctx, ctx->allocate_temp(DT_INT8, TensorShape({static_cast<int64>(ws_bytes + 256)}), &ws));
-    int8* raw = ws.flat<int8>().data();
-    void* aligned = raw + ((256 - (reinterpret_cast<uintptr_t>(raw) & 255u)) & 255u);
-    if (OPT == 0) {
-      OP_REQUIRES_OK(ctx, ToStatus(det_apply_rmsprop_dup(handle, k, g, nn, step, rho_, momentum_, epsilon_, centered_,
-                                                         eps_in_sqrt_, ip, init_ms_, aligned, ws_bytes, nullptr,
-                                                         StreamOf(ctx))));
-    } else {
-      OP_REQUIRES_OK(ctx, ToStatus(det_apply_adadelta_dup(handle, k, g, nn, step, rho_, epsilon_, ip, aligned, ws_bytes,
-                                                          nullptr, StreamOf(ctx))));
-    }
-  }
-
- private:
-  float rho_ = 0.9f, momentum_ = 0.f, epsilon_ = 1e-7f, init_ms_ = 0.f;
-  int centered_ = 0, eps_in_sqrt_ = 0;
+  const Rule rule_;
 };
 
 class DetSegmentReduceOp : public OpKernel {
@@ -495,26 +415,27 @@ class DetSegmentReduceOp : public OpKernel {
 
 REGISTER_KERNEL_BUILDER(Name("TFRA>DetLookupSparse").Device(DEVICE_GPU), DetLookupSparseOp);
 REGISTER_KERNEL_BUILDER(Name("TFRA>DetSegmentReduce").Device(DEVICE_GPU).HostMemory("num_segments"), DetSegmentReduceOp);
-REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplyAdagrad").Device(DEVICE_GPU).HostMemory("lr"), DetApplyAdagradOp);
-REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplyAdam").Device(DEVICE_GPU).HostMemory("alpha"), DetApplyAdamOp);
+REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplyAdagrad").Device(DEVICE_GPU).HostMemory("lr"),
+                        DetApplyOp<AdagradRule, false>);
+REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplyAdam").Device(DEVICE_GPU).HostMemory("alpha"), DetApplyOp<AdamRule, false>);
 REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplyAdagradDuplicateIndices").Device(DEVICE_GPU).HostMemory("lr"),
-                        DetApplyDuplicateIndicesOp<0>);
+                        DetApplyOp<AdagradRule, true>);
 REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplyAdamDuplicateIndices").Device(DEVICE_GPU).HostMemory("alpha"),
-                        DetApplyDuplicateIndicesOp<1>);
-REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplySgd").Device(DEVICE_GPU).HostMemory("lr"), DetApplySgdFtrlOp<0, false>);
-REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplyFtrl").Device(DEVICE_GPU).HostMemory("lr"), DetApplySgdFtrlOp<1, false>);
+                        DetApplyOp<AdamRule, true>);
+REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplySgd").Device(DEVICE_GPU).HostMemory("lr"), DetApplyOp<SgdRule, false>);
+REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplyFtrl").Device(DEVICE_GPU).HostMemory("lr"), DetApplyOp<FtrlRule, false>);
 REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplySgdDuplicateIndices").Device(DEVICE_GPU).HostMemory("lr"),
-                        DetApplySgdFtrlOp<0, true>);
+                        DetApplyOp<SgdRule, true>);
 REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplyFtrlDuplicateIndices").Device(DEVICE_GPU).HostMemory("lr"),
-                        DetApplySgdFtrlOp<1, true>);
+                        DetApplyOp<FtrlRule, true>);
 REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplyRmsprop").Device(DEVICE_GPU).HostMemory("lr"),
-                        DetApplyRmspropAdadeltaOp<0, false>);
+                        DetApplyOp<RmspropRule, false>);
 REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplyAdadelta").Device(DEVICE_GPU).HostMemory("lr"),
-                        DetApplyRmspropAdadeltaOp<1, false>);
+                        DetApplyOp<AdadeltaRule, false>);
 REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplyRmspropDuplicateIndices").Device(DEVICE_GPU).HostMemory("lr"),
-                        DetApplyRmspropAdadeltaOp<0, true>);
+                        DetApplyOp<RmspropRule, true>);
 REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplyAdadeltaDuplicateIndices").Device(DEVICE_GPU).HostMemory("lr"),
-                        DetApplyRmspropAdadeltaOp<1, true>);
+                        DetApplyOp<AdadeltaRule, true>);
 
 }  // namespace det_shim
 }  // namespace lookup

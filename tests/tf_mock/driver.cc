@@ -8,25 +8,11 @@
 // Prints "OK <checks>" on success, aborts with a message otherwise.
 #include <algorithm>
 #include <cmath>
-#include <cstdio>
-#include <cstdlib>
 #include <map>
 #include <numeric>
 
-#include "det_hashtable_of_tensors_gpu.h"
+#include "driver_util.h"
 
-using namespace tensorflow;
-using tensorflow::recommenders_addons::lookup::det_shim::DetHashTableOfTensorsGpu;
-
-static int g_checks = 0;
-#define CHECK_T(cond) do { if (!(cond)) { std::fprintf(stderr, "%s:%d: CHECK failed: %s\n", __FILE__, __LINE__, #cond); std::exit(1); } ++g_checks; } while (0)
-#define CHECK_OK(expr) do { Status _s = (expr); if (!_s.ok()) { std::fprintf(stderr, "%s:%d: %s\n", __FILE__, __LINE__, _s.message().c_str()); std::exit(1); } ++g_checks; } while (0)
-
-static Tensor I64(std::initializer_list<int64> v) {
-  Tensor t(DT_INT64, TensorShape({(int64)v.size()}));
-  std::copy(v.begin(), v.end(), t.flat<int64>().data());
-  return t;
-}
 template <class T> static Tensor Rows(DataType dt, std::initializer_list<T> per_row, int64 dim) {
   Tensor t(dt, TensorShape({(int64)per_row.size(), dim}));
   int64 r = 0;
@@ -44,15 +30,6 @@ struct Harness {   // one table op kernel + a context per call, like a TF sessio
     def.attr["value_shape"].shape = TensorShape({dim});
   }
 };
-struct DummyKernel : OpKernel {
-  using OpKernel::OpKernel;
-  void Compute(OpKernelContext*) override {}
-};
-static OpKernelContext Ctx(DataType vdt) {
-  OpKernelContext c;
-  c.out_dtypes = {{"keys", DT_INT64}, {"values", vdt}, {"scores", DT_INT64}, {"output", DT_FLOAT}};
-  return c;
-}
 
 template <class V> static void known_answers(DataType vdt, int64 dim) {
   Harness h(dim, 1024, 1 << 16, /*LRU*/ 0);

@@ -4,55 +4,8 @@
 // result is the fp32 step rounded to nearest even into the table's dtype, computed here; an int32 table is refused
 // with InvalidArgument.  Prints "OK <checks>" on success, exits non-zero otherwise.
 #include <cmath>
-#include <cstdio>
-#include <cstdlib>
-#include <cstring>
-#include <memory>
 
-#include "det_hashtable_of_tensors_gpu.h"
-
-using namespace tensorflow;
-using tensorflow::recommenders_addons::lookup::det_shim::DetHashTableOfTensorsGpu;
-
-static int g_checks = 0;
-#define CHECK_T(cond) do { if (!(cond)) { std::fprintf(stderr, "%s:%d: CHECK failed: %s\n", __FILE__, __LINE__, #cond); std::exit(1); } ++g_checks; } while (0)
-#define CHECK_OK(expr) do { Status _s = (expr); if (!_s.ok()) { std::fprintf(stderr, "%s:%d: %s\n", __FILE__, __LINE__, _s.message().c_str()); std::exit(1); } ++g_checks; } while (0)
-
-struct DummyKernel : OpKernel {
-  using OpKernel::OpKernel;
-  void Compute(OpKernelContext*) override {}
-};
-
-static OpKernelContext Ctx(DataType vdt) {
-  OpKernelContext c;
-  c.out_dtypes = {{"keys", DT_INT64}, {"values", vdt}, {"scores", DT_INT64}, {"output", DT_FLOAT}};
-  return c;
-}
-
-static NodeDef TableDef(int64 dim) {
-  NodeDef def;
-  def.attr["init_capacity"].i = 1024;
-  def.attr["max_capacity"].i = 1 << 16;
-  def.attr["max_hbm_for_vectors"].i = 0;
-  def.attr["strategy"].i = 0;
-  def.attr["step_per_epoch"].i = 0;
-  def.attr["value_shape"].shape = TensorShape({dim});
-  return def;
-}
-
-static Tensor I64(std::initializer_list<int64> v) {
-  Tensor t(DT_INT64, TensorShape({(int64)v.size()}));
-  int64 i = 0;
-  for (int64 x : v) t.flat<int64>()(i++) = x;
-  return t;
-}
-
-static Tensor F32Rows(std::initializer_list<float> per_row, int64 dim) {
-  Tensor t(DT_FLOAT, TensorShape({(int64)per_row.size(), dim}));
-  int64 r = 0;
-  for (float v : per_row) { for (int64 c = 0; c < dim; ++c) t.flat<float>()(r * dim + c) = v; ++r; }
-  return t;
-}
+#include "driver_util.h"
 
 // 16-bit patterns of a float rounded to nearest even (normal values of the format only, which is all this driver
 // makes), and back

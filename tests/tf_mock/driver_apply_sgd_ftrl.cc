@@ -3,75 +3,8 @@
 // libdetable.  Every result is the fp32 rule computed here (bf16: rounded to nearest even once); an int32 table is
 // refused with InvalidArgument.  Prints "OK <checks>" on success, exits non-zero otherwise.
 #include <cmath>
-#include <cstdio>
-#include <cstdlib>
-#include <cstring>
-#include <memory>
 
-#include "det_hashtable_of_tensors_gpu.h"
-
-using namespace tensorflow;
-using tensorflow::recommenders_addons::lookup::det_shim::DetHashTableOfTensorsGpu;
-
-static int g_checks = 0;
-#define CHECK_T(cond) do { if (!(cond)) { std::fprintf(stderr, "%s:%d: CHECK failed: %s\n", __FILE__, __LINE__, #cond); std::exit(1); } ++g_checks; } while (0)
-#define CHECK_OK(expr) do { Status _s = (expr); if (!_s.ok()) { std::fprintf(stderr, "%s:%d: %s\n", __FILE__, __LINE__, _s.message().c_str()); std::exit(1); } ++g_checks; } while (0)
-
-struct DummyKernel : OpKernel {
-  using OpKernel::OpKernel;
-  void Compute(OpKernelContext*) override {}
-};
-
-static OpKernelContext Ctx(DataType vdt) {
-  OpKernelContext c;
-  c.out_dtypes = {{"keys", DT_INT64}, {"values", vdt}, {"scores", DT_INT64}, {"output", DT_FLOAT}};
-  return c;
-}
-
-static NodeDef TableDef(int64 dim) {
-  NodeDef def;
-  def.attr["init_capacity"].i = 1024;
-  def.attr["max_capacity"].i = 1 << 16;
-  def.attr["max_hbm_for_vectors"].i = 0;
-  def.attr["strategy"].i = 0;
-  def.attr["step_per_epoch"].i = 0;
-  def.attr["value_shape"].shape = TensorShape({dim});
-  return def;
-}
-
-static Tensor I64(std::initializer_list<int64> v) {
-  Tensor t(DT_INT64, TensorShape({(int64)v.size()}));
-  int64 i = 0;
-  for (int64 x : v) t.flat<int64>()(i++) = x;
-  return t;
-}
-
-static Tensor F32Rows(std::initializer_list<float> per_row, int64 dim) {
-  Tensor t(DT_FLOAT, TensorShape({(int64)per_row.size(), dim}));
-  int64 r = 0;
-  for (float v : per_row) { for (int64 c = 0; c < dim; ++c) t.flat<float>()(r * dim + c) = v; ++r; }
-  return t;
-}
-
-// a float as stored by a table of `vdt` (bf16: rounded to nearest even, normal values only) and read back as float
-static float stored(DataType vdt, float f) {
-  if (vdt == DT_FLOAT) return f;
-  uint32_t b;
-  std::memcpy(&b, &f, 4);
-  b = ((b + 0x7fffu + ((b >> 16) & 1u)) >> 16) << 16;
-  std::memcpy(&f, &b, 4);
-  return f;
-}
-
-template <class V> static float first_of(const Tensor& t, int64 row, int64 dim, DataType vdt) {
-  if (vdt == DT_FLOAT) return reinterpret_cast<const float*>(t.flat<V>().data())[row * dim];
-  uint16_t h;
-  std::memcpy(&h, &t.flat<V>().data()[row * dim], 2);
-  const uint32_t b = (uint32_t)h << 16;
-  float f;
-  std::memcpy(&f, &b, 4);
-  return f;
-}
+#include "driver_util.h"
 
 template <class V> static void apply_on(DataType vdt) {
   const int64 dim = 4;
