@@ -326,6 +326,39 @@ det_status det_apply_rmsprop(det_table* t, const int64_t* keys, const float* gra
                              int full_size_init, float init_ms, det_stream_t stream);
 det_status det_apply_adadelta(det_table* t, const int64_t* keys, const float* grads, size_t n, float lr, float rho,
                               float epsilon, const float* init_param, int full_size_init, det_stream_t stream);
+/* The same step for Adamax, Nadam, ProximalAdagrad, ProximalGradientDescent and AdagradDA.  r1 = 1 - beta1 and
+ * r2 = 1 - beta2 are computed once in fp32; the scalars that depend only on the step are the caller's, in fp32.
+ * Adamax (Keras): m = m*beta1 + g*r1;  v = max(v*beta2, |g|);  p = p + nsl*(m / (v + eps)) with nsl = -lr_t and
+ *   lr_t = lr / (1 - beta1^t) from the caller.  Plane 1 = m, plane 2 = v (both initial 0).
+ * Nadam (Keras): g' = g / omsn;  m = m*beta1 + g*r1;  m' = m / omsx;  mbar = omt*g' + mt1*m';
+ *   v = v*beta2 + (g*g)*r2;  v' = v / vden;  p = p + (nlr*mbar) / (sqrt(v') + eps) with nlr = -lr.  The caller computes,
+ *   as Keras' _prepare_local: u_t = beta1*(1 - 0.5*0.96^(0.004*t)), u_t1 the same at t + 1, msn = m_cache*u_t,
+ *   msx = msn*u_t1, omsn = 1 - msn, omsx = 1 - msx, omt = 1 - u_t, mt1 = u_t1, vden = 1 - beta2^t (m_cache: the product
+ *   of the earlier steps' u, 1 before the first).  Plane 1 = m, plane 2 = v (both initial 0).
+ * Shrink: S(x, c) = sign(x)*max(|x| - c, 0) (sign(0) = 0).
+ * ProximalAdagrad (TF1): a = a + g*g;  eta = lr / sqrt(a);  q = p - g*eta;
+ *   p = l1 > 0 ? S(q, eta*l1) / (1 + l2*eta) : q / (1 + l2*eta).  A correctly rounded square root and one division
+ *   where TF multiplies by rsqrt (DESIGN.md section 4).  Plane 1 = accumulator (initial init_accum).
+ * ProximalGradientDescent (TF1): q = p - g*lr, then the same with eta = lr.  No slot plane; with l1 = l2 = 0 it is
+ *   det_apply_sgd bit for bit.
+ * AdagradDA (TF1): ga = ga + g;  gg = gg + g*g;  p = ((l1 > 0 ? -S(ga, l1*gs) : -ga) / ((l2*gs)*lr + sqrt(gg)))*lr,
+ *   with gs = global_step >= 1, TF1's step on the worker (its global step + 1).  Plane 1 = gradient_accumulator ga
+ *   (initial 0), plane 2 = gradient_squared_accumulator gg (initial init_gg).
+ * lr <= 0, a negative l1, l2 or initial accumulator (NaN included) of the proximal and DA steps, or global_step < 1:
+ * DET_INVALID_ARGUMENT.  Additive to ABI 8. */
+det_status det_apply_adamax(det_table* t, const int64_t* keys, const float* grads, size_t n, float lr_t, float beta1,
+                            float beta2, float epsilon, const float* init_param, int full_size_init, det_stream_t stream);
+det_status det_apply_nadam(det_table* t, const int64_t* keys, const float* grads, size_t n, float lr, float beta1,
+                           float beta2, float epsilon, float omsn, float omsx, float omt, float mt1, float vden,
+                           const float* init_param, int full_size_init, det_stream_t stream);
+det_status det_apply_proximal_adagrad(det_table* t, const int64_t* keys, const float* grads, size_t n, float lr, float l1,
+                                      float l2, const float* init_param, int full_size_init, float init_accum,
+                                      det_stream_t stream);
+det_status det_apply_proximal_sgd(det_table* t, const int64_t* keys, const float* grads, size_t n, float lr, float l1,
+                                  float l2, const float* init_param, int full_size_init, det_stream_t stream);
+det_status det_apply_adagrad_da(det_table* t, const int64_t* keys, const float* grads, size_t n, float lr, float l1,
+                                float l2, int64_t global_step, const float* init_param, int full_size_init,
+                                float init_gg, det_stream_t stream);
 
 /* ---- HOST-buffer entry points (the op placed on host tensors; used for end-to-end timing):
  * pinned or pageable HOST pointers; chunked H2D -> kernel -> D2H pipeline on internal streams;
@@ -376,6 +409,23 @@ det_status det_apply_rmsprop_dup(det_table* t, const int64_t* ids, const float* 
 det_status det_apply_adadelta_dup(det_table* t, const int64_t* ids, const float* grads, size_t n, float lr, float rho,
                                   float epsilon, const float* init_param, void* workspace, size_t workspace_bytes,
                                   int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_adamax_dup(det_table* t, const int64_t* ids, const float* grads, size_t n, float lr_t, float beta1,
+                                float beta2, float epsilon, const float* init_param, void* workspace,
+                                size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_nadam_dup(det_table* t, const int64_t* ids, const float* grads, size_t n, float lr, float beta1,
+                               float beta2, float epsilon, float omsn, float omsx, float omt, float mt1, float vden,
+                               const float* init_param, void* workspace, size_t workspace_bytes,
+                               int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_proximal_adagrad_dup(det_table* t, const int64_t* ids, const float* grads, size_t n, float lr,
+                                          float l1, float l2, const float* init_param, float init_accum, void* workspace,
+                                          size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_proximal_sgd_dup(det_table* t, const int64_t* ids, const float* grads, size_t n, float lr, float l1,
+                                      float l2, const float* init_param, void* workspace, size_t workspace_bytes,
+                                      int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_adagrad_da_dup(det_table* t, const int64_t* ids, const float* grads, size_t n, float lr, float l1,
+                                    float l2, int64_t global_step, const float* init_param, float init_gg,
+                                    void* workspace, size_t workspace_bytes, int64_t* n_unique_dev_out,
+                                    det_stream_t stream);
 
 /* The backward of det_lookup_sparse, fused: per-unique-id gradients straight from the output gradient (ABI >= 8).
  * Inputs are the forward's ids int64[nnz], segment_ids int32[nnz] (ascending, in [0, batch)), weights f32[nnz] or NULL
@@ -428,6 +478,29 @@ det_status det_apply_adadelta_sparse(det_table* t, const int64_t* ids, const int
                                      size_t nnz, size_t batch, int combiner, const float* gout, float lr, float rho,
                                      float epsilon, const float* init_param, void* workspace, size_t workspace_bytes,
                                      int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_adamax_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
+                                   size_t nnz, size_t batch, int combiner, const float* gout, float lr_t, float beta1,
+                                   float beta2, float epsilon, const float* init_param, void* workspace,
+                                   size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_nadam_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
+                                  size_t nnz, size_t batch, int combiner, const float* gout, float lr, float beta1,
+                                  float beta2, float epsilon, float omsn, float omsx, float omt, float mt1, float vden,
+                                  const float* init_param, void* workspace, size_t workspace_bytes,
+                                  int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_proximal_adagrad_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                             const float* weights, size_t nnz, size_t batch, int combiner,
+                                             const float* gout, float lr, float l1, float l2, const float* init_param,
+                                             float init_accum, void* workspace, size_t workspace_bytes,
+                                             int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_proximal_sgd_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                         const float* weights, size_t nnz, size_t batch, int combiner, const float* gout,
+                                         float lr, float l1, float l2, const float* init_param, void* workspace,
+                                         size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_adagrad_da_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                       const float* weights, size_t nnz, size_t batch, int combiner, const float* gout,
+                                       float lr, float l1, float l2, int64_t global_step, const float* init_param,
+                                       float init_gg, void* workspace, size_t workspace_bytes,
+                                       int64_t* n_unique_dev_out, det_stream_t stream);
 
 /* ---- key-hash sharding across GPUs (python/ops/dynamic_embedding_variable.py:165-197 default_partition_fn,
  * python/ops/shadow_embedding_ops.py:397-447 alltoall exchange) ----

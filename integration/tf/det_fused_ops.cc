@@ -156,6 +156,113 @@ REGISTER_OP("TFRA>DetApplyAdadeltaDuplicateIndices")
     .Attr("rho: float = 0.95")
     .Attr("epsilon: float = 1e-7");
 
+// Adamax and Nadam (Keras' _resource_apply_sparse), ProximalAdagrad, ProximalGradientDescent and AdagradDA (TF1's
+// SparseApplyProximalAdagrad / SparseApplyProximalGradientDescent / SparseApplyAdagradDA), as det_apply_adamax /
+// _nadam / _proximal_adagrad / _proximal_sgd / _adagrad_da.  The scalars that depend on the step are host-memory inputs:
+// Adamax's lr_t = lr / (1 - beta1^t); Nadam's schedule [omsn, omsx, omt, mt1, vden] (Keras' _prepare_local, see
+// include/detable.h); AdagradDA's global_step, TF1's step on the worker (its global step + 1).
+REGISTER_OP("TFRA>DetApplyAdamax")
+    .Input("table_handle: resource")
+    .Input("keys: int64")          // [n] unique
+    .Input("grads: float")         // [n, dim]
+    .Input("lr_t: float")
+    .Input("init_param: float")    // [dim] or [n, dim]
+    .Attr("beta1: float = 0.9")
+    .Attr("beta2: float = 0.999")
+    .Attr("epsilon: float = 1e-7");
+
+REGISTER_OP("TFRA>DetApplyNadam")
+    .Input("table_handle: resource")
+    .Input("keys: int64")
+    .Input("grads: float")
+    .Input("lr: float")
+    .Input("init_param: float")
+    .Input("schedule: float")      // [5]
+    .Attr("beta1: float = 0.9")
+    .Attr("beta2: float = 0.999")
+    .Attr("epsilon: float = 1e-7");
+
+REGISTER_OP("TFRA>DetApplyProximalAdagrad")
+    .Input("table_handle: resource")
+    .Input("keys: int64")
+    .Input("grads: float")
+    .Input("lr: float")
+    .Input("init_param: float")
+    .Attr("l1: float = 0.0")
+    .Attr("l2: float = 0.0")
+    .Attr("initial_accumulator_value: float = 0.1");
+
+REGISTER_OP("TFRA>DetApplyProximalGradientDescent")
+    .Input("table_handle: resource")
+    .Input("keys: int64")
+    .Input("grads: float")
+    .Input("lr: float")
+    .Input("init_param: float")
+    .Attr("l1: float = 0.0")
+    .Attr("l2: float = 0.0");
+
+REGISTER_OP("TFRA>DetApplyAdagradDA")
+    .Input("table_handle: resource")
+    .Input("keys: int64")
+    .Input("grads: float")
+    .Input("lr: float")
+    .Input("init_param: float")
+    .Input("global_step: int64")
+    .Attr("l1: float = 0.0")
+    .Attr("l2: float = 0.0")
+    .Attr("initial_gradient_squared_accumulator_value: float = 0.1");
+
+REGISTER_OP("TFRA>DetApplyAdamaxDuplicateIndices")
+    .Input("table_handle: resource")
+    .Input("ids: int64")
+    .Input("grads: float")
+    .Input("lr_t: float")
+    .Input("init_param: float")    // [dim]
+    .Attr("beta1: float = 0.9")
+    .Attr("beta2: float = 0.999")
+    .Attr("epsilon: float = 1e-7");
+
+REGISTER_OP("TFRA>DetApplyNadamDuplicateIndices")
+    .Input("table_handle: resource")
+    .Input("ids: int64")
+    .Input("grads: float")
+    .Input("lr: float")
+    .Input("init_param: float")
+    .Input("schedule: float")
+    .Attr("beta1: float = 0.9")
+    .Attr("beta2: float = 0.999")
+    .Attr("epsilon: float = 1e-7");
+
+REGISTER_OP("TFRA>DetApplyProximalAdagradDuplicateIndices")
+    .Input("table_handle: resource")
+    .Input("ids: int64")
+    .Input("grads: float")
+    .Input("lr: float")
+    .Input("init_param: float")
+    .Attr("l1: float = 0.0")
+    .Attr("l2: float = 0.0")
+    .Attr("initial_accumulator_value: float = 0.1");
+
+REGISTER_OP("TFRA>DetApplyProximalGradientDescentDuplicateIndices")
+    .Input("table_handle: resource")
+    .Input("ids: int64")
+    .Input("grads: float")
+    .Input("lr: float")
+    .Input("init_param: float")
+    .Attr("l1: float = 0.0")
+    .Attr("l2: float = 0.0");
+
+REGISTER_OP("TFRA>DetApplyAdagradDADuplicateIndices")
+    .Input("table_handle: resource")
+    .Input("ids: int64")
+    .Input("grads: float")
+    .Input("lr: float")
+    .Input("init_param: float")
+    .Input("global_step: int64")
+    .Attr("l1: float = 0.0")
+    .Attr("l2: float = 0.0")
+    .Attr("initial_gradient_squared_accumulator_value: float = 0.1");
+
 // The gradient dedupe in front of the sparse optimizer step: unsorted_segment_sum(values, idx, num_segments) as
 // _deduplicate_indexed_slices calls it before _resource_apply_sparse_duplicate_indices
 // (python/ops/dynamic_embedding_optimizer.py:150,184), with the rows of one segment added in position order
@@ -222,8 +329,10 @@ class DetLookupSparseOp : public OpKernel {
 };
 
 // What a TFRA>DetApply* op hands the library.  `step` is input 3: lr, or alpha for Adam.  `full` is 1 when init_param
-// holds one row per key (unique-key forms only); `ws` / `ws_bytes` are the duplicate-id forms' workspace.
+// holds one row per key (unique-key forms only); `ws` / `ws_bytes` are the duplicate-id forms' workspace.  `ctx`: for
+// the rules with more step inputs after init_param (Nadam, AdagradDA).
 struct ApplyArgs {
+  OpKernelContext* ctx;
   det_table* table;
   const int64_t* keys;
   const float* grads;
@@ -344,6 +453,104 @@ struct AdadeltaRule {
   }
 };
 
+struct AdamaxRule {
+  static constexpr const char* kName = "DetApplyAdamax";
+  float beta1 = 0.9f, beta2 = 0.999f, epsilon = 1e-7f;
+  explicit AdamaxRule(OpKernelConstruction* ctx) {
+    OP_REQUIRES_OK(ctx, ctx->GetAttr("beta1", &beta1));
+    OP_REQUIRES_OK(ctx, ctx->GetAttr("beta2", &beta2));
+    OP_REQUIRES_OK(ctx, ctx->GetAttr("epsilon", &epsilon));
+  }
+  det_status Unique(const ApplyArgs& a) const {
+    return det_apply_adamax(a.table, a.keys, a.grads, a.n, a.step, beta1, beta2, epsilon, a.init, a.full, a.stream);
+  }
+  det_status Dup(const ApplyArgs& a) const {
+    return det_apply_adamax_dup(a.table, a.keys, a.grads, a.n, a.step, beta1, beta2, epsilon, a.init, a.ws, a.ws_bytes,
+                                nullptr, a.stream);
+  }
+};
+
+struct NadamRule {
+  static constexpr const char* kName = "DetApplyNadam";
+  float beta1 = 0.9f, beta2 = 0.999f, epsilon = 1e-7f;
+  explicit NadamRule(OpKernelConstruction* ctx) {
+    OP_REQUIRES_OK(ctx, ctx->GetAttr("beta1", &beta1));
+    OP_REQUIRES_OK(ctx, ctx->GetAttr("beta2", &beta2));
+    OP_REQUIRES_OK(ctx, ctx->GetAttr("epsilon", &epsilon));
+  }
+  // input 5, the step's schedule [omsn, omsx, omt, mt1, vden]
+  static const float* Schedule(const ApplyArgs& a) {
+    const Tensor& s = a.ctx->input(5);
+    return s.NumElements() == 5 ? s.flat<float>().data() : nullptr;
+  }
+  det_status Unique(const ApplyArgs& a) const {
+    const float* s = Schedule(a);
+    if (!s) return DET_INVALID_ARGUMENT;
+    return det_apply_nadam(a.table, a.keys, a.grads, a.n, a.step, beta1, beta2, epsilon, s[0], s[1], s[2], s[3], s[4],
+                           a.init, a.full, a.stream);
+  }
+  det_status Dup(const ApplyArgs& a) const {
+    const float* s = Schedule(a);
+    if (!s) return DET_INVALID_ARGUMENT;
+    return det_apply_nadam_dup(a.table, a.keys, a.grads, a.n, a.step, beta1, beta2, epsilon, s[0], s[1], s[2], s[3],
+                               s[4], a.init, a.ws, a.ws_bytes, nullptr, a.stream);
+  }
+};
+
+struct ProximalAdagradRule {
+  static constexpr const char* kName = "DetApplyProximalAdagrad";
+  float l1 = 0.f, l2 = 0.f, init_accum = 0.1f;
+  explicit ProximalAdagradRule(OpKernelConstruction* ctx) {
+    OP_REQUIRES_OK(ctx, ctx->GetAttr("l1", &l1));
+    OP_REQUIRES_OK(ctx, ctx->GetAttr("l2", &l2));
+    OP_REQUIRES_OK(ctx, ctx->GetAttr("initial_accumulator_value", &init_accum));
+  }
+  det_status Unique(const ApplyArgs& a) const {
+    return det_apply_proximal_adagrad(a.table, a.keys, a.grads, a.n, a.step, l1, l2, a.init, a.full, init_accum,
+                                      a.stream);
+  }
+  det_status Dup(const ApplyArgs& a) const {
+    return det_apply_proximal_adagrad_dup(a.table, a.keys, a.grads, a.n, a.step, l1, l2, a.init, init_accum, a.ws,
+                                          a.ws_bytes, nullptr, a.stream);
+  }
+};
+
+struct ProximalSgdRule {
+  static constexpr const char* kName = "DetApplyProximalGradientDescent";
+  float l1 = 0.f, l2 = 0.f;
+  explicit ProximalSgdRule(OpKernelConstruction* ctx) {
+    OP_REQUIRES_OK(ctx, ctx->GetAttr("l1", &l1));
+    OP_REQUIRES_OK(ctx, ctx->GetAttr("l2", &l2));
+  }
+  det_status Unique(const ApplyArgs& a) const {
+    return det_apply_proximal_sgd(a.table, a.keys, a.grads, a.n, a.step, l1, l2, a.init, a.full, a.stream);
+  }
+  det_status Dup(const ApplyArgs& a) const {
+    return det_apply_proximal_sgd_dup(a.table, a.keys, a.grads, a.n, a.step, l1, l2, a.init, a.ws, a.ws_bytes, nullptr,
+                                      a.stream);
+  }
+};
+
+struct AdagradDARule {
+  static constexpr const char* kName = "DetApplyAdagradDA";
+  float l1 = 0.f, l2 = 0.f, init_gg = 0.1f;
+  explicit AdagradDARule(OpKernelConstruction* ctx) {
+    OP_REQUIRES_OK(ctx, ctx->GetAttr("l1", &l1));
+    OP_REQUIRES_OK(ctx, ctx->GetAttr("l2", &l2));
+    OP_REQUIRES_OK(ctx, ctx->GetAttr("initial_gradient_squared_accumulator_value", &init_gg));
+  }
+  // input 5, the step on the worker
+  static int64_t Step(const ApplyArgs& a) { return static_cast<int64_t>(a.ctx->input(5).scalar<int64>()()); }
+  det_status Unique(const ApplyArgs& a) const {
+    return det_apply_adagrad_da(a.table, a.keys, a.grads, a.n, a.step, l1, l2, Step(a), a.init, a.full, init_gg,
+                                a.stream);
+  }
+  det_status Dup(const ApplyArgs& a) const {
+    return det_apply_adagrad_da_dup(a.table, a.keys, a.grads, a.n, a.step, l1, l2, Step(a), a.init, init_gg, a.ws,
+                                    a.ws_bytes, nullptr, a.stream);
+  }
+};
+
 // TFRA>DetApply<Rule> (DUP false: unique keys, init_param [dim] or [n, dim]) and TFRA>DetApply<Rule>DuplicateIndices
 // (DUP true: ids with repeats, init_param [dim], a 256 B aligned workspace)
 template <class Rule, bool DUP>
@@ -382,6 +589,7 @@ class DetApplyOp : public OpKernel {
     a.init = init.flat<float>().data();
     a.full = init.NumElements() == dim ? 0 : 1;
     a.stream = StreamOf(ctx);
+    a.ctx = ctx;
     OP_REQUIRES_OK(ctx, ToStatus(DUP ? rule_.Dup(a) : rule_.Unique(a)));
   }
 
@@ -436,6 +644,25 @@ REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplyRmspropDuplicateIndices").Device(DEVI
                         DetApplyOp<RmspropRule, true>);
 REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplyAdadeltaDuplicateIndices").Device(DEVICE_GPU).HostMemory("lr"),
                         DetApplyOp<AdadeltaRule, true>);
+REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplyAdamax").Device(DEVICE_GPU).HostMemory("lr_t"), DetApplyOp<AdamaxRule, false>);
+REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplyNadam").Device(DEVICE_GPU).HostMemory("lr").HostMemory("schedule"),
+                        DetApplyOp<NadamRule, false>);
+REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplyProximalAdagrad").Device(DEVICE_GPU).HostMemory("lr"),
+                        DetApplyOp<ProximalAdagradRule, false>);
+REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplyProximalGradientDescent").Device(DEVICE_GPU).HostMemory("lr"),
+                        DetApplyOp<ProximalSgdRule, false>);
+REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplyAdagradDA").Device(DEVICE_GPU).HostMemory("lr").HostMemory("global_step"),
+                        DetApplyOp<AdagradDARule, false>);
+REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplyAdamaxDuplicateIndices").Device(DEVICE_GPU).HostMemory("lr_t"),
+                        DetApplyOp<AdamaxRule, true>);
+REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplyNadamDuplicateIndices").Device(DEVICE_GPU).HostMemory("lr").HostMemory("schedule"),
+                        DetApplyOp<NadamRule, true>);
+REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplyProximalAdagradDuplicateIndices").Device(DEVICE_GPU).HostMemory("lr"),
+                        DetApplyOp<ProximalAdagradRule, true>);
+REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplyProximalGradientDescentDuplicateIndices").Device(DEVICE_GPU).HostMemory("lr"),
+                        DetApplyOp<ProximalSgdRule, true>);
+REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplyAdagradDADuplicateIndices").Device(DEVICE_GPU).HostMemory("lr").HostMemory("global_step"),
+                        DetApplyOp<AdagradDARule, true>);
 
 }  // namespace det_shim
 }  // namespace lookup

@@ -106,6 +106,30 @@ SIGNATURES = {
                                       ctypes.c_float, ctypes.c_float, _i, _i, _vp, ctypes.c_float, _vp, _sz, _vp, _vp]),
     "det_apply_adadelta_sparse": (_i, [_vp, _vp, _vp, _vp, _sz, _sz, _i, _vp, ctypes.c_float, ctypes.c_float,
                                        ctypes.c_float, _vp, _vp, _sz, _vp, _vp]),
+    # Adamax, Nadam, ProximalAdagrad, ProximalGradientDescent, AdagradDA: unique keys, then _dup, then _sparse
+    "det_apply_adamax": (_i, [_vp, _vp, _vp, _sz] + [ctypes.c_float] * 4 + [_vp, _i, _vp]),
+    "det_apply_nadam": (_i, [_vp, _vp, _vp, _sz] + [ctypes.c_float] * 9 + [_vp, _i, _vp]),
+    "det_apply_proximal_adagrad": (_i, [_vp, _vp, _vp, _sz] + [ctypes.c_float] * 3 + [_vp, _i, ctypes.c_float, _vp]),
+    "det_apply_proximal_sgd": (_i, [_vp, _vp, _vp, _sz] + [ctypes.c_float] * 3 + [_vp, _i, _vp]),
+    "det_apply_adagrad_da": (_i, [_vp, _vp, _vp, _sz] + [ctypes.c_float] * 3 + [ctypes.c_int64, _vp, _i, ctypes.c_float,
+                                                                               _vp]),
+    "det_apply_adamax_dup": (_i, [_vp, _vp, _vp, _sz] + [ctypes.c_float] * 4 + [_vp, _vp, _sz, _vp, _vp]),
+    "det_apply_nadam_dup": (_i, [_vp, _vp, _vp, _sz] + [ctypes.c_float] * 9 + [_vp, _vp, _sz, _vp, _vp]),
+    "det_apply_proximal_adagrad_dup": (_i, [_vp, _vp, _vp, _sz] + [ctypes.c_float] * 3 + [_vp, ctypes.c_float, _vp, _sz,
+                                                                                         _vp, _vp]),
+    "det_apply_proximal_sgd_dup": (_i, [_vp, _vp, _vp, _sz] + [ctypes.c_float] * 3 + [_vp, _vp, _sz, _vp, _vp]),
+    "det_apply_adagrad_da_dup": (_i, [_vp, _vp, _vp, _sz] + [ctypes.c_float] * 3 + [ctypes.c_int64, _vp, ctypes.c_float,
+                                                                                   _vp, _sz, _vp, _vp]),
+    "det_apply_adamax_sparse": (_i, [_vp, _vp, _vp, _vp, _sz, _sz, _i, _vp] + [ctypes.c_float] * 4 + [_vp, _vp, _sz, _vp,
+                                                                                                     _vp]),
+    "det_apply_nadam_sparse": (_i, [_vp, _vp, _vp, _vp, _sz, _sz, _i, _vp] + [ctypes.c_float] * 9 + [_vp, _vp, _sz, _vp,
+                                                                                                    _vp]),
+    "det_apply_proximal_adagrad_sparse": (_i, [_vp, _vp, _vp, _vp, _sz, _sz, _i, _vp] + [ctypes.c_float] * 3 +
+                                          [_vp, ctypes.c_float, _vp, _sz, _vp, _vp]),
+    "det_apply_proximal_sgd_sparse": (_i, [_vp, _vp, _vp, _vp, _sz, _sz, _i, _vp] + [ctypes.c_float] * 3 +
+                                      [_vp, _vp, _sz, _vp, _vp]),
+    "det_apply_adagrad_da_sparse": (_i, [_vp, _vp, _vp, _vp, _sz, _sz, _i, _vp] + [ctypes.c_float] * 3 +
+                                    [ctypes.c_int64, _vp, ctypes.c_float, _vp, _sz, _vp, _vp]),
     "det_find_host": (_i, [_vp, _vp, _sz, _vp, _i, _vp, _vp]),
     "det_insert_host": (_i, [_vp, _vp, _vp, _sz]),
     "det_find_host_async": (_i, [_vp, _vp, _sz, _vp, _i, _vp, _vp]),

@@ -769,16 +769,43 @@ segment_sum_wide_kernel(TableView t, const long long* __restrict__ slots, const 
 // ------------------------------------------------------------------------------------------------
 // K7: fused find-or-insert + optimizer update
 // ------------------------------------------------------------------------------------------------
-// The optimizer of a K7 launch is its template parameter OPT (kAdagrad .. kAdadelta, host.h) with an OptHyper.
+// The optimizer of a K7 launch is its template parameter OPT (kAdagrad .. kAdagradDa, host.h) with an OptHyper (and,
+// for Nadam, a StepArg).
 
 // slot planes an optimizer reads and writes (planes 1 .. opt_slots(OPT)): Adagrad accumulator = plane 1; Adam m =
 // plane 1, v = plane 2; momentum = plane 1; FTRL accumulator n = plane 1, linear z = plane 2; RMSprop rms = plane 1,
 // then mg if centered, then momentum if momentum > 0 (kRmsprop1 .. kRmsprop3); Adadelta accum_grad = plane 1,
-// accum_var = plane 2
+// accum_var = plane 2; Adamax and Nadam m = plane 1, v = plane 2; ProximalAdagrad accumulator = plane 1;
+// ProximalGradientDescent none; AdagradDA gradient_accumulator = plane 1, gradient_squared_accumulator = plane 2
 __host__ __device__ constexpr int opt_slots(int opt) {
   return opt == kRmsprop3 ? 3
-         : opt == kAdam || opt == kFtrl || opt == kRmsprop2 || opt == kAdadelta ? 2
-         : opt == kSgd ? 0 : 1;
+         : opt == kAdam || opt == kFtrl || opt == kRmsprop2 || opt == kAdadelta || opt == kAdamax || opt == kNadam ||
+                   opt == kAdagradDa
+             ? 2
+         : opt == kSgd || opt == kProxSgd ? 0 : 1;
+}
+
+// The per-step scalars beyond OptHyper (host.h StepScalars), the trailing K7 kernel argument: Nadam's; EMPTY for every
+// other optimizer, which keeps their kernels' parameters as they were (like SlotPlanes, ScoreArg and InitArg).
+template <int OPT> struct StepArg {};
+template <> struct StepArg<kNadam> : StepScalars {};
+template <int OPT>
+static StepArg<OPT> step_arg(const StepScalars& sx) {
+  StepArg<OPT> x{};
+  if constexpr (OPT == kNadam) static_cast<StepScalars&>(x) = sx;
+  return x;
+}
+
+// sign(x) * max(|x| - t, 0), sign(0) = 0: the l1 shrink of TF's proximal and AdagradDA kernels
+__device__ __forceinline__ float shrink(float x, float t) {
+  const float s = x > 0.f ? 1.f : (x < 0.f ? -1.f : 0.f);
+  return s * fmaxf(fabsf(x) - t, 0.f);
+}
+// The proximal step of ProximalAdagrad and ProximalGradientDescent from q = p - g*eta: with l1 > 0 the shrink by
+// eta*l1, then the l2 division.  The branch is uniform over the launch.  l1 = l2 = 0 gives q / 1 = q exactly.
+__device__ __forceinline__ float prox_step(float q, float eta, float l1, float l2) {
+  const float d = 1.f + l2 * eta;
+  return l1 > 0.f ? shrink(q, eta * l1) / d : q / d;
 }
 
 // The slot values a key without slot state starts from: a slot 1, b slot 2, c slot 3.
@@ -788,9 +815,14 @@ __device__ __forceinline__ void opt_fresh(const OptHyper& h, FVec<VF>& a, FVec<V
     a.fill(h.init_slot);
     if constexpr (opt_slots(OPT) > 1) b.zero();
     if constexpr (opt_slots(OPT) > 2) c.zero();
-  } else if constexpr (OPT == kAdadelta) {
+  } else if constexpr (OPT == kAdadelta || OPT == kAdamax || OPT == kNadam) {
     a.zero();
     b.zero();
+  } else if constexpr (OPT == kProxAdagrad) {
+    a.fill(h.init_slot);
+  } else if constexpr (OPT == kAdagradDa) {
+    a.zero();
+    b.fill(h.init_slot);
   } else if constexpr (OPT == kAdagrad) {
     a.fill(h.init_slot);
   } else if constexpr (OPT == kAdam) {
@@ -817,10 +849,47 @@ __device__ __forceinline__ void opt_fresh(const OptHyper& h, FVec<VF>& a, FVec<V
 //   FTRL    : lr, eps = l1, beta1 = 2*l2, beta2 = 2*l2_shrinkage, init_slot = initial accumulator
 //   RMSprop : lr, eps = epsilon, beta1 = rho, beta2 = momentum, init_slot = initial rms, flags = kEpsInSqrt | kCentered
 //   Adadelta: lr, eps = epsilon, beta1 = rho
-// r = 1 - beta1 (RMSprop and Adadelta), computed once per step in fp32.
+//   Adamax  : lr = -lr / (1 - beta1^t), eps = epsilon, beta1, beta2
+//   Nadam   : lr = -lr, eps = epsilon, beta1, beta2; the StepArg x: omsn, omsx, omt, mt1, vden (host.h StepScalars)
+//   ProximalAdagrad : lr, eps = l1, beta1 = l2, init_slot = initial accumulator
+//   ProximalGD      : lr, eps = l1, beta1 = l2
+//   AdagradDA: lr, eps = l1*gs, beta1 = (l2*gs)*lr, init_slot = initial squared accumulator (gs >= 1, so eps > 0
+//              exactly when l1 > 0)
+// r = 1 - beta1 (RMSprop, Adadelta, Adamax, Nadam) and r2 = 1 - beta2 (Nadam), computed once per step in fp32.
+// Adamax and Nadam restate Keras' _resource_apply_sparse; ProximalAdagrad, ProximalGradientDescent and AdagradDA TF1's
+// SparseApplyProximalAdagrad, SparseApplyProximalGradientDescent and SparseApplyAdagradDA (ProximalAdagrad with a
+// correctly rounded square root and one division where TF multiplies by an Eigen rsqrt, DESIGN.md section 4).
 template <int OPT>
-__device__ __forceinline__ void opt_elem(const OptHyper& h, float r, float g, float& p, float& a, float& b, float& c3) {
-  if (OPT >= kRmsprop1 && OPT <= kRmsprop3) {
+__device__ __forceinline__ void opt_elem(const OptHyper& h, const StepArg<OPT>& x, float r, float r2, float g, float& p,
+                                         float& a, float& b, float& c3) {
+  if constexpr (OPT == kNadam) {
+    // a = m, b = v
+    const float gp = g / x.omsn;
+    a = a * h.beta1 + g * r;
+    const float mp = a / x.omsx;
+    const float mbar = x.omt * gp + x.mt1 * mp;
+    b = b * h.beta2 + (g * g) * r2;
+    const float vp = b / x.vden;
+    p = p + (h.lr * mbar) / (sqrtf(vp) + h.eps);
+  } else if (OPT == kAdamax) {
+    // a = m, b = v
+    a = a * h.beta1 + g * r;
+    b = fmaxf(b * h.beta2, fabsf(g));
+    p = p + h.lr * (a / (b + h.eps));
+  } else if (OPT == kProxAdagrad) {
+    // a = accumulator
+    a = a + g * g;
+    const float eta = h.lr / sqrtf(a);
+    p = prox_step(p - g * eta, eta, h.eps, h.beta1);
+  } else if (OPT == kProxSgd) {
+    p = prox_step(p - g * h.lr, h.lr, h.eps, h.beta1);
+  } else if (OPT == kAdagradDa) {
+    // a = gradient_accumulator, b = gradient_squared_accumulator
+    a = a + g;
+    b = b + g * g;
+    const float num = h.eps > 0.f ? -shrink(a, h.eps) : -a;
+    p = (num / (h.beta1 + sqrtf(b))) * h.lr;
+  } else if (OPT >= kRmsprop1 && OPT <= kRmsprop3) {
     // a = rms; kRmsprop2: b = mg (centered) or momentum; kRmsprop3: b = mg, c3 = momentum
     const bool centered = OPT == kRmsprop3 || (OPT == kRmsprop2 && (h.flags & kCentered));
     const bool mom = OPT == kRmsprop3 || (OPT == kRmsprop2 && !(h.flags & kCentered));
@@ -864,8 +933,8 @@ __device__ __forceinline__ void opt_elem(const OptHyper& h, float r, float g, fl
   }
 }
 template <int OPT, int VF>
-__device__ __forceinline__ void opt_step(const OptHyper& h, const FVec<VF>& g, FVec<VF>& p, FVec<VF>& a, FVec<VF>& b,
-                                         FVec<VF>& c) {
+__device__ __forceinline__ void opt_step(const OptHyper& h, const StepArg<OPT>& x, const FVec<VF>& g, FVec<VF>& p,
+                                         FVec<VF>& a, FVec<VF>& b, FVec<VF>& c) {
   if constexpr (OPT == kAdagrad) {
     // accum += g*g ; var -= lr*g / (sqrt(accum) + eps)
     a.zip(g, [](float& av, float gv) { av = av + gv * gv; });
@@ -887,8 +956,9 @@ __device__ __forceinline__ void opt_step(const OptHyper& h, const FVec<VF>& g, F
     float* bv = reinterpret_cast<float*>(&b.v);
     float* cv = reinterpret_cast<float*>(&c.v);
     const float r = 1.f - h.beta1;
+    const float r2 = 1.f - h.beta2;
 #pragma unroll
-    for (int e = 0; e < VF; ++e) opt_elem<OPT>(h, r, gv[e], pv[e], av[e], bv[e], cv[e]);
+    for (int e = 0; e < VF; ++e) opt_elem<OPT>(h, x, r, r2, gv[e], pv[e], av[e], bv[e], cv[e]);
   }
 }
 
@@ -919,8 +989,13 @@ static SlotPlanes<OPT> slot_planes_arg(const det_table* t) {
 // FTRL's two square roots and three divisions per element: left to its own heuristics ptxas spills the probe's
 // first-bucket loads to reach 4 CTAs per SM; asking for 3 (the register-held Adagrad / Adam kernels' occupancy) keeps
 // them in registers.  RMSprop spills the same way: its 1-plane kernel keeps 3 CTAs per SM, the 3-plane one (three slot
-// vectors in flight) 2.  0 = no minimum, the other optimizers' kernels as before.
-template <int OPT> constexpr int kApplyMinBlocks = OPT == kFtrl || OPT == kRmsprop1 ? 3 : OPT == kRmsprop3 ? 2 : 0;
+// vectors in flight) 2.  ProximalAdagrad and AdagradDA (a root and one or two divisions per element, the proximal
+// branch) spill 16 bytes at ptxas' own choice of 4 CTAs per SM; they keep 3.  0 = no minimum, the other optimizers'
+// kernels as before.
+template <int OPT>
+constexpr int kApplyMinBlocks = OPT == kFtrl || OPT == kRmsprop1 || OPT == kProxAdagrad || OPT == kAdagradDa ? 3
+                                : OPT == kRmsprop3                                                       ? 2
+                                                                                                         : 0;
 
 // KEYED: a new key's param starts from its row of the table's keyed initializer (init_param is NULL).
 // (keyed: 2 CTAs per SM, the register budget the generator's calls need without spilling, as segment_sum_kernel)
@@ -928,7 +1003,8 @@ template <int VF, int OPT, typename T = float, bool KEYED = false>
 __global__ void __launch_bounds__(kThreadsF, KEYED ? 2 : kApplyMinBlocks<OPT>)
 apply_kernel(TableView t, const long long* __restrict__ keys, const float* __restrict__ grads, size_t n,
              OptHyper h, const float* __restrict__ init_param, int full_init, unsigned vpr, unsigned lpr,
-             unsigned lpr_shift, int use_tma, SlotPlanes<OPT> sp, InitArg<KEYED> ki = InitArg<KEYED>()) {
+             unsigned lpr_shift, int use_tma, SlotPlanes<OPT> sp, InitArg<KEYED> ki = InitArg<KEYED>(),
+             StepArg<OPT> x = StepArg<OPT>()) {
   __shared__ __align__(128) long long s_keys[kStages][kTileKeys];
   __shared__ __align__(8) unsigned long long s_bar[kStages];
   __shared__ unsigned s_new, s_used;
@@ -1012,7 +1088,7 @@ apply_kernel(TableView t, const long long* __restrict__ keys, const float* __res
 #pragma unroll
         for (int u = 0; u < RU; ++u) {
           if (!ok[u]) continue;
-          opt_step<OPT>(h, g[u], p[u], a[u], b[u], c3[u]);
+          opt_step<OPT>(h, x, g[u], p[u], a[u], b[u], c3[u]);
           if (opt_slots(OPT) > 0) a[u].store(S1 + ro[u] + o);
           if (opt_slots(OPT) > 1) b[u].store(S2 + ro[u] + o);
           if constexpr (opt_slots(OPT) > 2) c3[u].store((float*)t.planes[3] + ro[u] + o);
@@ -1060,7 +1136,7 @@ __global__ void __launch_bounds__(kThreadsF)
 apply_staged_kernel(TableView t, const long long* __restrict__ keys, const float* __restrict__ grads, size_t n,
                     OptHyper h, const float* __restrict__ init_param, int full_init, unsigned vpr, unsigned lpr,
                     unsigned lpr_shift, int use_tma, ScoreArg<SCORED> sa, const long long* __restrict__ n_dev,
-                    SlotPlanes<OPT> sp, InitArg<KEYED> ki = InitArg<KEYED>()) {
+                    SlotPlanes<OPT> sp, InitArg<KEYED> ki = InitArg<KEYED>(), StepArg<OPT> x = StepArg<OPT>()) {
   if (n_dev) n = (size_t)*n_dev;        // key count produced on the device (det_apply_*_dup); the grid covers the bound
   constexpr int NS = 2 + opt_slots(OPT);  // streams per row: grad, param (, slot1 (, slot2 (, slot3)))
   DET_DYN_SHARED(dyn_smem);
@@ -1176,7 +1252,7 @@ apply_staged_kernel(TableView t, const long long* __restrict__ keys, const float
             if (NS > 3) b2.v = *sm(stage, st, 3);
             if constexpr (NS > 4) c3.v = *sm(stage, st, 4);
           }
-          opt_step<OPT>(h, g, p, a, b2, c3);
+          opt_step<OPT>(h, x, g, p, a, b2, c3);
           if (opt_slots(OPT) > 0) a.store(S1 + ro);
           if (opt_slots(OPT) > 1) b2.store(S2 + ro);
           if constexpr (opt_slots(OPT) > 2) c3.store((float*)t.planes[3] + ro);
@@ -1935,15 +2011,59 @@ static det_status adadelta_hyper(float lr, float rho, float epsilon, OptHyper* h
   return DET_OK;
 }
 
+// Adamax: lr_t = lr / (1 - beta1^t) from the caller; the rule adds -lr_t * (m / (v + eps)) (negation is exact)
+static det_status adamax_hyper(float lr_t, float beta1, float beta2, float epsilon, OptHyper* h, int* opt) {
+  h->lr = -lr_t; h->eps = epsilon; h->beta1 = beta1; h->beta2 = beta2; h->init_slot = 0.f;
+  *opt = kAdamax;
+  return DET_OK;
+}
+
+// Nadam: the step scalars the caller computed as Keras' _prepare_local does (StepScalars)
+static det_status nadam_hyper(float lr, float beta1, float beta2, float epsilon, float omsn, float omsx, float omt,
+                              float mt1, float vden, OptHyper* h, StepScalars* sx, int* opt) {
+  h->lr = -lr; h->eps = epsilon; h->beta1 = beta1; h->beta2 = beta2; h->init_slot = 0.f;
+  sx->omsn = omsn; sx->omsx = omsx; sx->omt = omt; sx->mt1 = mt1; sx->vden = vden;
+  *opt = kNadam;
+  return DET_OK;
+}
+
+// ProximalAdagrad (init_accum >= 0) and ProximalGradientDescent (init_accum unused): lr > 0, l1 >= 0, l2 >= 0 as TF's
+// kernels check them (NaN fails each test)
+static det_status proximal_hyper(const char* who, float lr, float l1, float l2, float init_accum, int adagrad,
+                                 OptHyper* h, int* opt) {
+  if (!(lr > 0.f)) return fail(DET_INVALID_ARGUMENT, std::string(who) + ": lr must be positive");
+  if (!(l1 >= 0.f) || !(l2 >= 0.f) || !(init_accum >= 0.f))
+    return fail(DET_INVALID_ARGUMENT, std::string(who) + ": l1, l2 and the initial accumulator must be >= 0");
+  h->lr = lr; h->eps = l1; h->beta1 = l2; h->beta2 = 0.f; h->init_slot = adagrad ? init_accum : 0.f;
+  *opt = adagrad ? kProxAdagrad : kProxSgd;
+  return DET_OK;
+}
+
+// AdagradDA: gs >= 1 is TF1's step on the worker (its global step + 1); l1*gs and (l2*gs)*lr are computed here once per
+// call, in fp32
+static det_status adagrad_da_hyper(float lr, float l1, float l2, int64_t gs, float init_gg, OptHyper* h, int* opt) {
+  if (!(lr > 0.f)) return fail(DET_INVALID_ARGUMENT, "det_apply_adagrad_da: lr must be positive");
+  if (!(l1 >= 0.f) || !(l2 >= 0.f) || !(init_gg >= 0.f))
+    return fail(DET_INVALID_ARGUMENT, "det_apply_adagrad_da: l1, l2 and the initial squared accumulator must be >= 0");
+  if (gs < 1) return fail(DET_INVALID_ARGUMENT, "det_apply_adagrad_da: global_step must be >= 1");
+  const float g = (float)gs;
+  h->lr = lr; h->eps = l1 * g; h->beta1 = (l2 * g) * lr; h->beta2 = 0.f; h->init_slot = init_gg;
+  *opt = kAdagradDa;
+  return DET_OK;
+}
+
 // det_table::slot_init, the slot values of a key created by insert / accum and never stepped: the initial accumulator
-// of Adagrad and FTRL (FTRL's z: 0), 0 for momentum, RMSprop's initial rms (its mg and momentum: 0), 0 for both Adadelta
-// planes; Adam and plain SGD leave them as they are.  Every optimizer entry point records them before it takes the
-// table lock.
+// of Adagrad, FTRL and ProximalAdagrad (FTRL's z: 0), 0 for momentum, RMSprop's initial rms (its mg and momentum: 0),
+// 0 for both Adadelta, Adamax and Nadam planes, AdagradDA's 0 and initial squared accumulator; Adam, plain SGD and
+// ProximalGradientDescent leave them as they are.  Every optimizer entry point records them before it takes the table
+// lock.
 static void record_slot_init(det_table* t, int opt, const OptHyper& h) {
   if (!t) return;
-  if (opt == kAdagrad || opt == kFtrl || (opt >= kRmsprop1 && opt <= kRmsprop3)) t->slot_init[1] = h.init_slot;
-  if (opt == kMomentum || opt == kAdadelta) t->slot_init[1] = 0.f;
-  if (opt == kFtrl || opt == kRmsprop2 || opt == kAdadelta) t->slot_init[2] = 0.f;
+  if (opt == kAdagrad || opt == kFtrl || (opt >= kRmsprop1 && opt <= kRmsprop3) || opt == kProxAdagrad)
+    t->slot_init[1] = h.init_slot;
+  if (opt == kMomentum || opt == kAdadelta || opt == kAdamax || opt == kNadam || opt == kAdagradDa) t->slot_init[1] = 0.f;
+  if (opt == kFtrl || opt == kRmsprop2 || opt == kAdadelta || opt == kAdamax || opt == kNadam) t->slot_init[2] = 0.f;
+  if (opt == kAdagradDa) t->slot_init[2] = h.init_slot;
   if (opt == kRmsprop3) t->slot_init[2] = t->slot_init[3] = 0.f;
 }
 
@@ -2103,9 +2223,10 @@ det_status det_lookup_sparse_clip(det_table* t, const int64_t* ids, const int32_
 
 // n_dev (nullable): the key count lives on the device (det_apply_*_dup); n is then its upper bound -- room is reserved
 // for n NEW keys (the unique keys themselves are not read by the host path) and only the staged kernels support it
+// sx: the step scalars beyond h (Nadam; ignored by the other optimizers)
 static det_status apply_common(det_table* t, const int64_t* keys, const float* grads, size_t n, OptHyper h,
                                const float* init_param, int full_init, int opt, cudaStream_t s,
-                               const long long* n_dev = nullptr) {
+                               const long long* n_dev = nullptr, const StepScalars& sx = StepScalars()) {
   if (!t) return fail(DET_INVALID_ARGUMENT, "det_apply: null table");
   det::MutLock _lk(t);
   const int vt = t->cfg.value_dtype;
@@ -2151,7 +2272,8 @@ static det_status apply_common(det_table* t, const int64_t* keys, const float* g
             int occ = 1;
             if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, kThreadsF, smem) != cudaSuccess || occ < 1) occ = 1;
             DET_LAUNCH(kern, grid_for(n, kTileKeys, t->sm_count, occ), kThreadsF, smem, s, v, k, grads, n, h, init_param,
-                       full_init, vpr, lpr, sh, tma, sa, n_dev, slot_planes_arg<decltype(OPT)::value>(t), init_arg<kKeyed>(t));
+                       full_init, vpr, lpr, sh, tma, sa, n_dev, slot_planes_arg<decltype(OPT)::value>(t), init_arg<kKeyed>(t),
+                       step_arg<decltype(OPT)::value>(sx));
             return DET_OK;
           });
         });
@@ -2170,7 +2292,8 @@ static det_status apply_common(det_table* t, const int64_t* keys, const float* g
           const auto kern = apply_kernel<decltype(VEC4)::value ? 4 : 1, decltype(OPT)::value, typename decltype(row)::type, kKeyed>;
           const int grid = grid_for(n, kTileKeys, t->sm_count, occupancy_of(kern, kThreadsF));
           DET_LAUNCH(kern, grid, kThreadsF, 0, s, v, k, grads, n, h, init_param, full_init, vpr, lpr, sh,
-                     (((uintptr_t)keys & 15u) == 0) ? 1 : 0, slot_planes_arg<decltype(OPT)::value>(t), init_arg<kKeyed>(t));
+                     (((uintptr_t)keys & 15u) == 0) ? 1 : 0, slot_planes_arg<decltype(OPT)::value>(t), init_arg<kKeyed>(t),
+                     step_arg<decltype(OPT)::value>(sx));
           return DET_OK;
         });
       });
@@ -2235,6 +2358,55 @@ det_status det_apply_adadelta(det_table* t, const int64_t* keys, const float* gr
   OptHyper h;
   int opt;
   if (det_status st = adadelta_hyper(lr, rho, epsilon, &h, &opt)) return st;
+  record_slot_init(t, opt, h);
+  return apply_common(t, keys, grads, n, h, init_param, full_size_init, opt, (cudaStream_t)stream);
+}
+
+det_status det_apply_adamax(det_table* t, const int64_t* keys, const float* grads, size_t n, float lr_t, float beta1,
+                            float beta2, float epsilon, const float* init_param, int full_size_init, det_stream_t stream) {
+  OptHyper h;
+  int opt;
+  if (det_status st = adamax_hyper(lr_t, beta1, beta2, epsilon, &h, &opt)) return st;
+  record_slot_init(t, opt, h);
+  return apply_common(t, keys, grads, n, h, init_param, full_size_init, opt, (cudaStream_t)stream);
+}
+
+det_status det_apply_nadam(det_table* t, const int64_t* keys, const float* grads, size_t n, float lr, float beta1,
+                           float beta2, float epsilon, float omsn, float omsx, float omt, float mt1, float vden,
+                           const float* init_param, int full_size_init, det_stream_t stream) {
+  OptHyper h;
+  StepScalars sx;
+  int opt;
+  if (det_status st = nadam_hyper(lr, beta1, beta2, epsilon, omsn, omsx, omt, mt1, vden, &h, &sx, &opt)) return st;
+  record_slot_init(t, opt, h);
+  return apply_common(t, keys, grads, n, h, init_param, full_size_init, opt, (cudaStream_t)stream, nullptr, sx);
+}
+
+det_status det_apply_proximal_adagrad(det_table* t, const int64_t* keys, const float* grads, size_t n, float lr, float l1,
+                                      float l2, const float* init_param, int full_size_init, float init_accum,
+                                      det_stream_t stream) {
+  OptHyper h;
+  int opt;
+  if (det_status st = proximal_hyper("det_apply_proximal_adagrad", lr, l1, l2, init_accum, 1, &h, &opt)) return st;
+  record_slot_init(t, opt, h);
+  return apply_common(t, keys, grads, n, h, init_param, full_size_init, opt, (cudaStream_t)stream);
+}
+
+det_status det_apply_proximal_sgd(det_table* t, const int64_t* keys, const float* grads, size_t n, float lr, float l1,
+                                  float l2, const float* init_param, int full_size_init, det_stream_t stream) {
+  OptHyper h;
+  int opt;
+  if (det_status st = proximal_hyper("det_apply_proximal_sgd", lr, l1, l2, 0.f, 0, &h, &opt)) return st;
+  record_slot_init(t, opt, h);
+  return apply_common(t, keys, grads, n, h, init_param, full_size_init, opt, (cudaStream_t)stream);
+}
+
+det_status det_apply_adagrad_da(det_table* t, const int64_t* keys, const float* grads, size_t n, float lr, float l1,
+                                float l2, int64_t global_step, const float* init_param, int full_size_init,
+                                float init_gg, det_stream_t stream) {
+  OptHyper h;
+  int opt;
+  if (det_status st = adagrad_da_hyper(lr, l1, l2, global_step, init_gg, &h, &opt)) return st;
   record_slot_init(t, opt, h);
   return apply_common(t, keys, grads, n, h, init_param, full_size_init, opt, (cudaStream_t)stream);
 }
@@ -2536,7 +2708,7 @@ size_t det_apply_sparse_workspace_bytes(size_t nnz, size_t batch, size_t dim) {
 static det_status apply_dup(det_table* t, const int64_t* ids, const float* grads, size_t n, OptHyper h,
                             const float* init_param, int opt, void* workspace, size_t workspace_bytes,
                             int64_t* n_unique_dev_out, cudaStream_t s, const long long* n_items_dev = nullptr,
-                            const SparseSrc* sp = nullptr) {
+                            const SparseSrc* sp = nullptr, const StepScalars& sx = StepScalars()) {
   if (!t) return fail(DET_INVALID_ARGUMENT, "det_apply_dup: null table");
   if (n == 0) return DET_OK;
   if (sp) {
@@ -2570,7 +2742,7 @@ static det_status apply_dup(det_table* t, const int64_t* ids, const float* grads
     st = seg_reduce_run(grads, w.idx, n, n, dim, w.gsum, w.sws, w.sws_bytes, w.cnt, s, n_items_dev);
   }
   if (st != DET_OK) return st;
-  st = apply_common(t, (const int64_t*)w.uniq, w.gsum, n, h, init_param, 0, opt, s, w.cnt);
+  st = apply_common(t, (const int64_t*)w.uniq, w.gsum, n, h, init_param, 0, opt, s, w.cnt, sx);
   if (st != DET_OK) return st;
   if (n_unique_dev_out) CUDA_TRY(cudaMemcpyAsync(n_unique_dev_out, w.cnt, sizeof(int64_t), cudaMemcpyDeviceToDevice, s));
   return DET_OK;
@@ -2633,6 +2805,60 @@ det_status det_apply_adadelta_dup(det_table* t, const int64_t* ids, const float*
   OptHyper h;
   int opt;
   if (det_status st = adadelta_hyper(lr, rho, epsilon, &h, &opt)) return st;
+  record_slot_init(t, opt, h);
+  return apply_dup(t, ids, grads, n, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out, (cudaStream_t)stream);
+}
+
+det_status det_apply_adamax_dup(det_table* t, const int64_t* ids, const float* grads, size_t n, float lr_t, float beta1,
+                                float beta2, float epsilon, const float* init_param, void* workspace,
+                                size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream) {
+  OptHyper h;
+  int opt;
+  if (det_status st = adamax_hyper(lr_t, beta1, beta2, epsilon, &h, &opt)) return st;
+  record_slot_init(t, opt, h);
+  return apply_dup(t, ids, grads, n, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out, (cudaStream_t)stream);
+}
+
+det_status det_apply_nadam_dup(det_table* t, const int64_t* ids, const float* grads, size_t n, float lr, float beta1,
+                               float beta2, float epsilon, float omsn, float omsx, float omt, float mt1, float vden,
+                               const float* init_param, void* workspace, size_t workspace_bytes,
+                               int64_t* n_unique_dev_out, det_stream_t stream) {
+  OptHyper h;
+  StepScalars sx;
+  int opt;
+  if (det_status st = nadam_hyper(lr, beta1, beta2, epsilon, omsn, omsx, omt, mt1, vden, &h, &sx, &opt)) return st;
+  record_slot_init(t, opt, h);
+  return apply_dup(t, ids, grads, n, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out, (cudaStream_t)stream,
+                   nullptr, nullptr, sx);
+}
+
+det_status det_apply_proximal_adagrad_dup(det_table* t, const int64_t* ids, const float* grads, size_t n, float lr,
+                                          float l1, float l2, const float* init_param, float init_accum, void* workspace,
+                                          size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream) {
+  OptHyper h;
+  int opt;
+  if (det_status st = proximal_hyper("det_apply_proximal_adagrad", lr, l1, l2, init_accum, 1, &h, &opt)) return st;
+  record_slot_init(t, opt, h);
+  return apply_dup(t, ids, grads, n, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out, (cudaStream_t)stream);
+}
+
+det_status det_apply_proximal_sgd_dup(det_table* t, const int64_t* ids, const float* grads, size_t n, float lr, float l1,
+                                      float l2, const float* init_param, void* workspace, size_t workspace_bytes,
+                                      int64_t* n_unique_dev_out, det_stream_t stream) {
+  OptHyper h;
+  int opt;
+  if (det_status st = proximal_hyper("det_apply_proximal_sgd", lr, l1, l2, 0.f, 0, &h, &opt)) return st;
+  record_slot_init(t, opt, h);
+  return apply_dup(t, ids, grads, n, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out, (cudaStream_t)stream);
+}
+
+det_status det_apply_adagrad_da_dup(det_table* t, const int64_t* ids, const float* grads, size_t n, float lr, float l1,
+                                    float l2, int64_t global_step, const float* init_param, float init_gg,
+                                    void* workspace, size_t workspace_bytes, int64_t* n_unique_dev_out,
+                                    det_stream_t stream) {
+  OptHyper h;
+  int opt;
+  if (det_status st = adagrad_da_hyper(lr, l1, l2, global_step, init_gg, &h, &opt)) return st;
   record_slot_init(t, opt, h);
   return apply_dup(t, ids, grads, n, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out, (cudaStream_t)stream);
 }
@@ -2716,6 +2942,75 @@ det_status det_apply_adadelta_sparse(det_table* t, const int64_t* ids, const int
                    (cudaStream_t)stream, nullptr, &sp);
 }
 
+det_status det_apply_adamax_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
+                                   size_t nnz, size_t batch, int combiner, const float* gout, float lr_t, float beta1,
+                                   float beta2, float epsilon, const float* init_param, void* workspace,
+                                   size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream) {
+  OptHyper h;
+  int opt;
+  if (det_status st = adamax_hyper(lr_t, beta1, beta2, epsilon, &h, &opt)) return st;
+  record_slot_init(t, opt, h);
+  const SparseSrc sp{segment_ids, weights, batch, combiner};
+  return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
+                   (cudaStream_t)stream, nullptr, &sp);
+}
+
+det_status det_apply_nadam_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
+                                  size_t nnz, size_t batch, int combiner, const float* gout, float lr, float beta1,
+                                  float beta2, float epsilon, float omsn, float omsx, float omt, float mt1, float vden,
+                                  const float* init_param, void* workspace, size_t workspace_bytes,
+                                  int64_t* n_unique_dev_out, det_stream_t stream) {
+  OptHyper h;
+  StepScalars sx;
+  int opt;
+  if (det_status st = nadam_hyper(lr, beta1, beta2, epsilon, omsn, omsx, omt, mt1, vden, &h, &sx, &opt)) return st;
+  record_slot_init(t, opt, h);
+  const SparseSrc sp{segment_ids, weights, batch, combiner};
+  return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
+                   (cudaStream_t)stream, nullptr, &sp, sx);
+}
+
+det_status det_apply_proximal_adagrad_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                             const float* weights, size_t nnz, size_t batch, int combiner,
+                                             const float* gout, float lr, float l1, float l2, const float* init_param,
+                                             float init_accum, void* workspace, size_t workspace_bytes,
+                                             int64_t* n_unique_dev_out, det_stream_t stream) {
+  OptHyper h;
+  int opt;
+  if (det_status st = proximal_hyper("det_apply_proximal_adagrad", lr, l1, l2, init_accum, 1, &h, &opt)) return st;
+  record_slot_init(t, opt, h);
+  const SparseSrc sp{segment_ids, weights, batch, combiner};
+  return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
+                   (cudaStream_t)stream, nullptr, &sp);
+}
+
+det_status det_apply_proximal_sgd_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                         const float* weights, size_t nnz, size_t batch, int combiner, const float* gout,
+                                         float lr, float l1, float l2, const float* init_param, void* workspace,
+                                         size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream) {
+  OptHyper h;
+  int opt;
+  if (det_status st = proximal_hyper("det_apply_proximal_sgd", lr, l1, l2, 0.f, 0, &h, &opt)) return st;
+  record_slot_init(t, opt, h);
+  const SparseSrc sp{segment_ids, weights, batch, combiner};
+  return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
+                   (cudaStream_t)stream, nullptr, &sp);
+}
+
+det_status det_apply_adagrad_da_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                       const float* weights, size_t nnz, size_t batch, int combiner, const float* gout,
+                                       float lr, float l1, float l2, int64_t global_step, const float* init_param,
+                                       float init_gg, void* workspace, size_t workspace_bytes,
+                                       int64_t* n_unique_dev_out, det_stream_t stream) {
+  OptHyper h;
+  int opt;
+  if (det_status st = adagrad_da_hyper(lr, l1, l2, global_step, init_gg, &h, &opt)) return st;
+  record_slot_init(t, opt, h);
+  const SparseSrc sp{segment_ids, weights, batch, combiner};
+  return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
+                   (cudaStream_t)stream, nullptr, &sp);
+}
+
 }  // extern "C"
 
 namespace det {
@@ -2723,11 +3018,12 @@ namespace det {
 // their count lives in *n_items_dev; h and opt come from adagrad_hyper or adam_hyper
 det_status apply_dup_on_device_count(det_table* t, const int64_t* ids, const float* grads, size_t n_bound,
                                      const long long* n_items_dev, const OptHyper& h, int opt, const float* init_param,
-                                     void* workspace, size_t workspace_bytes, cudaStream_t s) {
+                                     void* workspace, size_t workspace_bytes, cudaStream_t s, const StepScalars& sx) {
   record_slot_init(t, opt, h);
   // the owner side does not generate rows: the exchange always passes the initial param row
   if (!init_param) return fail(DET_INVALID_ARGUMENT, "det_peer_xchg_apply: null init_param");
-  return apply_dup(t, ids, grads, n_bound, h, init_param, opt, workspace, workspace_bytes, nullptr, s, n_items_dev);
+  return apply_dup(t, ids, grads, n_bound, h, init_param, opt, workspace, workspace_bytes, nullptr, s, n_items_dev,
+                   nullptr, sx);
 }
 }  // namespace det
 

@@ -278,9 +278,10 @@ void host_pipe_free(det_table* t);
 det_status rehash_to(det_table* t, uint64_t new_nb, cudaStream_t s);
 // fused.cu: the optimizers of the fused find-or-insert step (K7, its template parameter OPT) and their
 // hyper-parameters.  What each OptHyper field holds depends on the optimizer (listed at opt_step); only the builders
-// (adagrad_hyper, adam_hyper, sgd_hyper, ftrl_hyper, rmsprop_hyper, adadelta_hyper) fill them.  RMSprop has one id
-// per slot-plane count (kRmsprop1 .. kRmsprop3): the count is a compile-time property of a K7 instantiation.
-enum : int { kAdagrad, kAdam, kSgd, kMomentum, kFtrl, kRmsprop1, kRmsprop2, kRmsprop3, kAdadelta, kNumOpts };
+// (adagrad_hyper .. adagrad_da_hyper) fill them.  RMSprop has one id per slot-plane count (kRmsprop1 .. kRmsprop3):
+// the count is a compile-time property of a K7 instantiation.
+enum : int { kAdagrad, kAdam, kSgd, kMomentum, kFtrl, kRmsprop1, kRmsprop2, kRmsprop3, kAdadelta, kAdamax, kNadam,
+             kProxAdagrad, kProxSgd, kAdagradDa, kNumOpts };
 // OptHyper::flags (RMSprop only; 0 for the other optimizers)
 enum : unsigned { kEpsInSqrt = 1u, kCentered = 2u };
 struct OptHyper {
@@ -290,13 +291,24 @@ struct OptHyper {
   float init_slot;
   unsigned flags = 0;   // fills what was the struct's tail padding before an 8-byte kernel parameter
 };
+// Per-step scalars that do not fit OptHyper: Nadam's momentum schedule and bias correction (nadam_hyper fills them;
+// zero and unused for every other optimizer).  K7 receives them as a trailing kernel argument that is empty for every
+// other optimizer (StepArg, fused.cu), so OptHyper and the other kernels' parameters stay as they are.
+struct StepScalars {
+  float omsn = 0.f;   // 1 - m_schedule_new
+  float omsx = 0.f;   // 1 - m_schedule_next
+  float omt = 0.f;    // 1 - u_t
+  float mt1 = 0.f;    // u_{t+1}
+  float vden = 0.f;   // 1 - beta2^t
+};
 // validate the hyper-parameters, fill *h and set *opt
 det_status adagrad_hyper(float lr, float epsilon, float init_accum, OptHyper* h, int* opt);
 det_status adam_hyper(float alpha, float beta1, float beta2, float epsilon, OptHyper* h, int* opt);
 // unique -> position-order gradient sum -> fused optimizer step with the id count on the device (sharded.cu)
 det_status apply_dup_on_device_count(det_table* t, const int64_t* ids, const float* grads, size_t n_bound,
                                      const long long* n_items_dev, const OptHyper& h, int opt, const float* init_param,
-                                     void* workspace, size_t workspace_bytes, cudaStream_t s);
+                                     void* workspace, size_t workspace_bytes, cudaStream_t s,
+                                     const StepScalars& sx = StepScalars());
 // evict.cu (all called with t->mu held, except evict_insert which takes it)
 det_status evict_attach(det_table* t, int strategy);
 void evict_free(det_table* t);

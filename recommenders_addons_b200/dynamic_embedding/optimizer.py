@@ -469,6 +469,245 @@ class FusedAdadelta(_FusedBase):
                                                     ws.numel(), None, _stream_ptr(table.device)))
 
 
+class FusedAdamax(_FusedBase):
+  """Adamax on dynamic-embedding rows, with Keras' signature and sparse rule (tf.keras.optimizers.Adamax):
+  m = m*b1 + g*(1-b1); v = max(v*b2, |g|); var -= lr_t * m/(v + eps), lr_t = lr/(1 - b1^t) in float32.
+  torch.optim.Adamax puts eps inside the max, a different rule.  Slots: "m" and "v", both starting at 0."""
+  n_slots = 2
+  opt_name = "Adamax"
+  slot_plane_names = ("m", "v")
+
+  def __init__(self, learning_rate=0.001, beta_1=0.9, beta_2=0.999, epsilon=1e-7):
+    super().__init__()
+    self.learning_rate = float(learning_rate)
+    self.beta_1 = float(beta_1)
+    self.beta_2 = float(beta_2)
+    self.epsilon = float(epsilon)
+
+  def lr_t(self):
+    """lr / (1 - beta_1^t) in float32 at t = iterations (the step being taken)"""
+    f = np.float32
+    b1p = f(np.power(f(self.beta_1), f(self.iterations)))
+    return float(f(f(self.learning_rate) / (f(1) - b1p)))
+
+  def _hyper(self):
+    return (self.lr_t(), self.beta_1, self.beta_2, self.epsilon)
+
+  def _apply_table(self, params, table, keys, grads):
+    n = keys.numel()
+    init, full = _init_rows(params, n, table.device)
+    _lib.check(_lib.lib().det_apply_adamax(table.handle, _ptr(keys), _ptr(grads), n, *self._hyper(), _ptr(init), full,
+                                           _stream_ptr(table.device)))
+
+  def _apply_table_dup(self, table, ids, grads, n, init, ws):
+    _lib.check(_lib.lib().det_apply_adamax_dup(table.handle, _ptr(ids), _ptr(grads), n, *self._hyper(), _ptr(init),
+                                               _ptr(ws), ws.numel(), None, _stream_ptr(table.device)))
+
+  def _apply_table_sparse(self, table, h, gout, init, ws):
+    _lib.check(_lib.lib().det_apply_adamax_sparse(table.handle, _ptr(h.ids), _ptr(h.segment_ids), _ptr(h.weights),
+                                                  h.ids.numel(), h.batch, _lib.COMBINERS[h.combiner], _ptr(gout),
+                                                  *self._hyper(), _ptr(init), _ptr(ws), ws.numel(), None,
+                                                  _stream_ptr(table.device)))
+
+
+def nadam_step_scalars(beta_1, beta_2, t, m_cache):
+  """Keras Nadam's _prepare_local in float32 for step t (>= 1) and the m_cache of the steps before it:
+  returns (omsn, omsx, omt, mt1, vden, m_schedule_new), the scalars det_apply_nadam takes and the next m_cache."""
+  f = np.float32
+  b1, t = f(beta_1), f(t)
+  u_t = f(b1 * (f(1) - f(0.5) * f(np.power(f(0.96), f(f(0.004) * t)))))
+  u_t1 = f(b1 * (f(1) - f(0.5) * f(np.power(f(0.96), f(f(0.004) * f(t + f(1)))))))
+  msn = f(f(m_cache) * u_t)
+  msx = f(msn * u_t1)
+  vden = f(f(1) - f(np.power(f(beta_2), t)))
+  return (float(f(1) - msn), float(f(1) - msx), float(f(1) - u_t), float(u_t1), float(vden), float(msn))
+
+
+class FusedNadam(_FusedBase):
+  """Nadam on dynamic-embedding rows, with Keras' signature and sparse rule (tf.keras.optimizers.Nadam):
+  g' = g/omsn; m = m*b1 + g*(1-b1); m' = m/omsx; mbar = omt*g' + mt1*m'; v = v*b2 + (g*g)*(1-b2);
+  var -= lr*mbar / (sqrt(v/vden) + eps), with the step scalars of `nadam_step_scalars`.  torch.optim.NAdam has the same
+  algebra (through ComposedOptimizer, which rounds differently).  Slots: "m" and "v", both starting at 0.
+
+  `m_cache` (Keras' momentum cache, 1.0 before the first step) advances once per apply_gradients, after the step.
+  Callers that drive apply_sparse_duplicate_indices themselves advance `iterations` before the step and set
+  `m_cache = m_schedule_new()` after it, as apply_gradients does.  A restored run continues bit for bit when
+  `iterations` and `m_cache` are set back."""
+  n_slots = 2
+  opt_name = "Nadam"
+  slot_plane_names = ("m", "v")
+
+  def __init__(self, learning_rate=0.001, beta_1=0.9, beta_2=0.999, epsilon=1e-7):
+    super().__init__()
+    self.learning_rate = float(learning_rate)
+    self.beta_1 = float(beta_1)
+    self.beta_2 = float(beta_2)
+    self.epsilon = float(epsilon)
+    self.m_cache = 1.0
+
+  def m_schedule_new(self):
+    return nadam_step_scalars(self.beta_1, self.beta_2, self.iterations, self.m_cache)[5]
+
+  def apply_gradients(self, grads_and_vars):
+    super().apply_gradients(grads_and_vars)
+    self.m_cache = self.m_schedule_new()
+
+  def _hyper(self):
+    return (self.learning_rate, self.beta_1, self.beta_2, self.epsilon) + \
+        nadam_step_scalars(self.beta_1, self.beta_2, self.iterations, self.m_cache)[:5]
+
+  def _apply_table(self, params, table, keys, grads):
+    n = keys.numel()
+    init, full = _init_rows(params, n, table.device)
+    _lib.check(_lib.lib().det_apply_nadam(table.handle, _ptr(keys), _ptr(grads), n, *self._hyper(), _ptr(init), full,
+                                          _stream_ptr(table.device)))
+
+  def _apply_table_dup(self, table, ids, grads, n, init, ws):
+    _lib.check(_lib.lib().det_apply_nadam_dup(table.handle, _ptr(ids), _ptr(grads), n, *self._hyper(), _ptr(init),
+                                              _ptr(ws), ws.numel(), None, _stream_ptr(table.device)))
+
+  def _apply_table_sparse(self, table, h, gout, init, ws):
+    _lib.check(_lib.lib().det_apply_nadam_sparse(table.handle, _ptr(h.ids), _ptr(h.segment_ids), _ptr(h.weights),
+                                                 h.ids.numel(), h.batch, _lib.COMBINERS[h.combiner], _ptr(gout),
+                                                 *self._hyper(), _ptr(init), _ptr(ws), ws.numel(), None,
+                                                 _stream_ptr(table.device)))
+
+
+def _check_proximal(learning_rate, **nonneg):
+  if not learning_rate > 0:
+    raise ValueError("learning_rate must be positive, got %r" % (learning_rate,))
+  for name, v in nonneg.items():
+    if not v >= 0:
+      raise ValueError("%s must be >= 0, got %r" % (name, v))
+
+
+class FusedProximalAdagrad(_FusedBase):
+  """TF1 ProximalAdagradOptimizer on dynamic-embedding rows (SparseApplyProximalAdagrad): a = a + g*g;
+  eta = lr/sqrt(a); q = var - g*eta; var = l1 > 0 ? sign(q)*max(|q| - eta*l1, 0)/(1 + l2*eta) : q/(1 + l2*eta).
+  Slot: "accumulator", starting at initial_accumulator_value."""
+  n_slots = 1
+  opt_name = "ProximalAdagrad"
+  slot_plane_names = ("accumulator",)
+
+  def __init__(self, learning_rate, initial_accumulator_value=0.1, l1_regularization_strength=0.0,
+               l2_regularization_strength=0.0):
+    super().__init__()
+    _check_proximal(learning_rate, initial_accumulator_value=initial_accumulator_value,
+                    l1_regularization_strength=l1_regularization_strength,
+                    l2_regularization_strength=l2_regularization_strength)
+    self.learning_rate = float(learning_rate)
+    self.initial_accumulator_value = float(initial_accumulator_value)
+    self.l1 = float(l1_regularization_strength)
+    self.l2 = float(l2_regularization_strength)
+
+  def _apply_table(self, params, table, keys, grads):
+    n = keys.numel()
+    init, full = _init_rows(params, n, table.device)
+    _lib.check(_lib.lib().det_apply_proximal_adagrad(table.handle, _ptr(keys), _ptr(grads), n, self.learning_rate,
+                                                     self.l1, self.l2, _ptr(init), full, self.initial_accumulator_value,
+                                                     _stream_ptr(table.device)))
+
+  def _apply_table_dup(self, table, ids, grads, n, init, ws):
+    _lib.check(_lib.lib().det_apply_proximal_adagrad_dup(table.handle, _ptr(ids), _ptr(grads), n, self.learning_rate,
+                                                         self.l1, self.l2, _ptr(init), self.initial_accumulator_value,
+                                                         _ptr(ws), ws.numel(), None, _stream_ptr(table.device)))
+
+  def _apply_table_sparse(self, table, h, gout, init, ws):
+    _lib.check(_lib.lib().det_apply_proximal_adagrad_sparse(table.handle, _ptr(h.ids), _ptr(h.segment_ids),
+                                                            _ptr(h.weights), h.ids.numel(), h.batch,
+                                                            _lib.COMBINERS[h.combiner], _ptr(gout), self.learning_rate,
+                                                            self.l1, self.l2, _ptr(init), self.initial_accumulator_value,
+                                                            _ptr(ws), ws.numel(), None, _stream_ptr(table.device)))
+
+
+class FusedProximalGradientDescent(_FusedBase):
+  """TF1 ProximalGradientDescentOptimizer on dynamic-embedding rows (SparseApplyProximalGradientDescent):
+  q = var - g*lr; var = l1 > 0 ? sign(q)*max(|q| - lr*l1, 0)/(1 + l2*lr) : q/(1 + l2*lr).  No slot; with
+  l1 = l2 = 0 it is FusedSGD bit for bit."""
+  n_slots = 0
+  opt_name = "ProximalGradientDescent"
+  slot_plane_names = ()
+
+  def __init__(self, learning_rate, l1_regularization_strength=0.0, l2_regularization_strength=0.0):
+    super().__init__()
+    _check_proximal(learning_rate, l1_regularization_strength=l1_regularization_strength,
+                    l2_regularization_strength=l2_regularization_strength)
+    self.learning_rate = float(learning_rate)
+    self.l1 = float(l1_regularization_strength)
+    self.l2 = float(l2_regularization_strength)
+
+  def _apply_table(self, params, table, keys, grads):
+    n = keys.numel()
+    init, full = _init_rows(params, n, table.device)
+    _lib.check(_lib.lib().det_apply_proximal_sgd(table.handle, _ptr(keys), _ptr(grads), n, self.learning_rate, self.l1,
+                                                 self.l2, _ptr(init), full, _stream_ptr(table.device)))
+
+  def _apply_table_dup(self, table, ids, grads, n, init, ws):
+    _lib.check(_lib.lib().det_apply_proximal_sgd_dup(table.handle, _ptr(ids), _ptr(grads), n, self.learning_rate,
+                                                     self.l1, self.l2, _ptr(init), _ptr(ws), ws.numel(), None,
+                                                     _stream_ptr(table.device)))
+
+  def _apply_table_sparse(self, table, h, gout, init, ws):
+    _lib.check(_lib.lib().det_apply_proximal_sgd_sparse(table.handle, _ptr(h.ids), _ptr(h.segment_ids), _ptr(h.weights),
+                                                        h.ids.numel(), h.batch, _lib.COMBINERS[h.combiner], _ptr(gout),
+                                                        self.learning_rate, self.l1, self.l2, _ptr(init), _ptr(ws),
+                                                        ws.numel(), None, _stream_ptr(table.device)))
+
+
+class FusedAdagradDA(_FusedBase):
+  """TF1 AdagradDAOptimizer on dynamic-embedding rows (SparseApplyAdagradDA): ga = ga + g; gg = gg + g*g;
+  var = ((l1 > 0 ? -sign(ga)*max(|ga| - l1*gs, 0) : -ga) / ((l2*gs)*lr + sqrt(gg))) * lr, with gs = global_step + 1
+  (TF1's _global_step_on_worker).  `global_step`: an int or a zero-argument callable returning one, read on the host
+  at each step; None uses this optimizer's own step count before the step (`iterations - 1` once apply_gradients has
+  advanced it).  Slots: "gradient_accumulator" (starts at 0) and "gradient_squared_accumulator" (starts at
+  initial_gradient_squared_accumulator_value)."""
+  n_slots = 2
+  opt_name = "AdagradDA"
+  slot_plane_names = ("gradient_accumulator", "gradient_squared_accumulator")
+
+  def __init__(self, learning_rate, global_step=None, initial_gradient_squared_accumulator_value=0.1,
+               l1_regularization_strength=0.0, l2_regularization_strength=0.0):
+    super().__init__()
+    _check_proximal(learning_rate,
+                    initial_gradient_squared_accumulator_value=initial_gradient_squared_accumulator_value,
+                    l1_regularization_strength=l1_regularization_strength,
+                    l2_regularization_strength=l2_regularization_strength)
+    self.learning_rate = float(learning_rate)
+    self.global_step = global_step
+    self.initial_gradient_squared_accumulator_value = float(initial_gradient_squared_accumulator_value)
+    self.l1 = float(l1_regularization_strength)
+    self.l2 = float(l2_regularization_strength)
+
+  def step_on_worker(self):
+    """gs = global_step + 1"""
+    gs = self.global_step
+    if gs is None:
+      return int(self.iterations)
+    return int(gs() if callable(gs) else gs) + 1
+
+  def _hyper(self):
+    return (self.learning_rate, self.l1, self.l2, self.step_on_worker())
+
+  def _apply_table(self, params, table, keys, grads):
+    n = keys.numel()
+    init, full = _init_rows(params, n, table.device)
+    _lib.check(_lib.lib().det_apply_adagrad_da(table.handle, _ptr(keys), _ptr(grads), n, *self._hyper(), _ptr(init), full,
+                                               self.initial_gradient_squared_accumulator_value,
+                                               _stream_ptr(table.device)))
+
+  def _apply_table_dup(self, table, ids, grads, n, init, ws):
+    _lib.check(_lib.lib().det_apply_adagrad_da_dup(table.handle, _ptr(ids), _ptr(grads), n, *self._hyper(), _ptr(init),
+                                                   self.initial_gradient_squared_accumulator_value, _ptr(ws), ws.numel(),
+                                                   None, _stream_ptr(table.device)))
+
+  def _apply_table_sparse(self, table, h, gout, init, ws):
+    _lib.check(_lib.lib().det_apply_adagrad_da_sparse(table.handle, _ptr(h.ids), _ptr(h.segment_ids), _ptr(h.weights),
+                                                      h.ids.numel(), h.batch, _lib.COMBINERS[h.combiner], _ptr(gout),
+                                                      *self._hyper(), _ptr(init),
+                                                      self.initial_gradient_squared_accumulator_value, _ptr(ws),
+                                                      ws.numel(), None, _stream_ptr(table.device)))
+
+
 class ComposedOptimizer(object):
   """ANY torch.optim optimizer on dynamic-embedding rows, the way the reference patches a stock optimizer
   (dynamic_embedding_optimizer.py:137-204 `apply_grad_to_update_var`, :870-958 `create_slots`): per step and per
@@ -477,8 +716,8 @@ class ComposedOptimizer(object):
   write param and slots back (`TrainableWrapper.update_op`, embedding_weights.py:434-444).  Table passes per step:
   (1 + slots) finds + (1 + slots) upserts, all through the validated table kernels; Adagrad / Adam have the fused
   single-kernel path (FusedAdagrad / FusedAdam), which DynamicEmbeddingOptimizer picks by default.  SGD, momentum,
-  FTRL, RMSprop and Adadelta have fused steps too (FusedSGD / FusedFtrl / FusedRMSprop / FusedAdadelta), used when
-  passed explicitly.
+  FTRL, RMSprop, Adadelta, Adamax and Nadam have fused steps too (FusedSGD / FusedFtrl / FusedRMSprop / FusedAdadelta /
+  FusedAdamax / FusedNadam), used when passed explicitly.
 
   A key without slot state starts from the state a fresh torch optimizer gives a new parameter (zeros; Adagrad's
   `sum` from initial_accumulator_value) -- the reference's slot initializers.  State that is not per row (`step`,

@@ -10,9 +10,14 @@ rows.  Timed with CUDA events, in rounds that alternate the dtype order, median 
   * rmsprop (1 slot plane), rmsprop_c (centered), rmsprop_m (momentum 0.9), rmsprop_cm (centered + momentum, 3 slot
     planes), adadelta -- det_apply_rmsprop / det_apply_adadelta on 2^20 unique resident keys of two more variables
     (fp32, bf16) with three slot planes and 2/3 of --resident rows, made after the variables above are released, and the composed torch.optim.RMSprop / Adadelta next to FusedRMSprop /
-    FusedAdadelta on one more fp32 variable of --composed-resident rows.
+    FusedAdadelta on one more fp32 variable of --composed-resident rows;
+  * adamax, nadam, proxada, proxsgd, adagrad_da (the proximal and DA ones with l1, l2 > 0) -- det_apply_* on 2^20 unique
+    resident keys of two more two-plane variables (fp32, bf16), made after the variables above are released; each one's
+    _dup form at the c3 backward shape; and the composed torch.optim.Adamax / NAdam next to FusedAdamax / FusedNadam on
+    one more fp32 variable of --composed-resident rows (torch's Adamax is another rule: eps inside the max).
 Before the timing, the first step of each new optimizer on a sample of its keys (rows written by insert, no slot state
-yet) is checked bit for bit against tests/optimizer_oracle.py (RMSprop and Adadelta: tests/rmsprop_adadelta_oracle.py):
+yet) is checked bit for bit against tests/optimizer_oracle.py (RMSprop and Adadelta: tests/rmsprop_adadelta_oracle.py;
+the last five: tests/adamax_nadam_prox_oracle.py):
 params of both dtypes (bf16: the fp32 result rounded).
 
 Bytes per key are what the unique-key step must move at dim 64: key 8 + probed bucket 64 + fp32 gradient 256 + param
@@ -40,7 +45,8 @@ N_UNIQUE = 1 << 20
 N_DUP = 26 * 65536
 N_SAMPLE = 1 << 16
 SLOTS = {"sgd": 0, "momentum": 1, "ftrl": 2, "adagrad": 1, "adam": 2,
-         "rmsprop": 1, "rmsprop_c": 2, "rmsprop_m": 2, "rmsprop_cm": 3, "adadelta": 2}
+         "rmsprop": 1, "rmsprop_c": 2, "rmsprop_m": 2, "rmsprop_cm": 3, "adadelta": 2,
+         "adamax": 2, "nadam": 2, "proxada": 1, "proxsgd": 0, "adagrad_da": 2}
 RMS = {"rmsprop": (0.0, 0), "rmsprop_c": (0.0, 1), "rmsprop_m": (0.9, 0), "rmsprop_cm": (0.9, 1)}   # momentum, centered
 FTRL = dict(lr=0.05, l1=0.001, l2=0.01, l2_shrinkage=0.0)
 
@@ -204,6 +210,8 @@ def main():
   del vars_, small, comp, fused_small
   torch.cuda.empty_cache()
   res.update(rmsprop_adadelta_arms(args, lib, de, P, dev, gen, dts, fill, timed, mismatches))
+  torch.cuda.empty_cache()
+  res.update(adamax_nadam_prox_arms(args, lib, de, P, dev, gen, dts, fill, timed, mismatches))
   print(json.dumps({"metric": "fused optimizer step ms per call (median of rounds, CUDA events)", "card": info,
                     "resident": R, "dim": DIM, "rounds": args.rounds, "calls": args.calls,
                     "datasheet_hbm_TB_s": DATASHEET_HBM_BPS / 1e12, "oracle_mismatches": mismatches, "shapes": res}))
@@ -281,6 +289,110 @@ def rmsprop_adadelta_arms(args, lib, de, P, dev, gen, dts, fill, timed, mismatch
                 "bytes_per_key": bpk, "GB_s": round(bpk * N_UNIQUE / t / 1e6, 1),
                 "of_datasheet_hbm": round(bpk * N_UNIQUE / (t * 1e-3) / DATASHEET_HBM_BPS, 3)}
     row["ids"] = N_UNIQUE
+    res[shape] = row
+  for o, (comp, _) in pairs.items():
+    res["composed_vs_fused_fp32_" + o] = {"resident": Rc, "keys": N_UNIQUE, "composed_is": type(comp).__name__,
+                                          "composed_ms": round(float(np.median(mc[(o, "composed")])), 4),
+                                          "fused_ms": round(float(np.median(mc[(o, "fused")])), 4)}
+  for v in list(v3.values()) + [small]:   # released before the next arms' variables
+    for t in v.tables:
+      t.close()
+  return res
+
+
+def adamax_nadam_prox_arms(args, lib, de, P, dev, gen, dts, fill, timed, mismatches):
+  """Adamax, Nadam, ProximalAdagrad, ProximalGradientDescent and AdagradDA on their own two-plane variables: the
+  unique-key step, the _dup step at the c3 shape, and the composed torch Adamax / NAdam next to the fused ones"""
+  from oracle import oracle as O
+  from recommenders_addons_b200 import _lib
+  from tests import adamax_nadam_prox_oracle as PO
+  R = max(args.resident, 11 * N_UNIQUE)
+  v2 = {n: de.Variable(value_dtype=dt, dim=DIM, init_size=2 * R, initializer=0.0, name="fob5_" + n, num_slot_planes=2)
+        for n, dt in dts.items()}
+  fill(list(v2.values()), R)
+  part = R // 11
+  shapes = ("adamax", "nadam", "proxada", "proxsgd", "adagrad_da")
+  keys = {o: mix_keys(i * part + torch.randperm(part, device=dev, generator=gen)[:N_UNIQUE]) for i, o in enumerate(shapes)}
+  zipf = np.random.default_rng(5).zipf(1.2, N_DUP) - 1
+  ids_dup = {o: mix_keys((5 + i) * part + torch.as_tensor(zipf % part, device=dev)) for i, o in enumerate(shapes)}
+  g_uni = torch.randn(N_UNIQUE, DIM, device=dev, generator=gen) * 0.01
+  g_dup = torch.randn(N_DUP, DIM, device=dev, generator=gen) * 0.01
+  init = torch.zeros(DIM, device=dev)
+  wsb = int(lib.det_apply_dup_workspace_bytes(N_DUP, DIM))
+  ws = torch.empty(wsb + 256, dtype=torch.uint8, device=dev)
+  ws = ws[(-ws.data_ptr()) % 256:][:wsb]
+  nadam = de.FusedNadam(0.001)
+  nadam.iterations = 1
+  adamax = de.FusedAdamax(0.002)
+  adamax.iterations = 1
+  # the scalars after the gradients, the slot-init tail after init_param, and the restatement of a first step
+  hyper = {"adamax": (adamax._hyper(), ()), "nadam": (nadam._hyper(), ()), "proxada": ((0.05, 0.001, 0.01), (0.1,)),
+           "proxsgd": ((0.05, 0.001, 0.01), ()), "adagrad_da": ((0.05, 0.001, 0.01, 3), (0.1,))}
+  cname = {"adamax": "adamax", "nadam": "nadam", "proxada": "proximal_adagrad", "proxsgd": "proximal_sgd",
+           "adagrad_da": "adagrad_da"}
+  inits = {"adamax": [0.0, 0.0], "nadam": [0.0, 0.0], "proxada": [0.1], "proxsgd": [], "adagrad_da": [0.0, 0.1]}
+
+  def step(name, shape, k=None, g=None, n=N_UNIQUE, dup=False):
+    h = v2[name].tables[0].handle
+    args_, tail = hyper[shape]
+    if dup:
+      st = getattr(lib, "det_apply_%s_dup" % cname[shape])(h, P(ids_dup[shape]), P(g_dup), N_DUP, *args_, P(init), *tail,
+                                                           P(ws), wsb, None, None)
+    else:
+      k = keys[shape] if k is None else k
+      g = g_uni if g is None else g
+      st = getattr(lib, "det_apply_" + cname[shape])(h, P(k), P(g), n, *args_, P(init), 0, *tail, None)
+    _lib.check(st)
+
+  for shape in shapes:
+    k = keys[shape][:N_SAMPLE].contiguous()
+    g = g_uni[:N_SAMPLE].contiguous()
+    bad = 0
+    for name, dt in dts.items():
+      p0 = v2[name].lookup(k).float().cpu().numpy()
+      step(name, shape, k, g, N_SAMPLE)
+      got = v2[name].lookup(k).float().cpu().numpy()
+      pt = O.PortTable(DIM)
+      kn = k.cpu().numpy()
+      pt.insert(kn, p0)
+      exp = PO.sparse_step(cname[shape], pt, [O.PortTable(DIM) for _ in inits[shape]], kn, g.cpu().numpy(), init.cpu().numpy(),
+                           inits[shape], *hyper[shape][0])
+      exp = torch.from_numpy(exp).to(dt).float().numpy()
+      bad += int((got.view(np.uint32) != exp.view(np.uint32)).sum())
+    mismatches[shape] = bad
+
+  Rc = args.composed_resident
+  small = de.Variable(dim=DIM, init_size=2 * Rc, initializer=0.0, name="fob5_small", num_slot_planes=2)
+  fill([small], Rc)
+  keys_small = mix_keys(torch.randperm(Rc, device=dev, generator=gen)[:N_UNIQUE])
+  dummy = [torch.nn.Parameter(torch.zeros(1))]
+  fa, fn = de.FusedAdamax(0.002), de.FusedNadam(0.001)
+  fa.iterations = fn.iterations = 1
+  pairs = {"adamax": (de.DynamicEmbeddingOptimizer(torch.optim.Adamax(dummy, lr=0.002, eps=1e-7)), fa),
+           "nadam": (de.DynamicEmbeddingOptimizer(torch.optim.NAdam(dummy, lr=0.001, eps=1e-7)), fn)}
+  dup_shapes = tuple(s + "_dup" for s in shapes)
+  ms = {(n, s): [] for n in dts for s in shapes + dup_shapes}
+  mc = {(o, kind): [] for o in pairs for kind in ("composed", "fused")}
+  for r in range(args.rounds):
+    order = list(dts) if r % 2 == 0 else list(reversed(list(dts)))
+    for shape in shapes:
+      for n in order:
+        ms[(n, shape)].append(timed(lambda: step(n, shape), args.calls))
+        ms[(n, shape + "_dup")].append(timed(lambda: step(n, shape, dup=True), args.calls))
+    for o, (comp, fused) in pairs.items():
+      mc[(o, "composed")].append(timed(lambda: comp.apply_sparse(small, keys_small, g_uni), max(2, args.calls // 2)))
+      mc[(o, "fused")].append(timed(lambda: fused.apply_sparse(small, keys_small, g_uni), args.calls))
+  res = {}
+  for shape in shapes + dup_shapes:
+    row = {}
+    for n, dt in dts.items():
+      t = float(np.median(ms[(n, shape)]))
+      row[n] = {"ms": round(t, 4), "ms_spread": [round(min(ms[(n, shape)]), 4), round(max(ms[(n, shape)]), 4)]}
+      if not shape.endswith("_dup"):
+        bpk = bytes_per_key(shape, torch.empty(0, dtype=dt).element_size())
+        row[n].update({"bytes_per_key": bpk, "GB_s": round(bpk * N_UNIQUE / t / 1e6, 1),
+                       "of_datasheet_hbm": round(bpk * N_UNIQUE / (t * 1e-3) / DATASHEET_HBM_BPS, 3)})
+    row["ids"] = N_DUP if shape.endswith("_dup") else N_UNIQUE
     res[shape] = row
   for o, (comp, _) in pairs.items():
     res["composed_vs_fused_fp32_" + o] = {"resident": Rc, "keys": N_UNIQUE, "composed_is": type(comp).__name__,
