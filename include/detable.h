@@ -83,12 +83,15 @@ typedef struct det_config {
   int32_t dim;              /* value_shape[0] */
   int32_t device;           /* CUDA device ordinal */
   int32_t num_slot_planes;  /* 0..3 optimizer slot planes co-indexed with the value rows: fp32 rows of 4 * dim bytes
-                             * beside DET_FLOAT32, DET_FLOAT16 or DET_BFLOAT16 value rows (other dtypes: 0 only) */
+                             * beside DET_FLOAT32, DET_FLOAT16 or DET_BFLOAT16 value rows (other dtypes: 0 only); with
+                             * DET_FLAGS_SLOTS_IN_VALUE_DTYPE on a DET_FLOAT16 / DET_BFLOAT16 table, rows of that dtype
+                             * (2 * dim bytes) */
   uint64_t init_capacity;   /* keys; 0 -> 8192 (TF_HASHTABLE_INIT_SIZE default, cuckoo_hashtable_op.cc:199-205) */
   uint64_t max_capacity;    /* SLOTS (HKV's max_capacity); 0 -> grow without bound (cuckoo semantics); else the table
                              * holds at most max_load_factor * max_capacity keys and answers DET_TABLE_FULL beyond */
   float max_load_factor;    /* 0 -> 0.75 (0.875 with an eviction strategy) */
-  uint32_t flags;           /* bits 0..3: eviction strategy + 1 (DET_FLAGS_EVICT), 0 = none; other bits reserved, 0 */
+  uint32_t flags;           /* bits 0..3: eviction strategy + 1 (DET_FLAGS_EVICT), 0 = none; bit 4:
+                             * DET_FLAGS_SLOTS_IN_VALUE_DTYPE; other bits reserved, 0 */
   uint64_t max_hbm_for_vectors; /* ABI >= 3.  Bytes of HBM the VALUE rows may take (attr `max_hbm_for_vectors`,
                              * ops/hkv_hashtable_ops.cc:318-331 -> HashTableOptions, lookup_table_op_hkv.h:443-448);
                              * 0 = all rows in HBM.  Rows beyond the budget live in pinned HOST memory that the
@@ -113,6 +116,17 @@ enum {
   DET_EVICT_CUSTOMIZED = 4
 };
 #define DET_FLAGS_EVICT(strategy) ((uint32_t)((strategy) + 1) & 0xFu)
+
+/* Optimizer slot planes in the table's own value dtype (the layout of the reference, whose slot Variables take the
+ * param's value_dtype, python/ops/dynamic_embedding_optimizer.py:889-901).  On a DET_FLOAT16 / DET_BFLOAT16 table every
+ * slot plane holds rows of that dtype, 2 * dim bytes; on a DET_FLOAT32 table the flag changes nothing.  The fused step
+ * widens each slot element to fp32 (exact), runs the fp32 rule, and rounds every slot value it writes to nearest even
+ * into the dtype once, at its store, as it does the param; the new param comes from the unrounded fp32 slot values.  A
+ * slot without state (a key the step creates, or one written by insert / accum and never stepped) starts from its
+ * initial value rounded into the dtype.  fp32 planes stay the default: a half accumulator loses small updates (an fp16
+ * Adagrad accumulator drops g*g below |g| ~ 1.7e-4, DESIGN.md section 4).  det_table_create_in_region and the
+ * det_peer_* groups refuse a table with the flag (DET_UNIMPLEMENTED).  Additive to ABI 8. */
+#define DET_FLAGS_SLOTS_IN_VALUE_DTYPE (1u << 4)
 
 /* ---- lifetime: HashTableOp::Compute / LookupOrCreate, kernels/cuckoo_hashtable_op.h:59-110 ---- */
 det_status det_table_create(det_table** out, const det_config* cfg);
@@ -184,7 +198,9 @@ det_status det_reserve(det_table* t, uint64_t total_keys, det_stream_t stream);
 /* ExportValues (cuckoo_hashtable_op.cc:293-308): writes up to max_n (key,row) pairs in table order,
  * *n_out_host = number written (HOST).  plane = 0 value rows, 1..num_slot_planes an optimizer slot
  * plane (the reference keeps each slot in its own table `<var>/<opt>/<slot>`,
- * python/ops/dynamic_embedding_optimizer.py:870-958).  Synchronises `stream`. */
+ * python/ops/dynamic_embedding_optimizer.py:870-958) in the plane's dtype (fp32, or the table's dtype with
+ * DET_FLAGS_SLOTS_IN_VALUE_DTYPE); a slot row that was never stepped reads as the slot's initial value (rounded into the
+ * plane's dtype).  Synchronises `stream`. */
 det_status det_export(det_table* t, int plane, int64_t* keys_out, void* values_out, size_t max_n,
                       int64_t* n_out_host, det_stream_t stream);
 
@@ -286,8 +302,9 @@ det_status det_lookup_sparse_clip(det_table* t, const int64_t* ids, const int32_
  *   alpha = lr*sqrt(1-b2^t)/(1-b1^t) computed by the caller;  plane 1 = m, plane 2 = v.
  * Tables of DET_FLOAT32, DET_FLOAT16 and DET_BFLOAT16 values (other dtypes: DET_UNIMPLEMENTED).  On a half table the
  * stored param is widened to fp32 (exact), stepped by the fp32 rule above, and rounded to nearest even into the table's
- * dtype once (overflow to +-inf, subnormals kept, NaN stays NaN); the slot planes stay fp32.  grads and init_param are
- * fp32 whatever the table's dtype (a half initializer row widened to fp32 is exact). */
+ * dtype once (overflow to +-inf, subnormals kept, NaN stays NaN); the slot planes stay fp32, or are rounded the same way
+ * into the table's dtype with DET_FLAGS_SLOTS_IN_VALUE_DTYPE.  grads and init_param are fp32 whatever the table's dtype
+ * (a half initializer row widened to fp32 is exact). */
 det_status det_apply_adagrad(det_table* t, const int64_t* keys, const float* grads, size_t n,
                              float lr, float epsilon, const float* init_param, int full_size_init,
                              float init_accum, det_stream_t stream);
@@ -616,10 +633,15 @@ det_status det_load(det_table* t, const char* prefix, size_t buffer_keys, int cl
 /* Checkpointing the state of the FUSED optimizers.  The reference keeps every optimizer slot in its own table
  * `<var>/<opt>/<slot>` (python/ops/dynamic_embedding_optimizer.py:870-958), saved and restored like any variable;
  * here the slots are planes of the variable's own table, so they travel as one more raw file pair per plane:
- *   det_save_plane  = det_save of plane 1..num_slot_planes (fp32 rows; never-stepped keys carry the slot initializer),
+ *   det_save_plane  = det_save of plane 1..num_slot_planes (rows in the plane's dtype: fp32, or the table's fp16 / bf16
+ *                     with DET_FLAGS_SLOTS_IN_VALUE_DTYPE -- the reference's slot files of a half variable; never-stepped
+ *                     keys carry the slot initializer),
  *   det_load_plane  = the pair read back into the plane for the keys that are IN the table (restore the value plane
- *                     first); keys of the file that are not in the table are skipped,
- *   det_import_plane = the same from device buffers (keys int64 [n], rows fp32 [n, dim]), asynchronous on `stream`.
+ *                     first); keys of the file that are not in the table are skipped.  The `-values` file of an fp16 /
+ *                     bf16 plane must hold exactly n * dim * 2 bytes for the n keys of `-keys` (an fp32 file is refused
+ *                     with DET_IO_ERROR, not misread),
+ *   det_import_plane = the same from device buffers (keys int64 [n], rows fp32 [n, dim]), asynchronous on `stream`; rows
+ *                     are rounded to nearest even into an fp16 / bf16 plane (exact for rows widened from that dtype).
  * ABI >= 4. */
 det_status det_import_plane(det_table* t, int plane, const int64_t* keys, const float* rows, size_t n,
                             det_stream_t stream);
@@ -632,7 +654,7 @@ typedef struct det_stats {
   int64_t used_slots;  /* non-empty slots (live + tombstones) */
   uint64_t capacity;   /* slots */
   uint64_t buckets;
-  uint64_t hbm_bytes;  /* device bytes held by the table */
+  uint64_t hbm_bytes;  /* device bytes held by the table (slot planes at their element size) */
   uint32_t error_flags;
   uint32_t rehash_count;
   uint32_t evict_events;  /* eviction events so far (ABI >= 2) */

@@ -127,6 +127,10 @@ class DetHashTableOfTensorsGpu final : public LookupInterface {
     cfg.max_capacity = static_cast<uint64_t>(max_capacity);
     cfg.max_load_factor = 0.f;
     cfg.flags = DET_FLAGS_EVICT(strategy);
+    // TFRA_DET_SLOT_DTYPE=value: the slot planes of half and bfloat16 tables hold their own dtype, the reference's slot
+    // layout (its slot Variables take the param's value_dtype); the default keeps them fp32
+    const char* slot_dtype = std::getenv("TFRA_DET_SLOT_DTYPE");
+    if (slot_dtype && std::string(slot_dtype) == "value") cfg.flags |= DET_FLAGS_SLOTS_IN_VALUE_DTYPE;
     cfg.max_hbm_for_vectors = static_cast<uint64_t>(max_hbm_for_vectors);
     OP_REQUIRES_OK(ctx, ToStatus(det_table_create(&table_, &cfg)));
   }

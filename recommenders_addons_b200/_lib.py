@@ -17,6 +17,10 @@ COMBINERS = {"sum": 0, "mean": 1, "sqrtn": 2}
 EVICT_STRATEGIES = {"LRU": 0, "LFU": 1, "EPOCHLRU": 2, "EPOCHLFU": 3, "CUSTOMIZED": 4}
 
 
+# det_config.flags bit 4: optimizer slot planes in the table's fp16 / bf16 value dtype (fp32 planes otherwise)
+FLAGS_SLOTS_IN_VALUE_DTYPE = 1 << 4
+
+
 def flags_evict(strategy):
   return (int(strategy) + 1) & 0xF
 

@@ -5,7 +5,8 @@
 //   keys   : int64 [nb*8]            8-slot buckets = 64 B = two 32 B sectors, one DRAM burst
 //   values : V     [(nb*8+2)][dim]   row s belongs to slot s; 2 trailing rows serve the two key
 //                                    values that double as in-table sentinels (EMPTY/TOMB)
-//   slots_k: float [(nb*8+2)][dim]   optional optimizer planes (accumulator / m / v)
+//   slots_k: float [(nb*8+2)][dim]   optional optimizer planes (accumulator / m / v); V instead of float with
+//                                    DET_FLAGS_SLOTS_IN_VALUE_DTYPE on an fp16 / bf16 table
 // Probing: bucket b0 = mulhi64(fmix64(key), nb), linear over buckets.  A 4-lane subgroup owns one
 // key: each lane loads 16 B (2 keys) of the 64 B bucket, matches are found with __ballot_sync.
 //
@@ -16,6 +17,7 @@
 #include <cuda_runtime.h>
 #endif
 #include <stdint.h>
+#include <string.h>
 
 #include "../../include/detable.h"  // DET_EVICT_* (score rules)
 
@@ -29,6 +31,73 @@ constexpr int kMaxPlanes = 4;  // plane 0 = values, 1..3 = optimizer slots
 // first word of an optimizer-slot row whose key was created by insert/accum and never stepped (a quiet NaN
 // payload no optimizer produces): the fused optimizer treats such a row as "slot absent -> initializer"
 constexpr unsigned kSlotUninit = 0x7fc0de7au;
+// The same marker in the first element of a slot row that holds the table's fp16 / bf16 dtype
+// (DET_FLAGS_SLOTS_IN_VALUE_DTYPE): a 16-bit pattern that is a quiet NaN in both formats (so it fits dim 1) and that no
+// narrowing produces -- the device's fp16 and bf16 conversions give the canonical 0x7fff for every NaN (the SIMT
+// emulator's fp16 conversion 0x7e00 / 0xfe00), so a slot that a NaN gradient turned into NaN stays NaN.
+constexpr unsigned kSlotUninit16 = 0x7fdau;
+
+// Write the marker into the slot row `slot` of one slot plane with `esize`-byte elements (4: fp32, 2: fp16 / bf16).
+__device__ __forceinline__ void mark_slot_row(unsigned char* plane, size_t slot, unsigned dim, unsigned esize) {
+  unsigned char* p = plane + slot * dim * esize;
+  if (esize == 2) *reinterpret_cast<unsigned short*>(p) = (unsigned short)kSlotUninit16;
+  else *reinterpret_cast<unsigned*>(p) = kSlotUninit;
+}
+
+// fp32 -> fp16 (bf16 = false) or bf16 bits, rounded to nearest even, overflow to +-inf, subnormals kept, every NaN the
+// canonical 0x7fff (what the device's cvt.rn.f16.f32 / cvt.rn.bf16.f32 give).  Integer arithmetic only: the host side
+// (slot initial values, det_import_plane) and the emulator get the device's rounding.
+__host__ __device__ __forceinline__ unsigned short f32_to_half_bits(float f, bool bf16) {
+  unsigned x;
+  memcpy(&x, &f, 4);
+  const unsigned s = (x >> 16) & 0x8000u, a = x & 0x7fffffffu;
+  if (a > 0x7f800000u) return 0x7fffu;
+  if (bf16) return (unsigned short)((x + 0x7fffu + ((x >> 16) & 1u)) >> 16);
+  if (a >= 0x477ff000u) return (unsigned short)(s | 0x7c00u);   // |f| >= 65520 rounds to inf
+  unsigned r, rem, half;
+  if (a < 0x38800000u) {                                         // below 2^-14: an fp16 subnormal or zero
+    const unsigned e = a >> 23;
+    if (e < 102u) return (unsigned short)s;                      // below 2^-25: rounds to zero
+    const unsigned m = (a & 0x7fffffu) | 0x800000u, sh = 126u - e;
+    r = m >> sh;
+    rem = m & ((1u << sh) - 1u);
+    half = 1u << (sh - 1u);
+  } else {
+    r = (a >> 13) - (112u << 10);
+    rem = a & 0x1fffu;
+    half = 0x1000u;
+  }
+  if (rem > half || (rem == half && (r & 1u))) ++r;
+  return (unsigned short)(s | r);
+}
+// and back (exact)
+__host__ __device__ __forceinline__ float half_bits_to_f32(unsigned short h, bool bf16) {
+  unsigned x;
+  if (bf16) {
+    x = (unsigned)h << 16;
+  } else {
+    const unsigned s = (unsigned)(h & 0x8000u) << 16, e = (h >> 10) & 0x1fu, m = h & 0x3ffu;
+    if (e == 31u) {
+      x = s | 0x7f800000u | (m << 13);
+    } else if (e == 0u) {
+      if (m == 0u) {
+        x = s;
+      } else {                                                   // subnormal: normalise
+        unsigned ee = 113u, mm = m;
+        while (!(mm & 0x400u)) {
+          mm <<= 1;
+          --ee;
+        }
+        x = s | (ee << 23) | ((mm & 0x3ffu) << 13);
+      }
+    } else {
+      x = s | ((e + 112u) << 23) | (m << 13);
+    }
+  }
+  float f;
+  memcpy(&f, &x, 4);
+  return f;
+}
 
 enum : unsigned { kErrTableFull = 1u, kErrBadSegment = 2u };
 

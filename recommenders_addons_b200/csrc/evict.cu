@@ -145,14 +145,24 @@ static det_status repair_rounds(det_table* t, cudaStream_t s) {
   EvictState* ev = t->ev;
   const TableView v = t->view;
   const size_t cap = v.capacity();
-  const RowGeom gs = make_geom((unsigned)t->cfg.dim * 4u, 4);
+  const bool half_slots = t->slot_esize == 2;
+  const RowGeom gs = make_geom((unsigned)slot_row_bytes(t), 4);   // fp32 slot rows move as 4-byte vectors
   const int np = t->cfg.num_slot_planes;
   const int rgrid = grid_for(cap, kThreadsE, t->sm_count, 8);
   for (int round = 0; round < 256; ++round) {
     CUDA_TRY(cudaMemsetAsync(&ev->dev->n_moved, 0, 2 * sizeof(unsigned long long), s));  // n_moved, n_erased
     dispatch_vec(t->row_bytes, {}, [&](auto V, const RowGeom& g) -> det_status {
-      DET_LAUNCH(repair_move_kernel<decltype(V)::value>, rgrid, kThreadsE, 0, s, v, ev->scores, g, gs, np, ev->dev);
-      return DET_OK;
+      constexpr int VV = decltype(V)::value;
+      if (!half_slots) {
+        DET_LAUNCH(repair_move_kernel<VV>, rgrid, kThreadsE, 0, s, v, ev->scores, g, gs, np, ev->dev);
+        return DET_OK;
+      }
+      // half slot rows (2 * dim bytes) at the widest vector width their size allows, as the value rows
+      return dispatch_vec<2>(slot_row_bytes(t), {}, [&](auto SV, const RowGeom& gsv) -> det_status {
+        const auto kern = repair_move_kernel<VV, decltype(SV)::value>;
+        DET_LAUNCH(kern, rgrid, kThreadsE, 0, s, v, ev->scores, g, gsv, np, ev->dev);
+        return DET_OK;
+      });
     });
     DET_LAUNCH(repair_sweep_kernel, rgrid, kThreadsE, 0, s, v, ev->scores, ev->dev);
     CUDA_TRY(cudaGetLastError());
@@ -322,7 +332,8 @@ det_status evict_insert(det_table* t, const int64_t* keys, const void* values, c
     st = dispatch_vec(t->row_bytes, {{vals, "det_insert: values"}}, [&](auto V, const RowGeom& g) -> det_status {
       constexpr int VV = decltype(V)::value;
       const int grid = grid_for(m, kThreadsE, t->sm_count, occupancy_of(insert_scored_kernel<VV>, kThreadsE));
-      DET_LAUNCH(insert_scored_kernel<VV>, grid, kThreadsE, 0, s, v, k, vals, sc_in, mask, m, g, np, ev->scores, rule);
+      DET_LAUNCH(insert_scored_kernel<VV>, grid, kThreadsE, 0, s, v, k, vals, sc_in, mask, m, g, np, ev->scores, rule,
+                 t->slot_esize);
       CUDA_TRY(cudaGetLastError());
       return DET_OK;
     });

@@ -48,7 +48,8 @@ template <int VEC>
 __global__ void __launch_bounds__(kThreadsE)
 insert_scored_kernel(TableView t, const long long* __restrict__ keys, const unsigned char* __restrict__ values,
                      const unsigned long long* __restrict__ scores_in, const unsigned char* __restrict__ may_claim,
-                     size_t n, RowGeom g, int n_slot_planes, unsigned long long* __restrict__ sc, ScoreRule rule) {
+                     size_t n, RowGeom g, int n_slot_planes, unsigned long long* __restrict__ sc, ScoreRule rule,
+                     unsigned slot_esize = 4u) {
   __shared__ unsigned s_new, s_used;
   if (threadIdx.x == 0) {
     s_new = 0;
@@ -78,8 +79,7 @@ insert_scored_kernel(TableView t, const long long* __restrict__ keys, const unsi
     }
     warp_move_rows<VEC>(g, src, dst, lane);
     if (is_new && slot >= 0)
-      for (int p = 1; p <= n_slot_planes; ++p)
-        *reinterpret_cast<unsigned*>(t.planes[p] + (size_t)slot * t.dim * 4u) = kSlotUninit;
+      for (int p = 1; p <= n_slot_planes; ++p) mark_slot_row(t.planes[p], (size_t)slot, t.dim, slot_esize);
     if (valid && slot >= 0) {
       const unsigned long long old = is_new ? 0ull : sc[slot];
       sc[slot] = rule_score(rule, old, scores_in != nullptr, scores_in ? scores_in[i] : 0ull, now_ns());
@@ -303,7 +303,8 @@ evict_apply_kernel(TableView t, unsigned long long* __restrict__ sc, EvictDev* d
 //                        goes back to EMPTY (score 0).  EMPTY slots only appear here; a probe cut short by one of
 //                        them reports "no earlier copy" and the stale copy survives until the next round.
 // Freed slots may cut chains further on: the host repeats rounds until one moves nothing and erases nothing.
-template <int VEC>
+// Slot rows move as SVEC-byte vectors (gslot): 4 for fp32 planes; the widest width 2 * dim allows for fp16 / bf16 ones.
+template <int VEC, int SVEC = 4>
 __global__ void __launch_bounds__(kThreadsE)
 repair_move_kernel(TableView t, unsigned long long* __restrict__ sc, RowGeom g, RowGeom gslot, int n_planes,
                    EvictDev* d) {
@@ -346,7 +347,7 @@ repair_move_kernel(TableView t, unsigned long long* __restrict__ sc, RowGeom g, 
     warp_move_rows<VEC>(g, ok ? t.planes[0] + s * g.row_bytes : nullptr,
                         ok ? t.planes[0] + (size_t)ns * g.row_bytes : nullptr, lane);
     for (int p = 1; p <= n_planes; ++p)
-      warp_move_rows<4>(gslot, ok ? t.planes[p] + s * gslot.row_bytes : nullptr,
+      warp_move_rows<SVEC>(gslot, ok ? t.planes[p] + s * gslot.row_bytes : nullptr,
                         ok ? t.planes[p] + (size_t)ns * gslot.row_bytes : nullptr, lane);
     if (ok) sc[ns] = sc[s];
     const unsigned bm = __ballot_sync(kFull, ok), bu = __ballot_sync(kFull, ok && from_empty);

@@ -509,6 +509,15 @@ template <> struct FVec<1> {
   template <typename F> __device__ __forceinline__ void zip(const FVec& o, F f) { f(v, o.v); }
 };
 
+// Slot-plane storage S of the fused optimizer step: float, or the table's __half / __nv_bfloat16 with
+// DET_FLAGS_SLOTS_IN_VALUE_DTYPE (FVec loads widen it, stores round it to nearest even, as for the param).
+// slot_bits: the bits of a slot row's element 0, compared with the "no slot state" marker kSlotMark<S>.
+__device__ __forceinline__ unsigned slot_bits(const float* p) { return __float_as_uint(*p); }
+template <typename H> __device__ __forceinline__ unsigned slot_bits(const H* p) {
+  return *reinterpret_cast<const unsigned short*>(p);
+}
+template <typename S> constexpr unsigned kSlotMark = std::is_same<S, float>::value ? kSlotUninit : kSlotUninit16;
+
 // The row vector segment_sum_kernel holds while its loads are in flight.  An fp32 lane holds the row (or the default
 // row, kept in registers) itself.  A half lane holds the raw 16-bit elements, half the registers, widens them when they
 // are added, and reads the default row from L1 when an id is missing: widening early or keeping the fp32 default row
@@ -968,12 +977,17 @@ __device__ __forceinline__ void opt_step(const OptHyper& h, const StepArg<OPT>& 
 template <int OPT> struct SlotPlanes { int n; };
 template <> struct SlotPlanes<kAdagrad> {};
 template <> struct SlotPlanes<kAdam> {};
-template <int OPT>
+template <int OPT, typename S = float>
 __device__ __forceinline__ void mark_unwritten(const TableView& t, const SlotPlanes<OPT>& sp, long long slot) {
   // unrolled: a plane index known at compile time keeps the TableView parameter out of local memory
 #pragma unroll
-  for (int p = 1 + opt_slots(OPT); p < kMaxPlanes; ++p)
-    if (p <= sp.n) *reinterpret_cast<unsigned*>(t.planes[p] + (size_t)slot * t.dim * 4u) = kSlotUninit;
+  for (int p = 1 + opt_slots(OPT); p < kMaxPlanes; ++p) {
+    if constexpr (std::is_same<S, float>::value) {
+      if (p <= sp.n) *reinterpret_cast<unsigned*>(t.planes[p] + (size_t)slot * t.dim * 4u) = kSlotUninit;
+    } else {
+      if (p <= sp.n) *reinterpret_cast<unsigned short*>(t.planes[p] + (size_t)slot * t.dim * 2u) = (unsigned short)kSlotUninit16;
+    }
+  }
 }
 template <int OPT>
 static SlotPlanes<OPT> slot_planes_arg(const det_table* t) {
@@ -982,10 +996,11 @@ static SlotPlanes<OPT> slot_planes_arg(const det_table* t) {
   return sp;
 }
 
-// T: the table's param row storage type (float, __half or __nv_bfloat16).  Slot planes are fp32 whatever T is, and the
-// lane geometry is that of the fp32 gradient row: a half lane reads and writes 8 B of param row where an fp32 lane
-// moves 16 B.  A half param is widened after its load (exact), stepped in fp32, and rounded to nearest even into T
-// once, at its store.
+// T: the table's param row storage type (float, __half or __nv_bfloat16).  S: the slot planes' storage type, float or
+// (DET_FLAGS_SLOTS_IN_VALUE_DTYPE) T.  The lane geometry is that of the fp32 gradient row: a half lane reads and writes
+// 8 B of param (or slot) row where an fp32 lane moves 16 B.  A half param or slot element is widened after its load
+// (exact), stepped in fp32, and rounded to nearest even into its type once, at its store; the param is computed from
+// the unrounded fp32 slot values.
 // FTRL's two square roots and three divisions per element: left to its own heuristics ptxas spills the probe's
 // first-bucket loads to reach 4 CTAs per SM; asking for 3 (the register-held Adagrad / Adam kernels' occupancy) keeps
 // them in registers.  RMSprop spills the same way: its 1-plane kernel keeps 3 CTAs per SM, the 3-plane one (three slot
@@ -997,9 +1012,13 @@ constexpr int kApplyMinBlocks = OPT == kFtrl || OPT == kRmsprop1 || OPT == kProx
                                 : OPT == kRmsprop3                                                       ? 2
                                                                                                          : 0;
 
+// S of a launch: the table's row type T when its slot planes hold that dtype (HALF_SLOTS), else float
+template <typename T, bool HALF_SLOTS>
+using SlotT = std::conditional_t<HALF_SLOTS && !std::is_same<T, float>::value, T, float>;
+
 // KEYED: a new key's param starts from its row of the table's keyed initializer (init_param is NULL).
 // (keyed: 2 CTAs per SM, the register budget the generator's calls need without spilling, as segment_sum_kernel)
-template <int VF, int OPT, typename T = float, bool KEYED = false>
+template <int VF, int OPT, typename T = float, bool KEYED = false, typename S = float>
 __global__ void __launch_bounds__(kThreadsF, KEYED ? 2 : kApplyMinBlocks<OPT>)
 apply_kernel(TableView t, const long long* __restrict__ keys, const float* __restrict__ grads, size_t n,
              OptHyper h, const float* __restrict__ init_param, int full_init, unsigned vpr, unsigned lpr,
@@ -1019,8 +1038,8 @@ apply_kernel(TableView t, const long long* __restrict__ keys, const float* __res
   const unsigned sub = (unsigned)lane >> lpr_shift;
   const unsigned c0 = (unsigned)lane & (lpr - 1u);
   T* P = (T*)t.planes[0];
-  float* S1 = (float*)t.planes[1];
-  float* S2 = (float*)t.planes[2];
+  S* S1 = (S*)t.planes[1];
+  S* S2 = (S*)t.planes[2];
   KeyTiles kt;
   kt.init(s_keys, s_bar, keys, n, use_tma != 0);
   for (; kt.valid(); kt.next()) {
@@ -1055,14 +1074,14 @@ apply_kernel(TableView t, const long long* __restrict__ keys, const float* __res
         ro[u] = ok[u] ? (size_t)s * dim : 0;
         // slot state absent: key created in this launch, or created by insert/accum and never stepped.
         // Every lane reads the marker word BEFORE any lane of the row's group overwrites it.
-        mark[u] = ok[u] && opt_slots(OPT) > 0 ? __float_as_uint(S1[ro[u]]) : 0u;
+        mark[u] = ok[u] && opt_slots(OPT) > 0 ? slot_bits(S1 + ro[u]) : 0u;
         if constexpr (OPT >= kSgd) {
-          if (ok[u] && nwv[u] && c0 == 0) mark_unwritten(t, sp, s);
+          if (ok[u] && nwv[u] && c0 == 0) mark_unwritten<OPT, S>(t, sp, s);
         }
       }
       __syncwarp();
 #pragma unroll
-      for (int u = 0; u < RU; ++u) fresh[u] = nwv[u] || (mark[u] == kSlotUninit);
+      for (int u = 0; u < RU; ++u) fresh[u] = nwv[u] || (mark[u] == kSlotMark<S>);
       for (unsigned c = c0; c < vpr; c += lpr) {
         const size_t o = (size_t)c * VF;
         FVec<VF> g[RU], p[RU], a[RU], b[RU], c3[RU];
@@ -1082,7 +1101,7 @@ apply_kernel(TableView t, const long long* __restrict__ keys, const float* __res
           } else {
             if (opt_slots(OPT) > 0) a[u].load(S1 + ro[u] + o);
             if (opt_slots(OPT) > 1) b[u].load(S2 + ro[u] + o);
-            if constexpr (opt_slots(OPT) > 2) c3[u].load((const float*)t.planes[3] + ro[u] + o);
+            if constexpr (opt_slots(OPT) > 2) c3[u].load((const S*)t.planes[3] + ro[u] + o);
           }
         }
 #pragma unroll
@@ -1091,7 +1110,7 @@ apply_kernel(TableView t, const long long* __restrict__ keys, const float* __res
           opt_step<OPT>(h, x, g[u], p[u], a[u], b[u], c3[u]);
           if (opt_slots(OPT) > 0) a[u].store(S1 + ro[u] + o);
           if (opt_slots(OPT) > 1) b[u].store(S2 + ro[u] + o);
-          if constexpr (opt_slots(OPT) > 2) c3[u].store((float*)t.planes[3] + ro[u] + o);
+          if constexpr (opt_slots(OPT) > 2) c3[u].store((S*)t.planes[3] + ro[u] + o);
           p[u].store(P + ro[u] + o);
         }
       }
@@ -1127,11 +1146,13 @@ __device__ __forceinline__ void score_touch<true>(const ScoreArg<true>& sa, long
   if (valid && slot >= 0) sa.sc[slot] = rule_score(sa.rule, is_new ? 0ull : sa.sc[slot], false, 0ull, now_ns());
 }
 
-// T: the param row storage type, as in apply_kernel.  An existing key's half param vector is one 8 B cp.async into the
-// first half of its 16 B stage slot; a new key's is the 16 B fp32 init_param vector, as on an fp32 table.
+// T: the param row storage type, S the slot planes' storage type, as in apply_kernel.  An existing key's half param
+// vector is one 8 B cp.async into the first half of its 16 B stage slot; a new key's is the 16 B fp32 init_param vector,
+// as on an fp32 table.  A half slot vector is staged the same way (8 B into its 16 B stage slot, element 0 where the
+// marker test reads it) and widened by FVec::load.
 // KEYED: a new key's param vector is generated in registers from the table's keyed initializer instead of copied from
 // init_param (NULL); the key travels with the slot through the row-step shuffles.
-template <int OPT, bool SCORED = false, typename T = float, bool KEYED = false>
+template <int OPT, bool SCORED = false, typename T = float, bool KEYED = false, typename S = float>
 __global__ void __launch_bounds__(kThreadsF)
 apply_staged_kernel(TableView t, const long long* __restrict__ keys, const float* __restrict__ grads, size_t n,
                     OptHyper h, const float* __restrict__ init_param, int full_init, unsigned vpr, unsigned lpr,
@@ -1155,8 +1176,8 @@ apply_staged_kernel(TableView t, const long long* __restrict__ keys, const float
   const unsigned c0 = (unsigned)lane & (lpr - 1u);
   const bool lane_on = c0 < vpr;
   T* P = (T*)t.planes[0];
-  float* S1 = (float*)t.planes[1];
-  float* S2 = (float*)t.planes[2];
+  S* S1 = (S*)t.planes[1];
+  S* S2 = (S*)t.planes[2];
   // per warp: 2 stages x kStageSteps steps x NS streams x 32 lanes x 16 B
   float4* wbuf = reinterpret_cast<float4*>(dyn_smem) + (size_t)warp * (2 * kStageSteps * NS * 32);
   auto sm = [&](int stage, int step, int stream) -> float4* { return wbuf + ((stage * kStageSteps + step) * NS + stream) * 32 + lane; };
@@ -1203,9 +1224,15 @@ apply_staged_kernel(TableView t, const long long* __restrict__ keys, const float
               cp_async8(sm(stage, st, 1), P + ro);
           }
           if (!nw && NS > 2) {
-            cp_async16(sm(stage, st, 2), S1 + ro);
-            if (NS > 3) cp_async16(sm(stage, st, 3), S2 + ro);
-            if constexpr (NS > 4) cp_async16(sm(stage, st, 4), (const float*)t.planes[3] + ro);
+            if constexpr (std::is_same<S, float>::value) {
+              cp_async16(sm(stage, st, 2), S1 + ro);
+              if (NS > 3) cp_async16(sm(stage, st, 3), S2 + ro);
+              if constexpr (NS > 4) cp_async16(sm(stage, st, 4), (const float*)t.planes[3] + ro);
+            } else {
+              cp_async8(sm(stage, st, 2), S1 + ro);
+              if (NS > 3) cp_async8(sm(stage, st, 3), S2 + ro);
+              if constexpr (NS > 4) cp_async8(sm(stage, st, 4), (const S*)t.planes[3] + ro);
+            }
           }
         }
       }
@@ -1231,7 +1258,8 @@ apply_staged_kernel(TableView t, const long long* __restrict__ keys, const float
         const size_t gi = base + (j & 31u);
         const bool row_ok = step < steps_total && gi < n && sl >= 0;
         // slot state absent: key created in this launch, or created by insert/accum and never stepped
-        const bool fresh = nw || (NS > 2 && row_ok && __float_as_uint(*sm_mark(stage, st)) == kSlotUninit);
+        const bool fresh =
+            nw || (NS > 2 && row_ok && slot_bits(reinterpret_cast<const S*>(sm_mark(stage, st))) == kSlotMark<S>);
         if (row_ok && lane_on) {
           const size_t ro = (size_t)sl * dim + (size_t)c0 * 4;
           FVec<4> g, p, a, b2, c3;
@@ -1247,18 +1275,22 @@ apply_staged_kernel(TableView t, const long long* __restrict__ keys, const float
           }
           if (fresh) {
             opt_fresh<OPT>(h, a, b2, c3);
-          } else {
+          } else if constexpr (std::is_same<S, float>::value) {
             if (NS > 2) a.v = *sm(stage, st, 2);
             if (NS > 3) b2.v = *sm(stage, st, 3);
             if constexpr (NS > 4) c3.v = *sm(stage, st, 4);
+          } else {
+            if (NS > 2) a.load(reinterpret_cast<const S*>(sm(stage, st, 2)));
+            if (NS > 3) b2.load(reinterpret_cast<const S*>(sm(stage, st, 3)));
+            if constexpr (NS > 4) c3.load(reinterpret_cast<const S*>(sm(stage, st, 4)));
           }
           opt_step<OPT>(h, x, g, p, a, b2, c3);
           if (opt_slots(OPT) > 0) a.store(S1 + ro);
           if (opt_slots(OPT) > 1) b2.store(S2 + ro);
-          if constexpr (opt_slots(OPT) > 2) c3.store((float*)t.planes[3] + ro);
+          if constexpr (opt_slots(OPT) > 2) c3.store((S*)t.planes[3] + ro);
           p.store(P + ro);
           if constexpr (OPT >= kSgd) {
-            if (nw && c0 == 0) mark_unwritten(t, sp, sl);
+            if (nw && c0 == 0) mark_unwritten<OPT, S>(t, sp, sl);
           }
         }
       }
@@ -2252,29 +2284,35 @@ static det_status apply_common(det_table* t, const int64_t* keys, const float* g
   if (st != DET_OK) return st;
   const TableView v = t->view;
   const long long* k = (const long long*)keys;
+  // slot planes in the table's half dtype: a slot without state starts from its initial value rounded into that dtype
+  const bool half_slots = t->slot_esize == 2;
+  if (half_slots) h.init_slot = half_bits_to_f32(f32_to_half_bits(h.init_slot, vt == DET_BFLOAT16), vt == DET_BFLOAT16);
   if (vec4 && vpr <= lpr) {
     // cp.async-staged variant: 2 stages x kStageSteps x streams x 512 B per warp of dynamic shared memory
     const int ns = 2 + opt_slots(opt);
     const size_t smem = (size_t)(kThreadsF / 32) * 2 * kStageSteps * ns * 32 * 16;
     const int tma = (((uintptr_t)keys & 15u) == 0) ? 1 : 0;
     st = dispatch_row_type(vt, [&](auto row) -> det_status {
-      return dispatch_bit(t->ev != nullptr, [&](auto SCORED) -> det_status {
-        return dispatch_bit(keyed, [&](auto KEYED) -> det_status {
-          return dispatch_int<kNumOpts>(opt, [&](auto OPT) -> det_status {
-            constexpr bool kScored = decltype(SCORED)::value, kKeyed = decltype(KEYED)::value;
-            ScoreArg<kScored> sa;
-            if constexpr (kScored) {
-              sa.sc = evict_scores(t);
-              sa.rule = evict_rule(t);
-            }
-            const auto kern = apply_staged_kernel<decltype(OPT)::value, kScored, typename decltype(row)::type, kKeyed>;
-            CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            int occ = 1;
-            if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, kThreadsF, smem) != cudaSuccess || occ < 1) occ = 1;
-            DET_LAUNCH(kern, grid_for(n, kTileKeys, t->sm_count, occ), kThreadsF, smem, s, v, k, grads, n, h, init_param,
-                       full_init, vpr, lpr, sh, tma, sa, n_dev, slot_planes_arg<decltype(OPT)::value>(t), init_arg<kKeyed>(t),
-                       step_arg<decltype(OPT)::value>(sx));
-            return DET_OK;
+      return dispatch_bit(half_slots, [&](auto HS) -> det_status {
+        using S = SlotT<typename decltype(row)::type, decltype(HS)::value>;
+        return dispatch_bit(t->ev != nullptr, [&](auto SCORED) -> det_status {
+          return dispatch_bit(keyed, [&](auto KEYED) -> det_status {
+            return dispatch_int<kNumOpts>(opt, [&](auto OPT) -> det_status {
+              constexpr bool kScored = decltype(SCORED)::value, kKeyed = decltype(KEYED)::value;
+              ScoreArg<kScored> sa;
+              if constexpr (kScored) {
+                sa.sc = evict_scores(t);
+                sa.rule = evict_rule(t);
+              }
+              const auto kern = apply_staged_kernel<decltype(OPT)::value, kScored, typename decltype(row)::type, kKeyed, S>;
+              CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+              int occ = 1;
+              if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, kThreadsF, smem) != cudaSuccess || occ < 1) occ = 1;
+              DET_LAUNCH(kern, grid_for(n, kTileKeys, t->sm_count, occ), kThreadsF, smem, s, v, k, grads, n, h, init_param,
+                         full_init, vpr, lpr, sh, tma, sa, n_dev, slot_planes_arg<decltype(OPT)::value>(t), init_arg<kKeyed>(t),
+                         step_arg<decltype(OPT)::value>(sx));
+              return DET_OK;
+            });
           });
         });
       });
@@ -2285,16 +2323,19 @@ static det_status apply_common(det_table* t, const int64_t* keys, const float* g
     return DET_OK;   // scores of a table with an eviction strategy were written by the kernel itself
   }
   dispatch_row_type(vt, [&](auto row) -> det_status {
-    return dispatch_int<kNumOpts>(opt, [&](auto OPT) -> det_status {
-      return dispatch_bit(vec4, [&](auto VEC4) -> det_status {
-        return dispatch_bit(keyed, [&](auto KEYED) -> det_status {
-          constexpr bool kKeyed = decltype(KEYED)::value;
-          const auto kern = apply_kernel<decltype(VEC4)::value ? 4 : 1, decltype(OPT)::value, typename decltype(row)::type, kKeyed>;
-          const int grid = grid_for(n, kTileKeys, t->sm_count, occupancy_of(kern, kThreadsF));
-          DET_LAUNCH(kern, grid, kThreadsF, 0, s, v, k, grads, n, h, init_param, full_init, vpr, lpr, sh,
-                     (((uintptr_t)keys & 15u) == 0) ? 1 : 0, slot_planes_arg<decltype(OPT)::value>(t), init_arg<kKeyed>(t),
-                     step_arg<decltype(OPT)::value>(sx));
-          return DET_OK;
+    return dispatch_bit(half_slots, [&](auto HS) -> det_status {
+      using S = SlotT<typename decltype(row)::type, decltype(HS)::value>;
+      return dispatch_int<kNumOpts>(opt, [&](auto OPT) -> det_status {
+        return dispatch_bit(vec4, [&](auto VEC4) -> det_status {
+          return dispatch_bit(keyed, [&](auto KEYED) -> det_status {
+            constexpr bool kKeyed = decltype(KEYED)::value;
+            const auto kern = apply_kernel<decltype(VEC4)::value ? 4 : 1, decltype(OPT)::value, typename decltype(row)::type, kKeyed, S>;
+            const int grid = grid_for(n, kTileKeys, t->sm_count, occupancy_of(kern, kThreadsF));
+            DET_LAUNCH(kern, grid, kThreadsF, 0, s, v, k, grads, n, h, init_param, full_init, vpr, lpr, sh,
+                       (((uintptr_t)keys & 15u) == 0) ? 1 : 0, slot_planes_arg<decltype(OPT)::value>(t), init_arg<kKeyed>(t),
+                       step_arg<decltype(OPT)::value>(sx));
+            return DET_OK;
+          });
         });
       });
     });

@@ -205,6 +205,7 @@ struct det_table {
   uint64_t n_since_snap = 0;         // keys of mutating calls issued after the snapshot in flight
   uint32_t rehash_count = 0;
   float slot_init[det::kMaxPlanes];  // value given to slot-plane rows of keys created by insert/accum
+  unsigned slot_esize = 4;           // bytes per slot-plane element: 4 (fp32), 2 (DET_FLAGS_SLOTS_IN_VALUE_DTYPE, half table)
   bool keyed = false;                // det_table_set_initializer: missing rows come from `init` where a NULL row is passed
   det::KeyedInit init{};
   det::HostPipe* pipe = nullptr;   // host-buffer pipeline of det_find_host
@@ -239,6 +240,9 @@ struct det_table {
 };
 
 namespace det {
+// bytes per row of an optimizer slot plane
+inline size_t slot_row_bytes(const det_table* t) { return (size_t)t->cfg.dim * t->slot_esize; }
+
 // Lock of the mutating (and scratch-using) entry points.  Releasing it advances the table generation, which retires
 // every slot hint written before: the bump comes after the call has enqueued its kernels, so a find that read the old
 // generation may have run before them, and one that reads the new one runs after them (same stream).
@@ -276,6 +280,9 @@ det_status table_clear_async(det_table* t, cudaStream_t s);
 det_status table_scratch(det_table* t, size_t bytes, void** out);
 void host_pipe_free(det_table* t);
 det_status rehash_to(det_table* t, uint64_t new_nb, cudaStream_t s);
+// det_import_plane; rows in the plane's own dtype unless `narrow` (fp32 rows, rounded into an fp16 / bf16 plane)
+det_status import_plane_rows(det_table* t, int plane, const int64_t* keys, const void* rows, size_t n, bool narrow,
+                             cudaStream_t s);
 // fused.cu: the optimizers of the fused find-or-insert step (K7, its template parameter OPT) and their
 // hyper-parameters.  What each OptHyper field holds depends on the optimizer (listed at opt_step); only the builders
 // (adagrad_hyper .. adagrad_da_hyper) fill them.  RMSprop has one id per slot-plane count (kRmsprop1 .. kRmsprop3):

@@ -315,7 +315,7 @@ static det_status save_plane(det_table* t, int plane, const char* prefix, size_t
     const size_t want = n > 0 ? (size_t)n : 1;
     if (buffer_keys > want) buffer_keys = want;
   }
-  const size_t rb = plane == 0 ? t->row_bytes : (size_t)t->cfg.dim * 4u;   // slot planes are fp32 rows
+  const size_t rb = plane == 0 ? t->row_bytes : slot_row_bytes(t);   // slot planes: fp32 rows, or the table's half dtype
   long long* dk = nullptr;
   unsigned char* dv = nullptr;
   CUDA_TRY(cudaMalloc((void**)&dk, buffer_keys * 8));
@@ -379,13 +379,26 @@ det_status det_load_plane(det_table* t, int plane, const char* prefix, size_t bu
     if (fv) fclose(fv);
     return fail(DET_IO_ERROR, "det_load_plane: cannot open " + kf + " / " + vf);
   }
-  const size_t rb = (size_t)t->cfg.dim * 4u;
+  const size_t rb = slot_row_bytes(t);
   if (buffer_keys == 0) buffer_keys = 1u << 20;
   if (fseek(fk, 0, SEEK_END) == 0) {
     const long bytes = ftell(fk);
     const size_t n_file = bytes > 0 ? (size_t)bytes / 8 : 0;
     if (buffer_keys > n_file) buffer_keys = n_file ? n_file : 1;
     rewind(fk);
+    // an fp16 / bf16 plane reads rows of its own dtype: a file of any other row size (an fp32 slot file is twice as
+    // long) is refused instead of being misread
+    if (t->slot_esize == 2 && fseek(fv, 0, SEEK_END) == 0) {
+      const long vbytes = ftell(fv);
+      rewind(fv);
+      if (vbytes < 0 || (size_t)vbytes != n_file * rb) {
+        fclose(fk);
+        fclose(fv);
+        return fail(DET_IO_ERROR, "det_load_plane: " + vf + " holds " + std::to_string(vbytes) + " bytes, not the " +
+                                      std::to_string(n_file * rb) + " of " + std::to_string(n_file) + " rows of " +
+                                      std::to_string(t->cfg.dim) + " 2-byte elements");
+      }
+    }
   }
   std::vector<long long> hk(buffer_keys);
   std::vector<unsigned char> hv(buffer_keys * rb);
@@ -409,7 +422,7 @@ det_status det_load_plane(det_table* t, int plane, const char* prefix, size_t bu
       st = fail(DET_CUDA_ERROR, "det_load_plane: H2D copy failed");
       break;
     }
-    st = det_import_plane(t, plane, (const int64_t*)dk, (const float*)dv, m, nullptr);
+    st = import_plane_rows(t, plane, (const int64_t*)dk, dv, m, false, nullptr);
     if (st == DET_OK && cudaStreamSynchronize(nullptr) != cudaSuccess) st = fail(DET_CUDA_ERROR, "det_load_plane: import failed");
   }
   if (dk) cudaFree(dk);

@@ -653,8 +653,16 @@ extern "C" {
 
 size_t det_peer_handle_bytes(void) { return sizeof(PeerBlob); }
 
+// the sharded step runs on fp32 slot planes only: a shard with DET_FLAGS_SLOTS_IN_VALUE_DTYPE joins no group
+static det_status refuse_value_dtype_slots(const det_table* t, const char* who) {
+  if (t && (t->cfg.flags & DET_FLAGS_SLOTS_IN_VALUE_DTYPE))
+    return fail(DET_UNIMPLEMENTED, std::string(who) + ": shards with DET_FLAGS_SLOTS_IN_VALUE_DTYPE are not supported");
+  return DET_OK;
+}
+
 det_status det_peer_export(det_table* t, void* blob_out) {
   if (!t || !blob_out) return fail(DET_INVALID_ARGUMENT, "det_peer_export: null argument");
+  if (det_status st = refuse_value_dtype_slots(t, "det_peer_export")) return st;
   det::DevGuard _dg(t->cfg.device);
   PeerBlob b;
   memset(&b, 0, sizeof(b));
@@ -704,6 +712,8 @@ det_status det_peer_group_create(det_peer_group** out, det_table* const* tables,
     return fail(DET_INVALID_ARGUMENT, "det_peer_group_create: world must be in [1,8] and rank in [0,world)");
   det_table* local = tables[rank];
   if (!local) return fail(DET_INVALID_ARGUMENT, "det_peer_group_create: tables[rank] must be the local shard");
+  for (int p = 0; p < world; ++p)
+    if (det_status st = refuse_value_dtype_slots(tables[p], "det_peer_group_create")) return st;
   det::DevGuard _dg(local->cfg.device);
   det_peer_group* g = new det_peer_group();
   memset(g->opened, 0, sizeof(g->opened));
@@ -791,6 +801,7 @@ det_status det_peer_group_create_regions(det_peer_group** out, det_table* local,
   if (world < 1 || world > kMaxPeers || rank < 0 || rank >= world)
     return fail(DET_INVALID_ARGUMENT, "det_peer_group_create_regions: world must be in [1,8] and rank in [0,world)");
   if (!local->external) return fail(DET_INVALID_ARGUMENT, "det_peer_group_create_regions: the local shard must live in a region");
+  if (det_status st = refuse_value_dtype_slots(local, "det_peer_group_create_regions")) return st;
   det::DevGuard _dg(local->cfg.device);
   det_peer_group* g = new det_peer_group();
   memset(g->opened, 0, sizeof(g->opened));

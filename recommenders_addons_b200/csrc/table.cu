@@ -119,7 +119,8 @@ find_kernel_tma(TableView t, const long long* __restrict__ keys, size_t n,
 
 struct SlotInit {
   float v[kMaxPlanes];
-  int n_planes;  // number of slot planes (excluding values)
+  int n_planes;    // number of slot planes (excluding values)
+  unsigned esize;  // bytes per slot-plane element (det_table::slot_esize)
 };
 
 // K2: Insert (insert_or_assign).  HINTED: the host has checked that no mutation was enqueued since the find that wrote
@@ -157,8 +158,7 @@ __device__ __forceinline__ void insert_step(const TableView& t, long long key, s
   // reference keeps slots in separate tables, where such a key is simply absent and reads the slot
   // initializer at the next optimizer step)
   if (is_new && slot >= 0)
-    for (int p = 1; p <= si.n_planes; ++p)
-      *reinterpret_cast<unsigned*>(t.planes[p] + (size_t)slot * t.dim * 4u) = kSlotUninit;
+    for (int p = 1; p <= si.n_planes; ++p) mark_slot_row(t.planes[p], (size_t)slot, t.dim, si.esize);
 }
 
 // Key tiles as in find_kernel_tma<VEC, TMA>.
@@ -259,8 +259,7 @@ accum_kernel(TableView t, const long long* __restrict__ keys, const T* __restric
       }
     }
     if (is_new && slot >= 0)
-      for (int p = 1; p <= si.n_planes; ++p)
-        *reinterpret_cast<unsigned*>(t.planes[p] + (size_t)slot * dim * 4u) = kSlotUninit;
+      for (int p = 1; p <= si.n_planes; ++p) mark_slot_row(t.planes[p], (size_t)slot, dim, si.esize);
   }
   __syncthreads();
   if (threadIdx.x == 0 && s_new) {
@@ -353,8 +352,7 @@ accum_staged_kernel(TableView t, const long long* __restrict__ keys, const float
       }
     }
     if (is_new && slot >= 0)
-      for (int p = 1; p <= si.n_planes; ++p)
-        *reinterpret_cast<unsigned*>(t.planes[p] + (size_t)slot * dim * 4u) = kSlotUninit;
+      for (int p = 1; p <= si.n_planes; ++p) mark_slot_row(t.planes[p], (size_t)slot, dim, si.esize);
   }
   __syncthreads();
   if (threadIdx.x == 0 && s_new) {
@@ -612,16 +610,26 @@ set_plane_kernel(TableView t, int plane, const long long* __restrict__ keys, con
   }
 }
 
+// fp32 rows rounded to nearest even into an fp16 / bf16 slot plane's elements (det_import_plane)
+__global__ void narrow_rows_kernel(const float* __restrict__ in, unsigned short* __restrict__ out, size_t count, int bf16) {
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < count; i += (size_t)gridDim.x * blockDim.x)
+    out[i] = f32_to_half_bits(in[i], bf16 != 0);
+}
+
 // exported optimizer-slot rows that were never initialised read as the slot initializer value
-__global__ void export_fix_slot_rows_kernel(float* __restrict__ vals, const unsigned long long* __restrict__ n_rows,
-                                            unsigned dim, float init) {
+// (E = float with fp32 planes; unsigned short with fp16 / bf16 planes, `mark` and `init` then their 16-bit patterns)
+template <typename E = float>
+__global__ void export_fix_slot_rows_kernel(E* __restrict__ vals, const unsigned long long* __restrict__ n_rows,
+                                            unsigned dim, E init, unsigned mark = kSlotUninit) {
   const size_t n = (size_t)*n_rows;
   const size_t warp0 = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const size_t nwarps = ((size_t)gridDim.x * blockDim.x) >> 5;
   const int lane = threadIdx.x & 31;
   for (size_t r = warp0; r < n; r += nwarps) {
-    float* row = vals + r * dim;
-    const bool un = __float_as_uint(row[0]) == kSlotUninit;
+    E* row = vals + r * dim;
+    unsigned bits = 0;
+    memcpy(&bits, row, sizeof(E));
+    const bool un = bits == mark;
     __syncwarp();
     if (un)
       for (unsigned c = lane; c < dim; c += 32) row[c] = init;
@@ -629,8 +637,8 @@ __global__ void export_fix_slot_rows_kernel(float* __restrict__ vals, const unsi
   }
 }
 
-// Rehash: move every live slot of `src` into `dst` (fresh, all EMPTY).
-template <int VEC>
+// Rehash: move every live slot of `src` into `dst` (fresh, all EMPTY).  Slot rows move as SVEC-byte vectors (gslot).
+template <int VEC, int SVEC = 4>
 __global__ void __launch_bounds__(kThreads)
 rehash_kernel(TableView src, TableView dst, RowGeom g, RowGeom gslot, int n_planes) {
   const int lane = threadIdx.x & 31;
@@ -648,7 +656,7 @@ rehash_kernel(TableView src, TableView dst, RowGeom g, RowGeom gslot, int n_plan
     warp_move_rows<VEC>(g, ok ? src.planes[0] + s * g.row_bytes : nullptr,
                         ok ? dst.planes[0] + (size_t)ns * g.row_bytes : nullptr, lane);
     for (int p = 1; p <= n_planes; ++p)
-      warp_move_rows<4>(gslot, ok ? src.planes[p] + s * gslot.row_bytes : nullptr,
+      warp_move_rows<SVEC>(gslot, ok ? src.planes[p] + s * gslot.row_bytes : nullptr,
                         ok ? dst.planes[p] + (size_t)ns * gslot.row_bytes : nullptr, lane);
   }
 }
@@ -698,7 +706,7 @@ static det_status alloc_planes(det_table* t, uint64_t nb, TableView* v, void** r
   const size_t cap = nb * kBucket;
   const size_t key_bytes = cap * sizeof(long long);
   const size_t val_bytes = (cap + 2) * t->row_bytes;
-  const size_t slot_bytes = (cap + 2) * (size_t)t->cfg.dim * 4u;
+  const size_t slot_bytes = (cap + 2) * slot_row_bytes(t);
   for (int i = 0; i < 1 + kMaxPlanes; ++i) raw[i] = nullptr;
   cudaError_t e = cudaMalloc(&raw[0], key_bytes);
   if (e == cudaSuccess) e = alloc_value_plane(t, &raw[1], val_bytes);
@@ -729,7 +737,7 @@ static size_t planes_bytes(const det_table* t, uint64_t nb, size_t* host_bytes) 
   const size_t val_bytes = (cap + 2) * t->row_bytes;
   const size_t head = spill_head_bytes(t, val_bytes);
   if (host_bytes) *host_bytes = val_bytes - head;
-  return cap * 8 + head + (size_t)t->cfg.num_slot_planes * (cap + 2) * t->cfg.dim * 4u;
+  return cap * 8 + head + (size_t)t->cfg.num_slot_planes * (cap + 2) * slot_row_bytes(t);
 }
 
 det_status table_clear_async(det_table* t, cudaStream_t s) {
@@ -751,12 +759,22 @@ det_status rehash_to(det_table* t, uint64_t new_nb, cudaStream_t s) {
   const size_t ncap = new_nb * kBucket;
   DET_LAUNCH(fill_keys_kernel, grid_for(ncap, 4096, t->sm_count, 8), 1024, 0, s, nv.keys, ncap, kEmptyKey);
   const TableView ov = t->view;
-  const RowGeom gs = make_geom((unsigned)t->cfg.dim * 4u, 4);
+  const bool half_slots = t->slot_esize == 2;
+  const RowGeom gs = make_geom((unsigned)slot_row_bytes(t), 4);   // fp32 slot rows move as 4-byte vectors
   const int np = t->cfg.num_slot_planes;
   const int grid = grid_for(ov.capacity(), kThreads, t->sm_count, 8);
   dispatch_vec(t->row_bytes, {}, [&](auto V, const RowGeom& g) -> det_status {
-    DET_LAUNCH(rehash_kernel<decltype(V)::value>, grid, kThreads, 0, s, ov, nv, g, gs, np);
-    return DET_OK;
+    constexpr int VV = decltype(V)::value;
+    if (!half_slots) {
+      DET_LAUNCH(rehash_kernel<VV>, grid, kThreads, 0, s, ov, nv, g, gs, np);
+      return DET_OK;
+    }
+    // half slot rows (2 * dim bytes) move at the widest vector width their size allows, as the value rows do
+    return dispatch_vec<2>(slot_row_bytes(t), {}, [&](auto SV, const RowGeom& gsv) -> det_status {
+      const auto kern = rehash_kernel<VV, decltype(SV)::value>;
+      DET_LAUNCH(kern, grid, kThreads, 0, s, ov, nv, g, gsv, np);
+      return DET_OK;
+    });
   });
   // an error from here on must not leak the new planes (the table keeps its old ones and stays usable)
   auto drop_new = [&](det_status code) {
@@ -768,7 +786,7 @@ det_status rehash_to(det_table* t, uint64_t new_nb, cudaStream_t s) {
   };
   // special rows
   for (int p = 0; p <= np; ++p) {
-    const size_t rb = p == 0 ? t->row_bytes : (size_t)t->cfg.dim * 4u;
+    const size_t rb = p == 0 ? t->row_bytes : slot_row_bytes(t);
     const cudaError_t ce = cudaMemcpyAsync(nv.planes[p] + ncap * rb, ov.planes[p] + ov.capacity() * rb, 2 * rb,
                                            cudaMemcpyDeviceToDevice, s);
     if (ce != cudaSuccess) return drop_new(fail(DET_CUDA_ERROR, std::string("rehash: ") + cudaGetErrorString(ce)));
@@ -934,6 +952,7 @@ det_status table_scratch(det_table* t, size_t bytes, void** out) {
 SlotInit slot_init_of(const det_table* t) {
   SlotInit si;
   si.n_planes = t->cfg.num_slot_planes;
+  si.esize = t->slot_esize;
   for (int p = 0; p < kMaxPlanes; ++p) si.v[p] = t->slot_init[p];
   return si;
 }
@@ -1089,10 +1108,15 @@ static det_status create_common(det_table** out, const det_config* cfg, void* re
   if (cfg->dim <= 0) return fail(DET_INVALID_ARGUMENT, "det_table_create: dim must be positive (value_shape must be a vector)");
   if (cfg->num_slot_planes < 0 || cfg->num_slot_planes >= kMaxPlanes)
     return fail(DET_INVALID_ARGUMENT, "det_table_create: num_slot_planes must be in [0,3]");
-  // slot planes are fp32 rows of 4 * dim bytes beside value rows of fp32, fp16 or bf16 (the fused optimizer step)
+  // slot planes are fp32 rows of 4 * dim bytes beside value rows of fp32, fp16 or bf16 (the fused optimizer step), or
+  // rows of the table's fp16 / bf16 dtype with DET_FLAGS_SLOTS_IN_VALUE_DTYPE
   if (cfg->num_slot_planes > 0 && cfg->value_dtype != DET_FLOAT32 && cfg->value_dtype != DET_FLOAT16 &&
       cfg->value_dtype != DET_BFLOAT16)
     return fail(DET_INVALID_ARGUMENT, "det_table_create: optimizer slot planes need float32, float16 or bfloat16 values");
+  // region layouts are shared by peers, whose sharded step runs on fp32 slot planes only
+  if (region != nullptr && (cfg->flags & DET_FLAGS_SLOTS_IN_VALUE_DTYPE))
+    return fail(DET_UNIMPLEMENTED, "det_table_create_in_region: DET_FLAGS_SLOTS_IN_VALUE_DTYPE is not supported for tables "
+                                   "in a region");
   int ndev = 0;
   CUDA_TRY(cudaGetDeviceCount(&ndev));
   if (cfg->device < 0 || cfg->device >= ndev) return fail(DET_INVALID_ARGUMENT, "det_table_create: bad device ordinal");
@@ -1100,6 +1124,9 @@ static det_status create_common(det_table** out, const det_config* cfg, void* re
   det_table* t = new det_table();
   t->cfg = *cfg;
   t->row_bytes = es * (size_t)cfg->dim;
+  if ((cfg->flags & DET_FLAGS_SLOTS_IN_VALUE_DTYPE) &&
+      (cfg->value_dtype == DET_FLOAT16 || cfg->value_dtype == DET_BFLOAT16))
+    t->slot_esize = 2;
   const int evict_strategy = (int)(cfg->flags & 0xFu) - 1;  // DET_FLAGS_EVICT
   t->max_lf = cfg->max_load_factor > 0.f ? cfg->max_load_factor : (evict_strategy >= 0 ? 0.875f : 0.75f);
   if (t->max_lf > 0.9f) t->max_lf = 0.9f;
@@ -1441,16 +1468,21 @@ det_status det_export_window(det_table* t, int plane, uint64_t first, int64_t* k
   const int grid = grid_for(n_tiles, 1, t->sm_count, 8);
   DET_LAUNCH(export_count_kernel, grid, kThreads, 0, s, v, counts, n_tiles);
   DET_LAUNCH(export_scan_kernel, 1, 1024, 0, s, counts, offs, n_tiles, v.st);
-  const unsigned prb = plane == 0 ? (unsigned)t->row_bytes : (unsigned)t->cfg.dim * 4u;
+  const unsigned prb = plane == 0 ? (unsigned)t->row_bytes : (unsigned)slot_row_bytes(t);
   dispatch_vec(prb, {{values_out, "det_export: values"}}, [&](auto V, const RowGeom& g) -> det_status {
     DET_LAUNCH(export_write_kernel<decltype(V)::value>, grid, kThreads, 0, s, 
         v, plane, prb, offs, n_tiles, (long long*)keys_out, (unsigned char*)values_out, (size_t)first, max_n, g);
     return DET_OK;
   });
   DET_LAUNCH(export_special_kernel, 1, 128, 0, s, v, plane, prb, (long long*)keys_out, (unsigned char*)values_out, (size_t)first, max_n);
-  if (plane > 0 && values_out)
+  if (plane > 0 && values_out && t->slot_esize == 2) {
+    const unsigned short init = f32_to_half_bits(t->slot_init[plane], t->cfg.value_dtype == DET_BFLOAT16);
+    DET_LAUNCH(export_fix_slot_rows_kernel<unsigned short>, grid_for(max_n, 8, t->sm_count, 8), kThreads, 0, s,
+               (unsigned short*)values_out, &v.st->scratch[1], (unsigned)t->cfg.dim, init, kSlotUninit16);
+  } else if (plane > 0 && values_out) {
     DET_LAUNCH(export_fix_slot_rows_kernel, grid_for(max_n, 8, t->sm_count, 8), kThreads, 0, s, 
         (float*)values_out, &v.st->scratch[1], (unsigned)t->cfg.dim, t->slot_init[plane]);
+  }
   CUDA_TRY(cudaGetLastError());
   DevState ds;
   det_status st = read_state(t, s, &ds);
@@ -1464,8 +1496,12 @@ det_status det_export(det_table* t, int plane, int64_t* keys_out, void* values_o
   return det_export_window(t, plane, 0, keys_out, values_out, max_n, n_out_host, stream);
 }
 
-det_status det_import_plane(det_table* t, int plane, const int64_t* keys, const float* rows, size_t n,
-                            det_stream_t stream) {
+}  // extern "C"
+
+namespace det {
+// det_import_plane from rows already in the plane's dtype (slot_row_bytes(t) each); det_load_plane reads them from file
+det_status import_plane_rows(det_table* t, int plane, const int64_t* keys, const void* rows, size_t n, bool narrow,
+                             cudaStream_t s) {
   if (!t) return fail(DET_INVALID_ARGUMENT, "det_import_plane: null table");
   det::MutLock _lk(t);
   if (plane < 1 || plane > t->cfg.num_slot_planes)
@@ -1473,18 +1509,35 @@ det_status det_import_plane(det_table* t, int plane, const int64_t* keys, const 
                                           std::to_string(t->cfg.num_slot_planes) + ")");
   if (n == 0) return DET_OK;
   if (!keys || !rows) return fail(DET_INVALID_ARGUMENT, "det_import_plane: null keys/rows");
-  cudaStream_t s = (cudaStream_t)stream;
   det::DevGuard _dg(t->cfg.device);
-  const size_t rb = (size_t)t->cfg.dim * 4u;
+  const size_t rb = slot_row_bytes(t);
+  if (narrow && t->slot_esize == 2) {   // fp32 rows into an fp16 / bf16 plane: rounded once, in the table's scratch
+    void* sc = nullptr;
+    det_status sst = table_scratch(t, n * rb, &sc);
+    if (sst != DET_OK) return sst;
+    const size_t count = n * (size_t)t->cfg.dim;
+    DET_LAUNCH(narrow_rows_kernel, grid_for(count, 1024, t->sm_count, 8), 256, 0, s, (const float*)rows,
+               (unsigned short*)sc, count, t->cfg.value_dtype == DET_BFLOAT16 ? 1 : 0);
+    rows = sc;
+  }
   const int grid = grid_for(n, kThreads, t->sm_count, 8);
   const TableView v = t->view;
-  dispatch_vec(rb, {{rows, "det_import_plane: rows"}}, [&](auto V, const RowGeom& g) -> det_status {
+  det_status st = dispatch_vec(rb, {{rows, "det_import_plane: rows"}}, [&](auto V, const RowGeom& g) -> det_status {
     DET_LAUNCH(set_plane_kernel<decltype(V)::value>, grid, kThreads, 0, s, v, plane, (const long long*)keys,
                (const unsigned char*)rows, n, g);
     return DET_OK;
   });
+  if (st != DET_OK) return st;
   CUDA_TRY(cudaGetLastError());
   return DET_OK;
+}
+}  // namespace det
+
+extern "C" {
+
+det_status det_import_plane(det_table* t, int plane, const int64_t* keys, const float* rows, size_t n,
+                            det_stream_t stream) {
+  return det::import_plane_rows(t, plane, keys, rows, n, true, (cudaStream_t)stream);
 }
 
 det_status det_import(det_table* t, const int64_t* keys, const void* values, size_t n, det_stream_t stream) {

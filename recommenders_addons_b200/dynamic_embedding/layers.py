@@ -8,6 +8,7 @@ import torch
 from .ops import trainable_embedding_lookup_sparse
 from .optimizer import _FUSED_DTYPES, ComposedOptimizer, _FusedBase
 from .sharded import PeerShardedVariable, ShardedVariable
+from .table import slot_dtype_of
 from .variable import Variable, default_partition_fn, embedding_lookup_unique, gather_unique, unique
 
 
@@ -16,12 +17,13 @@ class Embedding(torch.nn.Module):
 
   num_slot_planes: float32 optimizer slot planes beside the rows, for the fused Adagrad / Adam step; kept for float32,
   float16 and bfloat16 rows (the step widens a half row, updates it in float32 and rounds it once), 0 for any other
-  value_dtype."""
+  value_dtype.  slot_dtype: None (float32 planes) or the layer's own float16 / bfloat16 value_dtype (planes in that
+  dtype, rounded once per step like the rows; the reference's slot layout)."""
 
   def __init__(self, embedding_size, key_dtype=torch.int64, value_dtype=torch.float32, combiner="sum", initializer=None,
                devices=None, name="DynamicEmbeddingLayer", with_unique=True, trainable=True, bp_v2=False,
                init_capacity=0, partitioner=default_partition_fn, kv_creator=None, max_norm=None, num_slot_planes=2,
-               restrict_policy=None, short_file_name=False):
+               restrict_policy=None, short_file_name=False, slot_dtype=None):
     super().__init__()
     if combiner not in ("sum", "mean", "sqrtn"):
       raise ValueError("combiner must be one of 'mean', 'sqrtn' or 'sum'")
@@ -33,7 +35,7 @@ class Embedding(torch.nn.Module):
                            partitioner=partitioner, name=name, initializer=initializer, trainable=trainable,
                            init_size=init_capacity, kv_creator=kv_creator, bp_v2=bp_v2, restrict_policy=restrict_policy,
                            num_slot_planes=num_slot_planes if value_dtype in _FUSED_DTYPES else 0,
-                           short_file_name=short_file_name)
+                           short_file_name=short_file_name, slot_dtype=slot_dtype)
     self._wrappers = []
 
   def call(self, ids):
@@ -149,7 +151,7 @@ class AllToAllEmbedding(torch.nn.Module):
   def __init__(self, embedding_size, capacity_per_shard=None, group=None, initializer=None, name="AllToAllEmbedding",
                num_slot_planes=2, with_unique=True, with_secondary_unique=True, mpi_size=None, batch_size=None,
                key_dtype=torch.int64, value_dtype=torch.float32, init_capacity=0, kv_creator=None, devices=None,
-               exchange_impls=None, evict_strategy=None, max_ids_per_rank=None, **kwargs):
+               exchange_impls=None, evict_strategy=None, max_ids_per_rank=None, slot_dtype=None, **kwargs):
     """The reference's arguments (embedding.py:545-563: with_unique, with_secondary_unique, mpi_size, batch_size and the
     base layer's) are accepted; the world size comes from `group`, lookups always dedupe once (unique -> one-sided
     find), and a published shard has a FIXED capacity: capacity_per_shard (default: init_capacity, else 1M slots)."""
@@ -158,6 +160,7 @@ class AllToAllEmbedding(torch.nn.Module):
     refuse_keyed(initializer, "AllToAllEmbedding")
     if key_dtype != torch.int64 or value_dtype != torch.float32:
       raise TypeError("AllToAllEmbedding: int64 keys and float32 rows")
+    slot_dtype_of(value_dtype, slot_dtype)   # float32 rows: float32 slot planes only
     self.embedding_size = int(embedding_size)
     self.with_unique, self.with_secondary_unique, self.batch_size = with_unique, with_secondary_unique, batch_size
     capacity_per_shard = int(capacity_per_shard or init_capacity or (1 << 20))

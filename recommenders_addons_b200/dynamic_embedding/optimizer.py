@@ -46,7 +46,10 @@ class SlotPlane(object):
     # create_slots (dynamic_embedding_optimizer.py:882-885)
     self.name = ("%s/%s" % (params.name, slot_name)) if getattr(params, "short_file_name", False) else \
         "%s/%s/%s" % (params.name, opt_name, slot_name)
-    self.dim, self.value_dtype, self.key_dtype, self.trainable = params.dim, torch.float32, params.key_dtype, False
+    # the plane's dtype: float32, or the variable's float16 / bfloat16 with slot_dtype (the reference's slot Variables
+    # take the param's value_dtype, dynamic_embedding_optimizer.py:889-901)
+    self.value_dtype = getattr(params, "slot_dtype", torch.float32)
+    self.dim, self.key_dtype, self.trainable = params.dim, params.key_dtype, False
 
   def size(self):
     return self.params.size()
@@ -56,7 +59,8 @@ class SlotPlane(object):
     return torch.cat(ks), torch.cat(vs)
 
   def upsert(self, keys, values):
-    """slot rows for keys of the variable (keys the variable does not hold are skipped)"""
+    """slot rows for keys of the variable (keys the variable does not hold are skipped); a float16 / bfloat16 plane
+    stores them rounded to nearest even"""
     grouped, perm, bounds = self.params._partition(keys.reshape(-1))
     values = values.reshape(-1, self.dim).to(torch.float32)
     if perm is not None:
@@ -84,7 +88,8 @@ class SlotPlane(object):
 
   def load_from_file_system_with_restore_function(self, dirpath, buffer_size=4194304):
     """reshard-on-load for a slot (the variable's own `load_from_file_system_with_restore_function` first): every
-    saved shard file of this slot, whatever topology wrote it, its rows routed to the shards that hold the keys now"""
+    saved shard file of this slot, whatever topology wrote it, its rows routed to the shards that hold the keys now.
+    The `-values` files hold rows of the slot's dtype (value_dtype: float32, float16 or bfloat16)."""
     import glob
     import os
     import re
@@ -101,10 +106,19 @@ class SlotPlane(object):
       if os.path.getsize(kf) == 0:
         continue
       keys = np.memmap(kf, dtype=np.int64, mode="r")
-      vals = np.memmap(kf[:-len("-keys")] + "-values", dtype=np.float32, mode="r").reshape(-1, self.dim)
+      vf = kf[:-len("-keys")] + "-values"
+      # bfloat16 has no NumPy dtype: its rows are read as uint16 and viewed as torch.bfloat16
+      npdt = {torch.float32: np.float32, torch.float16: np.float16, torch.bfloat16: np.uint16}[self.value_dtype]
+      want = keys.shape[0] * self.dim * np.dtype(npdt).itemsize
+      if os.path.getsize(vf) != want:
+        raise ValueError("%s holds %d bytes, not the %d of %d rows of %d %s elements" %
+                         (vf, os.path.getsize(vf), want, keys.shape[0], self.dim, self.value_dtype))
+      vals = np.memmap(vf, dtype=npdt, mode="r").reshape(-1, self.dim)
       for b in range(0, keys.shape[0], step):
-        self.upsert(torch.from_numpy(np.array(keys[b:b + step])).to(dev),      # np.array: a writable copy of the chunk
-                    torch.from_numpy(np.array(vals[b:b + step])).to(dev))
+        v = torch.from_numpy(np.array(vals[b:b + step]))     # np.array: a writable copy of the chunk
+        if self.value_dtype == torch.bfloat16:
+          v = v.view(torch.bfloat16)
+        self.upsert(torch.from_numpy(np.array(keys[b:b + step])).to(dev), v.to(dev))
 
 
 class _FusedBase(object):

@@ -29,6 +29,18 @@ VALID_VALUE_DTYPES = tuple(_TORCH_TO_NAME.keys())
 _DEVICE_TYPES = ("cuda",)
 
 
+def slot_dtype_of(value_dtype, slot_dtype):
+  """The dtype of a table's optimizer slot planes: float32 (slot_dtype None or torch.float32, the default), or the
+  table's own float16 / bfloat16 value dtype -- the reference's layout, whose slot Variables take the param's
+  value_dtype (python/ops/dynamic_embedding_optimizer.py:889-901).  Anything else is a TypeError."""
+  if slot_dtype is None or slot_dtype == torch.float32:
+    return torch.float32
+  if slot_dtype == value_dtype and value_dtype in (torch.float16, torch.bfloat16):
+    return slot_dtype
+  raise TypeError("slot_dtype must be None, torch.float32 or the variable's own float16 / bfloat16 value dtype; got %s "
+                  "for value dtype %s" % (slot_dtype, value_dtype))
+
+
 def _stream_ptr(device):
   return ctypes.c_void_p(torch.cuda.current_stream(device).cuda_stream)
 
@@ -101,7 +113,8 @@ class KVCreator(object):
                          "DynamicEmbeddingSaver.")
 
   def create(self, key_dtype=None, value_dtype=None, default_value=None, name=None, checkpoint=None,
-             init_size=None, config=None, device=None, shard_saveable_object_fn=None, num_slot_planes=0):
+             init_size=None, config=None, device=None, shard_saveable_object_fn=None, num_slot_planes=0,
+             slot_dtype=None):
     raise NotImplementedError("create function must be implemented")
 
 
@@ -156,7 +169,7 @@ class CuckooHashTable(object):
 
   def __init__(self, key_dtype, value_dtype, default_value, name="CuckooHashTable", checkpoint=True, init_size=0,
                config=None, device=None, shard_saveable_object_fn=None, num_slot_planes=0, max_capacity=0,
-               max_load_factor=0.0, region=None, evict_strategy=None, max_hbm_for_values=None):
+               max_load_factor=0.0, region=None, evict_strategy=None, max_hbm_for_values=None, slot_dtype=None):
     if key_dtype != torch.int64:
       raise TypeError("key dtype %s is not supported on GPU: keys must be int64" % (key_dtype,))
     if value_dtype not in _TORCH_TO_NAME:
@@ -178,6 +191,7 @@ class CuckooHashTable(object):
     self._init_size = int(init_size)
     self._config = config
     self._num_slot_planes = int(num_slot_planes)
+    self._slot_dtype = slot_dtype_of(value_dtype, slot_dtype)
     cfg = _lib.DetConfig()
     cfg.value_dtype = _lib.DTYPE_CODES[_TORCH_TO_NAME[value_dtype]]
     cfg.dim = self._dim
@@ -187,6 +201,8 @@ class CuckooHashTable(object):
     cfg.max_capacity = int(max_capacity)
     cfg.max_load_factor = float(max_load_factor)
     cfg.flags = 0 if evict_strategy is None else _lib.flags_evict(int(evict_strategy))
+    if self._slot_dtype != torch.float32:
+      cfg.flags |= _lib.FLAGS_SLOTS_IN_VALUE_DTYPE
     if max_hbm_for_values is not None and int(max_hbm_for_values) < 0:
       raise ValueError("params max_hbm_for_vectors less than 0")  # hkv_hashtable_op_gpu.cu.cc:87-89
     cfg.max_hbm_for_vectors = 0 if max_hbm_for_values is None else max(int(max_hbm_for_values), 1)
@@ -217,6 +233,11 @@ class CuckooHashTable(object):
   @property
   def key_dtype(self):
     return self._key_dtype
+
+  @property
+  def slot_dtype(self):
+    """dtype of the optimizer slot planes: torch.float32, or the table's float16 / bfloat16 value dtype"""
+    return self._slot_dtype
 
   @property
   def value_dtype(self):
@@ -340,7 +361,7 @@ class CuckooHashTable(object):
   def export(self, name=None, plane=0):
     """(keys, values) of everything in the table, in table order (undefined, as in the reference)."""
     n = int(self.size())
-    vdtype = self._value_dtype if plane == 0 else torch.float32
+    vdtype = self._value_dtype if plane == 0 else self._slot_dtype
     keys = torch.empty(n, dtype=torch.int64, device=self._device)
     values = torch.empty((n, self._dim), dtype=vdtype, device=self._device)
     got = ctypes.c_int64(0)
@@ -352,7 +373,7 @@ class CuckooHashTable(object):
     """(keys, values) of at most `max_keys` live keys starting at live key number `first` of the table order: bounded-
     memory streaming of a table (det_export_window; what det_save uses).  The table must not be mutated between the
     windows of one pass.  An empty result marks the end."""
-    vdtype = self._value_dtype if plane == 0 else torch.float32
+    vdtype = self._value_dtype if plane == 0 else self._slot_dtype
     keys = torch.empty(int(max_keys), dtype=torch.int64, device=self._device)
     values = torch.empty((int(max_keys), self._dim), dtype=vdtype, device=self._device)
     got = ctypes.c_int64(0)
@@ -429,7 +450,8 @@ class CuckooHashTable(object):
 
   # -- optimizer slot planes (state of the fused optimizers): restore / checkpoint ---------------------------------
   def import_plane(self, plane, keys, values):
-    """rows of slot plane `plane` (1..num_slot_planes) for keys that are in the table; others are skipped"""
+    """rows of slot plane `plane` (1..num_slot_planes) for keys that are in the table; others are skipped.  The rows are
+    fp32; a float16 / bfloat16 plane stores them rounded to nearest even (exact for rows widened from that dtype)."""
     keys = self._check_keys(keys).reshape(-1)
     values = torch.as_tensor(values, dtype=torch.float32).to(self._device).contiguous()
     if values.numel() != keys.numel() * self._dim:
@@ -473,7 +495,7 @@ class HkvHashTable(CuckooHashTable):
   def __init__(self, key_dtype, value_dtype, default_value, name="HkvHashTable", checkpoint=True, init_size=0,
                config=None, device=None, shard_saveable_object_fn=None, num_slot_planes=0, init_capacity=None,
                max_capacity=None, max_hbm_for_values=None, evict_strategy=None, step_per_epoch=0, gen_scores_fn=None,
-               reserved_key_start_bit=0):
+               reserved_key_start_bit=0, slot_dtype=None):
     # hkv_hashtable_ops.py:66-136: the capacity / eviction attributes may be given directly; a config, when given,
     # overrides every one of them
     if config is not None:
@@ -495,7 +517,8 @@ class HkvHashTable(CuckooHashTable):
     super().__init__(key_dtype, value_dtype, default_value, name=name, checkpoint=checkpoint, init_size=init, config=cfg,
                      device=device, num_slot_planes=num_slot_planes,
                      max_capacity=int(cfg.max_capacity) if strategy is not None else 0, max_load_factor=0.0,
-                     evict_strategy=strategy, max_hbm_for_values=getattr(cfg, "max_hbm_for_values", None))
+                     evict_strategy=strategy, max_hbm_for_values=getattr(cfg, "max_hbm_for_values", None),
+                     slot_dtype=slot_dtype)
     self._step_per_epoch = int(cfg.step_per_epoch or 0)
     self._gen_scores_fn = cfg.gen_scores_fn
     self._curr_epoch, self._curr_step = 0, 1
@@ -592,17 +615,19 @@ class CuckooHashTableCreator(KVCreator):
   """python/ops/dynamic_embedding_creator.py:89-138"""
 
   def create(self, key_dtype=None, value_dtype=None, default_value=None, name=None, checkpoint=None,
-             init_size=None, config=None, device=None, shard_saveable_object_fn=None, num_slot_planes=0):
+             init_size=None, config=None, device=None, shard_saveable_object_fn=None, num_slot_planes=0,
+             slot_dtype=None):
     return CuckooHashTable(key_dtype=key_dtype, value_dtype=value_dtype, default_value=default_value, name=name,
                            checkpoint=checkpoint, init_size=init_size or 0, config=config or self.config,
-                           device=device, num_slot_planes=num_slot_planes)
+                           device=device, num_slot_planes=num_slot_planes, slot_dtype=slot_dtype)
 
 
 class HkvHashTableCreator(KVCreator):
   """python/ops/dynamic_embedding_creator.py:172-240"""
 
   def create(self, key_dtype=None, value_dtype=None, default_value=None, name=None, checkpoint=None,
-             init_size=None, config=None, device=None, shard_saveable_object_fn=None, num_slot_planes=0):
+             init_size=None, config=None, device=None, shard_saveable_object_fn=None, num_slot_planes=0,
+             slot_dtype=None):
     return HkvHashTable(key_dtype=key_dtype, value_dtype=value_dtype, default_value=default_value, name=name,
                         checkpoint=checkpoint, init_size=init_size or 0, config=config or self.config,
-                        device=device, num_slot_planes=num_slot_planes)
+                        device=device, num_slot_planes=num_slot_planes, slot_dtype=slot_dtype)

@@ -4,7 +4,7 @@ python/ops/dynamic_embedding_ops.py:64-117) on torch CUDA tensors over the C ABI
 import torch
 
 from .. import _lib
-from .table import CuckooHashTableCreator, HkvHashTableCreator, KVCreator, _ptr, _stream_ptr
+from .table import CuckooHashTableCreator, HkvHashTableCreator, KVCreator, _ptr, _stream_ptr, slot_dtype_of
 
 _VARIABLES = {}
 
@@ -165,7 +165,7 @@ class Variable(object):
   def __init__(self, key_dtype=torch.int64, value_dtype=torch.float32, dim=1, devices=None,
                partitioner=default_partition_fn, shared_name=None, name="DynamicEmbedding_Variable",
                initializer=None, trainable=True, checkpoint=True, init_size=0, kv_creator=None,
-               restrict_policy=None, bp_v2=False, num_slot_planes=0, short_file_name=False):
+               restrict_policy=None, bp_v2=False, num_slot_planes=0, short_file_name=False, slot_dtype=None):
     self.key_dtype = key_dtype
     self.short_file_name = bool(short_file_name)   # :553-562: slot variables are named <var>/<slot>, not <var>/<opt>/<slot>
     self.value_dtype = value_dtype
@@ -190,13 +190,18 @@ class Variable(object):
     # a keyed initializer is set on every shard table below; the static default row is then never read
     static_default = torch.zeros(self.dim, dtype=value_dtype) if is_keyed(initializer) else \
         self._convert_anything_to_init(initializer, self.dim)
+    # slot_dtype: dtype of the fused optimizers' slot planes -- float32 (None, the default) or this variable's own
+    # float16 / bfloat16 value_dtype (the reference's layout: its slot Variables take the param's value_dtype)
+    self.slot_dtype = slot_dtype_of(value_dtype, slot_dtype)
+    # a creator that predates slot_dtype keeps working for float32 planes
+    slot_kw = {} if self.slot_dtype == torch.float32 else {"slot_dtype": self.slot_dtype}
     self._tables = []
     for idx, dev in enumerate(self.devices):
       self._tables.append(
           self.kv_creator.create(key_dtype=key_dtype, value_dtype=value_dtype, default_value=static_default,
                                  name=self._make_name(idx), checkpoint=checkpoint,
                                  init_size=int(self.init_size / self.shard_num), device=dev,
-                                 num_slot_planes=num_slot_planes))
+                                 num_slot_planes=num_slot_planes, **slot_kw))
       if is_keyed(initializer):
         self._tables[-1].set_initializer(initializer)
     # dynamic_embedding_variable.py:604-611
@@ -597,7 +602,7 @@ def embedding_lookup_unique(params, ids, partition_strategy=None, name=None, val
 def get_variable(name, key_dtype=torch.int64, value_dtype=torch.float32, dim=1, devices=None,
                  partitioner=default_partition_fn, shared_name="get_variable", initializer=None, trainable=True,
                  checkpoint=True, init_size=0, kv_creator=None, restrict_policy=None, bp_v2=False,
-                 num_slot_planes=0, short_file_name=False):
+                 num_slot_planes=0, short_file_name=False, slot_dtype=None):
   """de.get_variable (:1265-1359): one Variable per name."""
   if name in _VARIABLES:
     raise ValueError("Variable %s has already existed." % name)
@@ -605,7 +610,7 @@ def get_variable(name, key_dtype=torch.int64, value_dtype=torch.float32, dim=1, 
                  shared_name=shared_name, name=name, initializer=initializer, trainable=trainable,
                  checkpoint=checkpoint, init_size=init_size, kv_creator=kv_creator,
                  restrict_policy=restrict_policy, bp_v2=bp_v2, num_slot_planes=num_slot_planes,
-                 short_file_name=short_file_name)
+                 short_file_name=short_file_name, slot_dtype=slot_dtype)
   _VARIABLES[name] = var
   return var
 

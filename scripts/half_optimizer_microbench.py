@@ -1,26 +1,33 @@
 """The fused Adagrad / Adam step on float32, float16 and bfloat16 tables holding the same rows, timed in one process.
 
-Three variables get the same keys and the same rows; the rows are bf16 values that fp16 also represents exactly, so
-all three tables start from the same numbers.  Every variable has two fp32 slot planes.  Timed, with CUDA events, in
-rounds that alternate the dtype order:
+Five variables get the same keys and the same rows; the rows are bf16 values that fp16 also represents exactly, so
+all of them start from the same numbers.  Every variable has two slot planes: fp32 planes on the float32, float16 and
+bfloat16 variables, and planes in the variable's own dtype on `float16_slots` and `bfloat16_slots` (slot_dtype =
+value_dtype).  Timed, with CUDA events, in rounds that alternate the variable order:
   * adagrad_dup -- det_apply_adagrad_dup at the c3 backward shape: 26 x 65536 Zipf ids over one third of the keys
                    (unique, position-order gradient sum and the fused step, one call);
   * adagrad     -- det_apply_adagrad on 2^20 unique resident keys (another third of the keys);
   * adam        -- det_apply_adam on 2^20 unique resident keys (the last third).
-The three shapes touch disjoint keys, so before the timing one step of each shape runs from the same state on all three
-tables, and every half result is checked against the fp32 result rounded to the half dtype (bit for bit).  Also timed:
+The three shapes touch disjoint keys, so before the timing one step of each shape runs from the same state on all five
+tables, and every half param row it wrote -- and, on the half-slot tables, every slot row it wrote -- is checked against
+the fp32 result rounded to the half dtype (bit for bit).  That is the rule for half slots: the initial accumulator,
+0.125, is exact in every dtype, so the first step widens identical slot values, computes the param from the unrounded
+fp32 slot values, and rounds the param and the slots once.  Also timed:
 the composed step (`fused=False`: unique ids, finds of the param and slot rows, torch's dense Adagrad in bf16, upserts)
 that bf16 variables ran before, on a separate bf16 variable of --composed-resident rows (its slot Variables are tables
 of their own), next to the fused step on that same variable.
 
 Bytes per key are the bytes the unique-key step must move at dim 64 (key 8 + probed bucket 64 + fp32 gradient 256 +
-param row read and write + fp32 slot rows read and write); the rate is against the H100 SXM data-sheet HBM3 bandwidth
+param row read and write + slot rows read and write, 4 or 2 bytes per slot element); the rate is against the H100 SXM data-sheet HBM3 bandwidth
 of 3.35 TB/s (a data-sheet figure, not a measured peak).  Prints one JSON line.
 
-Three tables with two slot planes need 2072 B of HBM per slot (776 B fp32, 648 B fp16 and bf16), and each is sized
-at twice its resident keys, so the default of 1.2e7 resident keys takes ~50 GB of an 80 GB card; 4e7 would not fit.
+Per table slot at dim 64 with two slot planes: 776 B for the fp32 table (8 key + 256 row + 2 x 256 slots), 648 B for
+each half table with fp32 planes (8 + 128 + 2 x 256) and 392 B for each half table with half planes (8 + 128 + 2 x
+128): 2856 B for the five.  Each table is sized at twice its resident keys, so the default of 9e6 resident keys takes
+1.8e7 x 2856 B = 51.4 GB, plus 3.3 GB for the composed-step variable (2 x 2^22 slots x 392 B) and ~1 GB of ids,
+gradients and workspace: ~56 GB of an 80 GB card.  1.2e7 would need ~73 GB and leave no margin.
 
-  python scripts/half_optimizer_microbench.py [--resident 12000000] [--rounds 5] [--calls 10]
+  python scripts/half_optimizer_microbench.py [--resident 9000000] [--rounds 5] [--calls 10]
 """
 import argparse
 import ctypes
@@ -52,10 +59,10 @@ def card():
     return {"name": torch.cuda.get_device_name(0), "error": repr(ex)}
 
 
-def bytes_per_key(opt, elem_bytes):
+def bytes_per_key(opt, elem_bytes, slot_bytes=4):
   """HBM bytes the fused step moves per unique key: key, bucket, fp32 gradient, param read + write, slots read + write"""
   slots = 1 if opt == "adagrad" else 2
-  return 8 + BUCKET_BYTES + DIM * 4 + 2 * DIM * elem_bytes + slots * 2 * DIM * 4
+  return 8 + BUCKET_BYTES + DIM * 4 + 2 * DIM * elem_bytes + slots * 2 * DIM * slot_bytes
 
 
 def mix_keys(r):
@@ -64,7 +71,7 @@ def mix_keys(r):
 
 def main():
   ap = argparse.ArgumentParser()
-  ap.add_argument("--resident", type=int, default=12_000_000)
+  ap.add_argument("--resident", type=int, default=9_000_000)
   ap.add_argument("--composed-resident", type=int, default=1 << 22)
   ap.add_argument("--rounds", type=int, default=5)
   ap.add_argument("--calls", type=int, default=10)
@@ -79,9 +86,10 @@ def main():
   torch.cuda.set_device(0)
   info = card()
   R = args.resident
-  dts = {"float32": torch.float32, "float16": torch.float16, "bfloat16": torch.bfloat16}
-  vars_ = {n: de.Variable(value_dtype=dt, dim=DIM, init_size=2 * R, initializer=0.0, name="hom_" + n,
-                          num_slot_planes=2) for n, dt in dts.items()}
+  dts = {"float32": torch.float32, "float16": torch.float16, "bfloat16": torch.bfloat16,
+         "float16_slots": torch.float16, "bfloat16_slots": torch.bfloat16}
+  vars_ = {n: de.Variable(value_dtype=dt, dim=DIM, init_size=2 * R, initializer=0.0, name="hom_" + n, num_slot_planes=2,
+                          slot_dtype=dt if n.endswith("_slots") else None) for n, dt in dts.items()}
   gen = torch.Generator(device=dev).manual_seed(7)
 
   def fill(variables, n_rows):
@@ -112,12 +120,20 @@ def main():
   def step(name, shape, var=None):
     h = (var or vars_[name]).tables[0].handle
     if shape == "adagrad_dup":
-      st = lib.det_apply_adagrad_dup(h, P(ids_dup), P(g_dup), N_DUP, lr, 0.0, P(init), 0.1, P(ws), wsb, None, None)
+      st = lib.det_apply_adagrad_dup(h, P(ids_dup), P(g_dup), N_DUP, lr, 0.0, P(init), 0.125, P(ws), wsb, None, None)
     elif shape == "adagrad":
-      st = lib.det_apply_adagrad(h, P(keys_ada), P(g_uni), N_UNIQUE, lr, 0.0, P(init), 0, 0.1, None)
+      st = lib.det_apply_adagrad(h, P(keys_ada), P(g_uni), N_UNIQUE, lr, 0.0, P(init), 0, 0.125, None)
     else:
       st = lib.det_apply_adam(h, P(keys_adam), P(g_uni), N_UNIQUE, lr * 0.3, b1, b2, eps, P(init), 0, None)
     _lib.check(st)
+
+  def slot_rows(var, plane, keys):
+    """(keys, rows) of slot plane `plane` for `keys`, sorted by key"""
+    k, v = var.tables[0].export(plane=plane)
+    sel = torch.isin(k, keys)
+    k, v = k[sel], v[sel]
+    o = torch.argsort(k)
+    return k[o], v[o]
 
   shapes = ("adagrad_dup", "adagrad", "adam")
   touched = {"adagrad_dup": torch.unique(ids_dup), "adagrad": keys_ada, "adam": keys_adam}
@@ -127,7 +143,15 @@ def main():
       step(n, shape)
     ref = vars_["float32"].lookup(touched[shape])
     identical[shape] = all(torch.equal(vars_[n].lookup(touched[shape]).view(torch.int16), ref.to(dts[n]).view(torch.int16))
-                           for n in ("float16", "bfloat16"))
+                           for n in dts if n != "float32")
+    # the slot rows the step wrote on the half-slot tables: the fp32 table's rows rounded into the dtype
+    for plane in range(1, (1 if shape.startswith("adagrad") else 2) + 1):
+      kf, vf = slot_rows(vars_["float32"], plane, touched[shape])
+      for n in ("float16_slots", "bfloat16_slots"):
+        kh, vh = slot_rows(vars_[n], plane, touched[shape])
+        identical[shape] = identical[shape] and torch.equal(kh, kf) and vh.dtype == dts[n] and \
+            torch.equal(vh.view(torch.int16), vf.to(dts[n]).view(torch.int16))
+      del kf, vf
 
   def timed(fn, calls):
     fn()
@@ -166,11 +190,15 @@ def main():
       t = float(np.median(ms[(n, shape)]))
       row[n] = {"ms": round(t, 4), "ms_spread": [round(min(ms[(n, shape)]), 4), round(max(ms[(n, shape)]), 4)]}
       if shape != "adagrad_dup":
-        bpk = bytes_per_key(shape, torch.empty(0, dtype=dt).element_size())
+        es = torch.empty(0, dtype=dt).element_size()
+        bpk = bytes_per_key(shape, es, es if n.endswith("_slots") else 4)
         row[n].update({"bytes_per_key": bpk, "GB_s": round(bpk * N_UNIQUE / t / 1e6, 1),
                        "of_datasheet_hbm": round(bpk * N_UNIQUE / (t * 1e-3) / DATASHEET_HBM_BPS, 3)})
     row["bf16_speedup_vs_fp32"] = round(row["float32"]["ms"] / row["bfloat16"]["ms"], 3)
     row["fp16_speedup_vs_fp32"] = round(row["float32"]["ms"] / row["float16"]["ms"], 3)
+    # the same table dtype with its slot planes in that dtype instead of fp32
+    row["bf16_slots_speedup_vs_bf16"] = round(row["bfloat16"]["ms"] / row["bfloat16_slots"]["ms"], 3)
+    row["fp16_slots_speedup_vs_fp16"] = round(row["float16"]["ms"] / row["float16_slots"]["ms"], 3)
     row["ids"] = N_DUP if shape == "adagrad_dup" else N_UNIQUE
     res[shape] = row
   res["composed_vs_fused_bf16_adagrad"] = {"resident": Rc, "keys": N_UNIQUE,
