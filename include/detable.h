@@ -376,6 +376,24 @@ det_status det_apply_proximal_sgd(det_table* t, const int64_t* keys, const float
 det_status det_apply_adagrad_da(det_table* t, const int64_t* keys, const float* grads, size_t n, float lr, float l1,
                                 float l2, int64_t global_step, const float* init_param, int full_size_init,
                                 float init_gg, det_stream_t stream);
+/* The same step for AdamW (and AMSGrad) and Lion, Keras 3's dense update_step after its _apply_weight_decay.  Each
+ * fp32 operation is rounded on its own, in the order written; the step scalars are the caller's, in fp32.
+ * Weight decay, first, when weight_decay > 0: p = p - (p*weight_decay)*lr.  weight_decay == 0 skips the line (an inf
+ * param stays inf).
+ * AdamW: m = m + (g - m)*(1 - beta1);  v = v + (g*g - v)*(1 - beta2);  with amsgrad: vh = max(vh, v), then
+ *   p = p - (m*alpha) / (sqrt(vh) + epsilon); without it v takes vh's place.  alpha = lr*sqrt(1 - beta2^t)/(1 - beta1^t)
+ *   from the caller, as for det_apply_adam; lr is the decay's.  Plane 1 = m, plane 2 = v, plane 3 = vhat (amsgrad only;
+ *   all initial 0).  weight_decay = 0 with amsgrad = 0 is det_apply_adam bit for bit (param, m and v).  Keras' own
+ *   IndexedSlices branch rounds m and v in another order (DESIGN.md section 4).
+ * Lion: c = m*beta1 + g*r1;  p = p - lr*sign(c);  m = m*beta2 + g*r2, with r1 = 1 - beta1 and r2 = 1 - beta2 computed
+ *   once in fp32, sign(+-0) = 0 and sign(NaN) = NaN.  Plane 1 = m (initial 0).
+ * A negative or NaN weight_decay, or Lion betas outside [0, 1]: DET_INVALID_ARGUMENT.  Additive to ABI 8. */
+det_status det_apply_adamw(det_table* t, const int64_t* keys, const float* grads, size_t n, float alpha, float beta1,
+                           float beta2, float epsilon, float lr, float weight_decay, int amsgrad, const float* init_param,
+                           int full_size_init, det_stream_t stream);
+det_status det_apply_lion(det_table* t, const int64_t* keys, const float* grads, size_t n, float lr, float beta1,
+                          float beta2, float weight_decay, const float* init_param, int full_size_init,
+                          det_stream_t stream);
 
 /* ---- HOST-buffer entry points (the op placed on host tensors; used for end-to-end timing):
  * pinned or pageable HOST pointers; chunked H2D -> kernel -> D2H pipeline on internal streams;
@@ -443,6 +461,13 @@ det_status det_apply_adagrad_da_dup(det_table* t, const int64_t* ids, const floa
                                     float l2, int64_t global_step, const float* init_param, float init_gg,
                                     void* workspace, size_t workspace_bytes, int64_t* n_unique_dev_out,
                                     det_stream_t stream);
+det_status det_apply_adamw_dup(det_table* t, const int64_t* ids, const float* grads, size_t n, float alpha, float beta1,
+                               float beta2, float epsilon, float lr, float weight_decay, int amsgrad,
+                               const float* init_param, void* workspace, size_t workspace_bytes,
+                               int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_lion_dup(det_table* t, const int64_t* ids, const float* grads, size_t n, float lr, float beta1,
+                              float beta2, float weight_decay, const float* init_param, void* workspace,
+                              size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream);
 
 /* The backward of det_lookup_sparse, fused: per-unique-id gradients straight from the output gradient (ABI >= 8).
  * Inputs are the forward's ids int64[nnz], segment_ids int32[nnz] (ascending, in [0, batch)), weights f32[nnz] or NULL
@@ -518,6 +543,15 @@ det_status det_apply_adagrad_da_sparse(det_table* t, const int64_t* ids, const i
                                        float lr, float l1, float l2, int64_t global_step, const float* init_param,
                                        float init_gg, void* workspace, size_t workspace_bytes,
                                        int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_adamw_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
+                                  size_t nnz, size_t batch, int combiner, const float* gout, float alpha, float beta1,
+                                  float beta2, float epsilon, float lr, float weight_decay, int amsgrad,
+                                  const float* init_param, void* workspace, size_t workspace_bytes,
+                                  int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_lion_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
+                                 size_t nnz, size_t batch, int combiner, const float* gout, float lr, float beta1,
+                                 float beta2, float weight_decay, const float* init_param, void* workspace,
+                                 size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream);
 
 /* ---- key-hash sharding across GPUs (python/ops/dynamic_embedding_variable.py:165-197 default_partition_fn,
  * python/ops/shadow_embedding_ops.py:397-447 alltoall exchange) ----

@@ -263,6 +263,55 @@ REGISTER_OP("TFRA>DetApplyAdagradDADuplicateIndices")
     .Attr("l2: float = 0.0")
     .Attr("initial_gradient_squared_accumulator_value: float = 0.1");
 
+// AdamW (AMSGrad with amsgrad = 1) and Lion (Keras 3's dense update_step after its _apply_weight_decay), as
+// det_apply_adamw / _lion.  AdamW's input 3 is Adam's alpha = lr*sqrt(1 - beta2^t)/(1 - beta1^t) and its input 5 the
+// learning rate of the weight decay, both host-memory inputs; Lion's input 3 is lr.
+REGISTER_OP("TFRA>DetApplyAdamW")
+    .Input("table_handle: resource")
+    .Input("keys: int64")          // [n] unique
+    .Input("grads: float")         // [n, dim]
+    .Input("alpha: float")
+    .Input("init_param: float")    // [dim] or [n, dim]
+    .Input("lr: float")
+    .Attr("beta1: float = 0.9")
+    .Attr("beta2: float = 0.999")
+    .Attr("epsilon: float = 1e-7")
+    .Attr("weight_decay: float = 0.004")
+    .Attr("amsgrad: int = 0");
+
+REGISTER_OP("TFRA>DetApplyLion")
+    .Input("table_handle: resource")
+    .Input("keys: int64")
+    .Input("grads: float")
+    .Input("lr: float")
+    .Input("init_param: float")
+    .Attr("beta1: float = 0.9")
+    .Attr("beta2: float = 0.99")
+    .Attr("weight_decay: float = 0.0");
+
+REGISTER_OP("TFRA>DetApplyAdamWDuplicateIndices")
+    .Input("table_handle: resource")
+    .Input("ids: int64")
+    .Input("grads: float")
+    .Input("alpha: float")
+    .Input("init_param: float")    // [dim]
+    .Input("lr: float")
+    .Attr("beta1: float = 0.9")
+    .Attr("beta2: float = 0.999")
+    .Attr("epsilon: float = 1e-7")
+    .Attr("weight_decay: float = 0.004")
+    .Attr("amsgrad: int = 0");
+
+REGISTER_OP("TFRA>DetApplyLionDuplicateIndices")
+    .Input("table_handle: resource")
+    .Input("ids: int64")
+    .Input("grads: float")
+    .Input("lr: float")
+    .Input("init_param: float")
+    .Attr("beta1: float = 0.9")
+    .Attr("beta2: float = 0.99")
+    .Attr("weight_decay: float = 0.0");
+
 // The gradient dedupe in front of the sparse optimizer step: unsorted_segment_sum(values, idx, num_segments) as
 // _deduplicate_indexed_slices calls it before _resource_apply_sparse_duplicate_indices
 // (python/ops/dynamic_embedding_optimizer.py:150,184), with the rows of one segment added in position order
@@ -330,7 +379,7 @@ class DetLookupSparseOp : public OpKernel {
 
 // What a TFRA>DetApply* op hands the library.  `step` is input 3: lr, or alpha for Adam.  `full` is 1 when init_param
 // holds one row per key (unique-key forms only); `ws` / `ws_bytes` are the duplicate-id forms' workspace.  `ctx`: for
-// the rules with more step inputs after init_param (Nadam, AdagradDA).
+// the rules with more step inputs after init_param (Nadam, AdagradDA, AdamW).
 struct ApplyArgs {
   OpKernelContext* ctx;
   det_table* table;
@@ -551,6 +600,46 @@ struct AdagradDARule {
   }
 };
 
+struct AdamWRule {
+  static constexpr const char* kName = "DetApplyAdamW";
+  float beta1 = 0.9f, beta2 = 0.999f, epsilon = 1e-7f, weight_decay = 0.004f;
+  int amsgrad = 0;
+  explicit AdamWRule(OpKernelConstruction* ctx) {
+    OP_REQUIRES_OK(ctx, ctx->GetAttr("beta1", &beta1));
+    OP_REQUIRES_OK(ctx, ctx->GetAttr("beta2", &beta2));
+    OP_REQUIRES_OK(ctx, ctx->GetAttr("epsilon", &epsilon));
+    OP_REQUIRES_OK(ctx, ctx->GetAttr("weight_decay", &weight_decay));
+    OP_REQUIRES_OK(ctx, ctx->GetAttr("amsgrad", &amsgrad));
+  }
+  // input 5, the learning rate of the weight decay
+  static float Lr(const ApplyArgs& a) { return a.ctx->input(5).scalar<float>()(); }
+  det_status Unique(const ApplyArgs& a) const {
+    return det_apply_adamw(a.table, a.keys, a.grads, a.n, a.step, beta1, beta2, epsilon, Lr(a), weight_decay, amsgrad,
+                           a.init, a.full, a.stream);
+  }
+  det_status Dup(const ApplyArgs& a) const {
+    return det_apply_adamw_dup(a.table, a.keys, a.grads, a.n, a.step, beta1, beta2, epsilon, Lr(a), weight_decay,
+                               amsgrad, a.init, a.ws, a.ws_bytes, nullptr, a.stream);
+  }
+};
+
+struct LionRule {
+  static constexpr const char* kName = "DetApplyLion";
+  float beta1 = 0.9f, beta2 = 0.99f, weight_decay = 0.f;
+  explicit LionRule(OpKernelConstruction* ctx) {
+    OP_REQUIRES_OK(ctx, ctx->GetAttr("beta1", &beta1));
+    OP_REQUIRES_OK(ctx, ctx->GetAttr("beta2", &beta2));
+    OP_REQUIRES_OK(ctx, ctx->GetAttr("weight_decay", &weight_decay));
+  }
+  det_status Unique(const ApplyArgs& a) const {
+    return det_apply_lion(a.table, a.keys, a.grads, a.n, a.step, beta1, beta2, weight_decay, a.init, a.full, a.stream);
+  }
+  det_status Dup(const ApplyArgs& a) const {
+    return det_apply_lion_dup(a.table, a.keys, a.grads, a.n, a.step, beta1, beta2, weight_decay, a.init, a.ws,
+                              a.ws_bytes, nullptr, a.stream);
+  }
+};
+
 // TFRA>DetApply<Rule> (DUP false: unique keys, init_param [dim] or [n, dim]) and TFRA>DetApply<Rule>DuplicateIndices
 // (DUP true: ids with repeats, init_param [dim], a 256 B aligned workspace)
 template <class Rule, bool DUP>
@@ -663,6 +752,13 @@ REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplyProximalGradientDescentDuplicateIndic
                         DetApplyOp<ProximalSgdRule, true>);
 REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplyAdagradDADuplicateIndices").Device(DEVICE_GPU).HostMemory("lr").HostMemory("global_step"),
                         DetApplyOp<AdagradDARule, true>);
+REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplyAdamW").Device(DEVICE_GPU).HostMemory("alpha").HostMemory("lr"),
+                        DetApplyOp<AdamWRule, false>);
+REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplyLion").Device(DEVICE_GPU).HostMemory("lr"), DetApplyOp<LionRule, false>);
+REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplyAdamWDuplicateIndices").Device(DEVICE_GPU).HostMemory("alpha").HostMemory("lr"),
+                        DetApplyOp<AdamWRule, true>);
+REGISTER_KERNEL_BUILDER(Name("TFRA>DetApplyLionDuplicateIndices").Device(DEVICE_GPU).HostMemory("lr"),
+                        DetApplyOp<LionRule, true>);
 
 }  // namespace det_shim
 }  // namespace lookup

@@ -134,6 +134,15 @@ SIGNATURES = {
                                       [_vp, _vp, _sz, _vp, _vp]),
     "det_apply_adagrad_da_sparse": (_i, [_vp, _vp, _vp, _vp, _sz, _sz, _i, _vp] + [ctypes.c_float] * 3 +
                                     [ctypes.c_int64, _vp, ctypes.c_float, _vp, _sz, _vp, _vp]),
+    # AdamW (AMSGrad) and Lion: unique keys, then _dup, then _sparse
+    "det_apply_adamw": (_i, [_vp, _vp, _vp, _sz] + [ctypes.c_float] * 6 + [_i, _vp, _i, _vp]),
+    "det_apply_lion": (_i, [_vp, _vp, _vp, _sz] + [ctypes.c_float] * 4 + [_vp, _i, _vp]),
+    "det_apply_adamw_dup": (_i, [_vp, _vp, _vp, _sz] + [ctypes.c_float] * 6 + [_i, _vp, _vp, _sz, _vp, _vp]),
+    "det_apply_lion_dup": (_i, [_vp, _vp, _vp, _sz] + [ctypes.c_float] * 4 + [_vp, _vp, _sz, _vp, _vp]),
+    "det_apply_adamw_sparse": (_i, [_vp, _vp, _vp, _vp, _sz, _sz, _i, _vp] + [ctypes.c_float] * 6 +
+                               [_i, _vp, _vp, _sz, _vp, _vp]),
+    "det_apply_lion_sparse": (_i, [_vp, _vp, _vp, _vp, _sz, _sz, _i, _vp] + [ctypes.c_float] * 4 +
+                              [_vp, _vp, _sz, _vp, _vp]),
     "det_find_host": (_i, [_vp, _vp, _sz, _vp, _i, _vp, _vp]),
     "det_insert_host": (_i, [_vp, _vp, _vp, _sz]),
     "det_find_host_async": (_i, [_vp, _vp, _sz, _vp, _i, _vp, _vp]),

@@ -778,32 +778,45 @@ segment_sum_wide_kernel(TableView t, const long long* __restrict__ slots, const 
 // ------------------------------------------------------------------------------------------------
 // K7: fused find-or-insert + optimizer update
 // ------------------------------------------------------------------------------------------------
-// The optimizer of a K7 launch is its template parameter OPT (kAdagrad .. kAdagradDa, host.h) with an OptHyper (and,
-// for Nadam, a StepArg).
+// The optimizer of a K7 launch is its template parameter OPT (kAdagrad .. kLion, host.h) with an OptHyper (and, for
+// Nadam, AdamW and Lion, a StepArg).
 
 // slot planes an optimizer reads and writes (planes 1 .. opt_slots(OPT)): Adagrad accumulator = plane 1; Adam m =
 // plane 1, v = plane 2; momentum = plane 1; FTRL accumulator n = plane 1, linear z = plane 2; RMSprop rms = plane 1,
 // then mg if centered, then momentum if momentum > 0 (kRmsprop1 .. kRmsprop3); Adadelta accum_grad = plane 1,
 // accum_var = plane 2; Adamax and Nadam m = plane 1, v = plane 2; ProximalAdagrad accumulator = plane 1;
-// ProximalGradientDescent none; AdagradDA gradient_accumulator = plane 1, gradient_squared_accumulator = plane 2
+// ProximalGradientDescent none; AdagradDA gradient_accumulator = plane 1, gradient_squared_accumulator = plane 2;
+// AdamW m = plane 1, v = plane 2, with AMSGrad vhat = plane 3 (kAdamW3); Lion m = plane 1
 __host__ __device__ constexpr int opt_slots(int opt) {
-  return opt == kRmsprop3 ? 3
+  return opt == kRmsprop3 || opt == kAdamW3 ? 3
          : opt == kAdam || opt == kFtrl || opt == kRmsprop2 || opt == kAdadelta || opt == kAdamax || opt == kNadam ||
-                   opt == kAdagradDa
+                   opt == kAdagradDa || opt == kAdamW2
              ? 2
          : opt == kSgd || opt == kProxSgd ? 0 : 1;
 }
 
-// The per-step scalars beyond OptHyper (host.h StepScalars), the trailing K7 kernel argument: Nadam's; EMPTY for every
-// other optimizer, which keeps their kernels' parameters as they were (like SlotPlanes, ScoreArg and InitArg).
+// the optimizers with a decoupled weight decay (DecayScalars)
+__host__ __device__ constexpr bool opt_decays(int opt) { return opt == kAdamW2 || opt == kAdamW3 || opt == kLion; }
+
+// The per-step scalars beyond OptHyper (host.h StepScalars), the trailing K7 kernel argument: Nadam's schedule, the
+// weight decay of AdamW and Lion; EMPTY for every other optimizer, which keeps their kernels' parameters as they were
+// (like SlotPlanes, ScoreArg and InitArg).
 template <int OPT> struct StepArg {};
-template <> struct StepArg<kNadam> : StepScalars {};
+template <> struct StepArg<kNadam> : NadamScalars {};
+template <> struct StepArg<kAdamW2> : DecayScalars {};
+template <> struct StepArg<kAdamW3> : DecayScalars {};
+template <> struct StepArg<kLion> : DecayScalars {};
 template <int OPT>
 static StepArg<OPT> step_arg(const StepScalars& sx) {
   StepArg<OPT> x{};
-  if constexpr (OPT == kNadam) static_cast<StepScalars&>(x) = sx;
+  if constexpr (OPT == kNadam) static_cast<NadamScalars&>(x) = sx;
+  if constexpr (opt_decays(OPT)) static_cast<DecayScalars&>(x) = sx;
   return x;
 }
+
+// p = p - (p*wd)*lr, Keras' _apply_weight_decay ahead of the AdamW and Lion rules.  wd == 0 (uniform over the launch)
+// skips it, so an inf param does not become NaN.
+__device__ __forceinline__ float decay(float p, const DecayScalars& x) { return x.wd != 0.f ? p - (p * x.wd) * x.lr : p; }
 
 // sign(x) * max(|x| - t, 0), sign(0) = 0: the l1 shrink of TF's proximal and AdagradDA kernels
 __device__ __forceinline__ float shrink(float x, float t) {
@@ -824,9 +837,15 @@ __device__ __forceinline__ void opt_fresh(const OptHyper& h, FVec<VF>& a, FVec<V
     a.fill(h.init_slot);
     if constexpr (opt_slots(OPT) > 1) b.zero();
     if constexpr (opt_slots(OPT) > 2) c.zero();
-  } else if constexpr (OPT == kAdadelta || OPT == kAdamax || OPT == kNadam) {
+  } else if constexpr (OPT == kAdadelta || OPT == kAdamax || OPT == kNadam || OPT == kAdamW2) {
     a.zero();
     b.zero();
+  } else if constexpr (OPT == kAdamW3) {
+    a.zero();
+    b.zero();
+    c.zero();
+  } else if constexpr (OPT == kLion) {
+    a.zero();
   } else if constexpr (OPT == kProxAdagrad) {
     a.fill(h.init_slot);
   } else if constexpr (OPT == kAdagradDa) {
@@ -864,14 +883,25 @@ __device__ __forceinline__ void opt_fresh(const OptHyper& h, FVec<VF>& a, FVec<V
 //   ProximalGD      : lr, eps = l1, beta1 = l2
 //   AdagradDA: lr, eps = l1*gs, beta1 = (l2*gs)*lr, init_slot = initial squared accumulator (gs >= 1, so eps > 0
 //              exactly when l1 > 0)
-// r = 1 - beta1 (RMSprop, Adadelta, Adamax, Nadam) and r2 = 1 - beta2 (Nadam), computed once per step in fp32.
+//   AdamW   : as Adam; the StepArg x: wd, lr (host.h DecayScalars)
+//   Lion    : lr, beta1, beta2; the StepArg x: wd, lr
+// r = 1 - beta1 (RMSprop, Adadelta, Adamax, Nadam, Lion) and r2 = 1 - beta2 (Nadam, Lion), computed once per step in
+// fp32.  AdamW and Lion restate Keras 3's dense update_step after its _apply_weight_decay (AdamW on the dense Adam
+// expressions, DESIGN.md section 4).
 // Adamax and Nadam restate Keras' _resource_apply_sparse; ProximalAdagrad, ProximalGradientDescent and AdagradDA TF1's
 // SparseApplyProximalAdagrad, SparseApplyProximalGradientDescent and SparseApplyAdagradDA (ProximalAdagrad with a
 // correctly rounded square root and one division where TF multiplies by an Eigen rsqrt, DESIGN.md section 4).
 template <int OPT>
 __device__ __forceinline__ void opt_elem(const OptHyper& h, const StepArg<OPT>& x, float r, float r2, float g, float& p,
                                          float& a, float& b, float& c3) {
-  if constexpr (OPT == kNadam) {
+  if constexpr (OPT == kLion) {
+    // a = m.  sign(+-0) = 0, sign(NaN) = NaN
+    p = decay(p, x);
+    const float c = a * h.beta1 + g * r;
+    const float s = c > 0.f ? 1.f : (c < 0.f ? -1.f : (c == 0.f ? 0.f : c));
+    p = p - h.lr * s;
+    a = a * h.beta2 + g * r2;
+  } else if constexpr (OPT == kNadam) {
     // a = m, b = v
     const float gp = g / x.omsn;
     a = a * h.beta1 + g * r;
@@ -958,6 +988,16 @@ __device__ __forceinline__ void opt_step(const OptHyper& h, const StepArg<OPT>& 
     FVec<VF> upd = a;
     upd.zip(b, [&h](float& x, float vv) { x = (x * h.lr) / (sqrtf(vv) + h.eps); });
     p.zip(upd, [](float& pv, float x) { pv = pv - x; });
+  } else if constexpr (OPT == kAdamW2 || OPT == kAdamW3) {
+    // the weight decay, then Adam's expressions; AMSGrad (kAdamW3): vhat = max(vhat, v) takes v's place under the root
+    p.apply([&x](float& pv) { pv = decay(pv, x); });
+    const float omb1 = 1.f - h.beta1, omb2 = 1.f - h.beta2;
+    a.zip(g, [omb1](float& mv, float gv) { mv = mv + (gv - mv) * omb1; });
+    b.zip(g, [omb2](float& vv, float gv) { vv = vv + (gv * gv - vv) * omb2; });
+    if constexpr (OPT == kAdamW3) c.zip(b, [](float& vh, float vv) { vh = fmaxf(vh, vv); });
+    FVec<VF> upd = a;
+    upd.zip(OPT == kAdamW3 ? c : b, [&h](float& x, float vv) { x = (x * h.lr) / (sqrtf(vv) + h.eps); });
+    p.zip(upd, [](float& pv, float x) { pv = pv - x; });
   } else {
     const float* gv = reinterpret_cast<const float*>(&g.v);
     float* pv = reinterpret_cast<float*>(&p.v);
@@ -1005,12 +1045,13 @@ static SlotPlanes<OPT> slot_planes_arg(const det_table* t) {
 // first-bucket loads to reach 4 CTAs per SM; asking for 3 (the register-held Adagrad / Adam kernels' occupancy) keeps
 // them in registers.  RMSprop spills the same way: its 1-plane kernel keeps 3 CTAs per SM, the 3-plane one (three slot
 // vectors in flight) 2.  ProximalAdagrad and AdagradDA (a root and one or two divisions per element, the proximal
-// branch) spill 16 bytes at ptxas' own choice of 4 CTAs per SM; they keep 3.  0 = no minimum, the other optimizers'
-// kernels as before.
+// branch) spill 16 bytes at ptxas' own choice of 4 CTAs per SM; they keep 3, and so does two-plane AdamW (Adam's
+// vectors plus the decay's scalars spill 32 bytes at 4).  0 = no minimum, the other optimizers' kernels as before.
 template <int OPT>
-constexpr int kApplyMinBlocks = OPT == kFtrl || OPT == kRmsprop1 || OPT == kProxAdagrad || OPT == kAdagradDa ? 3
-                                : OPT == kRmsprop3                                                       ? 2
-                                                                                                         : 0;
+constexpr int kApplyMinBlocks =
+    OPT == kFtrl || OPT == kRmsprop1 || OPT == kProxAdagrad || OPT == kAdagradDa || OPT == kAdamW2 ? 3
+    : OPT == kRmsprop3                                                                             ? 2
+                                                                                                   : 0;
 
 // S of a launch: the table's row type T when its slot planes hold that dtype (HALF_SLOTS), else float
 template <typename T, bool HALF_SLOTS>
@@ -2084,19 +2125,46 @@ static det_status adagrad_da_hyper(float lr, float l1, float l2, int64_t gs, flo
   return DET_OK;
 }
 
+// AdamW (AMSGrad when amsgrad != 0, with vhat in plane 3): alpha = lr*sqrt(1 - beta2^t)/(1 - beta1^t) from the caller,
+// as for Adam; lr and weight_decay >= 0 (NaN fails the test) for the decay
+static det_status adamw_hyper(float alpha, float beta1, float beta2, float epsilon, float lr, float weight_decay,
+                              int amsgrad, OptHyper* h, StepScalars* sx, int* opt) {
+  if (!(weight_decay >= 0.f)) return fail(DET_INVALID_ARGUMENT, "det_apply_adamw: weight_decay must be >= 0");
+  h->lr = alpha; h->eps = epsilon; h->beta1 = beta1; h->beta2 = beta2; h->init_slot = 0.f;
+  sx->wd = weight_decay; sx->lr = lr;
+  *opt = amsgrad ? kAdamW3 : kAdamW2;
+  return DET_OK;
+}
+
+// Lion: betas in [0, 1] and weight_decay >= 0 (NaN fails each test)
+static det_status lion_hyper(float lr, float beta1, float beta2, float weight_decay, OptHyper* h, StepScalars* sx,
+                             int* opt) {
+  if (!(beta1 >= 0.f && beta1 <= 1.f) || !(beta2 >= 0.f && beta2 <= 1.f))
+    return fail(DET_INVALID_ARGUMENT, "det_apply_lion: beta1 and beta2 must be in [0, 1]");
+  if (!(weight_decay >= 0.f)) return fail(DET_INVALID_ARGUMENT, "det_apply_lion: weight_decay must be >= 0");
+  h->lr = lr; h->eps = 0.f; h->beta1 = beta1; h->beta2 = beta2; h->init_slot = 0.f;
+  sx->wd = weight_decay; sx->lr = lr;
+  *opt = kLion;
+  return DET_OK;
+}
+
 // det_table::slot_init, the slot values of a key created by insert / accum and never stepped: the initial accumulator
 // of Adagrad, FTRL and ProximalAdagrad (FTRL's z: 0), 0 for momentum, RMSprop's initial rms (its mg and momentum: 0),
-// 0 for both Adadelta, Adamax and Nadam planes, AdagradDA's 0 and initial squared accumulator; Adam, plain SGD and
-// ProximalGradientDescent leave them as they are.  Every optimizer entry point records them before it takes the table
-// lock.
+// 0 for both Adadelta, Adamax and Nadam planes, AdagradDA's 0 and initial squared accumulator, 0 for every AdamW and
+// Lion plane; Adam, plain SGD and ProximalGradientDescent leave them as they are.  Every optimizer entry point records
+// them before it takes the table lock.
 static void record_slot_init(det_table* t, int opt, const OptHyper& h) {
   if (!t) return;
   if (opt == kAdagrad || opt == kFtrl || (opt >= kRmsprop1 && opt <= kRmsprop3) || opt == kProxAdagrad)
     t->slot_init[1] = h.init_slot;
-  if (opt == kMomentum || opt == kAdadelta || opt == kAdamax || opt == kNadam || opt == kAdagradDa) t->slot_init[1] = 0.f;
-  if (opt == kFtrl || opt == kRmsprop2 || opt == kAdadelta || opt == kAdamax || opt == kNadam) t->slot_init[2] = 0.f;
+  if (opt == kMomentum || opt == kAdadelta || opt == kAdamax || opt == kNadam || opt == kAdagradDa || opt_decays(opt))
+    t->slot_init[1] = 0.f;
+  if (opt == kFtrl || opt == kRmsprop2 || opt == kAdadelta || opt == kAdamax || opt == kNadam || opt == kAdamW2 ||
+      opt == kAdamW3)
+    t->slot_init[2] = 0.f;
   if (opt == kAdagradDa) t->slot_init[2] = h.init_slot;
   if (opt == kRmsprop3) t->slot_init[2] = t->slot_init[3] = 0.f;
+  if (opt == kAdamW3) t->slot_init[3] = 0.f;
 }
 
 }  // namespace det
@@ -2255,7 +2323,7 @@ det_status det_lookup_sparse_clip(det_table* t, const int64_t* ids, const int32_
 
 // n_dev (nullable): the key count lives on the device (det_apply_*_dup); n is then its upper bound -- room is reserved
 // for n NEW keys (the unique keys themselves are not read by the host path) and only the staged kernels support it
-// sx: the step scalars beyond h (Nadam; ignored by the other optimizers)
+// sx: the step scalars beyond h (Nadam, AdamW, Lion; ignored by the other optimizers)
 static det_status apply_common(det_table* t, const int64_t* keys, const float* grads, size_t n, OptHyper h,
                                const float* init_param, int full_init, int opt, cudaStream_t s,
                                const long long* n_dev = nullptr, const StepScalars& sx = StepScalars()) {
@@ -2450,6 +2518,28 @@ det_status det_apply_adagrad_da(det_table* t, const int64_t* keys, const float* 
   if (det_status st = adagrad_da_hyper(lr, l1, l2, global_step, init_gg, &h, &opt)) return st;
   record_slot_init(t, opt, h);
   return apply_common(t, keys, grads, n, h, init_param, full_size_init, opt, (cudaStream_t)stream);
+}
+
+det_status det_apply_adamw(det_table* t, const int64_t* keys, const float* grads, size_t n, float alpha, float beta1,
+                           float beta2, float epsilon, float lr, float weight_decay, int amsgrad, const float* init_param,
+                           int full_size_init, det_stream_t stream) {
+  OptHyper h;
+  StepScalars sx;
+  int opt;
+  if (det_status st = adamw_hyper(alpha, beta1, beta2, epsilon, lr, weight_decay, amsgrad, &h, &sx, &opt)) return st;
+  record_slot_init(t, opt, h);
+  return apply_common(t, keys, grads, n, h, init_param, full_size_init, opt, (cudaStream_t)stream, nullptr, sx);
+}
+
+det_status det_apply_lion(det_table* t, const int64_t* keys, const float* grads, size_t n, float lr, float beta1,
+                          float beta2, float weight_decay, const float* init_param, int full_size_init,
+                          det_stream_t stream) {
+  OptHyper h;
+  StepScalars sx;
+  int opt;
+  if (det_status st = lion_hyper(lr, beta1, beta2, weight_decay, &h, &sx, &opt)) return st;
+  record_slot_init(t, opt, h);
+  return apply_common(t, keys, grads, n, h, init_param, full_size_init, opt, (cudaStream_t)stream, nullptr, sx);
 }
 
 size_t det_partition_workspace_bytes(size_t n, int num_shards) {
@@ -2904,6 +2994,31 @@ det_status det_apply_adagrad_da_dup(det_table* t, const int64_t* ids, const floa
   return apply_dup(t, ids, grads, n, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out, (cudaStream_t)stream);
 }
 
+det_status det_apply_adamw_dup(det_table* t, const int64_t* ids, const float* grads, size_t n, float alpha, float beta1,
+                               float beta2, float epsilon, float lr, float weight_decay, int amsgrad,
+                               const float* init_param, void* workspace, size_t workspace_bytes,
+                               int64_t* n_unique_dev_out, det_stream_t stream) {
+  OptHyper h;
+  StepScalars sx;
+  int opt;
+  if (det_status st = adamw_hyper(alpha, beta1, beta2, epsilon, lr, weight_decay, amsgrad, &h, &sx, &opt)) return st;
+  record_slot_init(t, opt, h);
+  return apply_dup(t, ids, grads, n, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out, (cudaStream_t)stream,
+                   nullptr, nullptr, sx);
+}
+
+det_status det_apply_lion_dup(det_table* t, const int64_t* ids, const float* grads, size_t n, float lr, float beta1,
+                              float beta2, float weight_decay, const float* init_param, void* workspace,
+                              size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream) {
+  OptHyper h;
+  StepScalars sx;
+  int opt;
+  if (det_status st = lion_hyper(lr, beta1, beta2, weight_decay, &h, &sx, &opt)) return st;
+  record_slot_init(t, opt, h);
+  return apply_dup(t, ids, grads, n, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out, (cudaStream_t)stream,
+                   nullptr, nullptr, sx);
+}
+
 det_status det_apply_adagrad_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
                                     size_t nnz, size_t batch, int combiner, const float* gout, float lr, float epsilon,
                                     const float* init_param, float init_accum, void* workspace, size_t workspace_bytes,
@@ -3050,6 +3165,35 @@ det_status det_apply_adagrad_da_sparse(det_table* t, const int64_t* ids, const i
   const SparseSrc sp{segment_ids, weights, batch, combiner};
   return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
                    (cudaStream_t)stream, nullptr, &sp);
+}
+
+det_status det_apply_adamw_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
+                                  size_t nnz, size_t batch, int combiner, const float* gout, float alpha, float beta1,
+                                  float beta2, float epsilon, float lr, float weight_decay, int amsgrad,
+                                  const float* init_param, void* workspace, size_t workspace_bytes,
+                                  int64_t* n_unique_dev_out, det_stream_t stream) {
+  OptHyper h;
+  StepScalars sx;
+  int opt;
+  if (det_status st = adamw_hyper(alpha, beta1, beta2, epsilon, lr, weight_decay, amsgrad, &h, &sx, &opt)) return st;
+  record_slot_init(t, opt, h);
+  const SparseSrc sp{segment_ids, weights, batch, combiner};
+  return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
+                   (cudaStream_t)stream, nullptr, &sp, sx);
+}
+
+det_status det_apply_lion_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
+                                 size_t nnz, size_t batch, int combiner, const float* gout, float lr, float beta1,
+                                 float beta2, float weight_decay, const float* init_param, void* workspace,
+                                 size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream) {
+  OptHyper h;
+  StepScalars sx;
+  int opt;
+  if (det_status st = lion_hyper(lr, beta1, beta2, weight_decay, &h, &sx, &opt)) return st;
+  record_slot_init(t, opt, h);
+  const SparseSrc sp{segment_ids, weights, batch, combiner};
+  return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
+                   (cudaStream_t)stream, nullptr, &sp, sx);
 }
 
 }  // extern "C"

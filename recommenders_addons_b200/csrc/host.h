@@ -285,10 +285,10 @@ det_status import_plane_rows(det_table* t, int plane, const int64_t* keys, const
                              cudaStream_t s);
 // fused.cu: the optimizers of the fused find-or-insert step (K7, its template parameter OPT) and their
 // hyper-parameters.  What each OptHyper field holds depends on the optimizer (listed at opt_step); only the builders
-// (adagrad_hyper .. adagrad_da_hyper) fill them.  RMSprop has one id per slot-plane count (kRmsprop1 .. kRmsprop3):
-// the count is a compile-time property of a K7 instantiation.
+// (adagrad_hyper .. lion_hyper) fill them.  RMSprop has one id per slot-plane count (kRmsprop1 .. kRmsprop3), and so
+// has AdamW (kAdamW2, kAdamW3 with AMSGrad's vhat): the count is a compile-time property of a K7 instantiation.
 enum : int { kAdagrad, kAdam, kSgd, kMomentum, kFtrl, kRmsprop1, kRmsprop2, kRmsprop3, kAdadelta, kAdamax, kNadam,
-             kProxAdagrad, kProxSgd, kAdagradDa, kNumOpts };
+             kProxAdagrad, kProxSgd, kAdagradDa, kAdamW2, kAdamW3, kLion, kNumOpts };
 // OptHyper::flags (RMSprop only; 0 for the other optimizers)
 enum : unsigned { kEpsInSqrt = 1u, kCentered = 2u };
 struct OptHyper {
@@ -298,16 +298,24 @@ struct OptHyper {
   float init_slot;
   unsigned flags = 0;   // fills what was the struct's tail padding before an 8-byte kernel parameter
 };
-// Per-step scalars that do not fit OptHyper: Nadam's momentum schedule and bias correction (nadam_hyper fills them;
-// zero and unused for every other optimizer).  K7 receives them as a trailing kernel argument that is empty for every
-// other optimizer (StepArg, fused.cu), so OptHyper and the other kernels' parameters stay as they are.
-struct StepScalars {
+// Per-step scalars that do not fit OptHyper (zero and unused for the optimizers that do not take them).  K7 receives
+// the ones its optimizer takes as a trailing kernel argument that is empty for every other optimizer (StepArg,
+// fused.cu), so OptHyper and the other kernels' parameters stay as they are.
+// Nadam's momentum schedule and bias correction (nadam_hyper fills them)
+struct NadamScalars {
   float omsn = 0.f;   // 1 - m_schedule_new
   float omsx = 0.f;   // 1 - m_schedule_next
   float omt = 0.f;    // 1 - u_t
   float mt1 = 0.f;    // u_{t+1}
   float vden = 0.f;   // 1 - beta2^t
 };
+// AdamW's and Lion's decoupled weight decay p = p - (p*wd)*lr before the step, none when wd == 0 (adamw_hyper and
+// lion_hyper fill them)
+struct DecayScalars {
+  float wd = 0.f;
+  float lr = 0.f;
+};
+struct StepScalars : NadamScalars, DecayScalars {};
 // validate the hyper-parameters, fill *h and set *opt
 det_status adagrad_hyper(float lr, float epsilon, float init_accum, OptHyper* h, int* opt);
 det_status adam_hyper(float alpha, float beta1, float beta2, float epsilon, OptHyper* h, int* opt);

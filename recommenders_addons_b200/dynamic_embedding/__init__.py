@@ -10,8 +10,8 @@ from .keyed_init import KeyedRandomNormal, KeyedRandomUniform, KeyedTruncatedNor
 from .ops import (SparseIds, SparseLookupTrainable, embedding_lookup_sparse, safe_embedding_lookup_sparse,
                   trainable_embedding_lookup_sparse)
 from .optimizer import (ComposedOptimizer, DynamicEmbeddingOptimizer, FusedAdadelta, FusedAdagrad, FusedAdagradDA,
-                        FusedAdam, FusedAdamax, FusedFtrl, FusedNadam, FusedProximalAdagrad, FusedProximalGradientDescent,
-                        FusedRMSprop, FusedSGD, SlotPlane)
+                        FusedAdam, FusedAdamax, FusedAdamW, FusedFtrl, FusedLion, FusedNadam, FusedProximalAdagrad,
+                        FusedProximalGradientDescent, FusedRMSprop, FusedSGD, SlotPlane)
 from .restrict_policies import FrequencyRestrictPolicy, RestrictPolicy, TimestampRestrictPolicy
 from .sharded import PeerShardedVariable, ShardedVariable
 from . import layers
@@ -24,7 +24,7 @@ __all__ = [
     "CuckooHashTable", "CuckooHashTableConfig", "CuckooHashTableCreator", "HkvEvictStrategy", "HkvHashTable", "HkvHashTableConfig",
     "HkvHashTableCreator", "KVCreator", "Variable", "default_partition_fn", "embedding_lookup",
     "embedding_lookup_unique", "get_variable", "unique", "segment_reduce", "SparseIds", "embedding_lookup_sparse",
-    "safe_embedding_lookup_sparse", "DynamicEmbeddingOptimizer", "FusedAdagrad", "FusedAdam", "FusedSGD", "FusedFtrl", "FusedRMSprop", "FusedAdadelta", "FusedAdamax", "FusedNadam", "FusedProximalAdagrad", "FusedProximalGradientDescent", "FusedAdagradDA", "ShardedVariable", "PeerShardedVariable", "layers",
+    "safe_embedding_lookup_sparse", "DynamicEmbeddingOptimizer", "FusedAdagrad", "FusedAdam", "FusedSGD", "FusedFtrl", "FusedRMSprop", "FusedAdadelta", "FusedAdamax", "FusedNadam", "FusedProximalAdagrad", "FusedProximalGradientDescent", "FusedAdagradDA", "FusedAdamW", "FusedLion", "ShardedVariable", "PeerShardedVariable", "layers",
     "RestrictPolicy", "TimestampRestrictPolicy", "FrequencyRestrictPolicy", "TrainableWrapper", "ModelMode",
     "enable_inference_mode", "enable_train_mode", "get_model_mode", "trainable_wrapper_filter", "shadow_ops",
     "ComposedOptimizer", "SlotPlane", "math", "data_flow", "keras", "GraphKeys", "FileSystemSaver", "FileSystemSaverConfig", "DynamicEmbeddingSaver",

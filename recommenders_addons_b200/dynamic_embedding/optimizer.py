@@ -271,19 +271,32 @@ class FusedAdagrad(_FusedBase):
                                                    _stream_ptr(table.device)))
 
 
-class FusedAdam(_FusedBase):
-  """TF Adam: m += (g-m)(1-b1); v += (g*g-v)(1-b2); var -= m*alpha/(sqrt(v)+eps) with
-  alpha = lr*sqrt(1-b2^t)/(1-b1^t) (fp32, like ApplyAdam)."""
+class _AdamFamily(_FusedBase):
+  """The state, step scalars and C calls FusedAdam and FusedAdamW share.  They are siblings rather than parent and
+  child, so `isinstance(o, FusedAdam)` never matches AdamW's rule."""
   n_slots = 2
-  opt_name = "Adam"
   slot_plane_names = ("m", "v")
+  weight_decay = 0.0
 
-  def __init__(self, learning_rate=0.001, beta_1=0.9, beta_2=0.999, epsilon=1e-8):
+  def __init__(self, learning_rate, beta_1, beta_2, epsilon, amsgrad):
     super().__init__()
     self.learning_rate = float(learning_rate)
     self.beta_1 = float(beta_1)
     self.beta_2 = float(beta_2)
     self.epsilon = float(epsilon)
+    self.amsgrad = bool(amsgrad)
+    if self.amsgrad:
+      self.n_slots = 3
+      self.slot_plane_names = ("m", "v", "vhat")
+
+  def _steps_adamw(self):
+    """whether the step is det_apply_adamw's (AMSGrad, or AdamW's weight decay) rather than det_apply_adam's"""
+    return self.amsgrad
+
+  def _adamw_hyper(self):
+    """det_apply_adamw's scalars between the gradients and init_param"""
+    return (self.alpha(), self.beta_1, self.beta_2, self.epsilon, self.learning_rate, self.weight_decay,
+            int(self.amsgrad))
 
   def alpha(self):
     f = np.float32
@@ -294,20 +307,51 @@ class FusedAdam(_FusedBase):
   def _apply_table(self, params, table, keys, grads):
     n = keys.numel()
     init, full = _init_rows(params, n, table.device)
+    if self._steps_adamw():
+      _lib.check(_lib.lib().det_apply_adamw(table.handle, _ptr(keys), _ptr(grads), n, *self._adamw_hyper(), _ptr(init),
+                                            full, _stream_ptr(table.device)))
+      return
     _lib.check(_lib.lib().det_apply_adam(table.handle, _ptr(keys), _ptr(grads), n, self.alpha(), self.beta_1,
                                          self.beta_2, self.epsilon, _ptr(init), full, _stream_ptr(table.device)))
 
 
   def _apply_table_dup(self, table, ids, grads, n, init, ws):
+    if self._steps_adamw():
+      _lib.check(_lib.lib().det_apply_adamw_dup(table.handle, _ptr(ids), _ptr(grads), n, *self._adamw_hyper(), _ptr(init),
+                                                _ptr(ws), ws.numel(), None, _stream_ptr(table.device)))
+      return
     _lib.check(_lib.lib().det_apply_adam_dup(table.handle, _ptr(ids), _ptr(grads), n, self.alpha(), self.beta_1, self.beta_2,
                                              self.epsilon, _ptr(init), _ptr(ws), ws.numel(), None,
                                              _stream_ptr(table.device)))
 
   def _apply_table_sparse(self, table, h, gout, init, ws):
+    if self._steps_adamw():
+      _lib.check(_lib.lib().det_apply_adamw_sparse(table.handle, _ptr(h.ids), _ptr(h.segment_ids), _ptr(h.weights),
+                                                   h.ids.numel(), h.batch, _lib.COMBINERS[h.combiner], _ptr(gout),
+                                                   *self._adamw_hyper(), _ptr(init), _ptr(ws), ws.numel(), None,
+                                                   _stream_ptr(table.device)))
+      return
     _lib.check(_lib.lib().det_apply_adam_sparse(table.handle, _ptr(h.ids), _ptr(h.segment_ids), _ptr(h.weights),
                                                 h.ids.numel(), h.batch, _lib.COMBINERS[h.combiner], _ptr(gout),
                                                 self.alpha(), self.beta_1, self.beta_2, self.epsilon, _ptr(init), _ptr(ws),
                                                 ws.numel(), None, _stream_ptr(table.device)))
+
+
+class FusedAdam(_AdamFamily):
+  """TF Adam: m += (g-m)(1-b1); v += (g*g-v)(1-b2); var -= m*alpha/(sqrt(v)+eps) with
+  alpha = lr*sqrt(1-b2^t)/(1-b1^t) (fp32, like ApplyAdam).  amsgrad=True is Keras' AMSGrad: vhat = max(vhat, v) takes
+  v's place under the root, in a third slot "vhat" starting at 0 (det_apply_adamw with weight_decay 0).
+  torch.optim.Adam(amsgrad=True) adds epsilon after the bias correction of sqrt(vhat), a different rounding, and
+  DynamicEmbeddingOptimizer leaves it on the composed path."""
+  opt_name = "Adam"
+
+  def __init__(self, learning_rate=0.001, beta_1=0.9, beta_2=0.999, epsilon=1e-8, amsgrad=False):
+    super().__init__(learning_rate, beta_1, beta_2, epsilon, amsgrad)
+
+
+def _check_weight_decay(weight_decay):
+  if not weight_decay >= 0:
+    raise ValueError("weight_decay must be >= 0, got %r" % (weight_decay,))
 
 
 class FusedSGD(_FusedBase):
@@ -722,6 +766,63 @@ class FusedAdagradDA(_FusedBase):
                                                       ws.numel(), None, _stream_ptr(table.device)))
 
 
+class FusedAdamW(_AdamFamily):
+  """Keras AdamW on dynamic-embedding rows (tf.keras.optimizers.AdamW, Keras 3's dense update_step): first the weight
+  decay var -= (var*wd)*lr (none when wd == 0), then FusedAdam's rule, AMSGrad's with amsgrad=True.  Slots: "m", "v"
+  and, with amsgrad, "vhat", all starting at 0.  With weight_decay=0 and amsgrad=False it is FusedAdam bit for bit.
+  torch.optim.AdamW decays by var*(1 - lr*wd) and places epsilon after the bias correction of sqrt(v), a different
+  rule: DynamicEmbeddingOptimizer(torch.optim.AdamW(...)) stays on the composed path."""
+  opt_name = "AdamW"
+
+  def __init__(self, learning_rate=0.001, weight_decay=0.004, beta_1=0.9, beta_2=0.999, epsilon=1e-7, amsgrad=False):
+    _check_weight_decay(weight_decay)
+    super().__init__(learning_rate, beta_1, beta_2, epsilon, amsgrad)
+    self.weight_decay = float(weight_decay)
+
+  def _steps_adamw(self):
+    return True
+
+
+class FusedLion(_FusedBase):
+  """Keras Lion on dynamic-embedding rows (tf.keras.optimizers.Lion, Keras 3's dense update_step): the weight decay
+  var -= (var*wd)*lr when weight_decay is set, then c = m*b1 + g*(1-b1); var -= lr*sign(c); m = m*b2 + g*(1-b2), with
+  sign(0) = 0 and sign(NaN) = NaN.  Slot: "m", starting at 0."""
+  n_slots = 1
+  opt_name = "Lion"
+  slot_plane_names = ("m",)
+
+  def __init__(self, learning_rate=1e-4, beta_1=0.9, beta_2=0.99, weight_decay=None):
+    super().__init__()
+    for name, b in (("beta_1", beta_1), ("beta_2", beta_2)):
+      if not 0 <= b <= 1:
+        raise ValueError("%s must be in [0, 1], got %r" % (name, b))
+    weight_decay = 0.0 if weight_decay is None else weight_decay
+    _check_weight_decay(weight_decay)
+    self.learning_rate = float(learning_rate)
+    self.beta_1 = float(beta_1)
+    self.beta_2 = float(beta_2)
+    self.weight_decay = float(weight_decay)
+
+  def _hyper(self):
+    return (self.learning_rate, self.beta_1, self.beta_2, self.weight_decay)
+
+  def _apply_table(self, params, table, keys, grads):
+    n = keys.numel()
+    init, full = _init_rows(params, n, table.device)
+    _lib.check(_lib.lib().det_apply_lion(table.handle, _ptr(keys), _ptr(grads), n, *self._hyper(), _ptr(init), full,
+                                         _stream_ptr(table.device)))
+
+  def _apply_table_dup(self, table, ids, grads, n, init, ws):
+    _lib.check(_lib.lib().det_apply_lion_dup(table.handle, _ptr(ids), _ptr(grads), n, *self._hyper(), _ptr(init),
+                                             _ptr(ws), ws.numel(), None, _stream_ptr(table.device)))
+
+  def _apply_table_sparse(self, table, h, gout, init, ws):
+    _lib.check(_lib.lib().det_apply_lion_sparse(table.handle, _ptr(h.ids), _ptr(h.segment_ids), _ptr(h.weights),
+                                                h.ids.numel(), h.batch, _lib.COMBINERS[h.combiner], _ptr(gout),
+                                                *self._hyper(), _ptr(init), _ptr(ws), ws.numel(), None,
+                                                _stream_ptr(table.device)))
+
+
 class ComposedOptimizer(object):
   """ANY torch.optim optimizer on dynamic-embedding rows, the way the reference patches a stock optimizer
   (dynamic_embedding_optimizer.py:137-204 `apply_grad_to_update_var`, :870-958 `create_slots`): per step and per
@@ -730,8 +831,9 @@ class ComposedOptimizer(object):
   write param and slots back (`TrainableWrapper.update_op`, embedding_weights.py:434-444).  Table passes per step:
   (1 + slots) finds + (1 + slots) upserts, all through the validated table kernels; Adagrad / Adam have the fused
   single-kernel path (FusedAdagrad / FusedAdam), which DynamicEmbeddingOptimizer picks by default.  SGD, momentum,
-  FTRL, RMSprop, Adadelta, Adamax and Nadam have fused steps too (FusedSGD / FusedFtrl / FusedRMSprop / FusedAdadelta /
-  FusedAdamax / FusedNadam), used when passed explicitly.
+  FTRL, RMSprop, Adadelta, Adamax, Nadam, AdamW, AMSGrad and Lion have fused steps too (FusedSGD / FusedFtrl /
+  FusedRMSprop / FusedAdadelta / FusedAdamax / FusedNadam / FusedAdamW / FusedAdam(amsgrad=True) / FusedLion), used
+  when passed explicitly.
 
   A key without slot state starts from the state a fresh torch optimizer gives a new parameter (zeros; Adagrad's
   `sum` from initial_accumulator_value) -- the reference's slot initializers.  State that is not per row (`step`,
@@ -873,7 +975,9 @@ def DynamicEmbeddingOptimizer(self, bp_v2=False, synchronous=False, fused=True, 
   (dynamic_embedding_optimizer.py:103).  Accepts a FusedAdagrad/FusedAdam (returned unchanged) or any
   torch.optim.Optimizer instance: Adagrad / Adam are carried over to the fused single-kernel path (fused=True, the
   default); every other optimizer -- or fused=False -- gets the reference's composed find -> dense rule -> upsert
-  path (ComposedOptimizer)."""
+  path (ComposedOptimizer).  torch.optim.AdamW and Adam(amsgrad=True) are composed too: torch's rules differ from
+  Keras' (decay by var*(1 - lr*wd), epsilon added after the bias correction of the root); de.FusedAdamW
+  and de.FusedAdam(amsgrad=True) are Keras' and are opted into explicitly."""
   if isinstance(self, (_FusedBase, ComposedOptimizer)):
     return self
   if fused and type(self) is torch.optim.Adagrad:

@@ -454,6 +454,12 @@ class PeerShardedVariable(object):
     gradient sum -> fused optimizer, every count on the device (no host synchronisation, no inbox round trip)"""
     import ctypes
     from .optimizer import FusedAdagrad, FusedAdam
+    # the owner-side exchange step has the Adagrad and Adam rules only: AMSGrad, AdamW and the other optimizers are
+    # refused, before any state changes, rather than run as another rule
+    adagrad = isinstance(optimizer, FusedAdagrad)
+    if not adagrad and not (isinstance(optimizer, FusedAdam) and not optimizer.amsgrad):
+      raise TypeError("PeerShardedVariable.apply_gradients: de.FusedAdagrad / de.FusedAdam (without amsgrad), got %s" %
+                      type(optimizer).__name__)
     flat = keys.reshape(-1).contiguous()
     g = grads.reshape(-1, self.dim).to(torch.float32).contiguous()
     need = int(self._lib.det_peer_xchg_apply_workspace_bytes(self._g))
@@ -465,16 +471,14 @@ class PeerShardedVariable(object):
     init = self._default.to(self.device).contiguous()
     p = lambda t: ctypes.c_void_p(t.data_ptr()) if t.numel() else None
     optimizer.iterations += 1
-    if isinstance(optimizer, FusedAdagrad):
+    if adagrad:
       self._libmod.check(self._lib.det_peer_xchg_apply_adagrad(self._g, p(flat), p(g), flat.numel(), optimizer.learning_rate,
                                                                optimizer.epsilon, p(init), optimizer.initial_accumulator_value,
                                                                p(ws), ws.numel(), self._sp()))
-    elif isinstance(optimizer, FusedAdam):
+    else:
       self._libmod.check(self._lib.det_peer_xchg_apply_adam(self._g, p(flat), p(g), flat.numel(), optimizer.alpha(),
                                                             optimizer.beta_1, optimizer.beta_2, optimizer.epsilon, p(init),
                                                             p(ws), ws.numel(), self._sp()))
-    else:
-      raise TypeError("PeerShardedVariable.apply_gradients: de.FusedAdagrad / de.FusedAdam")
 
   def size(self):
     if self._group is None and self.world > 1 and all(t is not None for t in self._tables):

@@ -14,10 +14,16 @@ rows.  Timed with CUDA events, in rounds that alternate the dtype order, median 
   * adamax, nadam, proxada, proxsgd, adagrad_da (the proximal and DA ones with l1, l2 > 0) -- det_apply_* on 2^20 unique
     resident keys of two more two-plane variables (fp32, bf16), made after the variables above are released; each one's
     _dup form at the c3 backward shape; and the composed torch.optim.Adamax / NAdam next to FusedAdamax / FusedNadam on
-    one more fp32 variable of --composed-resident rows (torch's Adamax is another rule: eps inside the max).
+    one more fp32 variable of --composed-resident rows (torch's Adamax is another rule: eps inside the max);
+  * adamw (weight decay 0.004), amsgrad (AdamW with AMSGrad, 3 slot planes), lion (weight decay 0.1) -- det_apply_adamw
+    / det_apply_lion on 2^20 unique resident keys of two more three-plane variables (fp32, bf16), made after the
+    variables above are released, next to their plane-count twins on the same variables in the same rounds (twin_adam,
+    twin_rmsprop_cm, twin_momentum: the same streams per key); each new one's _dup form at the c3 backward shape; and
+    the composed torch.optim.AdamW next to FusedAdamW on one more fp32 variable of --composed-resident rows (torch's
+    AdamW is another rule: decay by p*(1 - lr*wd), epsilon after the bias correction).
 Before the timing, the first step of each new optimizer on a sample of its keys (rows written by insert, no slot state
 yet) is checked bit for bit against tests/optimizer_oracle.py (RMSprop and Adadelta: tests/rmsprop_adadelta_oracle.py;
-the last five: tests/adamax_nadam_prox_oracle.py):
+Adamax to AdagradDA: tests/adamax_nadam_prox_oracle.py; AdamW, AMSGrad and Lion: tests/adamw_lion_oracle.py):
 params of both dtypes (bf16: the fp32 result rounded).
 
 Bytes per key are what the unique-key step must move at dim 64: key 8 + probed bucket 64 + fp32 gradient 256 + param
@@ -46,7 +52,8 @@ N_DUP = 26 * 65536
 N_SAMPLE = 1 << 16
 SLOTS = {"sgd": 0, "momentum": 1, "ftrl": 2, "adagrad": 1, "adam": 2,
          "rmsprop": 1, "rmsprop_c": 2, "rmsprop_m": 2, "rmsprop_cm": 3, "adadelta": 2,
-         "adamax": 2, "nadam": 2, "proxada": 1, "proxsgd": 0, "adagrad_da": 2}
+         "adamax": 2, "nadam": 2, "proxada": 1, "proxsgd": 0, "adagrad_da": 2,
+         "adamw": 2, "amsgrad": 3, "lion": 1, "twin_adam": 2, "twin_rmsprop_cm": 3, "twin_momentum": 1}
 RMS = {"rmsprop": (0.0, 0), "rmsprop_c": (0.0, 1), "rmsprop_m": (0.9, 0), "rmsprop_cm": (0.9, 1)}   # momentum, centered
 FTRL = dict(lr=0.05, l1=0.001, l2=0.01, l2_shrinkage=0.0)
 
@@ -212,6 +219,8 @@ def main():
   res.update(rmsprop_adadelta_arms(args, lib, de, P, dev, gen, dts, fill, timed, mismatches))
   torch.cuda.empty_cache()
   res.update(adamax_nadam_prox_arms(args, lib, de, P, dev, gen, dts, fill, timed, mismatches))
+  torch.cuda.empty_cache()
+  res.update(adamw_lion_arms(args, lib, de, P, dev, gen, dts, fill, timed, mismatches))
   print(json.dumps({"metric": "fused optimizer step ms per call (median of rounds, CUDA events)", "card": info,
                     "resident": R, "dim": DIM, "rounds": args.rounds, "calls": args.calls,
                     "datasheet_hbm_TB_s": DATASHEET_HBM_BPS / 1e12, "oracle_mismatches": mismatches, "shapes": res}))
@@ -398,6 +407,115 @@ def adamax_nadam_prox_arms(args, lib, de, P, dev, gen, dts, fill, timed, mismatc
     res["composed_vs_fused_fp32_" + o] = {"resident": Rc, "keys": N_UNIQUE, "composed_is": type(comp).__name__,
                                           "composed_ms": round(float(np.median(mc[(o, "composed")])), 4),
                                           "fused_ms": round(float(np.median(mc[(o, "fused")])), 4)}
+  for v in list(v2.values()) + [small]:   # released before the next arms' variables
+    for t in v.tables:
+      t.close()
+  return res
+
+
+def adamw_lion_arms(args, lib, de, P, dev, gen, dts, fill, timed, mismatches):
+  """AdamW, AMSGrad and Lion on their own three-plane variables next to their plane-count twins (Adam, centered
+  RMSprop with momentum, momentum SGD), the new ones' _dup step at the c3 shape, and the composed torch AdamW next to
+  FusedAdamW"""
+  from oracle import oracle as O
+  from recommenders_addons_b200 import _lib
+  from tests import adamw_lion_oracle as WL
+  new = ("adamw", "amsgrad", "lion")
+  twins = ("twin_adam", "twin_rmsprop_cm", "twin_momentum")
+  shapes = new + twins
+  R = max(args.resident, (len(shapes) + len(new)) * N_UNIQUE)
+  v3 = {n: de.Variable(value_dtype=dt, dim=DIM, init_size=2 * R, initializer=0.0, name="fob6_" + n, num_slot_planes=3)
+        for n, dt in dts.items()}
+  fill(list(v3.values()), R)
+  part = R // (len(shapes) + len(new))
+  keys = {o: mix_keys(i * part + torch.randperm(part, device=dev, generator=gen)[:N_UNIQUE]) for i, o in enumerate(shapes)}
+  zipf = np.random.default_rng(6).zipf(1.2, N_DUP) - 1
+  ids_dup = {o: mix_keys((len(shapes) + i) * part + torch.as_tensor(zipf % part, device=dev)) for i, o in enumerate(new)}
+  g_uni = torch.randn(N_UNIQUE, DIM, device=dev, generator=gen) * 0.01
+  g_dup = torch.randn(N_DUP, DIM, device=dev, generator=gen) * 0.01
+  init = torch.zeros(DIM, device=dev)
+  wsb = int(lib.det_apply_dup_workspace_bytes(N_DUP, DIM))
+  ws = torch.empty(wsb + 256, dtype=torch.uint8, device=dev)
+  ws = ws[(-ws.data_ptr()) % 256:][:wsb]
+  adamw, ams, lion = de.FusedAdamW(0.001), de.FusedAdamW(0.001, amsgrad=True), de.FusedLion(1e-4, weight_decay=0.1)
+  adamw.iterations = ams.iterations = 1
+  hyper = {"adamw": ("adamw", adamw._adamw_hyper()), "amsgrad": ("adamw", ams._adamw_hyper()),
+           "lion": ("lion", lion._hyper())}
+  alpha = float(O.adam_scalars(0.001, 0.9, 0.999, 1))
+
+  def step(name, shape, k=None, g=None, n=N_UNIQUE, dup=False):
+    h = v3[name].tables[0].handle
+    if dup:
+      c, a = hyper[shape]
+      _lib.check(getattr(lib, "det_apply_%s_dup" % c)(h, P(ids_dup[shape]), P(g_dup), N_DUP, *a, P(init), P(ws), wsb,
+                                                      None, None))
+      return
+    k = keys[shape] if k is None else k
+    g = g_uni if g is None else g
+    if shape == "twin_adam":
+      st = lib.det_apply_adam(h, P(k), P(g), n, alpha, 0.9, 0.999, 1e-7, P(init), 0, None)
+    elif shape == "twin_rmsprop_cm":
+      st = lib.det_apply_rmsprop(h, P(k), P(g), n, 0.001, 0.9, 0.9, 1e-7, 1, 1, P(init), 0, 0.0, None)
+    elif shape == "twin_momentum":
+      st = lib.det_apply_sgd(h, P(k), P(g), n, 0.01, 0.9, 0, P(init), 0, None)
+    else:
+      c, a = hyper[shape]
+      st = getattr(lib, "det_apply_" + c)(h, P(k), P(g), n, *a, P(init), 0, None)
+    _lib.check(st)
+
+  for shape in new:
+    k = keys[shape][:N_SAMPLE].contiguous()
+    g = g_uni[:N_SAMPLE].contiguous()
+    bad = 0
+    for name, dt in dts.items():
+      p0 = v3[name].lookup(k).float().cpu().numpy()
+      step(name, shape, k, g, N_SAMPLE)
+      got = v3[name].lookup(k).float().cpu().numpy()
+      pt = O.PortTable(DIM)
+      kn = k.cpu().numpy()
+      pt.insert(kn, p0)
+      c, a = hyper[shape]
+      exp = WL.sparse_step(c, pt, [O.PortTable(DIM) for _ in range(SLOTS[shape])], kn, g.cpu().numpy(),
+                           init.cpu().numpy(), [0.0] * SLOTS[shape], *a)
+      exp = torch.from_numpy(exp).to(dt).float().numpy()
+      bad += int((got.view(np.uint32) != exp.view(np.uint32)).sum())
+    mismatches[shape] = bad
+
+  Rc = args.composed_resident
+  small = de.Variable(dim=DIM, init_size=2 * Rc, initializer=0.0, name="fob6_small", num_slot_planes=2)
+  fill([small], Rc)
+  keys_small = mix_keys(torch.randperm(Rc, device=dev, generator=gen)[:N_UNIQUE])
+  dummy = [torch.nn.Parameter(torch.zeros(1))]
+  comp = de.DynamicEmbeddingOptimizer(torch.optim.AdamW(dummy, lr=0.001, weight_decay=0.004, eps=1e-7))
+  fused = de.FusedAdamW(0.001)
+  fused.iterations = 1
+  dup_shapes = tuple(s + "_dup" for s in new)
+  ms = {(n, s): [] for n in dts for s in shapes + dup_shapes}
+  mc = {kind: [] for kind in ("composed", "fused")}
+  for r in range(args.rounds):
+    order = list(dts) if r % 2 == 0 else list(reversed(list(dts)))
+    for shape in shapes:
+      for n in order:
+        ms[(n, shape)].append(timed(lambda: step(n, shape), args.calls))
+        if shape in new:
+          ms[(n, shape + "_dup")].append(timed(lambda: step(n, shape, dup=True), args.calls))
+    mc["composed"].append(timed(lambda: comp.apply_sparse(small, keys_small, g_uni), max(2, args.calls // 2)))
+    mc["fused"].append(timed(lambda: fused.apply_sparse(small, keys_small, g_uni), args.calls))
+  res = {}
+  for shape in shapes + dup_shapes:
+    row = {}
+    for n, dt in dts.items():
+      t = float(np.median(ms[(n, shape)]))
+      row[n] = {"ms": round(t, 4), "ms_spread": [round(min(ms[(n, shape)]), 4), round(max(ms[(n, shape)]), 4)]}
+      if not shape.endswith("_dup"):
+        bpk = bytes_per_key(shape, torch.empty(0, dtype=dt).element_size())
+        row[n].update({"bytes_per_key": bpk, "GB_s": round(bpk * N_UNIQUE / t / 1e6, 1),
+                       "of_datasheet_hbm": round(bpk * N_UNIQUE / (t * 1e-3) / DATASHEET_HBM_BPS, 3)})
+    row["ids"] = N_DUP if shape.endswith("_dup") else N_UNIQUE
+    res[shape] = row
+  res["composed_vs_fused_fp32_adamw"] = {"resident": Rc, "keys": N_UNIQUE, "composed_is": type(comp).__name__,
+                                         "composed_ms": round(float(np.median(mc["composed"])), 4),
+                                         "fused_ms": round(float(np.median(mc["fused"])), 4)}
   return res
 
 
