@@ -292,6 +292,24 @@ det_status det_lookup_sparse_clip(det_table* t, const int64_t* ids, const int32_
                                   const float* weights, size_t nnz, size_t batch, int combiner,
                                   const float* default_row, float max_norm, float* out, det_stream_t stream);
 
+/* safe_embedding_lookup_sparse forward, fused (python/ops/dynamic_embedding_ops.py:296-438; ABI >= 8).  The inputs are
+ * the RAW sparse ids: ids int64[nnz], segment_ids int32[nnz] = the flattened row of every entry (for ids of rank r >= 2,
+ * row = sum_k idx[:, k] * stride_k over the leading r - 1 dims; batch = their product), ascending (canonical order),
+ * weights f32[nnz] or NULL.  Before the lookup, the list is cleaned on the device, as the reference rewrites it:
+ *   prune:  only with weights and combiner != DET_COMBINER_SUM, an entry is kept iff w > 0 (NaN weights are pruned);
+ *           a pruned id is not looked up and adds nothing to any denominator;
+ *   fill:   a row left without an entry (empty, or all of its entries pruned) gets one entry (default_id, weight 1) at
+ *           its row position when has_default_id != 0 -- its output is that id's row, bit for bit;
+ *           has_default_id == 0: its output row is +0.0 (no entry is added);
+ * then out[b] is det_lookup_sparse of the cleaned list (same arithmetic, default_row and dtype rules).  The cleaned
+ * count never leaves the device: no host synchronisation.  Rows of `out` are in the flattened row order (reshape to
+ * dense_shape[:-1] + (dim,)).  Malformed segment ids (not ascending, or outside [0, batch)) leave every output row +0.0
+ * and raise the table's bad-segment error flag (det_get_stats).  Any dim det_lookup_sparse covers; no max_norm.  Uses
+ * the table's scratch buffer: one stream per table at a time. */
+det_status det_lookup_sparse_safe(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
+                                  size_t nnz, size_t batch, int combiner, int has_default_id, int64_t default_id,
+                                  const float* default_row, float* out, det_stream_t stream);
+
 /* One DynamicEmbeddingOptimizer step on unique keys, fused (find param + find slot(s) -> dense
  * rule -> upsert param + upsert slot(s); python/ops/dynamic_embedding_optimizer.py:161-204,
  * python/ops/embedding_weights.py:434-444).  Missing keys start from init_param[dim]
@@ -552,6 +570,101 @@ det_status det_apply_lion_sparse(det_table* t, const int64_t* ids, const int32_t
                                  size_t nnz, size_t batch, int combiner, const float* gout, float lr, float beta1,
                                  float beta2, float weight_decay, const float* init_param, void* workspace,
                                  size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream);
+
+/* The backward of det_lookup_sparse_safe (ABI >= 8): the raw inputs of the forward, its combiner, has_default_id and
+ * default_id, and gout f32[batch, dim].  The list is cleaned as the forward cleans it, except that with
+ * has_default_id == 0 every empty row still gets its fill entry (id 0, weight 1): the reference looks id 0 up for
+ * such rows and zeroes their output afterwards, so id 0 joins the unique set -- it is created and stepped -- with a
+ * gradient contribution of exactly +0.0 from each such row, whatever gout holds there.  Every other gradient is
+ * det_lookup_sparse_grad's rule on the cleaned list (positions of the cleaned list, first-occurrence order of its
+ * ids).  Malformed segment ids give an empty cleaned list: no unique id, no step.  nnz == 0 is valid (every row is
+ * empty); batch == 0 with nnz > 0 is DET_INVALID_ARGUMENT.
+ *
+ * det_lookup_sparse_safe_grad: the backward alone.  unique_out int64[nnz + batch], grads_out f32[nnz + batch, dim] (the
+ * first *n_unique_dev rows are written).  workspace: det_lookup_sparse_safe_grad_workspace_bytes(nnz, batch, dim)
+ * bytes, 256 B aligned. */
+size_t det_lookup_sparse_safe_grad_workspace_bytes(size_t nnz, size_t batch, size_t dim);
+det_status det_lookup_sparse_safe_grad(const int64_t* ids, const int32_t* segment_ids, const float* weights, size_t nnz,
+                                       size_t batch, int combiner, int has_default_id, int64_t default_id,
+                                       const float* gout, size_t dim, int64_t* unique_out, float* grads_out,
+                                       int64_t* n_unique_dev, void* workspace, size_t workspace_bytes,
+                                       det_stream_t stream);
+/* det_apply_*_sparse_safe: that backward chained into the fused step of det_apply_*_sparse, in one call with every
+ * count on the device.  The arguments are those of det_apply_*_sparse plus has_default_id and default_id; the
+ * hyper-parameters, init_param, dtypes and refusals are the same (rows of dim % 4 == 0 and dim <= 128).
+ * workspace: det_apply_sparse_safe_workspace_bytes(nnz, batch, dim) bytes, 256 B aligned. */
+size_t det_apply_sparse_safe_workspace_bytes(size_t nnz, size_t batch, size_t dim);
+det_status det_apply_adagrad_sparse_safe(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                         const float* weights, size_t nnz, size_t batch, int combiner,
+                                         int has_default_id, int64_t default_id, const float* gout, float lr,
+                                         float epsilon, const float* init_param, float init_accum, void* workspace,
+                                         size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_adam_sparse_safe(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                      const float* weights, size_t nnz, size_t batch, int combiner, int has_default_id,
+                                      int64_t default_id, const float* gout, float alpha, float beta1, float beta2,
+                                      float epsilon, const float* init_param, void* workspace, size_t workspace_bytes,
+                                      int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_sgd_sparse_safe(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
+                                     size_t nnz, size_t batch, int combiner, int has_default_id, int64_t default_id,
+                                     const float* gout, float lr, float momentum, int nesterov, const float* init_param,
+                                     void* workspace, size_t workspace_bytes, int64_t* n_unique_dev_out,
+                                     det_stream_t stream);
+det_status det_apply_ftrl_sparse_safe(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                      const float* weights, size_t nnz, size_t batch, int combiner, int has_default_id,
+                                      int64_t default_id, const float* gout, float lr, float l1, float l2,
+                                      float l2_shrinkage, const float* init_param, float init_accum, void* workspace,
+                                      size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_rmsprop_sparse_safe(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                         const float* weights, size_t nnz, size_t batch, int combiner,
+                                         int has_default_id, int64_t default_id, const float* gout, float lr, float rho,
+                                         float momentum, float epsilon, int centered, int eps_in_sqrt,
+                                         const float* init_param, float init_ms, void* workspace,
+                                         size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_adadelta_sparse_safe(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                          const float* weights, size_t nnz, size_t batch, int combiner,
+                                          int has_default_id, int64_t default_id, const float* gout, float lr,
+                                          float rho, float epsilon, const float* init_param, void* workspace,
+                                          size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_adamax_sparse_safe(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                        const float* weights, size_t nnz, size_t batch, int combiner,
+                                        int has_default_id, int64_t default_id, const float* gout, float lr_t,
+                                        float beta1, float beta2, float epsilon, const float* init_param,
+                                        void* workspace, size_t workspace_bytes, int64_t* n_unique_dev_out,
+                                        det_stream_t stream);
+det_status det_apply_nadam_sparse_safe(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                       const float* weights, size_t nnz, size_t batch, int combiner, int has_default_id,
+                                       int64_t default_id, const float* gout, float lr, float beta1, float beta2,
+                                       float epsilon, float omsn, float omsx, float omt, float mt1, float vden,
+                                       const float* init_param, void* workspace, size_t workspace_bytes,
+                                       int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_proximal_adagrad_sparse_safe(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                                  const float* weights, size_t nnz, size_t batch, int combiner,
+                                                  int has_default_id, int64_t default_id, const float* gout, float lr,
+                                                  float l1, float l2, const float* init_param, float init_accum,
+                                                  void* workspace, size_t workspace_bytes, int64_t* n_unique_dev_out,
+                                                  det_stream_t stream);
+det_status det_apply_proximal_sgd_sparse_safe(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                              const float* weights, size_t nnz, size_t batch, int combiner,
+                                              int has_default_id, int64_t default_id, const float* gout, float lr,
+                                              float l1, float l2, const float* init_param, void* workspace,
+                                              size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_adagrad_da_sparse_safe(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                            const float* weights, size_t nnz, size_t batch, int combiner,
+                                            int has_default_id, int64_t default_id, const float* gout, float lr,
+                                            float l1, float l2, int64_t global_step, const float* init_param,
+                                            float init_gg, void* workspace, size_t workspace_bytes,
+                                            int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_adamw_sparse_safe(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                       const float* weights, size_t nnz, size_t batch, int combiner, int has_default_id,
+                                       int64_t default_id, const float* gout, float alpha, float beta1, float beta2,
+                                       float epsilon, float lr, float weight_decay, int amsgrad,
+                                       const float* init_param, void* workspace, size_t workspace_bytes,
+                                       int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_lion_sparse_safe(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                      const float* weights, size_t nnz, size_t batch, int combiner, int has_default_id,
+                                      int64_t default_id, const float* gout, float lr, float beta1, float beta2,
+                                      float weight_decay, const float* init_param, void* workspace,
+                                      size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream);
 
 /* ---- key-hash sharding across GPUs (python/ops/dynamic_embedding_variable.py:165-197 default_partition_fn,
  * python/ops/shadow_embedding_ops.py:397-447 alltoall exchange) ----

@@ -143,6 +143,12 @@ SIGNATURES = {
                                [_i, _vp, _vp, _sz, _vp, _vp]),
     "det_apply_lion_sparse": (_i, [_vp, _vp, _vp, _vp, _sz, _sz, _i, _vp] + [ctypes.c_float] * 4 +
                               [_vp, _vp, _sz, _vp, _vp]),
+    # safe_embedding_lookup_sparse: the forward, its backward, and the _sparse forms with (has_default_id, default_id)
+    "det_lookup_sparse_safe": (_i, [_vp, _vp, _vp, _vp, _sz, _sz, _i, _i, ctypes.c_int64, _vp, _vp, _vp]),
+    "det_lookup_sparse_safe_grad_workspace_bytes": (_sz, [_sz, _sz, _sz]),
+    "det_lookup_sparse_safe_grad": (_i, [_vp, _vp, _vp, _sz, _sz, _i, _i, ctypes.c_int64, _vp, _sz, _vp, _vp, _vp, _vp,
+                                         _sz, _vp]),
+    "det_apply_sparse_safe_workspace_bytes": (_sz, [_sz, _sz, _sz]),
     "det_find_host": (_i, [_vp, _vp, _sz, _vp, _i, _vp, _vp]),
     "det_insert_host": (_i, [_vp, _vp, _vp, _sz]),
     "det_find_host_async": (_i, [_vp, _vp, _sz, _vp, _i, _vp, _vp]),
@@ -188,6 +194,11 @@ SIGNATURES = {
     "det_set_global_epoch": (_i, [_vp, ctypes.c_uint64]),
     "det_evict": (_i, [_vp, ctypes.c_uint64, ctypes.POINTER(ctypes.c_int64), _vp]),
 }
+
+# det_apply_<opt>_sparse_safe: det_apply_<opt>_sparse's arguments with (has_default_id, default_id) after the combiner
+for _name in [n for n in SIGNATURES if n.startswith("det_apply_") and n.endswith("_sparse")]:
+  _res, _args = SIGNATURES[_name]
+  SIGNATURES[_name + "_safe"] = (_res, _args[:7] + [_i, ctypes.c_int64] + _args[7:])
 
 _LIB = None
 

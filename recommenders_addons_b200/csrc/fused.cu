@@ -206,10 +206,12 @@ static size_t unique_ws_layout(size_t n, unsigned char* base, UniqueWs* w) {
 // seg_start[b] = first position i with segment_ids[i] >= b ; seg_start[batch] = nnz
 // run_if_set (nullable): the flag lookup_identity_kernel leaves behind -- zero means "exactly one id per output row was
 // verified and served", the Criteo shape; the general kernels then have nothing to do
+// n_dev (nullable): the id count lives on the device (the cleaned list of the safe lookup); nnz is its bound
 __global__ void segment_offsets_kernel(const int* __restrict__ seg, size_t nnz, size_t batch,
                                        long long* __restrict__ seg_start, DevState* st, const unsigned* run_if_set,
-                                       unsigned epoch) {
+                                       unsigned epoch, const long long* __restrict__ n_dev) {
   if (run_if_set && *run_if_set != epoch) return;   // one id per row, verified by lookup_identity_kernel: nothing to do
+  if (n_dev) nnz = (size_t)*n_dev;
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i > nnz) return;
   const long long cur = i < nnz ? (long long)seg[i] : (long long)batch;
@@ -225,8 +227,10 @@ __global__ void segment_offsets_kernel(const int* __restrict__ seg, size_t nnz, 
 // det_find; only 8 B per id leave the kernel (the [nnz, dim] gather of the reference is never materialised)
 __global__ void __launch_bounds__(kThreadsF)
 resolve_slots_kernel(TableView t, const long long* __restrict__ ids, size_t nnz, long long* __restrict__ slots,
-                     int use_tma, const unsigned* __restrict__ run_if_set, unsigned epoch) {
+                     int use_tma, const unsigned* __restrict__ run_if_set, unsigned epoch,
+                     const long long* __restrict__ n_dev) {
   if (run_if_set && *run_if_set != epoch) return;   // the one-id-per-row kernel has served this call
+  if (n_dev) nnz = (size_t)*n_dev;                  // the id count lives on the device; the grid covers its bound
   __shared__ __align__(128) long long s_keys[kStages][kTileKeys];
   __shared__ __align__(8) unsigned long long s_bar[kStages];
   const int lane = threadIdx.x & 31;
@@ -272,6 +276,95 @@ lookup_identity_kernel(TableView t, const long long* __restrict__ ids, const int
     }
     warp_move_rows<VEC, KEYED>(g, src, dst, lane, default_row, ki, key);
   }
+}
+
+// ---- safe_embedding_lookup_sparse: the cleaned id list, built on the device ---------------------------------------
+// The reference rewrites the sparse ids before its lookup (python/ops/dynamic_embedding_ops.py:349-383): entries with a
+// weight <= 0 (or NaN) are pruned when there are weights and the combiner is not "sum", and every row left without an
+// entry gets one (fill_id, weight 1) entry at its row position.  Here one thread walks one row of the raw list (through
+// its seg_start, as segment_coef_kernel does): row b contributes max(kept_b, 1) entries when filling, kept_b otherwise;
+// an exclusive scan of those counts places every row's entries, in their raw order.  The cleaned count stays in device
+// memory (scan_sums_kernel's total); the host only knows its bound nnz + batch.  Malformed raw segment ids (flagged in
+// `st` by segment_offsets_kernel) give every row 0 entries: the cleaned list is empty.
+struct SafeRows {
+  const long long* seg_start;   // [batch + 1] of the raw list
+  const float* weights;         // raw weights or NULL
+  size_t batch;
+  int prune;                    // weights given and combiner != sum: keep iff w > 0
+  int fill;                     // give every empty row its fill entry
+  const DevState* st;
+};
+
+__device__ __forceinline__ bool safe_keep(const SafeRows& r, long long j) {
+  return !r.prune || __ldg(r.weights + j) > 0.f;    // NaN > 0 is false: pruned
+}
+
+// entries of row b in the cleaned list (0 for b >= batch)
+__device__ __forceinline__ unsigned safe_row_entries(const SafeRows& r, size_t b, bool bad) {
+  if (b >= r.batch || bad) return 0u;
+  const long long st = r.seg_start[b], en = r.seg_start[b + 1];
+  unsigned k = 0;
+  for (long long j = st; j < en; ++j) k += safe_keep(r, j) ? 1u : 0u;
+  return (r.fill && k == 0u) ? 1u : k;
+}
+
+// the entry count of every row summed per block of kScanBlock rows (then scan_sums_kernel: block offsets + the total)
+__global__ void __launch_bounds__(kScanBlock)
+safe_count_kernel(SafeRows r, unsigned* __restrict__ block_sums, const unsigned* __restrict__ run_if_set,
+                  unsigned epoch) {
+  if (run_if_set && *run_if_set != epoch) return;   // the one-id-per-row kernel has served this call
+  __shared__ unsigned s_warp[33];
+  const bool bad = (r.st->error & kErrBadSegment) != 0;
+  unsigned total;
+  block_exclusive_scan(safe_row_entries(r, (size_t)blockIdx.x * kScanBlock + threadIdx.x, bad), s_warp, total);
+  if (threadIdx.x == 0) block_sums[blockIdx.x] = total;
+}
+
+// writes the cleaned list: (id, row, weight, is_fill) of every kept entry and of every empty row's fill entry.
+// out_w / out_fill are NULL when not needed (no weights: every cleaned weight is 1; a forward: no is_fill).
+// report (nullable): where a malformed raw list is also flagged (the table's DevState of a forward)
+__global__ void __launch_bounds__(kScanBlock)
+safe_scatter_kernel(SafeRows r, const long long* __restrict__ ids, long long fill_id,
+                    const unsigned* __restrict__ block_offsets, long long* __restrict__ out_ids, int* __restrict__ out_seg,
+                    float* __restrict__ out_w, unsigned char* __restrict__ out_fill, DevState* report,
+                    const unsigned* __restrict__ run_if_set, unsigned epoch) {
+  if (run_if_set && *run_if_set != epoch) return;
+  __shared__ unsigned s_warp[33];
+  const bool bad = (r.st->error & kErrBadSegment) != 0;
+  if (bad && report && blockIdx.x == 0 && threadIdx.x == 0) atomicOr(&report->error, kErrBadSegment);
+  const size_t b = (size_t)blockIdx.x * kScanBlock + threadIdx.x;
+  const unsigned v = safe_row_entries(r, b, bad);
+  unsigned total;
+  const unsigned excl = block_exclusive_scan(v, s_warp, total);
+  if (v == 0u) return;
+  size_t o = (size_t)block_offsets[blockIdx.x] + excl;
+  const long long st = r.seg_start[b], en = r.seg_start[b + 1];
+  bool any = false;
+  for (long long j = st; j < en; ++j) {
+    if (!safe_keep(r, j)) continue;
+    out_ids[o] = __ldg(ids + j);
+    out_seg[o] = (int)b;
+    if (out_w) out_w[o] = __ldg(r.weights + j);
+    if (out_fill) out_fill[o] = 0;
+    ++o;
+    any = true;
+  }
+  if (!any) {   // v == 1: the row's fill entry
+    out_ids[o] = fill_id;
+    out_seg[o] = (int)b;
+    if (out_w) out_w[o] = 1.f;
+    if (out_fill) out_fill[o] = 1;
+  }
+}
+
+// The backward with default_id None: a fill entry joins the unique set (id 0 is created and stepped), but its gradient
+// contribution is exactly +0, whatever gout holds -- its position is left out of the gradient sum (K9 drops an index
+// outside [0, n_groups)).  Leaving out a +0 term changes no sum: a sum started from +0 is never -0.
+__global__ void safe_drop_fill_kernel(const unsigned char* __restrict__ is_fill, int* __restrict__ idx, size_t n,
+                                      const long long* __restrict__ n_dev) {
+  n = (size_t)*n_dev;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
+    if (is_fill[i]) idx[i] = -1;
 }
 
 // ---- fp16 / bf16 tables: rows are read in their storage type and widened to fp32 in registers (exact) --------------
@@ -2205,9 +2298,67 @@ det_status det_unique(const int64_t* ids, size_t n, int64_t* unique_out, int32_t
   return unique_run(ids, n, unique_out, idx_out, n_unique_dev, workspace, workspace_bytes, nullptr, (cudaStream_t)stream);
 }
 
+// ---- safe_embedding_lookup_sparse: the cleaned list of nnz raw entries over batch rows (bound nnz + batch) --------
+struct SafeWs {
+  long long* ids;           // [bound] cleaned ids
+  int* seg;                 // [bound] their rows, ascending
+  float* w;                 // [bound] their weights (used when the raw list has weights)
+  unsigned char* fill;      // [bound] 1 for a fill entry (used by the backward)
+  long long* raw_start;     // [batch + 1] seg_start of the raw list
+  unsigned* block_sums;     // per kScanBlock rows
+  long long* n;             // the cleaned count, on the device
+  DevState* st;             // malformed raw segment ids
+};
+
+static size_t safe_layout(size_t nnz, size_t batch, unsigned char* base, SafeWs* w) {
+  const size_t m = nnz + batch, nblocks = (batch + kScanBlock - 1) / kScanBlock;
+  WsCarver c(base);
+  long long* ids = c.take<long long>(m * 8);
+  int* seg = c.take<int>(m * 4);
+  float* wt = c.take<float>(m * 4);
+  unsigned char* fill = c.take(m);
+  long long* raw = c.take<long long>((batch + 1) * 8);
+  unsigned* bs = c.take<unsigned>((nblocks + 1) * 4);
+  long long* n = c.take<long long>(16);
+  DevState* st = c.take<DevState>(sizeof(DevState));
+  if (w) {
+    w->ids = ids; w->seg = seg; w->w = wt; w->fill = fill; w->raw_start = raw; w->block_sums = bs; w->n = n; w->st = st;
+  }
+  return c.off;
+}
+
+// What makes a lookup "safe": the fill id of empty rows, when given (has_default_id), and whether fill entries are
+// needed at all (a forward without default_id leaves empty rows at +0 and needs none)
+struct SafeSpec {
+  int has_default_id;
+  long long default_id;
+};
+
+// prune when there are weights and the combiner is not "sum"
+static bool safe_prunes(const float* weights, int combiner) { return weights != nullptr && combiner != DET_COMBINER_SUM; }
+
+// raw (ids, segment_ids, weights) -> the cleaned list in w (count in *w.n); gate / epoch as for the K6 kernels
+static det_status safe_compact_run(const int64_t* ids, const int32_t* segment_ids, const float* weights, size_t nnz,
+                                   size_t batch, int combiner, bool fill, long long fill_id, const SafeWs& w,
+                                   bool fill_flags, DevState* report, const unsigned* gate, unsigned epoch,
+                                   cudaStream_t s) {
+  CUDA_TRY(cudaMemsetAsync(w.st, 0, sizeof(DevState), s));
+  DET_LAUNCH(segment_offsets_kernel, (int)((nnz + 1 + 255) / 256), 256, 0, s, segment_ids, nnz, batch, w.raw_start, w.st,
+             gate, epoch, (const long long*)nullptr);
+  const SafeRows r{w.raw_start, weights, batch, safe_prunes(weights, combiner) ? 1 : 0, fill ? 1 : 0, w.st};
+  const size_t nblocks = (batch + kScanBlock - 1) / kScanBlock;
+  DET_LAUNCH(safe_count_kernel, (int)nblocks, kScanBlock, 0, s, r, w.block_sums, gate, epoch);
+  DET_LAUNCH(scan_sums_kernel, 1, kScanBlock, 0, s, w.block_sums, nblocks, w.n);
+  DET_LAUNCH(safe_scatter_kernel, (int)nblocks, kScanBlock, 0, s, r, (const long long*)ids, fill_id, w.block_sums, w.ids,
+             w.seg, weights ? w.w : nullptr, fill_flags ? w.fill : nullptr, report, gate, epoch);
+  CUDA_TRY(cudaGetLastError());
+  return DET_OK;
+}
+
+// safe (nullable): safe_embedding_lookup_sparse's rules on the raw list (det_lookup_sparse_safe)
 static det_status lookup_sparse_impl(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
                                      size_t nnz, size_t batch, int combiner, const float* default_row, float max_norm,
-                                     float* out, det_stream_t stream) {
+                                     float* out, det_stream_t stream, const SafeSpec* safe = nullptr) {
   if (!t) return fail(DET_INVALID_ARGUMENT, "det_lookup_sparse: null table");
   if (!(max_norm >= 0.f)) return fail(DET_INVALID_ARGUMENT, "det_lookup_sparse: max_norm must be >= 0 (0 = no clipping)");
   det::MutLock _lk(t);
@@ -2228,17 +2379,27 @@ static det_status lookup_sparse_impl(det_table* t, const int64_t* ids, const int
     return fail(DET_INVALID_ARGUMENT, "det_lookup_sparse: null default_row (the table has no keyed initializer)");
   cudaStream_t s = (cudaStream_t)stream;
   det::DevGuard _dg(t->cfg.device);
+  // a safe lookup that neither prunes nor fills reads the raw list as it is
+  if (safe && !safe->has_default_id && !safe_prunes(weights, combiner)) safe = nullptr;
+  if (safe && (nnz >= 0x7fffffffull || batch >= 0x7fffffffull))
+    return fail(DET_INVALID_ARGUMENT, "det_lookup_sparse_safe: nnz / batch too large");
+  // the slot list holds the cleaned list of a safe lookup: at most nnz + batch entries
+  const size_t n_slots = safe ? nnz + batch : (nnz ? nnz : 1);
   long long* seg_start = nullptr;
   long long* slots = nullptr;
   unsigned* not_identity = nullptr;
+  SafeWs sw{};
   {
     void* sc = nullptr;
     const size_t seg_bytes = align256((batch + 1) * sizeof(long long));
-    det_status sst = table_scratch(t, 256 + seg_bytes + (nnz ? nnz : 1) * sizeof(long long), &sc);
+    const size_t slot_bytes = align256(n_slots * sizeof(long long));
+    const size_t safe_bytes = safe ? safe_layout(nnz, batch, nullptr, nullptr) : 0;
+    det_status sst = table_scratch(t, 256 + seg_bytes + slot_bytes + safe_bytes, &sc);
     if (sst != DET_OK) return sst;
     not_identity = (unsigned*)sc;
     seg_start = (long long*)((unsigned char*)sc + 256);
     slots = (long long*)((unsigned char*)sc + 256 + seg_bytes);
+    if (safe) safe_layout(nnz, batch, (unsigned char*)sc + 256 + seg_bytes + slot_bytes, &sw);
   }
   const unsigned dim = (unsigned)t->cfg.dim;
   const bool vec4 = (dim % 4 == 0) && ((((uintptr_t)default_row | (uintptr_t)out) & 15u) == 0);
@@ -2280,9 +2441,22 @@ static det_status lookup_sparse_impl(det_table* t, const int64_t* ids, const int
       });
     });
   }
-  DET_LAUNCH(segment_offsets_kernel, (int)((nnz + 1 + 255) / 256), 256, 0, s, segment_ids, nnz, batch, seg_start, t->view.st, gate, epoch);
+  // a safe lookup: everything below reads the cleaned list, whose count lives on the device
+  const long long* n_dev = nullptr;
+  if (safe) {
+    const det_status cs = safe_compact_run(ids, segment_ids, weights, nnz, batch, combiner, safe->has_default_id != 0,
+                                           safe->default_id, sw, false, t->view.st, gate, epoch, s);
+    if (cs != DET_OK) return cs;
+    ids = (const int64_t*)sw.ids;
+    segment_ids = sw.seg;
+    weights = weights ? sw.w : nullptr;
+    nnz = n_slots;
+    n_dev = sw.n;
+  }
+  DET_LAUNCH(segment_offsets_kernel, (int)((nnz + 1 + 255) / 256), 256, 0, s, segment_ids, nnz, batch, seg_start, t->view.st, gate, epoch,
+             n_dev);
   if (nnz)
-    DET_LAUNCH(resolve_slots_kernel, grid_for(nnz, kTileKeys, t->sm_count, occupancy_of(resolve_slots_kernel, kThreadsF)), kThreadsF, 0, s, t->view, (const long long*)ids, nnz, slots, (((uintptr_t)ids & 15u) == 0) ? 1 : 0, gate, epoch);
+    DET_LAUNCH(resolve_slots_kernel, grid_for(nnz, kTileKeys, t->sm_count, occupancy_of(resolve_slots_kernel, kThreadsF)), kThreadsF, 0, s, t->view, (const long long*)ids, nnz, slots, (((uintptr_t)ids & 15u) == 0) ? 1 : 0, gate, epoch, n_dev);
   det_status rc = DET_OK;
   if (max_norm > 0.f && !(vpr <= lpr)) {
     rc = fail(DET_UNIMPLEMENTED, "det_lookup_sparse_clip: max_norm is fused for rows of at most 32 vectors (dim <= 128 when "
@@ -2319,6 +2493,13 @@ det_status det_lookup_sparse_clip(det_table* t, const int64_t* ids, const int32_
                                   size_t nnz, size_t batch, int combiner, const float* default_row, float max_norm,
                                   float* out, det_stream_t stream) {
   return lookup_sparse_impl(t, ids, segment_ids, weights, nnz, batch, combiner, default_row, max_norm, out, stream);
+}
+
+det_status det_lookup_sparse_safe(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
+                                  size_t nnz, size_t batch, int combiner, int has_default_id, int64_t default_id,
+                                  const float* default_row, float* out, det_stream_t stream) {
+  const SafeSpec sp{has_default_id ? 1 : 0, (long long)default_id};
+  return lookup_sparse_impl(t, ids, segment_ids, weights, nnz, batch, combiner, default_row, 0.f, out, stream, &sp);
 }
 
 // n_dev (nullable): the key count lives on the device (det_apply_*_dup); n is then its upper bound -- room is reserved
@@ -2628,7 +2809,8 @@ det_status det_sparse_segment_sum(const float* rows, size_t dim, const int64_t* 
   v.row_bytes = (unsigned)dim * 4u;
   v.st = st;
   const int sms = current_sm_count();
-  DET_LAUNCH(segment_offsets_kernel, (int)((nnz + 1 + 255) / 256), 256, 0, s, segment_ids, nnz, batch, seg_start, st, (const unsigned*)nullptr, 0u);
+  DET_LAUNCH(segment_offsets_kernel, (int)((nnz + 1 + 255) / 256), 256, 0, s, segment_ids, nnz, batch, seg_start, st, (const unsigned*)nullptr, 0u,
+             (const long long*)nullptr);
   const long long* slots = (const long long*)row_idx;
   const bool vec4 = (dim % 4 == 0) && ((((uintptr_t)default_row | (uintptr_t)out | (uintptr_t)rows) & 15u) == 0);
   unsigned vpr, lpr, sh;
@@ -2778,29 +2960,54 @@ struct SparseSrc {
   const float* weights;
   size_t batch;
   int combiner;
+  // safe_embedding_lookup_sparse (det_*_sparse_safe): the ids are the raw list, cleaned on the device first
+  int safe = 0;
+  int has_default_id = 0;
+  long long default_id = 0;
 };
 
 static det_status check_sparse(const int64_t* ids, const SparseSrc& sp, size_t nnz, const float* gout, const char* who) {
   const std::string w(who);
   if (sp.combiner < DET_COMBINER_SUM || sp.combiner > DET_COMBINER_SQRTN)
     return fail(DET_INVALID_ARGUMENT, w + ": combiner must be one of 'mean', 'sqrtn' or 'sum'");
-  if (!ids || !sp.seg || !gout) return fail(DET_INVALID_ARGUMENT, w + ": null ids, segment_ids or gout");
+  if ((nnz && (!ids || !sp.seg)) || !gout) return fail(DET_INVALID_ARGUMENT, w + ": null ids, segment_ids or gout");
   if (sp.batch == 0) return fail(DET_INVALID_ARGUMENT, w + ": batch is 0 but there are ids");
   if (nnz >= 0x7fffffffull || sp.batch >= 0x7fffffffull) return fail(DET_INVALID_ARGUMENT, w + ": nnz / batch too large");
   return DET_OK;
 }
 
-// unique ids -> uniq (count -> cnt, on the device); their summed gradients -> gsum [n_unique, dim]
+// the entries a backward works on: nnz raw entries, or the nnz + batch bound of a safe lookup's cleaned list
+static size_t sparse_bound(const SparseSrc& sp, size_t nnz) { return sp.safe ? nnz + sp.batch : nnz; }
+
+// unique ids -> uniq (count -> cnt, on the device); their summed gradients -> gsum [n_unique, dim].
+// A safe lookup's raw list (nnz entries) is first cleaned into sw; n is then the bound nnz + batch.
 static det_status sparse_grad_run(const int64_t* ids, const SparseSrc& sp, size_t n, const float* gout, size_t dim,
-                                  const DupWs& w, int64_t* uniq, int64_t* cnt, float* gsum, int sms, cudaStream_t s) {
-  det_status st = unique_run(ids, n, uniq, w.idx, cnt, w.uws, w.uws_bytes, nullptr, s);
+                                  const DupWs& w, int64_t* uniq, int64_t* cnt, float* gsum, int sms, cudaStream_t s,
+                                  const SafeWs* sw = nullptr, size_t nnz = 0) {
+  const int32_t* seg = sp.seg;
+  const float* weights = sp.weights;
+  const long long* n_dev = nullptr;
+  if (sw) {
+    // default_id None: the fill entries are 0 and add nothing to its gradient (safe_drop_fill_kernel)
+    det_status cs = safe_compact_run(ids, sp.seg, sp.weights, nnz, sp.batch, sp.combiner, true,
+                                     sp.has_default_id ? sp.default_id : 0, *sw, !sp.has_default_id, nullptr, nullptr,
+                                     0u, s);
+    if (cs != DET_OK) return cs;
+    ids = (const int64_t*)sw->ids;
+    seg = sw->seg;
+    weights = weights ? sw->w : nullptr;
+    n_dev = sw->n;
+  }
+  det_status st = unique_run(ids, n, uniq, w.idx, cnt, w.uws, w.uws_bytes, n_dev, s);
   if (st != DET_OK) return st;
+  if (sw && !sp.has_default_id)
+    DET_LAUNCH(safe_drop_fill_kernel, grid_for(n, 256, sms, 8), 256, 0, s, sw->fill, w.idx, n, n_dev);
   CUDA_TRY(cudaMemsetAsync(w.st, 0, sizeof(DevState), s));
-  DET_LAUNCH(segment_offsets_kernel, (int)((n + 1 + 255) / 256), 256, 0, s, sp.seg, n, sp.batch, w.seg_start, w.st,
-             (const unsigned*)nullptr, 0u);
-  DET_LAUNCH(segment_coef_kernel, grid_for(sp.batch > n ? sp.batch : n, 256, sms, 8), 256, 0, s, w.seg_start, sp.weights, n,
+  DET_LAUNCH(segment_offsets_kernel, (int)((n + 1 + 255) / 256), 256, 0, s, seg, n, sp.batch, w.seg_start, w.st,
+             (const unsigned*)nullptr, 0u, n_dev);
+  DET_LAUNCH(segment_coef_kernel, grid_for(sp.batch > n ? sp.batch : n, 256, sms, 8), 256, 0, s, w.seg_start, weights, n,
              sp.batch, sp.combiner, w.st, w.coef);
-  return seg_reduce_run(gout, w.idx, n, n, dim, gsum, w.sws, w.sws_bytes, (const long long*)cnt, s, nullptr, w.coef);
+  return seg_reduce_run(gout, w.idx, n, n, dim, gsum, w.sws, w.sws_bytes, (const long long*)cnt, s, n_dev, w.coef);
 }
 
 size_t det_lookup_sparse_grad_workspace_bytes(size_t nnz, size_t batch, size_t dim) {
@@ -2831,8 +3038,50 @@ det_status det_lookup_sparse_grad(const int64_t* ids, const int32_t* segment_ids
   return sparse_grad_run(ids, sp, nnz, gout, dim, w, unique_out, n_unique_dev, grads_out, current_sm_count(), s);
 }
 
+size_t det_lookup_sparse_safe_grad_workspace_bytes(size_t nnz, size_t batch, size_t dim) {
+  (void)dim;
+  const size_t b = batch ? batch : 1;
+  return dup_layout(nnz + b, 0, nullptr, nullptr, b) + safe_layout(nnz, b, nullptr, nullptr);
+}
+
+det_status det_lookup_sparse_safe_grad(const int64_t* ids, const int32_t* segment_ids, const float* weights, size_t nnz,
+                                       size_t batch, int combiner, int has_default_id, int64_t default_id,
+                                       const float* gout, size_t dim, int64_t* unique_out, float* grads_out,
+                                       int64_t* n_unique_dev, void* workspace, size_t workspace_bytes,
+                                       det_stream_t stream) {
+  cudaStream_t s = (cudaStream_t)stream;
+  if (!n_unique_dev) return fail(DET_INVALID_ARGUMENT, "det_lookup_sparse_safe_grad: null n_unique");
+  if (batch == 0 && nnz == 0) {
+    CUDA_TRY(cudaMemsetAsync(n_unique_dev, 0, sizeof(int64_t), s));
+    return DET_OK;
+  }
+  SparseSrc sp{segment_ids, weights, batch, combiner};
+  sp.safe = 1;
+  sp.has_default_id = has_default_id ? 1 : 0;
+  sp.default_id = (long long)default_id;
+  det_status st = check_sparse(ids, sp, nnz, gout, "det_lookup_sparse_safe_grad");
+  if (st != DET_OK) return st;
+  if (dim == 0 || dim >= 0x7fffffffull) return fail(DET_INVALID_ARGUMENT, "det_lookup_sparse_safe_grad: dim must be in [1, 2^31)");
+  if (!unique_out || !grads_out || !workspace) return fail(DET_INVALID_ARGUMENT, "det_lookup_sparse_safe_grad: null argument");
+  if (workspace_bytes < det_lookup_sparse_safe_grad_workspace_bytes(nnz, batch, dim))
+    return fail(DET_INVALID_ARGUMENT, "det_lookup_sparse_safe_grad: workspace too small");
+  if (((uintptr_t)workspace & 255u) != 0)
+    return fail(DET_INVALID_ARGUMENT, "det_lookup_sparse_safe_grad: workspace must be 256 B aligned");
+  const size_t m = nnz + batch;
+  DupWs w;
+  const size_t off = dup_layout(m, 0, (unsigned char*)workspace, &w, batch);
+  SafeWs sw;
+  safe_layout(nnz, batch, (unsigned char*)workspace + off, &sw);
+  return sparse_grad_run(ids, sp, m, gout, dim, w, unique_out, n_unique_dev, grads_out, current_sm_count(), s, &sw, nnz);
+}
+
 size_t det_apply_sparse_workspace_bytes(size_t nnz, size_t batch, size_t dim) {
   return dup_layout(nnz ? nnz : 1, dim ? dim : 1, nullptr, nullptr, batch ? batch : 1);
+}
+
+size_t det_apply_sparse_safe_workspace_bytes(size_t nnz, size_t batch, size_t dim) {
+  const size_t b = batch ? batch : 1;
+  return dup_layout(nnz + b, dim ? dim : 1, nullptr, nullptr, b) + safe_layout(nnz, b, nullptr, nullptr);
 }
 
 // sp (nullable): the ids are those of a det_lookup_sparse call and `grads` is its output gradient [batch, dim]
@@ -2841,12 +3090,15 @@ static det_status apply_dup(det_table* t, const int64_t* ids, const float* grads
                             int64_t* n_unique_dev_out, cudaStream_t s, const long long* n_items_dev = nullptr,
                             const SparseSrc* sp = nullptr, const StepScalars& sx = StepScalars()) {
   if (!t) return fail(DET_INVALID_ARGUMENT, "det_apply_dup: null table");
-  if (n == 0) return DET_OK;
+  // a safe lookup steps its fill entries even when there are no ids: n is the raw count, the cleaned list's bound is
+  // n + batch
+  const bool safe = sp && sp->safe;
+  if (n == 0 && !(safe && sp->batch)) return DET_OK;
   if (sp) {
-    const det_status cs = check_sparse(ids, *sp, n, grads, "det_apply_*_sparse");
+    const det_status cs = check_sparse(ids, *sp, n, grads, safe ? "det_apply_*_sparse_safe" : "det_apply_*_sparse");
     if (cs != DET_OK) return cs;
   }
-  if (!ids || !grads || !workspace) return fail(DET_INVALID_ARGUMENT, "det_apply_dup: null argument");
+  if ((!ids && !safe) || !grads || !workspace) return fail(DET_INVALID_ARGUMENT, "det_apply_dup: null argument");
   if (!init_param) {
     bool keyed;
     {
@@ -2857,14 +3109,21 @@ static det_status apply_dup(det_table* t, const int64_t* ids, const float* grads
   }
   if (n >= 0x7fffffffull) return fail(DET_INVALID_ARGUMENT, "det_apply_dup: n too large");
   const size_t dim = (size_t)t->cfg.dim;
-  if (workspace_bytes < (sp ? det_apply_sparse_workspace_bytes(n, sp->batch, dim) : det_apply_dup_workspace_bytes(n, dim)))
-    return fail(DET_INVALID_ARGUMENT, "det_apply_dup: workspace too small");
+  const size_t need = safe ? det_apply_sparse_safe_workspace_bytes(n, sp->batch, dim)
+                      : sp ? det_apply_sparse_workspace_bytes(n, sp->batch, dim) : det_apply_dup_workspace_bytes(n, dim);
+  if (workspace_bytes < need) return fail(DET_INVALID_ARGUMENT, "det_apply_dup: workspace too small");
   if (((uintptr_t)workspace & 255u) != 0) return fail(DET_INVALID_ARGUMENT, "det_apply_dup: workspace must be 256 B aligned");
   det::DevGuard _dg(t->cfg.device);
+  const size_t nnz = n;
+  if (safe) n = nnz + sp->batch;   // the bound of the cleaned list: every count below lives on the device
   DupWs w;
-  dup_layout(n, dim, (unsigned char*)workspace, &w, sp ? sp->batch : 0);
+  const size_t off = dup_layout(n, dim, (unsigned char*)workspace, &w, sp ? sp->batch : 0);
   det_status st;
-  if (sp) {
+  if (safe) {
+    SafeWs sw;
+    safe_layout(nnz, sp->batch, (unsigned char*)workspace + off, &sw);
+    st = sparse_grad_run(ids, *sp, n, grads, dim, w, (int64_t*)w.uniq, (int64_t*)w.cnt, w.gsum, t->sm_count, s, &sw, nnz);
+  } else if (sp) {
     st = sparse_grad_run(ids, *sp, n, grads, dim, w, (int64_t*)w.uniq, (int64_t*)w.cnt, w.gsum, t->sm_count, s);
   } else {
     // n_items_dev: the id count itself lives on the device (owner side of the sharded backward); n is its bound
@@ -3192,6 +3451,195 @@ det_status det_apply_lion_sparse(det_table* t, const int64_t* ids, const int32_t
   if (det_status st = lion_hyper(lr, beta1, beta2, weight_decay, &h, &sx, &opt)) return st;
   record_slot_init(t, opt, h);
   const SparseSrc sp{segment_ids, weights, batch, combiner};
+  return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
+                   (cudaStream_t)stream, nullptr, &sp, sx);
+}
+
+// ---- det_apply_*_sparse_safe: the backward of det_lookup_sparse_safe chained into the same steps ------------------
+static SparseSrc safe_src(const int32_t* segment_ids, const float* weights, size_t batch, int combiner,
+                          int has_default_id, int64_t default_id) {
+  SparseSrc sp{segment_ids, weights, batch, combiner};
+  sp.safe = 1;
+  sp.has_default_id = has_default_id ? 1 : 0;
+  sp.default_id = (long long)default_id;
+  return sp;
+}
+
+det_status det_apply_adagrad_sparse_safe(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                         const float* weights, size_t nnz, size_t batch, int combiner,
+                                         int has_default_id, int64_t default_id, const float* gout, float lr,
+                                         float epsilon, const float* init_param, float init_accum, void* workspace,
+                                         size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream) {
+  OptHyper h;
+  int opt;
+  if (det_status st = adagrad_hyper(lr, epsilon, init_accum, &h, &opt)) return st;
+  record_slot_init(t, opt, h);
+  const SparseSrc sp = safe_src(segment_ids, weights, batch, combiner, has_default_id, default_id);
+  return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
+                   (cudaStream_t)stream, nullptr, &sp);
+}
+det_status det_apply_adam_sparse_safe(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                      const float* weights, size_t nnz, size_t batch, int combiner, int has_default_id,
+                                      int64_t default_id, const float* gout, float alpha, float beta1, float beta2,
+                                      float epsilon, const float* init_param, void* workspace, size_t workspace_bytes,
+                                      int64_t* n_unique_dev_out, det_stream_t stream) {
+  OptHyper h;
+  int opt;
+  if (det_status st = adam_hyper(alpha, beta1, beta2, epsilon, &h, &opt)) return st;
+  record_slot_init(t, opt, h);
+  const SparseSrc sp = safe_src(segment_ids, weights, batch, combiner, has_default_id, default_id);
+  return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
+                   (cudaStream_t)stream, nullptr, &sp);
+}
+det_status det_apply_sgd_sparse_safe(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
+                                     size_t nnz, size_t batch, int combiner, int has_default_id, int64_t default_id,
+                                     const float* gout, float lr, float momentum, int nesterov, const float* init_param,
+                                     void* workspace, size_t workspace_bytes, int64_t* n_unique_dev_out,
+                                     det_stream_t stream) {
+  OptHyper h;
+  int opt;
+  if (det_status st = sgd_hyper(lr, momentum, nesterov, &h, &opt)) return st;
+  record_slot_init(t, opt, h);
+  const SparseSrc sp = safe_src(segment_ids, weights, batch, combiner, has_default_id, default_id);
+  return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
+                   (cudaStream_t)stream, nullptr, &sp);
+}
+det_status det_apply_ftrl_sparse_safe(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                      const float* weights, size_t nnz, size_t batch, int combiner, int has_default_id,
+                                      int64_t default_id, const float* gout, float lr, float l1, float l2,
+                                      float l2_shrinkage, const float* init_param, float init_accum, void* workspace,
+                                      size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream) {
+  OptHyper h;
+  int opt;
+  if (det_status st = ftrl_hyper(lr, l1, l2, l2_shrinkage, init_accum, &h, &opt)) return st;
+  record_slot_init(t, opt, h);
+  const SparseSrc sp = safe_src(segment_ids, weights, batch, combiner, has_default_id, default_id);
+  return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
+                   (cudaStream_t)stream, nullptr, &sp);
+}
+det_status det_apply_rmsprop_sparse_safe(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                         const float* weights, size_t nnz, size_t batch, int combiner,
+                                         int has_default_id, int64_t default_id, const float* gout, float lr, float rho,
+                                         float momentum, float epsilon, int centered, int eps_in_sqrt,
+                                         const float* init_param, float init_ms, void* workspace,
+                                         size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream) {
+  OptHyper h;
+  int opt;
+  if (det_status st = rmsprop_hyper(lr, rho, momentum, epsilon, centered, eps_in_sqrt, init_ms, &h, &opt)) return st;
+  record_slot_init(t, opt, h);
+  const SparseSrc sp = safe_src(segment_ids, weights, batch, combiner, has_default_id, default_id);
+  return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
+                   (cudaStream_t)stream, nullptr, &sp);
+}
+det_status det_apply_adadelta_sparse_safe(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                          const float* weights, size_t nnz, size_t batch, int combiner,
+                                          int has_default_id, int64_t default_id, const float* gout, float lr,
+                                          float rho, float epsilon, const float* init_param, void* workspace,
+                                          size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream) {
+  OptHyper h;
+  int opt;
+  if (det_status st = adadelta_hyper(lr, rho, epsilon, &h, &opt)) return st;
+  record_slot_init(t, opt, h);
+  const SparseSrc sp = safe_src(segment_ids, weights, batch, combiner, has_default_id, default_id);
+  return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
+                   (cudaStream_t)stream, nullptr, &sp);
+}
+det_status det_apply_adamax_sparse_safe(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                        const float* weights, size_t nnz, size_t batch, int combiner,
+                                        int has_default_id, int64_t default_id, const float* gout, float lr_t,
+                                        float beta1, float beta2, float epsilon, const float* init_param,
+                                        void* workspace, size_t workspace_bytes, int64_t* n_unique_dev_out,
+                                        det_stream_t stream) {
+  OptHyper h;
+  int opt;
+  if (det_status st = adamax_hyper(lr_t, beta1, beta2, epsilon, &h, &opt)) return st;
+  record_slot_init(t, opt, h);
+  const SparseSrc sp = safe_src(segment_ids, weights, batch, combiner, has_default_id, default_id);
+  return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
+                   (cudaStream_t)stream, nullptr, &sp);
+}
+det_status det_apply_nadam_sparse_safe(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                       const float* weights, size_t nnz, size_t batch, int combiner, int has_default_id,
+                                       int64_t default_id, const float* gout, float lr, float beta1, float beta2,
+                                       float epsilon, float omsn, float omsx, float omt, float mt1, float vden,
+                                       const float* init_param, void* workspace, size_t workspace_bytes,
+                                       int64_t* n_unique_dev_out, det_stream_t stream) {
+  OptHyper h;
+  StepScalars sx;
+  int opt;
+  if (det_status st = nadam_hyper(lr, beta1, beta2, epsilon, omsn, omsx, omt, mt1, vden, &h, &sx, &opt)) return st;
+  record_slot_init(t, opt, h);
+  const SparseSrc sp = safe_src(segment_ids, weights, batch, combiner, has_default_id, default_id);
+  return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
+                   (cudaStream_t)stream, nullptr, &sp, sx);
+}
+det_status det_apply_proximal_adagrad_sparse_safe(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                                  const float* weights, size_t nnz, size_t batch, int combiner,
+                                                  int has_default_id, int64_t default_id, const float* gout, float lr,
+                                                  float l1, float l2, const float* init_param, float init_accum,
+                                                  void* workspace, size_t workspace_bytes, int64_t* n_unique_dev_out,
+                                                  det_stream_t stream) {
+  OptHyper h;
+  int opt;
+  if (det_status st = proximal_hyper("det_apply_proximal_adagrad", lr, l1, l2, init_accum, 1, &h, &opt)) return st;
+  record_slot_init(t, opt, h);
+  const SparseSrc sp = safe_src(segment_ids, weights, batch, combiner, has_default_id, default_id);
+  return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
+                   (cudaStream_t)stream, nullptr, &sp);
+}
+det_status det_apply_proximal_sgd_sparse_safe(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                              const float* weights, size_t nnz, size_t batch, int combiner,
+                                              int has_default_id, int64_t default_id, const float* gout, float lr,
+                                              float l1, float l2, const float* init_param, void* workspace,
+                                              size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream) {
+  OptHyper h;
+  int opt;
+  if (det_status st = proximal_hyper("det_apply_proximal_sgd", lr, l1, l2, 0.f, 0, &h, &opt)) return st;
+  record_slot_init(t, opt, h);
+  const SparseSrc sp = safe_src(segment_ids, weights, batch, combiner, has_default_id, default_id);
+  return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
+                   (cudaStream_t)stream, nullptr, &sp);
+}
+det_status det_apply_adagrad_da_sparse_safe(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                            const float* weights, size_t nnz, size_t batch, int combiner,
+                                            int has_default_id, int64_t default_id, const float* gout, float lr,
+                                            float l1, float l2, int64_t global_step, const float* init_param,
+                                            float init_gg, void* workspace, size_t workspace_bytes,
+                                            int64_t* n_unique_dev_out, det_stream_t stream) {
+  OptHyper h;
+  int opt;
+  if (det_status st = adagrad_da_hyper(lr, l1, l2, global_step, init_gg, &h, &opt)) return st;
+  record_slot_init(t, opt, h);
+  const SparseSrc sp = safe_src(segment_ids, weights, batch, combiner, has_default_id, default_id);
+  return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
+                   (cudaStream_t)stream, nullptr, &sp);
+}
+det_status det_apply_adamw_sparse_safe(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                       const float* weights, size_t nnz, size_t batch, int combiner, int has_default_id,
+                                       int64_t default_id, const float* gout, float alpha, float beta1, float beta2,
+                                       float epsilon, float lr, float weight_decay, int amsgrad,
+                                       const float* init_param, void* workspace, size_t workspace_bytes,
+                                       int64_t* n_unique_dev_out, det_stream_t stream) {
+  OptHyper h;
+  StepScalars sx;
+  int opt;
+  if (det_status st = adamw_hyper(alpha, beta1, beta2, epsilon, lr, weight_decay, amsgrad, &h, &sx, &opt)) return st;
+  record_slot_init(t, opt, h);
+  const SparseSrc sp = safe_src(segment_ids, weights, batch, combiner, has_default_id, default_id);
+  return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
+                   (cudaStream_t)stream, nullptr, &sp, sx);
+}
+det_status det_apply_lion_sparse_safe(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                      const float* weights, size_t nnz, size_t batch, int combiner, int has_default_id,
+                                      int64_t default_id, const float* gout, float lr, float beta1, float beta2,
+                                      float weight_decay, const float* init_param, void* workspace,
+                                      size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream) {
+  OptHyper h;
+  StepScalars sx;
+  int opt;
+  if (det_status st = lion_hyper(lr, beta1, beta2, weight_decay, &h, &sx, &opt)) return st;
+  record_slot_init(t, opt, h);
+  const SparseSrc sp = safe_src(segment_ids, weights, batch, combiner, has_default_id, default_id);
   return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
                    (cudaStream_t)stream, nullptr, &sp, sx);
 }

@@ -8,7 +8,7 @@ from .variable import (GraphKeys, ModelMode, TrainableWrapper, Variable, default
                        load_de_variable_from_file_system, make_partition, segment_reduce, trainable_wrapper_filter, unique)
 from .keyed_init import KeyedRandomNormal, KeyedRandomUniform, KeyedTruncatedNormal
 from .ops import (SparseIds, SparseLookupTrainable, embedding_lookup_sparse, safe_embedding_lookup_sparse,
-                  trainable_embedding_lookup_sparse)
+                  trainable_embedding_lookup_sparse, trainable_safe_embedding_lookup_sparse)
 from .optimizer import (ComposedOptimizer, DynamicEmbeddingOptimizer, FusedAdadelta, FusedAdagrad, FusedAdagradDA,
                         FusedAdam, FusedAdamax, FusedAdamW, FusedFtrl, FusedLion, FusedNadam, FusedProximalAdagrad,
                         FusedProximalGradientDescent, FusedRMSprop, FusedSGD, SlotPlane)
@@ -29,5 +29,5 @@ __all__ = [
     "enable_inference_mode", "enable_train_mode", "get_model_mode", "trainable_wrapper_filter", "shadow_ops",
     "ComposedOptimizer", "SlotPlane", "math", "data_flow", "keras", "GraphKeys", "FileSystemSaver", "FileSystemSaverConfig", "DynamicEmbeddingSaver",
     "KeyedRandomNormal", "KeyedRandomUniform", "KeyedTruncatedNormal", "SparseLookupTrainable",
-    "trainable_embedding_lookup_sparse",
+    "trainable_embedding_lookup_sparse", "trainable_safe_embedding_lookup_sparse",
 ]

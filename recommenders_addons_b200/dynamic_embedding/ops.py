@@ -63,6 +63,26 @@ def lookup_sparse_fused(params, ids, segment_ids, weights, batch, combiner, defa
   return out
 
 
+def lookup_sparse_safe_fused(params, ids, rows, weights, batch, combiner, default_id, out=None):
+  """det_lookup_sparse_safe: the raw ids, their flattened rows (ascending int32) and weights are cleaned on the device
+  (prune, fill) and looked up in one chain, with no host synchronisation.  `out` (optional): a contiguous float32
+  tensor of batch * dim elements on the table's device, written in place (any shape)."""
+  table = params.tables[0]
+  dev = table.device
+  ids = ids.reshape(-1).to(dev).contiguous()
+  seg = rows.reshape(-1).to(device=dev, dtype=torch.int32).contiguous()
+  w = None if weights is None else weights.reshape(-1).to(device=dev, dtype=torch.float32).contiguous()
+  default_row = None
+  if table.keyed_initializer is None:   # None: the kernels generate missing rows from the table's keyed initializer
+    default_row = table._default_value.to(device=dev, dtype=torch.float32).contiguous()
+  if out is None:
+    out = torch.empty((batch, params.dim), dtype=torch.float32, device=dev)
+  _lib.check(_lib.lib().det_lookup_sparse_safe(table.handle, _ptr(ids), _ptr(seg), _ptr(w), ids.numel(), batch,
+                                               _lib.COMBINERS[combiner], int(default_id is not None),
+                                               int(default_id or 0), _ptr(default_row), _ptr(out), _stream_ptr(dev)))
+  return out
+
+
 class _SparseSegmentSum(torch.autograd.Function):
   """gather(rows, idx) * weights -> segment sum -> normalise over a DENSE [U, dim] matrix (det_sparse_segment_sum: the
   kernels of the fused forward; the ids of a segment are added in order, so the result is deterministic and
@@ -174,32 +194,92 @@ class SparseLookupTrainable(object):
   """What a training step needs from one `trainable_embedding_lookup_sparse` call: the forward's inputs (`params`,
   `ids`, `segment_ids` int32, `weights` or None, `batch`, `combiner`) and its output `out`, whose `.grad` is dL/dout.
   A fused optimizer turns them into one det_apply_*_sparse call; `ComposedOptimizer` into det_lookup_sparse_grad and
-  its own step."""
+  its own step.  `safe`: a `trainable_safe_embedding_lookup_sparse` call, whose `ids`, `segment_ids` (flattened rows)
+  and `weights` are the raw list and `default_id` its fill id (or None); the steps are then det_apply_*_sparse_safe
+  and det_lookup_sparse_safe_grad."""
 
-  def __init__(self, params, ids, segment_ids, weights, batch, combiner, out):
+  def __init__(self, params, ids, segment_ids, weights, batch, combiner, out, safe=False, default_id=None):
     self.params, self.ids, self.segment_ids, self.weights = params, ids, segment_ids, weights
     self.batch, self.combiner, self.out = int(batch), combiner, out
+    self.safe, self.default_id = bool(safe), default_id
+
+  def safe_args(self):
+    """(has_default_id, default_id) of the _safe C calls"""
+    return int(self.default_id is not None), int(self.default_id or 0)
+
+  def touched_ids(self):
+    """the ids a step updates: `ids`, or for a safe lookup the kept ids plus the fill id when a row is empty (a host
+    synchronisation: only a restrict policy asks for them)"""
+    if not self.safe:
+      return self.ids
+    ids = self.ids
+    if self.weights is not None and self.combiner != "sum":
+      keep = self.weights > 0
+      ids, rows = ids[keep], self.segment_ids[keep]
+    else:
+      rows = self.segment_ids
+    present = torch.zeros(self.batch, dtype=torch.bool, device=ids.device)
+    present[rows.long()] = True
+    if bool((~present).any()):
+      ids = torch.cat([ids, torch.full((1,), self.default_id or 0, dtype=ids.dtype, device=ids.device)])
+    return ids
 
   def grad_rows(self, gout=None):
-    """(unique ids, their summed gradients [n_unique, dim]) from dL/dout (default: `out.grad`) -- det_lookup_sparse_grad.
-    The unique count is read on the host."""
+    """(unique ids, their summed gradients [n_unique, dim]) from dL/dout (default: `out.grad`) -- det_lookup_sparse_grad
+    (det_lookup_sparse_safe_grad for a safe lookup).  The unique count is read on the host."""
     gout = self.out.grad if gout is None else gout
     dev = self.ids.device
     gout = gout.to(device=dev, dtype=torch.float32).contiguous()
     nnz, dim = self.ids.numel(), self.params.dim
-    uniq = torch.empty(nnz, dtype=torch.int64, device=dev)
-    grads = torch.empty((nnz, dim), dtype=torch.float32, device=dev)
+    bound = nnz + self.batch if self.safe else nnz    # the cleaned list of a safe lookup has at most nnz + batch ids
+    uniq = torch.empty(max(bound, 1), dtype=torch.int64, device=dev)
+    grads = torch.empty((max(bound, 1), dim), dtype=torch.float32, device=dev)
     cnt = torch.zeros(1, dtype=torch.int64, device=dev)
     lib = _lib.lib()
-    ws_bytes = int(lib.det_lookup_sparse_grad_workspace_bytes(nnz, self.batch, dim))
+    if self.safe:
+      ws_bytes = int(lib.det_lookup_sparse_safe_grad_workspace_bytes(nnz, self.batch, dim))
+    else:
+      ws_bytes = int(lib.det_lookup_sparse_grad_workspace_bytes(nnz, self.batch, dim))
     raw = torch.empty(ws_bytes + 256, dtype=torch.uint8, device=dev)
     off = (-raw.data_ptr()) % 256          # the C ABI wants a 256 B aligned workspace (CUDA allocations already are)
     ws = raw[off:off + ws_bytes]
-    _lib.check(lib.det_lookup_sparse_grad(_ptr(self.ids), _ptr(self.segment_ids), _ptr(self.weights), nnz, self.batch,
-                                          _lib.COMBINERS[self.combiner], _ptr(gout), dim, _ptr(uniq), _ptr(grads), _ptr(cnt),
-                                          _ptr(ws), ws_bytes, _stream_ptr(dev)))
+    head = (_ptr(self.ids), _ptr(self.segment_ids), _ptr(self.weights), nnz, self.batch, _lib.COMBINERS[self.combiner])
+    tail = (_ptr(gout), dim, _ptr(uniq), _ptr(grads), _ptr(cnt), _ptr(ws), ws_bytes, _stream_ptr(dev))
+    if self.safe:
+      _lib.check(lib.det_lookup_sparse_safe_grad(*(head + self.safe_args() + tail)))
+    else:
+      _lib.check(lib.det_lookup_sparse_grad(*(head + tail)))
     n = int(cnt.item())
     return uniq[:n], grads[:n]
+
+
+def _check_trainable_sparse(params, sp_ids, sp_weights, combiner, who, composed):
+  """the refusals of the fused training lookups; `composed`: the function whose return_trainable=True path covers the
+  rest"""
+  if combiner not in ("mean", "sqrtn", "sum"):
+    raise ValueError("combiner must be one of 'mean', 'sqrtn' or 'sum'")
+  if not isinstance(sp_ids, SparseIds):
+    raise TypeError("sp_ids must be SparseTensor")
+  if sp_weights is not None and not isinstance(sp_weights, SparseIds):
+    raise TypeError("sp_weights must be either None or SparseTensor")
+  if not isinstance(params, Variable):
+    raise TypeError("params should be a Variable instance.")
+  if params.key_dtype != sp_ids.values.dtype:
+    raise TypeError("params.key_dtype should be same with sp_ids.dtype: {} vs. {}".format(params.key_dtype,
+                                                                                           sp_ids.values.dtype))
+  if params.shard_num != 1:
+    raise ValueError("%s: one shard only (got %d); use %s(return_trainable=True)" % (who, params.shard_num, composed))
+  if params.value_dtype not in _FUSED_DTYPES:
+    raise TypeError("%s: float32, float16 or bfloat16 variables, got %s" % (who, params.value_dtype))
+  from .keyed_init import is_keyed
+  if callable(params.initializer) and not is_keyed(params.initializer):
+    raise ValueError("%s: a callable initializer draws rows per lookup; use a constant or a keyed initializer "
+                     "(de.KeyedRandomUniform / de.KeyedRandomNormal / de.KeyedTruncatedNormal), or the composed path "
+                     "%s(return_trainable=True)" % (who, composed))
+  if params.bp_v2:
+    raise ValueError("%s: bp_v2 is not supported; use %s(return_trainable=True)" % (who, composed))
+  if params.dim % 4 != 0 or params.dim > 128:
+    raise ValueError("%s: dim must be a multiple of 4 and at most 128, got %d" % (who, params.dim))
 
 
 def trainable_embedding_lookup_sparse(params, sp_ids, sp_weights=None, combiner="mean"):
@@ -213,32 +293,8 @@ def trainable_embedding_lookup_sparse(params, sp_ids, sp_weights=None, combiner=
 
   Single-shard float32 / float16 / bfloat16 variables with a constant or keyed initializer, dim % 4 == 0 and
   dim <= 128; no max_norm.  Everything else takes `embedding_lookup_sparse(..., return_trainable=True)`."""
-  if combiner not in ("mean", "sqrtn", "sum"):
-    raise ValueError("combiner must be one of 'mean', 'sqrtn' or 'sum'")
-  if not isinstance(sp_ids, SparseIds):
-    raise TypeError("sp_ids must be SparseTensor")
-  if sp_weights is not None and not isinstance(sp_weights, SparseIds):
-    raise TypeError("sp_weights must be either None or SparseTensor")
-  if not isinstance(params, Variable):
-    raise TypeError("params should be a Variable instance.")
-  if params.key_dtype != sp_ids.values.dtype:
-    raise TypeError("params.key_dtype should be same with sp_ids.dtype: {} vs. {}".format(params.key_dtype,
-                                                                                           sp_ids.values.dtype))
-  if params.shard_num != 1:
-    raise ValueError("trainable_embedding_lookup_sparse: one shard only (got %d); use embedding_lookup_sparse("
-                     "return_trainable=True)" % params.shard_num)
-  if params.value_dtype not in _FUSED_DTYPES:
-    raise TypeError("trainable_embedding_lookup_sparse: float32, float16 or bfloat16 variables, got %s" % (params.value_dtype,))
-  from .keyed_init import is_keyed
-  if callable(params.initializer) and not is_keyed(params.initializer):
-    raise ValueError("trainable_embedding_lookup_sparse: a callable initializer draws rows per lookup; use a constant or "
-                     "a keyed initializer (de.KeyedRandomUniform / de.KeyedRandomNormal / de.KeyedTruncatedNormal), or the "
-                     "composed path embedding_lookup_sparse(return_trainable=True)")
-  if params.bp_v2:
-    raise ValueError("trainable_embedding_lookup_sparse: bp_v2 is not supported; use embedding_lookup_sparse("
-                     "return_trainable=True)")
-  if params.dim % 4 != 0 or params.dim > 128:
-    raise ValueError("trainable_embedding_lookup_sparse: dim must be a multiple of 4 and at most 128, got %d" % params.dim)
+  _check_trainable_sparse(params, sp_ids, sp_weights, combiner, "trainable_embedding_lookup_sparse",
+                          "embedding_lookup_sparse")
   dev = params.tables[0].device
   ids = sp_ids.values.reshape(-1).to(dev).contiguous()
   seg = sp_ids.indices[:, 0].to(device=dev, dtype=torch.int32).contiguous()
@@ -310,12 +366,44 @@ def _safe_preprocess(sparse_ids, sparse_weights, combiner, default_id):
   return sp2, sw2, empty_rows, shape
 
 
+def _flat_rows(sparse_ids):
+  """(the row of every entry over the leading dims, int32 on the ids' device; their count; the dense shape)"""
+  shape = sparse_ids.dense_shape
+  if len(shape) < 2:
+    raise ValueError("sparse_ids must have rank >= 2, got dense_shape %s" % (shape,))
+  idx = sparse_ids.indices
+  lead = 1
+  for d in shape[:-1]:
+    lead *= d
+  row = idx[:, 0]
+  for k in range(1, len(shape) - 1):
+    row = row * shape[k] + idx[:, k]
+  return row.to(torch.int32), lead, shape
+
+
 def safe_embedding_lookup_sparse(embedding_weights, sparse_ids, sparse_weights=None, combiner="mean",
                                  default_id=None, name="safe_embedding_lookup_sparse", partition_strategy=None,
                                  max_norm=None, return_trainable=False):
   """dynamic_embedding_ops.py:296-438: flatten leading dims, prune weights <= 0 (unless combiner is "sum"),
-  give empty rows `default_id` (or a zero vector when default_id is None), then embedding_lookup_sparse."""
+  give empty rows `default_id` (or a zero vector when default_id is None), then embedding_lookup_sparse.
+
+  Forward-only calls on a single-shard float32, float16 or bfloat16 variable with a constant or keyed initializer and
+  no `max_norm` run det_lookup_sparse_safe: the cleaning and the lookup are one chain on the device, with no host
+  synchronisation, bit-identical to the composed path below.  `return_trainable=True`, sharded variables, `max_norm`
+  and callable initializers take the composed path (see trainable_safe_embedding_lookup_sparse for the fused
+  training path)."""
   verify_embedding_param_weights(embedding_weights, sparse_ids, sparse_weights)
+  if combiner not in ("mean", "sqrtn", "sum"):
+    raise ValueError("combiner must be one of 'mean', 'sqrtn' or 'sum'")
+  params = embedding_weights
+  static_default = params.initializer is None or not callable(params.initializer)
+  if (not return_trainable and max_norm is None and static_default and isinstance(params, Variable) and
+      _fused_ok(params, params.tables[0]._default_value) and
+      params.tables[0].device.type in _table_device_types()):
+    rows, lead, shape = _flat_rows(sparse_ids)
+    w = None if sparse_weights is None else sparse_weights.values
+    out = lookup_sparse_safe_fused(params, sparse_ids.values, rows, w, lead, combiner, default_id)
+    return out.reshape(tuple(shape[:-1]) + (params.dim,))
   sp2, sw2, empty_rows, shape = _safe_preprocess(sparse_ids, sparse_weights, combiner, default_id)
   r = embedding_lookup_sparse(embedding_weights, sp2, sw2, combiner=combiner, max_norm=max_norm,
                               return_trainable=return_trainable)
@@ -325,3 +413,31 @@ def safe_embedding_lookup_sparse(embedding_weights, sparse_ids, sparse_weights=N
     result[empty_rows] = 0
   final = result.reshape(tuple(shape[:-1]) + (result.shape[-1],))
   return (final, tw) if return_trainable else final
+
+
+def trainable_safe_embedding_lookup_sparse(params, sp_ids, sp_weights=None, combiner="mean", default_id=None):
+  """safe_embedding_lookup_sparse for training through the fused kernels: returns (out, SparseLookupTrainable).
+
+  `out` [*dense_shape[:-1], dim] float32 is det_lookup_sparse_safe's forward, allocated in that shape, so in TRAIN mode
+  on a trainable variable the leaf that requires grad is the tensor returned.  After backward,
+  `optimizer.apply_gradients([(out.grad, handle)])` steps the table in one det_apply_*_sparse_safe call (no host
+  synchronisation): the ids of the cleaned list (pruned entries take no part; an empty row's fill id does) get the
+  gradients of trainable_embedding_lookup_sparse.  With default_id None, id 0 is stepped whenever a row is empty, with
+  a gradient of +0.0 from each such row, as the reference's composed path does.
+
+  Same restrictions as trainable_embedding_lookup_sparse; everything else takes
+  `safe_embedding_lookup_sparse(..., return_trainable=True)`."""
+  _check_trainable_sparse(params, sp_ids, sp_weights, combiner, "trainable_safe_embedding_lookup_sparse",
+                          "safe_embedding_lookup_sparse")
+  verify_embedding_param_weights(params, sp_ids, sp_weights)
+  dev = params.tables[0].device
+  rows, lead, shape = _flat_rows(sp_ids)
+  ids = sp_ids.values.reshape(-1).to(dev).contiguous()
+  seg = rows.to(dev).contiguous()
+  w = None if sp_weights is None else sp_weights.values.reshape(-1).to(device=dev, dtype=torch.float32).contiguous()
+  out = torch.empty(tuple(shape[:-1]) + (params.dim,), dtype=torch.float32, device=dev)
+  lookup_sparse_safe_fused(params, ids, seg, w, lead, combiner, default_id, out=out)
+  from .variable import ModelMode
+  if params.trainable and ModelMode.CURRENT_SETTING == ModelMode.TRAIN:
+    out.requires_grad_(True)
+  return out, SparseLookupTrainable(params, ids, seg, w, lead, combiner, out, safe=True, default_id=default_id)

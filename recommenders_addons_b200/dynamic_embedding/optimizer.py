@@ -222,19 +222,33 @@ class _FusedBase(object):
 
   def _apply_lookup_sparse(self, h, gout):
     """one step from dL/dout of a trainable_embedding_lookup_sparse call: det_apply_*_sparse (the backward of the fused
-    lookup chained into the fused step; the unique count stays on the device)"""
+    lookup chained into the fused step; the unique count stays on the device); det_apply_*_sparse_safe for a
+    trainable_safe_embedding_lookup_sparse call, whose empty rows are stepped even without ids"""
     params = h.params
     self._check(params)
     t = params.tables[0]
     nnz = h.ids.numel()
-    if nnz:
+    if nnz or (h.safe and h.batch):
       gout = gout.to(device=t.device, dtype=torch.float32).contiguous()
-      ws = self._workspace(int(_lib.lib().det_apply_sparse_workspace_bytes(nnz, h.batch, params.dim)), t.device)
+      lib = _lib.lib()
+      ws_fn = lib.det_apply_sparse_safe_workspace_bytes if h.safe else lib.det_apply_sparse_workspace_bytes
+      ws = self._workspace(int(ws_fn(nnz, h.batch, params.dim)), t.device)
       init = None if t.keyed_initializer is not None else t._default_value.to(device=t.device, dtype=torch.float32).contiguous()
       self._apply_table_sparse(t, h, gout, init, ws)
     policy = getattr(params, "restrict_policy", None)
     if policy is not None:
-      policy.apply_update(h.ids)
+      policy.apply_update(h.touched_ids())
+
+  def _sparse_call(self, name, table, h, gout, *rest):
+    """det_apply_<name>_sparse(table, ids, segment_ids, weights, nnz, batch, combiner, gout, *rest), or its _safe form
+    (has_default_id and default_id after the combiner) for a safe lookup"""
+    lib = _lib.lib()
+    head = (table.handle, _ptr(h.ids), _ptr(h.segment_ids), _ptr(h.weights), h.ids.numel(), h.batch,
+            _lib.COMBINERS[h.combiner])
+    if h.safe:
+      _lib.check(getattr(lib, "det_apply_%s_sparse_safe" % name)(*(head + h.safe_args()), _ptr(gout), *rest))
+    else:
+      _lib.check(getattr(lib, "det_apply_%s_sparse" % name)(*head, _ptr(gout), *rest))
 
 
 class FusedAdagrad(_FusedBase):
@@ -264,11 +278,8 @@ class FusedAdagrad(_FusedBase):
                                                 _stream_ptr(table.device)))
 
   def _apply_table_sparse(self, table, h, gout, init, ws):
-    _lib.check(_lib.lib().det_apply_adagrad_sparse(table.handle, _ptr(h.ids), _ptr(h.segment_ids), _ptr(h.weights),
-                                                   h.ids.numel(), h.batch, _lib.COMBINERS[h.combiner], _ptr(gout),
-                                                   self.learning_rate, self.epsilon, _ptr(init),
-                                                   self.initial_accumulator_value, _ptr(ws), ws.numel(), None,
-                                                   _stream_ptr(table.device)))
+    self._sparse_call("adagrad", table, h, gout, self.learning_rate, self.epsilon, _ptr(init),
+                      self.initial_accumulator_value, _ptr(ws), ws.numel(), None, _stream_ptr(table.device))
 
 
 class _AdamFamily(_FusedBase):
@@ -326,15 +337,11 @@ class _AdamFamily(_FusedBase):
 
   def _apply_table_sparse(self, table, h, gout, init, ws):
     if self._steps_adamw():
-      _lib.check(_lib.lib().det_apply_adamw_sparse(table.handle, _ptr(h.ids), _ptr(h.segment_ids), _ptr(h.weights),
-                                                   h.ids.numel(), h.batch, _lib.COMBINERS[h.combiner], _ptr(gout),
-                                                   *self._adamw_hyper(), _ptr(init), _ptr(ws), ws.numel(), None,
-                                                   _stream_ptr(table.device)))
+      self._sparse_call("adamw", table, h, gout, *self._adamw_hyper(), _ptr(init), _ptr(ws), ws.numel(), None,
+                        _stream_ptr(table.device))
       return
-    _lib.check(_lib.lib().det_apply_adam_sparse(table.handle, _ptr(h.ids), _ptr(h.segment_ids), _ptr(h.weights),
-                                                h.ids.numel(), h.batch, _lib.COMBINERS[h.combiner], _ptr(gout),
-                                                self.alpha(), self.beta_1, self.beta_2, self.epsilon, _ptr(init), _ptr(ws),
-                                                ws.numel(), None, _stream_ptr(table.device)))
+    self._sparse_call("adam", table, h, gout, self.alpha(), self.beta_1, self.beta_2, self.epsilon, _ptr(init),
+                      _ptr(ws), ws.numel(), None, _stream_ptr(table.device))
 
 
 class FusedAdam(_AdamFamily):
@@ -386,10 +393,8 @@ class FusedSGD(_FusedBase):
                                             _stream_ptr(table.device)))
 
   def _apply_table_sparse(self, table, h, gout, init, ws):
-    _lib.check(_lib.lib().det_apply_sgd_sparse(table.handle, _ptr(h.ids), _ptr(h.segment_ids), _ptr(h.weights),
-                                               h.ids.numel(), h.batch, _lib.COMBINERS[h.combiner], _ptr(gout),
-                                               self.learning_rate, self.momentum, int(self.nesterov), _ptr(init), _ptr(ws),
-                                               ws.numel(), None, _stream_ptr(table.device)))
+    self._sparse_call("sgd", table, h, gout, self.learning_rate, self.momentum, int(self.nesterov), _ptr(init),
+                      _ptr(ws), ws.numel(), None, _stream_ptr(table.device))
 
 
 class FusedFtrl(_FusedBase):
@@ -438,11 +443,8 @@ class FusedFtrl(_FusedBase):
                                              _ptr(ws), ws.numel(), None, _stream_ptr(table.device)))
 
   def _apply_table_sparse(self, table, h, gout, init, ws):
-    _lib.check(_lib.lib().det_apply_ftrl_sparse(table.handle, _ptr(h.ids), _ptr(h.segment_ids), _ptr(h.weights),
-                                                h.ids.numel(), h.batch, _lib.COMBINERS[h.combiner], _ptr(gout),
-                                                self.learning_rate, self.l1, self.l2, self.l2_shrinkage, _ptr(init),
-                                                self.initial_accumulator_value, _ptr(ws), ws.numel(), None,
-                                                _stream_ptr(table.device)))
+    self._sparse_call("ftrl", table, h, gout, self.learning_rate, self.l1, self.l2, self.l2_shrinkage, _ptr(init),
+                      self.initial_accumulator_value, _ptr(ws), ws.numel(), None, _stream_ptr(table.device))
 
 
 class FusedRMSprop(_FusedBase):
@@ -489,10 +491,8 @@ class FusedRMSprop(_FusedBase):
                                                 _stream_ptr(table.device)))
 
   def _apply_table_sparse(self, table, h, gout, init, ws):
-    _lib.check(_lib.lib().det_apply_rmsprop_sparse(table.handle, _ptr(h.ids), _ptr(h.segment_ids), _ptr(h.weights),
-                                                   h.ids.numel(), h.batch, _lib.COMBINERS[h.combiner], _ptr(gout),
-                                                   *self._hyper(), _ptr(init), self.initial_accumulator_value, _ptr(ws),
-                                                   ws.numel(), None, _stream_ptr(table.device)))
+    self._sparse_call("rmsprop", table, h, gout, *self._hyper(), _ptr(init), self.initial_accumulator_value, _ptr(ws),
+                      ws.numel(), None, _stream_ptr(table.device))
 
 
 class FusedAdadelta(_FusedBase):
@@ -521,10 +521,8 @@ class FusedAdadelta(_FusedBase):
                                                  _stream_ptr(table.device)))
 
   def _apply_table_sparse(self, table, h, gout, init, ws):
-    _lib.check(_lib.lib().det_apply_adadelta_sparse(table.handle, _ptr(h.ids), _ptr(h.segment_ids), _ptr(h.weights),
-                                                    h.ids.numel(), h.batch, _lib.COMBINERS[h.combiner], _ptr(gout),
-                                                    self.learning_rate, self.rho, self.epsilon, _ptr(init), _ptr(ws),
-                                                    ws.numel(), None, _stream_ptr(table.device)))
+    self._sparse_call("adadelta", table, h, gout, self.learning_rate, self.rho, self.epsilon, _ptr(init), _ptr(ws),
+                      ws.numel(), None, _stream_ptr(table.device))
 
 
 class FusedAdamax(_FusedBase):
@@ -562,10 +560,8 @@ class FusedAdamax(_FusedBase):
                                                _ptr(ws), ws.numel(), None, _stream_ptr(table.device)))
 
   def _apply_table_sparse(self, table, h, gout, init, ws):
-    _lib.check(_lib.lib().det_apply_adamax_sparse(table.handle, _ptr(h.ids), _ptr(h.segment_ids), _ptr(h.weights),
-                                                  h.ids.numel(), h.batch, _lib.COMBINERS[h.combiner], _ptr(gout),
-                                                  *self._hyper(), _ptr(init), _ptr(ws), ws.numel(), None,
-                                                  _stream_ptr(table.device)))
+    self._sparse_call("adamax", table, h, gout, *self._hyper(), _ptr(init), _ptr(ws), ws.numel(), None,
+                      _stream_ptr(table.device))
 
 
 def nadam_step_scalars(beta_1, beta_2, t, m_cache):
@@ -625,10 +621,8 @@ class FusedNadam(_FusedBase):
                                               _ptr(ws), ws.numel(), None, _stream_ptr(table.device)))
 
   def _apply_table_sparse(self, table, h, gout, init, ws):
-    _lib.check(_lib.lib().det_apply_nadam_sparse(table.handle, _ptr(h.ids), _ptr(h.segment_ids), _ptr(h.weights),
-                                                 h.ids.numel(), h.batch, _lib.COMBINERS[h.combiner], _ptr(gout),
-                                                 *self._hyper(), _ptr(init), _ptr(ws), ws.numel(), None,
-                                                 _stream_ptr(table.device)))
+    self._sparse_call("nadam", table, h, gout, *self._hyper(), _ptr(init), _ptr(ws), ws.numel(), None,
+                      _stream_ptr(table.device))
 
 
 def _check_proximal(learning_rate, **nonneg):
@@ -671,11 +665,8 @@ class FusedProximalAdagrad(_FusedBase):
                                                          _ptr(ws), ws.numel(), None, _stream_ptr(table.device)))
 
   def _apply_table_sparse(self, table, h, gout, init, ws):
-    _lib.check(_lib.lib().det_apply_proximal_adagrad_sparse(table.handle, _ptr(h.ids), _ptr(h.segment_ids),
-                                                            _ptr(h.weights), h.ids.numel(), h.batch,
-                                                            _lib.COMBINERS[h.combiner], _ptr(gout), self.learning_rate,
-                                                            self.l1, self.l2, _ptr(init), self.initial_accumulator_value,
-                                                            _ptr(ws), ws.numel(), None, _stream_ptr(table.device)))
+    self._sparse_call("proximal_adagrad", table, h, gout, self.learning_rate, self.l1, self.l2, _ptr(init),
+                      self.initial_accumulator_value, _ptr(ws), ws.numel(), None, _stream_ptr(table.device))
 
 
 class FusedProximalGradientDescent(_FusedBase):
@@ -706,10 +697,8 @@ class FusedProximalGradientDescent(_FusedBase):
                                                      _stream_ptr(table.device)))
 
   def _apply_table_sparse(self, table, h, gout, init, ws):
-    _lib.check(_lib.lib().det_apply_proximal_sgd_sparse(table.handle, _ptr(h.ids), _ptr(h.segment_ids), _ptr(h.weights),
-                                                        h.ids.numel(), h.batch, _lib.COMBINERS[h.combiner], _ptr(gout),
-                                                        self.learning_rate, self.l1, self.l2, _ptr(init), _ptr(ws),
-                                                        ws.numel(), None, _stream_ptr(table.device)))
+    self._sparse_call("proximal_sgd", table, h, gout, self.learning_rate, self.l1, self.l2, _ptr(init), _ptr(ws),
+                      ws.numel(), None, _stream_ptr(table.device))
 
 
 class FusedAdagradDA(_FusedBase):
@@ -759,11 +748,9 @@ class FusedAdagradDA(_FusedBase):
                                                    None, _stream_ptr(table.device)))
 
   def _apply_table_sparse(self, table, h, gout, init, ws):
-    _lib.check(_lib.lib().det_apply_adagrad_da_sparse(table.handle, _ptr(h.ids), _ptr(h.segment_ids), _ptr(h.weights),
-                                                      h.ids.numel(), h.batch, _lib.COMBINERS[h.combiner], _ptr(gout),
-                                                      *self._hyper(), _ptr(init),
-                                                      self.initial_gradient_squared_accumulator_value, _ptr(ws),
-                                                      ws.numel(), None, _stream_ptr(table.device)))
+    self._sparse_call("adagrad_da", table, h, gout, *self._hyper(), _ptr(init),
+                      self.initial_gradient_squared_accumulator_value, _ptr(ws), ws.numel(), None,
+                      _stream_ptr(table.device))
 
 
 class FusedAdamW(_AdamFamily):
@@ -817,10 +804,8 @@ class FusedLion(_FusedBase):
                                              _ptr(ws), ws.numel(), None, _stream_ptr(table.device)))
 
   def _apply_table_sparse(self, table, h, gout, init, ws):
-    _lib.check(_lib.lib().det_apply_lion_sparse(table.handle, _ptr(h.ids), _ptr(h.segment_ids), _ptr(h.weights),
-                                                h.ids.numel(), h.batch, _lib.COMBINERS[h.combiner], _ptr(gout),
-                                                *self._hyper(), _ptr(init), _ptr(ws), ws.numel(), None,
-                                                _stream_ptr(table.device)))
+    self._sparse_call("lion", table, h, gout, *self._hyper(), _ptr(init), _ptr(ws), ws.numel(), None,
+                      _stream_ptr(table.device))
 
 
 class ComposedOptimizer(object):

@@ -9,12 +9,20 @@ dim 64, on a variable holding --resident rows with one Adagrad plane, timed in o
       step: lookup_sparse_fused + apply_sparse_duplicate_indices on the [nnz, dim] output gradient;
   (3) the backward alone at shape (1): det_apply_adagrad_sparse against torch's gout[seg] * c materialisation followed by
       det_apply_adagrad_dup.
+With --safe, safe_embedding_lookup_sparse instead, at the shapes of (1) and (2) with about 5 % of the bags empty and
+about 10 % of the weights <= 0 (pruned), default_id None:
+  (s1) the forward: the composed surgery (_safe_preprocess in torch, then the fused lookup) against
+       det_lookup_sparse_safe (de.safe_embedding_lookup_sparse), outputs checked bit for bit;
+  (s2) the training step: safe_embedding_lookup_sparse(return_trainable=True) with the composed step against
+       trainable_safe_embedding_lookup_sparse with det_apply_adagrad_sparse_safe, rows checked bit for bit after one
+       unweighted step of each from the same state;
+  (s3) one id per row, no weights: de.safe_embedding_lookup_sparse with default_id None and 0 against det_lookup_sparse.
 CUDA events, median of --rounds rounds that alternate the order of the arms.  A sample of every arm's result is checked
 against the oracle: the sampled ids' rows after one step of each arm (the fused arms bit for bit against
 tests/sparse_grad_oracle.py + oracle.sparse_adagrad_step; the composed arm, whose weighted denominators are summed by
 atomics, to 1e-4 relative).  The card name, power limit and max SM clock are read in the same run.  Prints one JSON line.
 
-  python scripts/sparse_train_microbench.py [--resident 40000000] [--rounds 5] [--calls 5]
+  python scripts/sparse_train_microbench.py [--resident 40000000] [--rounds 5] [--calls 5] [--safe]
 """
 import argparse
 import json
@@ -70,9 +78,12 @@ def main():
   ap.add_argument("--rounds", type=int, default=5)
   ap.add_argument("--calls", type=int, default=5)
   ap.add_argument("--sample", type=int, default=2000)
+  ap.add_argument("--safe", action="store_true", help="measure safe_embedding_lookup_sparse instead")
   args = ap.parse_args()
   if not torch.cuda.is_available():
     raise SystemExit("sparse_train_microbench.py needs a GPU")
+  if args.safe:
+    return safe_main(args)
   from oracle import oracle as O
   from recommenders_addons_b200 import _lib
   from recommenders_addons_b200 import dynamic_embedding as de
@@ -220,6 +231,112 @@ def main():
     c3_floor()
   result["one_per_row"] = dict(zip(("composed_public", "fused_public", "harness_floor"),
                                    medians(args.rounds, args.calls, [c3_composed, c3_fused, c3_floor])))
+  result["checks"] = checks
+  result["ok"] = all(checks.values())
+  print(json.dumps(result))
+
+
+def safe_main(args):
+  from recommenders_addons_b200 import dynamic_embedding as de
+  from recommenders_addons_b200.dynamic_embedding import ops
+  dev = torch.device("cuda", torch.cuda.current_device())
+  rng = np.random.default_rng(1)
+  result = {"metric": "safe_embedding_lookup_sparse microbenchmark", "dim": DIM, "resident": args.resident,
+            "card": card(), "unit": "ms"}
+
+  def variable(name):
+    v = de.Variable(dim=DIM, initializer=0.0, num_slot_planes=1, devices=[str(dev)], name=name,
+                    init_size=2 * args.resident)
+    g = torch.Generator(device=dev)
+    g.manual_seed(5)
+    step = 1 << 22
+    for b in range(0, args.resident, step):
+      k = torch.arange(b, min(b + step, args.resident), dtype=torch.int64, device=dev)
+      v.upsert(k, torch.randn(k.numel(), DIM, device=dev, generator=g) * 0.05)
+    return v
+
+  va = variable("safe_bench_a")
+  ids_all = torch.as_tensor(rng.integers(0, args.resident, BAGS * PER_BAG), device=dev)
+  counts = np.full(BAGS, PER_BAG)
+  counts[rng.random(BAGS) < 0.05] = 0                       # about 5 % of the bags empty
+  rows = torch.as_tensor(np.repeat(np.arange(BAGS), counts), device=dev)
+  cols = torch.as_tensor(np.concatenate([np.arange(c) for c in counts]), device=dev)
+  nnz = rows.numel()
+  ind = torch.stack([rows, cols], 1)
+  ids = ids_all[:nnz].contiguous()
+  w = rng.uniform(0.5, 2.0, nnz).astype(np.float32)
+  w[rng.random(nnz) < 0.1] = -0.5                           # about 10 % pruned
+  sp, sw = de.SparseIds(ind, ids, (BAGS, PER_BAG)), de.SparseIds(ind, torch.as_tensor(w, device=dev), (BAGS, PER_BAG))
+
+  def fwd_old():
+    sp2, sw2, empty, shape = ops._safe_preprocess(sp, sw, "mean", None)
+    r = ops.embedding_lookup_sparse(va, sp2, sw2, combiner="mean")
+    if empty.numel():
+      r = r.clone()
+      r[empty] = 0
+    return r.reshape(tuple(shape[:-1]) + (DIM,))
+
+  def fwd_new():
+    return de.safe_embedding_lookup_sparse(va, sp, sw, combiner="mean")
+
+  checks = {"forward": bool(torch.equal(fwd_old().view(torch.int32), fwd_new().view(torch.int32)))}
+  for _ in range(2):
+    fwd_old()
+    fwd_new()
+  result["forward"] = dict(zip(("composed", "fused_safe"), medians(args.rounds, args.calls, [fwd_old, fwd_new])))
+
+  # training: unweighted bags (the composed path's denominators are then exact, so the two steps agree bit for bit)
+  gout = torch.randn(BAGS, DIM, device=dev) * 1e-3
+  vb = variable("safe_bench_b")
+  oa, ob = de.FusedAdagrad(LR, INIT_ACCUM), de.FusedAdagrad(LR, INIT_ACCUM)
+
+  def step_composed(v=va, o=oa):
+    out, tw = de.safe_embedding_lookup_sparse(v, sp, None, combiner="mean", return_trainable=True)
+    out.backward(gout)
+    o.apply_gradients([(tw.values.grad, tw)])
+
+  def step_fused(v=vb, o=ob):
+    out, h = de.trainable_safe_embedding_lookup_sparse(v, sp, None, combiner="mean")
+    out.backward(gout)
+    o.apply_gradients([(out.grad, h)])
+
+  step_composed()
+  step_fused()
+  torch.cuda.synchronize()
+  pick = torch.as_tensor(np.concatenate([[0], rng.choice(ids.cpu().numpy(), args.sample)]), device=dev)
+  checks["train_step"] = bool(torch.equal(va.lookup(pick).view(torch.int32), vb.lookup(pick).view(torch.int32)))
+  for _ in range(2):
+    step_composed()
+    step_fused()
+  result["train_step"] = dict(zip(("composed_public", "fused_safe_public"),
+                                  medians(args.rounds, args.calls, [step_composed, step_fused])))
+
+  # one id per row, no weights
+  n1 = FEATURES * BAGS
+  ids1 = ids_all[:n1].contiguous() if ids_all.numel() >= n1 else torch.as_tensor(
+      rng.integers(0, args.resident, n1), device=dev)
+  ind1 = torch.stack([torch.arange(n1, device=dev), torch.zeros(n1, dtype=torch.int64, device=dev)], 1)
+  sp1 = de.SparseIds(ind1, ids1, (n1, 1))
+  seg1 = torch.arange(n1, dtype=torch.int32, device=dev)
+
+  def one_plain():
+    return ops.lookup_sparse_fused(va, ids1, seg1, None, n1, "sum")
+
+  def one_safe_none():
+    return de.safe_embedding_lookup_sparse(va, sp1, None, combiner="sum")
+
+  def one_safe_default():
+    return de.safe_embedding_lookup_sparse(va, sp1, None, combiner="sum", default_id=0)
+
+  ref = one_plain()
+  checks["one_per_row"] = bool(torch.equal(ref.view(torch.int32), one_safe_none().view(torch.int32)) and
+                               torch.equal(ref.view(torch.int32), one_safe_default().view(torch.int32)))
+  for _ in range(2):
+    one_plain()
+    one_safe_none()
+    one_safe_default()
+  result["one_per_row"] = dict(zip(("det_lookup_sparse", "safe_default_none", "safe_default_0"),
+                                   medians(args.rounds, args.calls, [one_plain, one_safe_none, one_safe_default])))
   result["checks"] = checks
   result["ok"] = all(checks.values())
   print(json.dumps(result))
