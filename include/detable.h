@@ -304,11 +304,18 @@ det_status det_lookup_sparse_clip(det_table* t, const int64_t* ids, const int32_
  * then out[b] is det_lookup_sparse of the cleaned list (same arithmetic, default_row and dtype rules).  The cleaned
  * count never leaves the device: no host synchronisation.  Rows of `out` are in the flattened row order (reshape to
  * dense_shape[:-1] + (dim,)).  Malformed segment ids (not ascending, or outside [0, batch)) leave every output row +0.0
- * and raise the table's bad-segment error flag (det_get_stats).  Any dim det_lookup_sparse covers; no max_norm.  Uses
+ * and raise the table's bad-segment error flag (det_get_stats).  Any dim det_lookup_sparse covers; max_norm:
+ * det_lookup_sparse_safe_clip.  Uses
  * the table's scratch buffer: one stream per table at a time. */
 det_status det_lookup_sparse_safe(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
                                   size_t nnz, size_t batch, int combiner, int has_default_id, int64_t default_id,
                                   const float* default_row, float* out, det_stream_t stream);
+/* The same with `max_norm` (safe_embedding_lookup_sparse(..., max_norm); ABI >= 8): every row of the cleaned list,
+ * fill rows included, is clipped as det_lookup_sparse_clip clips it, with the same limits and refusals. */
+det_status det_lookup_sparse_safe_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                       const float* weights, size_t nnz, size_t batch, int combiner, int has_default_id,
+                                       int64_t default_id, const float* default_row, float max_norm, float* out,
+                                       det_stream_t stream);
 
 /* One DynamicEmbeddingOptimizer step on unique keys, fused (find param + find slot(s) -> dense
  * rule -> upsert param + upsert slot(s); python/ops/dynamic_embedding_optimizer.py:161-204,
@@ -665,6 +672,173 @@ det_status det_apply_lion_sparse_safe(det_table* t, const int64_t* ids, const in
                                       int64_t default_id, const float* gout, float lr, float beta1, float beta2,
                                       float weight_decay, const float* init_param, void* workspace,
                                       size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream);
+
+/* det_apply_*_sparse_clip and det_apply_*_sparse_safe_clip: the steps of det_lookup_sparse_clip and
+ * det_lookup_sparse_safe_clip (ABI >= 8).  The arguments are those of det_apply_*_sparse / det_apply_*_sparse_safe plus
+ * max_norm after the combiner.  Each unique id's summed gradient G (det_lookup_sparse_grad's rule, unchanged) is taken
+ * through the backward of the clip row -> row * c / max(||row||_2, c), c = max_norm, at the fp32 row p the step reads
+ * (the stored row, or for a key the step creates its init_param / keyed initializer row: the row the clipped forward
+ * read), then the optimizer rule runs on the result G':
+ *   ss  = sum_k p_k * p_k, and dot = sum_k p_k * G_k, each reduced as det_lookup_sparse_clip reduces ||row||^2: every
+ *         lane of a row group of lpr lanes (lpr = the power of two >= dim / 4) adds the products of its 4 elements in
+ *         order, then an xor butterfly over the lpr lanes;
+ *   !(sqrtf(ss) > c): G' = G bit for bit (the forward did not clip: its scale was exactly 1);
+ *   otherwise:        s = c / sqrtf(ss), t = (s * dot) / ss, G'_k = G_k * s - p_k * t (J^T G, one fp32 rounding each).
+ * The clip applies once per unique id, after the position-order sum, as the reference clips the unique rows before the
+ * gather.  The step and the forward agree bit for bit on which rows were clipped when the forward ran its 16-byte
+ * geometry: dim % 4 == 0 and `out` and `default_row` 16 B aligned (every cudaMalloc / torch allocation is).  With an
+ * unaligned `out` or `default_row` the forward sums each row's squares one float per lane, in another order, so a row
+ * whose norm is within rounding of max_norm may be clipped by one and not by the other.  max_norm == 0 is the unclipped call bit for bit; a negative or NaN max_norm is DET_INVALID_ARGUMENT;
+ * max_norm > 0 on a DET_FLOAT16 / DET_BFLOAT16 table is DET_UNIMPLEMENTED (as det_lookup_sparse_clip).  Rows, eviction
+ * scores, keyed initializers, slot dtypes and workspaces: as det_apply_*_sparse(_safe). */
+det_status det_apply_adagrad_sparse_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                         const float* weights, size_t nnz, size_t batch, int combiner, float max_norm,
+                                         const float* gout, float lr, float epsilon, const float* init_param,
+                                         float init_accum, void* workspace, size_t workspace_bytes,
+                                         int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_adam_sparse_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                      const float* weights, size_t nnz, size_t batch, int combiner, float max_norm,
+                                      const float* gout, float alpha, float beta1, float beta2, float epsilon,
+                                      const float* init_param, void* workspace, size_t workspace_bytes,
+                                      int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_sgd_sparse_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
+                                     size_t nnz, size_t batch, int combiner, float max_norm, const float* gout,
+                                     float lr, float momentum, int nesterov, const float* init_param, void* workspace,
+                                     size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_ftrl_sparse_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                      const float* weights, size_t nnz, size_t batch, int combiner, float max_norm,
+                                      const float* gout, float lr, float l1, float l2, float l2_shrinkage,
+                                      const float* init_param, float init_accum, void* workspace,
+                                      size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_rmsprop_sparse_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                         const float* weights, size_t nnz, size_t batch, int combiner, float max_norm,
+                                         const float* gout, float lr, float rho, float momentum, float epsilon,
+                                         int centered, int eps_in_sqrt, const float* init_param, float init_ms,
+                                         void* workspace, size_t workspace_bytes, int64_t* n_unique_dev_out,
+                                         det_stream_t stream);
+det_status det_apply_adadelta_sparse_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                          const float* weights, size_t nnz, size_t batch, int combiner, float max_norm,
+                                          const float* gout, float lr, float rho, float epsilon,
+                                          const float* init_param, void* workspace, size_t workspace_bytes,
+                                          int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_adamax_sparse_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                        const float* weights, size_t nnz, size_t batch, int combiner, float max_norm,
+                                        const float* gout, float lr_t, float beta1, float beta2, float epsilon,
+                                        const float* init_param, void* workspace, size_t workspace_bytes,
+                                        int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_nadam_sparse_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                       const float* weights, size_t nnz, size_t batch, int combiner, float max_norm,
+                                       const float* gout, float lr, float beta1, float beta2, float epsilon, float omsn,
+                                       float omsx, float omt, float mt1, float vden, const float* init_param,
+                                       void* workspace, size_t workspace_bytes, int64_t* n_unique_dev_out,
+                                       det_stream_t stream);
+det_status det_apply_proximal_adagrad_sparse_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                                  const float* weights, size_t nnz, size_t batch, int combiner,
+                                                  float max_norm, const float* gout, float lr, float l1, float l2,
+                                                  const float* init_param, float init_accum, void* workspace,
+                                                  size_t workspace_bytes, int64_t* n_unique_dev_out,
+                                                  det_stream_t stream);
+det_status det_apply_proximal_sgd_sparse_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                              const float* weights, size_t nnz, size_t batch, int combiner,
+                                              float max_norm, const float* gout, float lr, float l1, float l2,
+                                              const float* init_param, void* workspace, size_t workspace_bytes,
+                                              int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_adagrad_da_sparse_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                            const float* weights, size_t nnz, size_t batch, int combiner,
+                                            float max_norm, const float* gout, float lr, float l1, float l2,
+                                            int64_t global_step, const float* init_param, float init_gg,
+                                            void* workspace, size_t workspace_bytes, int64_t* n_unique_dev_out,
+                                            det_stream_t stream);
+det_status det_apply_adamw_sparse_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                       const float* weights, size_t nnz, size_t batch, int combiner, float max_norm,
+                                       const float* gout, float alpha, float beta1, float beta2, float epsilon,
+                                       float lr, float weight_decay, int amsgrad, const float* init_param,
+                                       void* workspace, size_t workspace_bytes, int64_t* n_unique_dev_out,
+                                       det_stream_t stream);
+det_status det_apply_lion_sparse_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                      const float* weights, size_t nnz, size_t batch, int combiner, float max_norm,
+                                      const float* gout, float lr, float beta1, float beta2, float weight_decay,
+                                      const float* init_param, void* workspace, size_t workspace_bytes,
+                                      int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_adagrad_sparse_safe_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                              const float* weights, size_t nnz, size_t batch, int combiner,
+                                              float max_norm, int has_default_id, int64_t default_id, const float* gout,
+                                              float lr, float epsilon, const float* init_param, float init_accum,
+                                              void* workspace, size_t workspace_bytes, int64_t* n_unique_dev_out,
+                                              det_stream_t stream);
+det_status det_apply_adam_sparse_safe_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                           const float* weights, size_t nnz, size_t batch, int combiner, float max_norm,
+                                           int has_default_id, int64_t default_id, const float* gout, float alpha,
+                                           float beta1, float beta2, float epsilon, const float* init_param,
+                                           void* workspace, size_t workspace_bytes, int64_t* n_unique_dev_out,
+                                           det_stream_t stream);
+det_status det_apply_sgd_sparse_safe_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                          const float* weights, size_t nnz, size_t batch, int combiner, float max_norm,
+                                          int has_default_id, int64_t default_id, const float* gout, float lr,
+                                          float momentum, int nesterov, const float* init_param, void* workspace,
+                                          size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_ftrl_sparse_safe_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                           const float* weights, size_t nnz, size_t batch, int combiner, float max_norm,
+                                           int has_default_id, int64_t default_id, const float* gout, float lr,
+                                           float l1, float l2, float l2_shrinkage, const float* init_param,
+                                           float init_accum, void* workspace, size_t workspace_bytes,
+                                           int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_rmsprop_sparse_safe_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                              const float* weights, size_t nnz, size_t batch, int combiner,
+                                              float max_norm, int has_default_id, int64_t default_id, const float* gout,
+                                              float lr, float rho, float momentum, float epsilon, int centered,
+                                              int eps_in_sqrt, const float* init_param, float init_ms, void* workspace,
+                                              size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_adadelta_sparse_safe_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                               const float* weights, size_t nnz, size_t batch, int combiner,
+                                               float max_norm, int has_default_id, int64_t default_id,
+                                               const float* gout, float lr, float rho, float epsilon,
+                                               const float* init_param, void* workspace, size_t workspace_bytes,
+                                               int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_adamax_sparse_safe_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                             const float* weights, size_t nnz, size_t batch, int combiner,
+                                             float max_norm, int has_default_id, int64_t default_id, const float* gout,
+                                             float lr_t, float beta1, float beta2, float epsilon,
+                                             const float* init_param, void* workspace, size_t workspace_bytes,
+                                             int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_nadam_sparse_safe_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                            const float* weights, size_t nnz, size_t batch, int combiner,
+                                            float max_norm, int has_default_id, int64_t default_id, const float* gout,
+                                            float lr, float beta1, float beta2, float epsilon, float omsn, float omsx,
+                                            float omt, float mt1, float vden, const float* init_param, void* workspace,
+                                            size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_proximal_adagrad_sparse_safe_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                                       const float* weights, size_t nnz, size_t batch, int combiner,
+                                                       float max_norm, int has_default_id, int64_t default_id,
+                                                       const float* gout, float lr, float l1, float l2,
+                                                       const float* init_param, float init_accum, void* workspace,
+                                                       size_t workspace_bytes, int64_t* n_unique_dev_out,
+                                                       det_stream_t stream);
+det_status det_apply_proximal_sgd_sparse_safe_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                                   const float* weights, size_t nnz, size_t batch, int combiner,
+                                                   float max_norm, int has_default_id, int64_t default_id,
+                                                   const float* gout, float lr, float l1, float l2,
+                                                   const float* init_param, void* workspace, size_t workspace_bytes,
+                                                   int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_adagrad_da_sparse_safe_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                                 const float* weights, size_t nnz, size_t batch, int combiner,
+                                                 float max_norm, int has_default_id, int64_t default_id,
+                                                 const float* gout, float lr, float l1, float l2, int64_t global_step,
+                                                 const float* init_param, float init_gg, void* workspace,
+                                                 size_t workspace_bytes, int64_t* n_unique_dev_out,
+                                                 det_stream_t stream);
+det_status det_apply_adamw_sparse_safe_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                            const float* weights, size_t nnz, size_t batch, int combiner,
+                                            float max_norm, int has_default_id, int64_t default_id, const float* gout,
+                                            float alpha, float beta1, float beta2, float epsilon, float lr,
+                                            float weight_decay, int amsgrad, const float* init_param, void* workspace,
+                                            size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream);
+det_status det_apply_lion_sparse_safe_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                           const float* weights, size_t nnz, size_t batch, int combiner, float max_norm,
+                                           int has_default_id, int64_t default_id, const float* gout, float lr,
+                                           float beta1, float beta2, float weight_decay, const float* init_param,
+                                           void* workspace, size_t workspace_bytes, int64_t* n_unique_dev_out,
+                                           det_stream_t stream);
 
 /* ---- key-hash sharding across GPUs (python/ops/dynamic_embedding_variable.py:165-197 default_partition_fn,
  * python/ops/shadow_embedding_ops.py:397-447 alltoall exchange) ----

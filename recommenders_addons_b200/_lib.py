@@ -145,6 +145,8 @@ SIGNATURES = {
                               [_vp, _vp, _sz, _vp, _vp]),
     # safe_embedding_lookup_sparse: the forward, its backward, and the _sparse forms with (has_default_id, default_id)
     "det_lookup_sparse_safe": (_i, [_vp, _vp, _vp, _vp, _sz, _sz, _i, _i, ctypes.c_int64, _vp, _vp, _vp]),
+    "det_lookup_sparse_safe_clip": (_i, [_vp, _vp, _vp, _vp, _sz, _sz, _i, _i, ctypes.c_int64, _vp, ctypes.c_float, _vp,
+                                         _vp]),
     "det_lookup_sparse_safe_grad_workspace_bytes": (_sz, [_sz, _sz, _sz]),
     "det_lookup_sparse_safe_grad": (_i, [_vp, _vp, _vp, _sz, _sz, _i, _i, ctypes.c_int64, _vp, _sz, _vp, _vp, _vp, _vp,
                                          _sz, _vp]),
@@ -195,10 +197,13 @@ SIGNATURES = {
     "det_evict": (_i, [_vp, ctypes.c_uint64, ctypes.POINTER(ctypes.c_int64), _vp]),
 }
 
-# det_apply_<opt>_sparse_safe: det_apply_<opt>_sparse's arguments with (has_default_id, default_id) after the combiner
+# det_apply_<opt>_sparse_safe: det_apply_<opt>_sparse's arguments with (has_default_id, default_id) after the combiner;
+# det_apply_<opt>_sparse_clip and _sparse_safe_clip: those of their unclipped twins with max_norm after the combiner
 for _name in [n for n in SIGNATURES if n.startswith("det_apply_") and n.endswith("_sparse")]:
   _res, _args = SIGNATURES[_name]
   SIGNATURES[_name + "_safe"] = (_res, _args[:7] + [_i, ctypes.c_int64] + _args[7:])
+  SIGNATURES[_name + "_clip"] = (_res, _args[:7] + [ctypes.c_float] + _args[7:])
+  SIGNATURES[_name + "_safe_clip"] = (_res, _args[:7] + [ctypes.c_float, _i, ctypes.c_int64] + _args[7:])
 
 _LIB = None
 

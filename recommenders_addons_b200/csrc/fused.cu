@@ -668,6 +668,33 @@ template <> struct ClipArg<true> { float max_norm; };
 template <bool CLIP> __device__ __forceinline__ float clip_norm_of(const ClipArg<CLIP>&) { return 0.f; }
 template <> __device__ __forceinline__ float clip_norm_of<true>(const ClipArg<true>& c) { return c.max_norm; }
 
+// sum_k a_k * b_k over the row an lpr-lane group holds, one vector per lane: each lane adds its own products in element
+// order, then an xor butterfly over the group's lanes (lanes beyond the row hold zeros).  The clipped gather (K6) and
+// the clip's backward in the fused step (apply_staged_kernel) both reduce through here, so they agree bit for bit on
+// whether a row was clipped.  Every lane of the warp must call it.
+template <int VF>
+__device__ __forceinline__ float group_dot(const FVec<VF>& a, FVec<VF> b, unsigned lpr) {
+  float s = 0.f;
+  b.zip(a, [&s](float& y, float x) { s = s + x * y; });
+  for (unsigned o = lpr >> 1; o > 0; o >>= 1) s = s + __shfl_xor_sync(kFull, s, (int)o);
+  return s;
+}
+
+// The backward of the clip row -> row * c / max(||row||, c) (c = max_norm > 0) at the row p, applied to its summed
+// gradient g: with ss = ||p||^2 (group_dot), a row that was not clipped (!(sqrtf(ss) > c)) keeps g bit for bit;
+// otherwise g <- s*g - p*t with s = c / sqrtf(ss), t = (s * dot) / ss, dot = group_dot(p, g).  That is J^T g for the
+// clip's Jacobian J = (c/n) I - (c/n^3) p p^T, n = ||p||, one fp32 rounding per operation in this order.
+__device__ __forceinline__ void clip_grad(FVec<4>& g, const FVec<4>& p, float c, unsigned lpr) {
+  const float ss = group_dot(p, p, lpr);
+  const float dot = group_dot(p, g, lpr);
+  const float n = sqrtf(ss);
+  if (n > c) {
+    const float s = c / n;
+    const float t = (s * dot) / ss;
+    g.zip(p, [s, t](float& a, float b) { a = a * s - b * t; });
+  }
+}
+
 // T: the table's row storage type (float, __half or __nv_bfloat16); the lane geometry is that of the fp32 output row,
 // so a lane that reads a 16 B float4 of an fp32 row reads 8 B of a half row.
 // KEYED: a missing id's row is generated from the table's keyed initializer for ki.ids[i] (default_row is NULL).
@@ -747,9 +774,7 @@ segment_sum_kernel(TableView t, const long long* __restrict__ slots, const long 
         const float mx = clip_norm_of(clip);
 #pragma unroll
         for (int u = 0; u < U; ++u) {
-          float ss = 0.f;
-          x[u].apply([&ss](float& a) { ss = ss + a * a; });
-          for (unsigned o = lpr >> 1; o > 0; o >>= 1) ss = ss + __shfl_xor_sync(kFull, ss, (int)o);
+          const float ss = group_dot<VF>(x[u], x[u], lpr);
           const float scale = mx / fmaxf(sqrtf(ss), mx);
           x[u].apply([scale](float& a) { a = a * scale; });
         }
@@ -1280,18 +1305,28 @@ __device__ __forceinline__ void score_touch<true>(const ScoreArg<true>& sa, long
   if (valid && slot >= 0) sa.sc[slot] = rule_score(sa.rule, is_new ? 0ull : sa.sc[slot], false, 0ull, now_ns());
 }
 
+// CTAs per SM the clipping step (apply_staged_clip_kernel) is built for: those of its unclipped twin, which ptxas
+// chooses on its own.  SGD, momentum, ProximalGradientDescent and Lion fit in 64 registers (4 CTAs of kThreadsF); the
+// three-plane rules are held to 2 by their stage buffers; every other rule runs 3 (at most 80 registers).
+constexpr int clip_min_blocks(int opt) {
+  return opt == kSgd || opt == kMomentum || opt == kProxSgd || opt == kLion ? 4 : opt_slots(opt) >= 3 ? 2 : 3;
+}
+
 // T: the param row storage type, S the slot planes' storage type, as in apply_kernel.  An existing key's half param
 // vector is one 8 B cp.async into the first half of its 16 B stage slot; a new key's is the 16 B fp32 init_param vector,
 // as on an fp32 table.  A half slot vector is staged the same way (8 B into its 16 B stage slot, element 0 where the
 // marker test reads it) and widened by FVec::load.
 // KEYED: a new key's param vector is generated in registers from the table's keyed initializer instead of copied from
 // init_param (NULL); the key travels with the slot through the row-step shuffles.
-template <int OPT, bool SCORED = false, typename T = float, bool KEYED = false, typename S = float>
-__global__ void __launch_bounds__(kThreadsF)
-apply_staged_kernel(TableView t, const long long* __restrict__ keys, const float* __restrict__ grads, size_t n,
-                    OptHyper h, const float* __restrict__ init_param, int full_init, unsigned vpr, unsigned lpr,
-                    unsigned lpr_shift, int use_tma, ScoreArg<SCORED> sa, const long long* __restrict__ n_dev,
-                    SlotPlanes<OPT> sp, InitArg<KEYED> ki = InitArg<KEYED>(), StepArg<OPT> x = StepArg<OPT>()) {
+// CLIP (fp32 rows only): the gradients are those of a max_norm-clipped lookup; each is first taken through the clip's
+// backward at the row the step reads (clip_grad), then the rule runs on the result.  The body is shared by two kernels
+// so that the unclipped one keeps its launch bounds (an explicit minimum of 1 CTA already changes ptxas' choice).
+template <int OPT, bool SCORED, typename T, bool KEYED, typename S, bool CLIP>
+__device__ __forceinline__ void
+apply_staged_body(TableView t, const long long* __restrict__ keys, const float* __restrict__ grads, size_t n,
+                  OptHyper h, const float* __restrict__ init_param, int full_init, unsigned vpr, unsigned lpr,
+                  unsigned lpr_shift, int use_tma, ScoreArg<SCORED> sa, const long long* __restrict__ n_dev,
+                  SlotPlanes<OPT> sp, InitArg<KEYED> ki, StepArg<OPT> x, ClipArg<CLIP> clip) {
   if (n_dev) n = (size_t)*n_dev;        // key count produced on the device (det_apply_*_dup); the grid covers the bound
   constexpr int NS = 2 + opt_slots(OPT);  // streams per row: grad, param (, slot1 (, slot2 (, slot3)))
   DET_DYN_SHARED(dyn_smem);
@@ -1394,9 +1429,9 @@ apply_staged_kernel(TableView t, const long long* __restrict__ keys, const float
         // slot state absent: key created in this launch, or created by insert/accum and never stepped
         const bool fresh =
             nw || (NS > 2 && row_ok && slot_bits(reinterpret_cast<const S*>(sm_mark(stage, st))) == kSlotMark<S>);
-        if (row_ok && lane_on) {
-          const size_t ro = (size_t)sl * dim + (size_t)c0 * 4;
-          FVec<4> g, p, a, b2, c3;
+        const bool on = row_ok && lane_on;
+        FVec<4> g, p, a, b2, c3;
+        if (on) {
           g.v = *sm(stage, st, 0);
           if constexpr (KEYED) {
             if (nw) p.keyed(ki, kj, c0 * 4u);
@@ -1407,6 +1442,16 @@ apply_staged_kernel(TableView t, const long long* __restrict__ keys, const float
             else if (nw) p.v = *sm(stage, st, 1);
             else p.load(reinterpret_cast<const T*>(sm(stage, st, 1)));
           }
+        }
+        if constexpr (CLIP) {   // the shuffles need every lane of the warp: lanes without a row contribute zeros
+          if (!on) {
+            g.zero();
+            p.zero();
+          }
+          clip_grad(g, p, clip_norm_of(clip), lpr);
+        }
+        if (on) {
+          const size_t ro = (size_t)sl * dim + (size_t)c0 * 4;
           if (fresh) {
             opt_fresh<OPT>(h, a, b2, c3);
           } else if constexpr (std::is_same<S, float>::value) {
@@ -1436,6 +1481,27 @@ apply_staged_kernel(TableView t, const long long* __restrict__ keys, const float
     atomicAdd(&t.st->size, (unsigned long long)s_new);
     atomicAdd(&t.st->used, (unsigned long long)s_used);
   }
+}
+
+template <int OPT, bool SCORED = false, typename T = float, bool KEYED = false, typename S = float>
+__global__ void __launch_bounds__(kThreadsF)
+apply_staged_kernel(TableView t, const long long* __restrict__ keys, const float* __restrict__ grads, size_t n,
+                    OptHyper h, const float* __restrict__ init_param, int full_init, unsigned vpr, unsigned lpr,
+                    unsigned lpr_shift, int use_tma, ScoreArg<SCORED> sa, const long long* __restrict__ n_dev,
+                    SlotPlanes<OPT> sp, InitArg<KEYED> ki = InitArg<KEYED>(), StepArg<OPT> x = StepArg<OPT>()) {
+  apply_staged_body<OPT, SCORED, T, KEYED, S, false>(t, keys, grads, n, h, init_param, full_init, vpr, lpr, lpr_shift,
+                                                     use_tma, sa, n_dev, sp, ki, x, ClipArg<false>());
+}
+
+// fp32 rows and slot planes only (the clip of a half row is not fused)
+template <int OPT, bool SCORED, bool KEYED>
+__global__ void __launch_bounds__(kThreadsF, clip_min_blocks(OPT))
+apply_staged_clip_kernel(TableView t, const long long* __restrict__ keys, const float* __restrict__ grads, size_t n,
+                         OptHyper h, const float* __restrict__ init_param, int full_init, unsigned vpr, unsigned lpr,
+                         unsigned lpr_shift, int use_tma, ScoreArg<SCORED> sa, const long long* __restrict__ n_dev,
+                         SlotPlanes<OPT> sp, InitArg<KEYED> ki, StepArg<OPT> x, ClipArg<true> clip) {
+  apply_staged_body<OPT, SCORED, float, KEYED, float, true>(t, keys, grads, n, h, init_param, full_init, vpr, lpr,
+                                                            lpr_shift, use_tma, sa, n_dev, sp, ki, x, clip);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -2502,12 +2568,23 @@ det_status det_lookup_sparse_safe(det_table* t, const int64_t* ids, const int32_
   return lookup_sparse_impl(t, ids, segment_ids, weights, nnz, batch, combiner, default_row, 0.f, out, stream, &sp);
 }
 
+det_status det_lookup_sparse_safe_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                       const float* weights, size_t nnz, size_t batch, int combiner, int has_default_id,
+                                       int64_t default_id, const float* default_row, float max_norm, float* out,
+                                       det_stream_t stream) {
+  const SafeSpec sp{has_default_id ? 1 : 0, (long long)default_id};
+  return lookup_sparse_impl(t, ids, segment_ids, weights, nnz, batch, combiner, default_row, max_norm, out, stream, &sp);
+}
+
 // n_dev (nullable): the key count lives on the device (det_apply_*_dup); n is then its upper bound -- room is reserved
 // for n NEW keys (the unique keys themselves are not read by the host path) and only the staged kernels support it
 // sx: the step scalars beyond h (Nadam, AdamW, Lion; ignored by the other optimizers)
+// max_norm > 0 (fp32 tables, staged kernel only; apply_dup checks both): `grads` are those of a max_norm-clipped
+// lookup, taken through the clip's backward inside the step (clip_grad)
 static det_status apply_common(det_table* t, const int64_t* keys, const float* grads, size_t n, OptHyper h,
                                const float* init_param, int full_init, int opt, cudaStream_t s,
-                               const long long* n_dev = nullptr, const StepScalars& sx = StepScalars()) {
+                               const long long* n_dev = nullptr, const StepScalars& sx = StepScalars(),
+                               float max_norm = 0.f) {
   if (!t) return fail(DET_INVALID_ARGUMENT, "det_apply: null table");
   det::MutLock _lk(t);
   const int vt = t->cfg.value_dtype;
@@ -2546,21 +2623,39 @@ static det_status apply_common(det_table* t, const int64_t* keys, const float* g
         using S = SlotT<typename decltype(row)::type, decltype(HS)::value>;
         return dispatch_bit(t->ev != nullptr, [&](auto SCORED) -> det_status {
           return dispatch_bit(keyed, [&](auto KEYED) -> det_status {
-            return dispatch_int<kNumOpts>(opt, [&](auto OPT) -> det_status {
-              constexpr bool kScored = decltype(SCORED)::value, kKeyed = decltype(KEYED)::value;
-              ScoreArg<kScored> sa;
-              if constexpr (kScored) {
-                sa.sc = evict_scores(t);
-                sa.rule = evict_rule(t);
+            return dispatch_bit(max_norm > 0.f, [&](auto CLIP) -> det_status {
+              using T = typename decltype(row)::type;
+              constexpr bool kClip = decltype(CLIP)::value;
+              if constexpr (kClip && !std::is_same<T, float>::value) {
+                return fail(DET_UNIMPLEMENTED, "det_apply: max_norm on float16 / bfloat16 tables is not fused");
+              } else {
+                return dispatch_int<kNumOpts>(opt, [&](auto OPT) -> det_status {
+                  constexpr bool kScored = decltype(SCORED)::value, kKeyed = decltype(KEYED)::value;
+                  ScoreArg<kScored> sa;
+                  if constexpr (kScored) {
+                    sa.sc = evict_scores(t);
+                    sa.rule = evict_rule(t);
+                  }
+                  // the clipping kernel takes max_norm as one more argument
+                  auto launch = [&](auto kern, auto... clip) -> det_status {
+                    CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+                    int occ = 1;
+                    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, kThreadsF, smem) != cudaSuccess || occ < 1) occ = 1;
+                    DET_LAUNCH(kern, grid_for(n, kTileKeys, t->sm_count, occ), kThreadsF, smem, s, v, k, grads, n, h,
+                               init_param, full_init, vpr, lpr, sh, tma, sa, n_dev,
+                               slot_planes_arg<decltype(OPT)::value>(t), init_arg<kKeyed>(t),
+                               step_arg<decltype(OPT)::value>(sx), clip...);
+                    return DET_OK;
+                  };
+                  if constexpr (kClip) {
+                    ClipArg<true> clip;
+                    clip.max_norm = max_norm;
+                    return launch(apply_staged_clip_kernel<decltype(OPT)::value, kScored, kKeyed>, clip);
+                  } else {
+                    return launch(apply_staged_kernel<decltype(OPT)::value, kScored, T, kKeyed, S>);
+                  }
+                });
               }
-              const auto kern = apply_staged_kernel<decltype(OPT)::value, kScored, typename decltype(row)::type, kKeyed, S>;
-              CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-              int occ = 1;
-              if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, kThreadsF, smem) != cudaSuccess || occ < 1) occ = 1;
-              DET_LAUNCH(kern, grid_for(n, kTileKeys, t->sm_count, occ), kThreadsF, smem, s, v, k, grads, n, h, init_param,
-                         full_init, vpr, lpr, sh, tma, sa, n_dev, slot_planes_arg<decltype(OPT)::value>(t), init_arg<kKeyed>(t),
-                         step_arg<decltype(OPT)::value>(sx));
-              return DET_OK;
             });
           });
         });
@@ -2960,6 +3055,9 @@ struct SparseSrc {
   const float* weights;
   size_t batch;
   int combiner;
+  // > 0: the forward clipped every row to this norm (det_lookup_sparse_clip / _safe_clip); the step applies the clip's
+  // backward to each unique id's summed gradient (clip_grad)
+  float max_norm = 0.f;
   // safe_embedding_lookup_sparse (det_*_sparse_safe): the ids are the raw list, cleaned on the device first
   int safe = 0;
   int has_default_id = 0;
@@ -3097,6 +3195,12 @@ static det_status apply_dup(det_table* t, const int64_t* ids, const float* grads
   if (sp) {
     const det_status cs = check_sparse(ids, *sp, n, grads, safe ? "det_apply_*_sparse_safe" : "det_apply_*_sparse");
     if (cs != DET_OK) return cs;
+    if (!(sp->max_norm >= 0.f))
+      return fail(DET_INVALID_ARGUMENT, "det_apply_*_sparse_clip: max_norm must be >= 0 (0 = no clipping)");
+    // the reference clips in the table's own dtype (as det_lookup_sparse_clip)
+    if (sp->max_norm > 0.f && t->cfg.value_dtype != DET_FLOAT32)
+      return fail(DET_UNIMPLEMENTED, "det_apply_*_sparse_clip: max_norm on float16 / bfloat16 tables is not fused; use "
+                                     "the composed path (lookup, clip in the table's dtype, segment sum)");
   }
   if ((!ids && !safe) || !grads || !workspace) return fail(DET_INVALID_ARGUMENT, "det_apply_dup: null argument");
   if (!init_param) {
@@ -3132,7 +3236,7 @@ static det_status apply_dup(det_table* t, const int64_t* ids, const float* grads
     st = seg_reduce_run(grads, w.idx, n, n, dim, w.gsum, w.sws, w.sws_bytes, w.cnt, s, n_items_dev);
   }
   if (st != DET_OK) return st;
-  st = apply_common(t, (const int64_t*)w.uniq, w.gsum, n, h, init_param, 0, opt, s, w.cnt, sx);
+  st = apply_common(t, (const int64_t*)w.uniq, w.gsum, n, h, init_param, 0, opt, s, w.cnt, sx, sp ? sp->max_norm : 0.f);
   if (st != DET_OK) return st;
   if (n_unique_dev_out) CUDA_TRY(cudaMemcpyAsync(n_unique_dev_out, w.cnt, sizeof(int64_t), cudaMemcpyDeviceToDevice, s));
   return DET_OK;
@@ -3278,203 +3382,343 @@ det_status det_apply_lion_dup(det_table* t, const int64_t* ids, const float* gra
                    nullptr, nullptr, sx);
 }
 
-det_status det_apply_adagrad_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
-                                    size_t nnz, size_t batch, int combiner, const float* gout, float lr, float epsilon,
-                                    const float* init_param, float init_accum, void* workspace, size_t workspace_bytes,
-                                    int64_t* n_unique_dev_out, det_stream_t stream) {
+det_status det_apply_adagrad_sparse_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                         const float* weights, size_t nnz, size_t batch, int combiner, float max_norm,
+                                         const float* gout, float lr, float epsilon, const float* init_param,
+                                         float init_accum, void* workspace, size_t workspace_bytes,
+                                         int64_t* n_unique_dev_out, det_stream_t stream) {
   OptHyper h;
   int opt;
   if (det_status st = adagrad_hyper(lr, epsilon, init_accum, &h, &opt)) return st;
   record_slot_init(t, opt, h);
-  const SparseSrc sp{segment_ids, weights, batch, combiner};
+  const SparseSrc sp{segment_ids, weights, batch, combiner, max_norm};
   return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
                    (cudaStream_t)stream, nullptr, &sp);
 }
+det_status det_apply_adagrad_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
+                                    size_t nnz, size_t batch, int combiner, const float* gout, float lr, float epsilon,
+                                    const float* init_param, float init_accum, void* workspace, size_t workspace_bytes,
+                                    int64_t* n_unique_dev_out, det_stream_t stream) {
+  return det_apply_adagrad_sparse_clip(t, ids, segment_ids, weights, nnz, batch, combiner, 0.f, gout, lr, epsilon,
+                                       init_param, init_accum, workspace, workspace_bytes, n_unique_dev_out, stream);
+}
 
-det_status det_apply_adam_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
-                                 size_t nnz, size_t batch, int combiner, const float* gout, float alpha, float beta1,
-                                 float beta2, float epsilon, const float* init_param, void* workspace,
-                                 size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream) {
+det_status det_apply_adam_sparse_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                      const float* weights, size_t nnz, size_t batch, int combiner, float max_norm,
+                                      const float* gout, float alpha, float beta1, float beta2, float epsilon,
+                                      const float* init_param, void* workspace, size_t workspace_bytes,
+                                      int64_t* n_unique_dev_out, det_stream_t stream) {
   OptHyper h;
   int opt;
   if (det_status st = adam_hyper(alpha, beta1, beta2, epsilon, &h, &opt)) return st;
   record_slot_init(t, opt, h);
-  const SparseSrc sp{segment_ids, weights, batch, combiner};
+  const SparseSrc sp{segment_ids, weights, batch, combiner, max_norm};
   return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
                    (cudaStream_t)stream, nullptr, &sp);
 }
+det_status det_apply_adam_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
+                                 size_t nnz, size_t batch, int combiner, const float* gout, float alpha, float beta1,
+                                 float beta2, float epsilon, const float* init_param, void* workspace,
+                                 size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream) {
+  return det_apply_adam_sparse_clip(t, ids, segment_ids, weights, nnz, batch, combiner, 0.f, gout, alpha, beta1, beta2,
+                                    epsilon, init_param, workspace, workspace_bytes, n_unique_dev_out, stream);
+}
 
-det_status det_apply_sgd_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
-                                size_t nnz, size_t batch, int combiner, const float* gout, float lr, float momentum,
-                                int nesterov, const float* init_param, void* workspace, size_t workspace_bytes,
-                                int64_t* n_unique_dev_out, det_stream_t stream) {
+det_status det_apply_sgd_sparse_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
+                                     size_t nnz, size_t batch, int combiner, float max_norm, const float* gout,
+                                     float lr, float momentum, int nesterov, const float* init_param, void* workspace,
+                                     size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream) {
   OptHyper h;
   int opt;
   if (det_status st = sgd_hyper(lr, momentum, nesterov, &h, &opt)) return st;
   record_slot_init(t, opt, h);
-  const SparseSrc sp{segment_ids, weights, batch, combiner};
+  const SparseSrc sp{segment_ids, weights, batch, combiner, max_norm};
   return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
                    (cudaStream_t)stream, nullptr, &sp);
 }
+det_status det_apply_sgd_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
+                                size_t nnz, size_t batch, int combiner, const float* gout, float lr, float momentum,
+                                int nesterov, const float* init_param, void* workspace, size_t workspace_bytes,
+                                int64_t* n_unique_dev_out, det_stream_t stream) {
+  return det_apply_sgd_sparse_clip(t, ids, segment_ids, weights, nnz, batch, combiner, 0.f, gout, lr, momentum,
+                                   nesterov, init_param, workspace, workspace_bytes, n_unique_dev_out, stream);
+}
 
-det_status det_apply_ftrl_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
-                                 size_t nnz, size_t batch, int combiner, const float* gout, float lr, float l1, float l2,
-                                 float l2_shrinkage, const float* init_param, float init_accum, void* workspace,
-                                 size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream) {
+det_status det_apply_ftrl_sparse_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                      const float* weights, size_t nnz, size_t batch, int combiner, float max_norm,
+                                      const float* gout, float lr, float l1, float l2, float l2_shrinkage,
+                                      const float* init_param, float init_accum, void* workspace,
+                                      size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream) {
   OptHyper h;
   int opt;
   if (det_status st = ftrl_hyper(lr, l1, l2, l2_shrinkage, init_accum, &h, &opt)) return st;
   record_slot_init(t, opt, h);
-  const SparseSrc sp{segment_ids, weights, batch, combiner};
+  const SparseSrc sp{segment_ids, weights, batch, combiner, max_norm};
   return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
                    (cudaStream_t)stream, nullptr, &sp);
 }
+det_status det_apply_ftrl_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
+                                 size_t nnz, size_t batch, int combiner, const float* gout, float lr, float l1,
+                                 float l2, float l2_shrinkage, const float* init_param, float init_accum,
+                                 void* workspace, size_t workspace_bytes, int64_t* n_unique_dev_out,
+                                 det_stream_t stream) {
+  return det_apply_ftrl_sparse_clip(t, ids, segment_ids, weights, nnz, batch, combiner, 0.f, gout, lr, l1, l2,
+                                    l2_shrinkage, init_param, init_accum, workspace, workspace_bytes, n_unique_dev_out,
+                                    stream);
+}
 
+det_status det_apply_rmsprop_sparse_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                         const float* weights, size_t nnz, size_t batch, int combiner, float max_norm,
+                                         const float* gout, float lr, float rho, float momentum, float epsilon,
+                                         int centered, int eps_in_sqrt, const float* init_param, float init_ms,
+                                         void* workspace, size_t workspace_bytes, int64_t* n_unique_dev_out,
+                                         det_stream_t stream) {
+  OptHyper h;
+  int opt;
+  if (det_status st = rmsprop_hyper(lr, rho, momentum, epsilon, centered, eps_in_sqrt, init_ms, &h, &opt)) return st;
+  record_slot_init(t, opt, h);
+  const SparseSrc sp{segment_ids, weights, batch, combiner, max_norm};
+  return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
+                   (cudaStream_t)stream, nullptr, &sp);
+}
 det_status det_apply_rmsprop_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
                                     size_t nnz, size_t batch, int combiner, const float* gout, float lr, float rho,
                                     float momentum, float epsilon, int centered, int eps_in_sqrt,
                                     const float* init_param, float init_ms, void* workspace, size_t workspace_bytes,
                                     int64_t* n_unique_dev_out, det_stream_t stream) {
-  OptHyper h;
-  int opt;
-  if (det_status st = rmsprop_hyper(lr, rho, momentum, epsilon, centered, eps_in_sqrt, init_ms, &h, &opt)) return st;
-  record_slot_init(t, opt, h);
-  const SparseSrc sp{segment_ids, weights, batch, combiner};
-  return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
-                   (cudaStream_t)stream, nullptr, &sp);
+  return det_apply_rmsprop_sparse_clip(t, ids, segment_ids, weights, nnz, batch, combiner, 0.f, gout, lr, rho, momentum,
+                                       epsilon, centered, eps_in_sqrt, init_param, init_ms, workspace, workspace_bytes,
+                                       n_unique_dev_out, stream);
 }
 
-det_status det_apply_adadelta_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
-                                     size_t nnz, size_t batch, int combiner, const float* gout, float lr, float rho,
-                                     float epsilon, const float* init_param, void* workspace, size_t workspace_bytes,
-                                     int64_t* n_unique_dev_out, det_stream_t stream) {
+det_status det_apply_adadelta_sparse_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                          const float* weights, size_t nnz, size_t batch, int combiner, float max_norm,
+                                          const float* gout, float lr, float rho, float epsilon,
+                                          const float* init_param, void* workspace, size_t workspace_bytes,
+                                          int64_t* n_unique_dev_out, det_stream_t stream) {
   OptHyper h;
   int opt;
   if (det_status st = adadelta_hyper(lr, rho, epsilon, &h, &opt)) return st;
   record_slot_init(t, opt, h);
-  const SparseSrc sp{segment_ids, weights, batch, combiner};
+  const SparseSrc sp{segment_ids, weights, batch, combiner, max_norm};
   return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
                    (cudaStream_t)stream, nullptr, &sp);
 }
+det_status det_apply_adadelta_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
+                                     size_t nnz, size_t batch, int combiner, const float* gout, float lr, float rho,
+                                     float epsilon, const float* init_param, void* workspace, size_t workspace_bytes,
+                                     int64_t* n_unique_dev_out, det_stream_t stream) {
+  return det_apply_adadelta_sparse_clip(t, ids, segment_ids, weights, nnz, batch, combiner, 0.f, gout, lr, rho, epsilon,
+                                        init_param, workspace, workspace_bytes, n_unique_dev_out, stream);
+}
 
-det_status det_apply_adamax_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
-                                   size_t nnz, size_t batch, int combiner, const float* gout, float lr_t, float beta1,
-                                   float beta2, float epsilon, const float* init_param, void* workspace,
-                                   size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream) {
+det_status det_apply_adamax_sparse_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                        const float* weights, size_t nnz, size_t batch, int combiner, float max_norm,
+                                        const float* gout, float lr_t, float beta1, float beta2, float epsilon,
+                                        const float* init_param, void* workspace, size_t workspace_bytes,
+                                        int64_t* n_unique_dev_out, det_stream_t stream) {
   OptHyper h;
   int opt;
   if (det_status st = adamax_hyper(lr_t, beta1, beta2, epsilon, &h, &opt)) return st;
   record_slot_init(t, opt, h);
-  const SparseSrc sp{segment_ids, weights, batch, combiner};
+  const SparseSrc sp{segment_ids, weights, batch, combiner, max_norm};
   return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
                    (cudaStream_t)stream, nullptr, &sp);
 }
+det_status det_apply_adamax_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
+                                   size_t nnz, size_t batch, int combiner, const float* gout, float lr_t, float beta1,
+                                   float beta2, float epsilon, const float* init_param, void* workspace,
+                                   size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream) {
+  return det_apply_adamax_sparse_clip(t, ids, segment_ids, weights, nnz, batch, combiner, 0.f, gout, lr_t, beta1, beta2,
+                                      epsilon, init_param, workspace, workspace_bytes, n_unique_dev_out, stream);
+}
 
-det_status det_apply_nadam_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
-                                  size_t nnz, size_t batch, int combiner, const float* gout, float lr, float beta1,
-                                  float beta2, float epsilon, float omsn, float omsx, float omt, float mt1, float vden,
-                                  const float* init_param, void* workspace, size_t workspace_bytes,
-                                  int64_t* n_unique_dev_out, det_stream_t stream) {
+det_status det_apply_nadam_sparse_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                       const float* weights, size_t nnz, size_t batch, int combiner, float max_norm,
+                                       const float* gout, float lr, float beta1, float beta2, float epsilon, float omsn,
+                                       float omsx, float omt, float mt1, float vden, const float* init_param,
+                                       void* workspace, size_t workspace_bytes, int64_t* n_unique_dev_out,
+                                       det_stream_t stream) {
   OptHyper h;
   StepScalars sx;
   int opt;
   if (det_status st = nadam_hyper(lr, beta1, beta2, epsilon, omsn, omsx, omt, mt1, vden, &h, &sx, &opt)) return st;
   record_slot_init(t, opt, h);
-  const SparseSrc sp{segment_ids, weights, batch, combiner};
+  const SparseSrc sp{segment_ids, weights, batch, combiner, max_norm};
   return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
                    (cudaStream_t)stream, nullptr, &sp, sx);
 }
+det_status det_apply_nadam_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
+                                  size_t nnz, size_t batch, int combiner, const float* gout, float lr, float beta1,
+                                  float beta2, float epsilon, float omsn, float omsx, float omt, float mt1, float vden,
+                                  const float* init_param, void* workspace, size_t workspace_bytes,
+                                  int64_t* n_unique_dev_out, det_stream_t stream) {
+  return det_apply_nadam_sparse_clip(t, ids, segment_ids, weights, nnz, batch, combiner, 0.f, gout, lr, beta1, beta2,
+                                     epsilon, omsn, omsx, omt, mt1, vden, init_param, workspace, workspace_bytes,
+                                     n_unique_dev_out, stream);
+}
 
+det_status det_apply_proximal_adagrad_sparse_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                                  const float* weights, size_t nnz, size_t batch, int combiner,
+                                                  float max_norm, const float* gout, float lr, float l1, float l2,
+                                                  const float* init_param, float init_accum, void* workspace,
+                                                  size_t workspace_bytes, int64_t* n_unique_dev_out,
+                                                  det_stream_t stream) {
+  OptHyper h;
+  int opt;
+  if (det_status st = proximal_hyper("det_apply_proximal_adagrad", lr, l1, l2, init_accum, 1, &h, &opt)) return st;
+  record_slot_init(t, opt, h);
+  const SparseSrc sp{segment_ids, weights, batch, combiner, max_norm};
+  return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
+                   (cudaStream_t)stream, nullptr, &sp);
+}
 det_status det_apply_proximal_adagrad_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids,
                                              const float* weights, size_t nnz, size_t batch, int combiner,
                                              const float* gout, float lr, float l1, float l2, const float* init_param,
                                              float init_accum, void* workspace, size_t workspace_bytes,
                                              int64_t* n_unique_dev_out, det_stream_t stream) {
-  OptHyper h;
-  int opt;
-  if (det_status st = proximal_hyper("det_apply_proximal_adagrad", lr, l1, l2, init_accum, 1, &h, &opt)) return st;
-  record_slot_init(t, opt, h);
-  const SparseSrc sp{segment_ids, weights, batch, combiner};
-  return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
-                   (cudaStream_t)stream, nullptr, &sp);
+  return det_apply_proximal_adagrad_sparse_clip(t, ids, segment_ids, weights, nnz, batch, combiner, 0.f, gout, lr, l1,
+                                                l2, init_param, init_accum, workspace, workspace_bytes,
+                                                n_unique_dev_out, stream);
 }
 
-det_status det_apply_proximal_sgd_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids,
-                                         const float* weights, size_t nnz, size_t batch, int combiner, const float* gout,
-                                         float lr, float l1, float l2, const float* init_param, void* workspace,
-                                         size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream) {
+det_status det_apply_proximal_sgd_sparse_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                              const float* weights, size_t nnz, size_t batch, int combiner,
+                                              float max_norm, const float* gout, float lr, float l1, float l2,
+                                              const float* init_param, void* workspace, size_t workspace_bytes,
+                                              int64_t* n_unique_dev_out, det_stream_t stream) {
   OptHyper h;
   int opt;
   if (det_status st = proximal_hyper("det_apply_proximal_sgd", lr, l1, l2, 0.f, 0, &h, &opt)) return st;
   record_slot_init(t, opt, h);
-  const SparseSrc sp{segment_ids, weights, batch, combiner};
+  const SparseSrc sp{segment_ids, weights, batch, combiner, max_norm};
   return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
                    (cudaStream_t)stream, nullptr, &sp);
 }
+det_status det_apply_proximal_sgd_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                         const float* weights, size_t nnz, size_t batch, int combiner,
+                                         const float* gout, float lr, float l1, float l2, const float* init_param,
+                                         void* workspace, size_t workspace_bytes, int64_t* n_unique_dev_out,
+                                         det_stream_t stream) {
+  return det_apply_proximal_sgd_sparse_clip(t, ids, segment_ids, weights, nnz, batch, combiner, 0.f, gout, lr, l1, l2,
+                                            init_param, workspace, workspace_bytes, n_unique_dev_out, stream);
+}
 
+det_status det_apply_adagrad_da_sparse_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                            const float* weights, size_t nnz, size_t batch, int combiner,
+                                            float max_norm, const float* gout, float lr, float l1, float l2,
+                                            int64_t global_step, const float* init_param, float init_gg,
+                                            void* workspace, size_t workspace_bytes, int64_t* n_unique_dev_out,
+                                            det_stream_t stream) {
+  OptHyper h;
+  int opt;
+  if (det_status st = adagrad_da_hyper(lr, l1, l2, global_step, init_gg, &h, &opt)) return st;
+  record_slot_init(t, opt, h);
+  const SparseSrc sp{segment_ids, weights, batch, combiner, max_norm};
+  return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
+                   (cudaStream_t)stream, nullptr, &sp);
+}
 det_status det_apply_adagrad_da_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids,
                                        const float* weights, size_t nnz, size_t batch, int combiner, const float* gout,
                                        float lr, float l1, float l2, int64_t global_step, const float* init_param,
                                        float init_gg, void* workspace, size_t workspace_bytes,
                                        int64_t* n_unique_dev_out, det_stream_t stream) {
-  OptHyper h;
-  int opt;
-  if (det_status st = adagrad_da_hyper(lr, l1, l2, global_step, init_gg, &h, &opt)) return st;
-  record_slot_init(t, opt, h);
-  const SparseSrc sp{segment_ids, weights, batch, combiner};
-  return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
-                   (cudaStream_t)stream, nullptr, &sp);
+  return det_apply_adagrad_da_sparse_clip(t, ids, segment_ids, weights, nnz, batch, combiner, 0.f, gout, lr, l1, l2,
+                                          global_step, init_param, init_gg, workspace, workspace_bytes,
+                                          n_unique_dev_out, stream);
 }
 
-det_status det_apply_adamw_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
-                                  size_t nnz, size_t batch, int combiner, const float* gout, float alpha, float beta1,
-                                  float beta2, float epsilon, float lr, float weight_decay, int amsgrad,
-                                  const float* init_param, void* workspace, size_t workspace_bytes,
-                                  int64_t* n_unique_dev_out, det_stream_t stream) {
+det_status det_apply_adamw_sparse_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                       const float* weights, size_t nnz, size_t batch, int combiner, float max_norm,
+                                       const float* gout, float alpha, float beta1, float beta2, float epsilon,
+                                       float lr, float weight_decay, int amsgrad, const float* init_param,
+                                       void* workspace, size_t workspace_bytes, int64_t* n_unique_dev_out,
+                                       det_stream_t stream) {
   OptHyper h;
   StepScalars sx;
   int opt;
   if (det_status st = adamw_hyper(alpha, beta1, beta2, epsilon, lr, weight_decay, amsgrad, &h, &sx, &opt)) return st;
   record_slot_init(t, opt, h);
-  const SparseSrc sp{segment_ids, weights, batch, combiner};
+  const SparseSrc sp{segment_ids, weights, batch, combiner, max_norm};
   return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
                    (cudaStream_t)stream, nullptr, &sp, sx);
 }
+det_status det_apply_adamw_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
+                                  size_t nnz, size_t batch, int combiner, const float* gout, float alpha, float beta1,
+                                  float beta2, float epsilon, float lr, float weight_decay, int amsgrad,
+                                  const float* init_param, void* workspace, size_t workspace_bytes,
+                                  int64_t* n_unique_dev_out, det_stream_t stream) {
+  return det_apply_adamw_sparse_clip(t, ids, segment_ids, weights, nnz, batch, combiner, 0.f, gout, alpha, beta1, beta2,
+                                     epsilon, lr, weight_decay, amsgrad, init_param, workspace, workspace_bytes,
+                                     n_unique_dev_out, stream);
+}
 
-det_status det_apply_lion_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
-                                 size_t nnz, size_t batch, int combiner, const float* gout, float lr, float beta1,
-                                 float beta2, float weight_decay, const float* init_param, void* workspace,
-                                 size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream) {
+det_status det_apply_lion_sparse_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                      const float* weights, size_t nnz, size_t batch, int combiner, float max_norm,
+                                      const float* gout, float lr, float beta1, float beta2, float weight_decay,
+                                      const float* init_param, void* workspace, size_t workspace_bytes,
+                                      int64_t* n_unique_dev_out, det_stream_t stream) {
   OptHyper h;
   StepScalars sx;
   int opt;
   if (det_status st = lion_hyper(lr, beta1, beta2, weight_decay, &h, &sx, &opt)) return st;
   record_slot_init(t, opt, h);
-  const SparseSrc sp{segment_ids, weights, batch, combiner};
+  const SparseSrc sp{segment_ids, weights, batch, combiner, max_norm};
   return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
                    (cudaStream_t)stream, nullptr, &sp, sx);
 }
+det_status det_apply_lion_sparse(det_table* t, const int64_t* ids, const int32_t* segment_ids, const float* weights,
+                                 size_t nnz, size_t batch, int combiner, const float* gout, float lr, float beta1,
+                                 float beta2, float weight_decay, const float* init_param, void* workspace,
+                                 size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream) {
+  return det_apply_lion_sparse_clip(t, ids, segment_ids, weights, nnz, batch, combiner, 0.f, gout, lr, beta1, beta2,
+                                    weight_decay, init_param, workspace, workspace_bytes, n_unique_dev_out, stream);
+}
 
 // ---- det_apply_*_sparse_safe: the backward of det_lookup_sparse_safe chained into the same steps ------------------
-static SparseSrc safe_src(const int32_t* segment_ids, const float* weights, size_t batch, int combiner,
+static SparseSrc safe_src(const int32_t* segment_ids, const float* weights, size_t batch, int combiner, float max_norm,
                           int has_default_id, int64_t default_id) {
-  SparseSrc sp{segment_ids, weights, batch, combiner};
+  SparseSrc sp{segment_ids, weights, batch, combiner, max_norm};
   sp.safe = 1;
   sp.has_default_id = has_default_id ? 1 : 0;
   sp.default_id = (long long)default_id;
   return sp;
 }
 
+det_status det_apply_adagrad_sparse_safe_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                              const float* weights, size_t nnz, size_t batch, int combiner,
+                                              float max_norm, int has_default_id, int64_t default_id, const float* gout,
+                                              float lr, float epsilon, const float* init_param, float init_accum,
+                                              void* workspace, size_t workspace_bytes, int64_t* n_unique_dev_out,
+                                              det_stream_t stream) {
+  OptHyper h;
+  int opt;
+  if (det_status st = adagrad_hyper(lr, epsilon, init_accum, &h, &opt)) return st;
+  record_slot_init(t, opt, h);
+  const SparseSrc sp = safe_src(segment_ids, weights, batch, combiner, max_norm, has_default_id, default_id);
+  return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
+                   (cudaStream_t)stream, nullptr, &sp);
+}
 det_status det_apply_adagrad_sparse_safe(det_table* t, const int64_t* ids, const int32_t* segment_ids,
                                          const float* weights, size_t nnz, size_t batch, int combiner,
                                          int has_default_id, int64_t default_id, const float* gout, float lr,
                                          float epsilon, const float* init_param, float init_accum, void* workspace,
                                          size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream) {
+  return det_apply_adagrad_sparse_safe_clip(t, ids, segment_ids, weights, nnz, batch, combiner, 0.f, has_default_id,
+                                            default_id, gout, lr, epsilon, init_param, init_accum, workspace,
+                                            workspace_bytes, n_unique_dev_out, stream);
+}
+det_status det_apply_adam_sparse_safe_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                           const float* weights, size_t nnz, size_t batch, int combiner, float max_norm,
+                                           int has_default_id, int64_t default_id, const float* gout, float alpha,
+                                           float beta1, float beta2, float epsilon, const float* init_param,
+                                           void* workspace, size_t workspace_bytes, int64_t* n_unique_dev_out,
+                                           det_stream_t stream) {
   OptHyper h;
   int opt;
-  if (det_status st = adagrad_hyper(lr, epsilon, init_accum, &h, &opt)) return st;
+  if (det_status st = adam_hyper(alpha, beta1, beta2, epsilon, &h, &opt)) return st;
   record_slot_init(t, opt, h);
-  const SparseSrc sp = safe_src(segment_ids, weights, batch, combiner, has_default_id, default_id);
+  const SparseSrc sp = safe_src(segment_ids, weights, batch, combiner, max_norm, has_default_id, default_id);
   return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
                    (cudaStream_t)stream, nullptr, &sp);
 }
@@ -3483,11 +3727,20 @@ det_status det_apply_adam_sparse_safe(det_table* t, const int64_t* ids, const in
                                       int64_t default_id, const float* gout, float alpha, float beta1, float beta2,
                                       float epsilon, const float* init_param, void* workspace, size_t workspace_bytes,
                                       int64_t* n_unique_dev_out, det_stream_t stream) {
+  return det_apply_adam_sparse_safe_clip(t, ids, segment_ids, weights, nnz, batch, combiner, 0.f, has_default_id,
+                                         default_id, gout, alpha, beta1, beta2, epsilon, init_param, workspace,
+                                         workspace_bytes, n_unique_dev_out, stream);
+}
+det_status det_apply_sgd_sparse_safe_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                          const float* weights, size_t nnz, size_t batch, int combiner, float max_norm,
+                                          int has_default_id, int64_t default_id, const float* gout, float lr,
+                                          float momentum, int nesterov, const float* init_param, void* workspace,
+                                          size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream) {
   OptHyper h;
   int opt;
-  if (det_status st = adam_hyper(alpha, beta1, beta2, epsilon, &h, &opt)) return st;
+  if (det_status st = sgd_hyper(lr, momentum, nesterov, &h, &opt)) return st;
   record_slot_init(t, opt, h);
-  const SparseSrc sp = safe_src(segment_ids, weights, batch, combiner, has_default_id, default_id);
+  const SparseSrc sp = safe_src(segment_ids, weights, batch, combiner, max_norm, has_default_id, default_id);
   return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
                    (cudaStream_t)stream, nullptr, &sp);
 }
@@ -3496,11 +3749,21 @@ det_status det_apply_sgd_sparse_safe(det_table* t, const int64_t* ids, const int
                                      const float* gout, float lr, float momentum, int nesterov, const float* init_param,
                                      void* workspace, size_t workspace_bytes, int64_t* n_unique_dev_out,
                                      det_stream_t stream) {
+  return det_apply_sgd_sparse_safe_clip(t, ids, segment_ids, weights, nnz, batch, combiner, 0.f, has_default_id,
+                                        default_id, gout, lr, momentum, nesterov, init_param, workspace,
+                                        workspace_bytes, n_unique_dev_out, stream);
+}
+det_status det_apply_ftrl_sparse_safe_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                           const float* weights, size_t nnz, size_t batch, int combiner, float max_norm,
+                                           int has_default_id, int64_t default_id, const float* gout, float lr,
+                                           float l1, float l2, float l2_shrinkage, const float* init_param,
+                                           float init_accum, void* workspace, size_t workspace_bytes,
+                                           int64_t* n_unique_dev_out, det_stream_t stream) {
   OptHyper h;
   int opt;
-  if (det_status st = sgd_hyper(lr, momentum, nesterov, &h, &opt)) return st;
+  if (det_status st = ftrl_hyper(lr, l1, l2, l2_shrinkage, init_accum, &h, &opt)) return st;
   record_slot_init(t, opt, h);
-  const SparseSrc sp = safe_src(segment_ids, weights, batch, combiner, has_default_id, default_id);
+  const SparseSrc sp = safe_src(segment_ids, weights, batch, combiner, max_norm, has_default_id, default_id);
   return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
                    (cudaStream_t)stream, nullptr, &sp);
 }
@@ -3509,11 +3772,21 @@ det_status det_apply_ftrl_sparse_safe(det_table* t, const int64_t* ids, const in
                                       int64_t default_id, const float* gout, float lr, float l1, float l2,
                                       float l2_shrinkage, const float* init_param, float init_accum, void* workspace,
                                       size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream) {
+  return det_apply_ftrl_sparse_safe_clip(t, ids, segment_ids, weights, nnz, batch, combiner, 0.f, has_default_id,
+                                         default_id, gout, lr, l1, l2, l2_shrinkage, init_param, init_accum, workspace,
+                                         workspace_bytes, n_unique_dev_out, stream);
+}
+det_status det_apply_rmsprop_sparse_safe_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                              const float* weights, size_t nnz, size_t batch, int combiner,
+                                              float max_norm, int has_default_id, int64_t default_id, const float* gout,
+                                              float lr, float rho, float momentum, float epsilon, int centered,
+                                              int eps_in_sqrt, const float* init_param, float init_ms, void* workspace,
+                                              size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream) {
   OptHyper h;
   int opt;
-  if (det_status st = ftrl_hyper(lr, l1, l2, l2_shrinkage, init_accum, &h, &opt)) return st;
+  if (det_status st = rmsprop_hyper(lr, rho, momentum, epsilon, centered, eps_in_sqrt, init_ms, &h, &opt)) return st;
   record_slot_init(t, opt, h);
-  const SparseSrc sp = safe_src(segment_ids, weights, batch, combiner, has_default_id, default_id);
+  const SparseSrc sp = safe_src(segment_ids, weights, batch, combiner, max_norm, has_default_id, default_id);
   return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
                    (cudaStream_t)stream, nullptr, &sp);
 }
@@ -3523,11 +3796,21 @@ det_status det_apply_rmsprop_sparse_safe(det_table* t, const int64_t* ids, const
                                          float momentum, float epsilon, int centered, int eps_in_sqrt,
                                          const float* init_param, float init_ms, void* workspace,
                                          size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream) {
+  return det_apply_rmsprop_sparse_safe_clip(t, ids, segment_ids, weights, nnz, batch, combiner, 0.f, has_default_id,
+                                            default_id, gout, lr, rho, momentum, epsilon, centered, eps_in_sqrt,
+                                            init_param, init_ms, workspace, workspace_bytes, n_unique_dev_out, stream);
+}
+det_status det_apply_adadelta_sparse_safe_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                               const float* weights, size_t nnz, size_t batch, int combiner,
+                                               float max_norm, int has_default_id, int64_t default_id,
+                                               const float* gout, float lr, float rho, float epsilon,
+                                               const float* init_param, void* workspace, size_t workspace_bytes,
+                                               int64_t* n_unique_dev_out, det_stream_t stream) {
   OptHyper h;
   int opt;
-  if (det_status st = rmsprop_hyper(lr, rho, momentum, epsilon, centered, eps_in_sqrt, init_ms, &h, &opt)) return st;
+  if (det_status st = adadelta_hyper(lr, rho, epsilon, &h, &opt)) return st;
   record_slot_init(t, opt, h);
-  const SparseSrc sp = safe_src(segment_ids, weights, batch, combiner, has_default_id, default_id);
+  const SparseSrc sp = safe_src(segment_ids, weights, batch, combiner, max_norm, has_default_id, default_id);
   return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
                    (cudaStream_t)stream, nullptr, &sp);
 }
@@ -3536,11 +3819,21 @@ det_status det_apply_adadelta_sparse_safe(det_table* t, const int64_t* ids, cons
                                           int has_default_id, int64_t default_id, const float* gout, float lr,
                                           float rho, float epsilon, const float* init_param, void* workspace,
                                           size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream) {
+  return det_apply_adadelta_sparse_safe_clip(t, ids, segment_ids, weights, nnz, batch, combiner, 0.f, has_default_id,
+                                             default_id, gout, lr, rho, epsilon, init_param, workspace, workspace_bytes,
+                                             n_unique_dev_out, stream);
+}
+det_status det_apply_adamax_sparse_safe_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                             const float* weights, size_t nnz, size_t batch, int combiner,
+                                             float max_norm, int has_default_id, int64_t default_id, const float* gout,
+                                             float lr_t, float beta1, float beta2, float epsilon,
+                                             const float* init_param, void* workspace, size_t workspace_bytes,
+                                             int64_t* n_unique_dev_out, det_stream_t stream) {
   OptHyper h;
   int opt;
-  if (det_status st = adadelta_hyper(lr, rho, epsilon, &h, &opt)) return st;
+  if (det_status st = adamax_hyper(lr_t, beta1, beta2, epsilon, &h, &opt)) return st;
   record_slot_init(t, opt, h);
-  const SparseSrc sp = safe_src(segment_ids, weights, batch, combiner, has_default_id, default_id);
+  const SparseSrc sp = safe_src(segment_ids, weights, batch, combiner, max_norm, has_default_id, default_id);
   return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
                    (cudaStream_t)stream, nullptr, &sp);
 }
@@ -3550,13 +3843,24 @@ det_status det_apply_adamax_sparse_safe(det_table* t, const int64_t* ids, const 
                                         float beta1, float beta2, float epsilon, const float* init_param,
                                         void* workspace, size_t workspace_bytes, int64_t* n_unique_dev_out,
                                         det_stream_t stream) {
+  return det_apply_adamax_sparse_safe_clip(t, ids, segment_ids, weights, nnz, batch, combiner, 0.f, has_default_id,
+                                           default_id, gout, lr_t, beta1, beta2, epsilon, init_param, workspace,
+                                           workspace_bytes, n_unique_dev_out, stream);
+}
+det_status det_apply_nadam_sparse_safe_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                            const float* weights, size_t nnz, size_t batch, int combiner,
+                                            float max_norm, int has_default_id, int64_t default_id, const float* gout,
+                                            float lr, float beta1, float beta2, float epsilon, float omsn, float omsx,
+                                            float omt, float mt1, float vden, const float* init_param, void* workspace,
+                                            size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream) {
   OptHyper h;
+  StepScalars sx;
   int opt;
-  if (det_status st = adamax_hyper(lr_t, beta1, beta2, epsilon, &h, &opt)) return st;
+  if (det_status st = nadam_hyper(lr, beta1, beta2, epsilon, omsn, omsx, omt, mt1, vden, &h, &sx, &opt)) return st;
   record_slot_init(t, opt, h);
-  const SparseSrc sp = safe_src(segment_ids, weights, batch, combiner, has_default_id, default_id);
+  const SparseSrc sp = safe_src(segment_ids, weights, batch, combiner, max_norm, has_default_id, default_id);
   return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
-                   (cudaStream_t)stream, nullptr, &sp);
+                   (cudaStream_t)stream, nullptr, &sp, sx);
 }
 det_status det_apply_nadam_sparse_safe(det_table* t, const int64_t* ids, const int32_t* segment_ids,
                                        const float* weights, size_t nnz, size_t batch, int combiner, int has_default_id,
@@ -3564,14 +3868,24 @@ det_status det_apply_nadam_sparse_safe(det_table* t, const int64_t* ids, const i
                                        float epsilon, float omsn, float omsx, float omt, float mt1, float vden,
                                        const float* init_param, void* workspace, size_t workspace_bytes,
                                        int64_t* n_unique_dev_out, det_stream_t stream) {
+  return det_apply_nadam_sparse_safe_clip(t, ids, segment_ids, weights, nnz, batch, combiner, 0.f, has_default_id,
+                                          default_id, gout, lr, beta1, beta2, epsilon, omsn, omsx, omt, mt1, vden,
+                                          init_param, workspace, workspace_bytes, n_unique_dev_out, stream);
+}
+det_status det_apply_proximal_adagrad_sparse_safe_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                                       const float* weights, size_t nnz, size_t batch, int combiner,
+                                                       float max_norm, int has_default_id, int64_t default_id,
+                                                       const float* gout, float lr, float l1, float l2,
+                                                       const float* init_param, float init_accum, void* workspace,
+                                                       size_t workspace_bytes, int64_t* n_unique_dev_out,
+                                                       det_stream_t stream) {
   OptHyper h;
-  StepScalars sx;
   int opt;
-  if (det_status st = nadam_hyper(lr, beta1, beta2, epsilon, omsn, omsx, omt, mt1, vden, &h, &sx, &opt)) return st;
+  if (det_status st = proximal_hyper("det_apply_proximal_adagrad", lr, l1, l2, init_accum, 1, &h, &opt)) return st;
   record_slot_init(t, opt, h);
-  const SparseSrc sp = safe_src(segment_ids, weights, batch, combiner, has_default_id, default_id);
+  const SparseSrc sp = safe_src(segment_ids, weights, batch, combiner, max_norm, has_default_id, default_id);
   return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
-                   (cudaStream_t)stream, nullptr, &sp, sx);
+                   (cudaStream_t)stream, nullptr, &sp);
 }
 det_status det_apply_proximal_adagrad_sparse_safe(det_table* t, const int64_t* ids, const int32_t* segment_ids,
                                                   const float* weights, size_t nnz, size_t batch, int combiner,
@@ -3579,11 +3893,21 @@ det_status det_apply_proximal_adagrad_sparse_safe(det_table* t, const int64_t* i
                                                   float l1, float l2, const float* init_param, float init_accum,
                                                   void* workspace, size_t workspace_bytes, int64_t* n_unique_dev_out,
                                                   det_stream_t stream) {
+  return det_apply_proximal_adagrad_sparse_safe_clip(t, ids, segment_ids, weights, nnz, batch, combiner, 0.f,
+                                                     has_default_id, default_id, gout, lr, l1, l2, init_param,
+                                                     init_accum, workspace, workspace_bytes, n_unique_dev_out, stream);
+}
+det_status det_apply_proximal_sgd_sparse_safe_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                                   const float* weights, size_t nnz, size_t batch, int combiner,
+                                                   float max_norm, int has_default_id, int64_t default_id,
+                                                   const float* gout, float lr, float l1, float l2,
+                                                   const float* init_param, void* workspace, size_t workspace_bytes,
+                                                   int64_t* n_unique_dev_out, det_stream_t stream) {
   OptHyper h;
   int opt;
-  if (det_status st = proximal_hyper("det_apply_proximal_adagrad", lr, l1, l2, init_accum, 1, &h, &opt)) return st;
+  if (det_status st = proximal_hyper("det_apply_proximal_sgd", lr, l1, l2, 0.f, 0, &h, &opt)) return st;
   record_slot_init(t, opt, h);
-  const SparseSrc sp = safe_src(segment_ids, weights, batch, combiner, has_default_id, default_id);
+  const SparseSrc sp = safe_src(segment_ids, weights, batch, combiner, max_norm, has_default_id, default_id);
   return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
                    (cudaStream_t)stream, nullptr, &sp);
 }
@@ -3592,11 +3916,22 @@ det_status det_apply_proximal_sgd_sparse_safe(det_table* t, const int64_t* ids, 
                                               int has_default_id, int64_t default_id, const float* gout, float lr,
                                               float l1, float l2, const float* init_param, void* workspace,
                                               size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream) {
+  return det_apply_proximal_sgd_sparse_safe_clip(t, ids, segment_ids, weights, nnz, batch, combiner, 0.f,
+                                                 has_default_id, default_id, gout, lr, l1, l2, init_param, workspace,
+                                                 workspace_bytes, n_unique_dev_out, stream);
+}
+det_status det_apply_adagrad_da_sparse_safe_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                                 const float* weights, size_t nnz, size_t batch, int combiner,
+                                                 float max_norm, int has_default_id, int64_t default_id,
+                                                 const float* gout, float lr, float l1, float l2, int64_t global_step,
+                                                 const float* init_param, float init_gg, void* workspace,
+                                                 size_t workspace_bytes, int64_t* n_unique_dev_out,
+                                                 det_stream_t stream) {
   OptHyper h;
   int opt;
-  if (det_status st = proximal_hyper("det_apply_proximal_sgd", lr, l1, l2, 0.f, 0, &h, &opt)) return st;
+  if (det_status st = adagrad_da_hyper(lr, l1, l2, global_step, init_gg, &h, &opt)) return st;
   record_slot_init(t, opt, h);
-  const SparseSrc sp = safe_src(segment_ids, weights, batch, combiner, has_default_id, default_id);
+  const SparseSrc sp = safe_src(segment_ids, weights, batch, combiner, max_norm, has_default_id, default_id);
   return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
                    (cudaStream_t)stream, nullptr, &sp);
 }
@@ -3606,13 +3941,24 @@ det_status det_apply_adagrad_da_sparse_safe(det_table* t, const int64_t* ids, co
                                             float l1, float l2, int64_t global_step, const float* init_param,
                                             float init_gg, void* workspace, size_t workspace_bytes,
                                             int64_t* n_unique_dev_out, det_stream_t stream) {
+  return det_apply_adagrad_da_sparse_safe_clip(t, ids, segment_ids, weights, nnz, batch, combiner, 0.f, has_default_id,
+                                               default_id, gout, lr, l1, l2, global_step, init_param, init_gg,
+                                               workspace, workspace_bytes, n_unique_dev_out, stream);
+}
+det_status det_apply_adamw_sparse_safe_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                            const float* weights, size_t nnz, size_t batch, int combiner,
+                                            float max_norm, int has_default_id, int64_t default_id, const float* gout,
+                                            float alpha, float beta1, float beta2, float epsilon, float lr,
+                                            float weight_decay, int amsgrad, const float* init_param, void* workspace,
+                                            size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream) {
   OptHyper h;
+  StepScalars sx;
   int opt;
-  if (det_status st = adagrad_da_hyper(lr, l1, l2, global_step, init_gg, &h, &opt)) return st;
+  if (det_status st = adamw_hyper(alpha, beta1, beta2, epsilon, lr, weight_decay, amsgrad, &h, &sx, &opt)) return st;
   record_slot_init(t, opt, h);
-  const SparseSrc sp = safe_src(segment_ids, weights, batch, combiner, has_default_id, default_id);
+  const SparseSrc sp = safe_src(segment_ids, weights, batch, combiner, max_norm, has_default_id, default_id);
   return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
-                   (cudaStream_t)stream, nullptr, &sp);
+                   (cudaStream_t)stream, nullptr, &sp, sx);
 }
 det_status det_apply_adamw_sparse_safe(det_table* t, const int64_t* ids, const int32_t* segment_ids,
                                        const float* weights, size_t nnz, size_t batch, int combiner, int has_default_id,
@@ -3620,12 +3966,22 @@ det_status det_apply_adamw_sparse_safe(det_table* t, const int64_t* ids, const i
                                        float epsilon, float lr, float weight_decay, int amsgrad,
                                        const float* init_param, void* workspace, size_t workspace_bytes,
                                        int64_t* n_unique_dev_out, det_stream_t stream) {
+  return det_apply_adamw_sparse_safe_clip(t, ids, segment_ids, weights, nnz, batch, combiner, 0.f, has_default_id,
+                                          default_id, gout, alpha, beta1, beta2, epsilon, lr, weight_decay, amsgrad,
+                                          init_param, workspace, workspace_bytes, n_unique_dev_out, stream);
+}
+det_status det_apply_lion_sparse_safe_clip(det_table* t, const int64_t* ids, const int32_t* segment_ids,
+                                           const float* weights, size_t nnz, size_t batch, int combiner, float max_norm,
+                                           int has_default_id, int64_t default_id, const float* gout, float lr,
+                                           float beta1, float beta2, float weight_decay, const float* init_param,
+                                           void* workspace, size_t workspace_bytes, int64_t* n_unique_dev_out,
+                                           det_stream_t stream) {
   OptHyper h;
   StepScalars sx;
   int opt;
-  if (det_status st = adamw_hyper(alpha, beta1, beta2, epsilon, lr, weight_decay, amsgrad, &h, &sx, &opt)) return st;
+  if (det_status st = lion_hyper(lr, beta1, beta2, weight_decay, &h, &sx, &opt)) return st;
   record_slot_init(t, opt, h);
-  const SparseSrc sp = safe_src(segment_ids, weights, batch, combiner, has_default_id, default_id);
+  const SparseSrc sp = safe_src(segment_ids, weights, batch, combiner, max_norm, has_default_id, default_id);
   return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
                    (cudaStream_t)stream, nullptr, &sp, sx);
 }
@@ -3634,14 +3990,9 @@ det_status det_apply_lion_sparse_safe(det_table* t, const int64_t* ids, const in
                                       int64_t default_id, const float* gout, float lr, float beta1, float beta2,
                                       float weight_decay, const float* init_param, void* workspace,
                                       size_t workspace_bytes, int64_t* n_unique_dev_out, det_stream_t stream) {
-  OptHyper h;
-  StepScalars sx;
-  int opt;
-  if (det_status st = lion_hyper(lr, beta1, beta2, weight_decay, &h, &sx, &opt)) return st;
-  record_slot_init(t, opt, h);
-  const SparseSrc sp = safe_src(segment_ids, weights, batch, combiner, has_default_id, default_id);
-  return apply_dup(t, ids, gout, nnz, h, init_param, opt, workspace, workspace_bytes, n_unique_dev_out,
-                   (cudaStream_t)stream, nullptr, &sp, sx);
+  return det_apply_lion_sparse_safe_clip(t, ids, segment_ids, weights, nnz, batch, combiner, 0.f, has_default_id,
+                                         default_id, gout, lr, beta1, beta2, weight_decay, init_param, workspace,
+                                         workspace_bytes, n_unique_dev_out, stream);
 }
 
 }  // extern "C"

@@ -84,13 +84,14 @@ class SparseEmbedding(Embedding):
   `forward(sp_ids, sp_weights=None)` is `trainable_embedding_lookup_sparse` (the fused embedding_lookup_sparse), and
   `apply_gradients(optimizer)` steps the table from the output gradient -- one det_apply_*_sparse call per forward with
   a fused optimizer.  One shard, float32 / float16 / bfloat16 rows, a constant or keyed initializer, embedding_size a
-  multiple of 4 up to 128."""
+  multiple of 4 up to 128.  `max_norm` clips every looked-up row, and the step trains through the clip (float32)."""
 
   def __init__(self, embedding_size, combiner="mean", **kwargs):
     super().__init__(embedding_size, combiner=combiner, **kwargs)
 
   def forward(self, sp_ids, sp_weights=None):
-    out, h = trainable_embedding_lookup_sparse(self.params, sp_ids, sp_weights, combiner=self.combiner)
+    out, h = trainable_embedding_lookup_sparse(self.params, sp_ids, sp_weights, combiner=self.combiner,
+                                               max_norm=self.max_norm)
     if self.training and self.params.trainable:
       self._wrappers.append(h)
     return out

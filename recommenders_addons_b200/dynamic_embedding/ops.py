@@ -63,10 +63,10 @@ def lookup_sparse_fused(params, ids, segment_ids, weights, batch, combiner, defa
   return out
 
 
-def lookup_sparse_safe_fused(params, ids, rows, weights, batch, combiner, default_id, out=None):
-  """det_lookup_sparse_safe: the raw ids, their flattened rows (ascending int32) and weights are cleaned on the device
-  (prune, fill) and looked up in one chain, with no host synchronisation.  `out` (optional): a contiguous float32
-  tensor of batch * dim elements on the table's device, written in place (any shape)."""
+def lookup_sparse_safe_fused(params, ids, rows, weights, batch, combiner, default_id, out=None, max_norm=None):
+  """det_lookup_sparse_safe[_clip]: the raw ids, their flattened rows (ascending int32) and weights are cleaned on the
+  device (prune, fill) and looked up in one chain, with no host synchronisation.  `out` (optional): a contiguous
+  float32 tensor of batch * dim elements on the table's device, written in place (any shape)."""
   table = params.tables[0]
   dev = table.device
   ids = ids.reshape(-1).to(dev).contiguous()
@@ -77,9 +77,12 @@ def lookup_sparse_safe_fused(params, ids, rows, weights, batch, combiner, defaul
     default_row = table._default_value.to(device=dev, dtype=torch.float32).contiguous()
   if out is None:
     out = torch.empty((batch, params.dim), dtype=torch.float32, device=dev)
-  _lib.check(_lib.lib().det_lookup_sparse_safe(table.handle, _ptr(ids), _ptr(seg), _ptr(w), ids.numel(), batch,
-                                               _lib.COMBINERS[combiner], int(default_id is not None),
-                                               int(default_id or 0), _ptr(default_row), _ptr(out), _stream_ptr(dev)))
+  head = (table.handle, _ptr(ids), _ptr(seg), _ptr(w), ids.numel(), batch, _lib.COMBINERS[combiner],
+          int(default_id is not None), int(default_id or 0), _ptr(default_row))
+  if max_norm is not None:
+    _lib.check(_lib.lib().det_lookup_sparse_safe_clip(*head, float(max_norm), _ptr(out), _stream_ptr(dev)))
+  else:
+    _lib.check(_lib.lib().det_lookup_sparse_safe(*head, _ptr(out), _stream_ptr(dev)))
   return out
 
 
@@ -196,12 +199,18 @@ class SparseLookupTrainable(object):
   A fused optimizer turns them into one det_apply_*_sparse call; `ComposedOptimizer` into det_lookup_sparse_grad and
   its own step.  `safe`: a `trainable_safe_embedding_lookup_sparse` call, whose `ids`, `segment_ids` (flattened rows)
   and `weights` are the raw list and `default_id` its fill id (or None); the steps are then det_apply_*_sparse_safe
-  and det_lookup_sparse_safe_grad."""
+  and det_lookup_sparse_safe_grad.  `max_norm` (or None): the forward clipped every row to that norm; the steps are
+  then the _clip forms, which take each unique id's gradient through the clip's backward.  0 means no clipping, as in
+  the C calls, for every optimizer."""
 
-  def __init__(self, params, ids, segment_ids, weights, batch, combiner, out, safe=False, default_id=None):
+  def __init__(self, params, ids, segment_ids, weights, batch, combiner, out, safe=False, default_id=None,
+               max_norm=None):
     self.params, self.ids, self.segment_ids, self.weights = params, ids, segment_ids, weights
     self.batch, self.combiner, self.out = int(batch), combiner, out
     self.safe, self.default_id = bool(safe), default_id
+    self.max_norm = None if max_norm is None else float(max_norm)
+    if self.max_norm is not None and not self.max_norm >= 0:
+      raise ValueError("max_norm must be >= 0 (0 = no clipping) or None, got %r" % (max_norm,))
 
   def safe_args(self):
     """(has_default_id, default_id) of the _safe C calls"""
@@ -226,7 +235,12 @@ class SparseLookupTrainable(object):
 
   def grad_rows(self, gout=None):
     """(unique ids, their summed gradients [n_unique, dim]) from dL/dout (default: `out.grad`) -- det_lookup_sparse_grad
-    (det_lookup_sparse_safe_grad for a safe lookup).  The unique count is read on the host."""
+    (det_lookup_sparse_safe_grad for a safe lookup).  The unique count is read on the host.
+
+    With `max_norm`, each gradient is then taken through the clip's backward at the id's current row (the stored row,
+    or the row a lookup of a missing id returns), with the rule of the fused _clip steps restated in torch.  torch's
+    reductions round differently from the kernel's lane-group sums, so this is close to, not bit-exact with, the
+    gradient the fused step applies."""
     gout = self.out.grad if gout is None else gout
     dev = self.ids.device
     gout = gout.to(device=dev, dtype=torch.float32).contiguous()
@@ -250,10 +264,23 @@ class SparseLookupTrainable(object):
     else:
       _lib.check(lib.det_lookup_sparse_grad(*(head + tail)))
     n = int(cnt.item())
-    return uniq[:n], grads[:n]
+    uniq, grads = uniq[:n], grads[:n]
+    if self.max_norm and n:
+      grads = _clip_grad(self.params.lookup(uniq).to(torch.float32), grads, self.max_norm)
+    return uniq, grads
 
 
-def _check_trainable_sparse(params, sp_ids, sp_weights, combiner, who, composed):
+def _clip_grad(p, g, c):
+  """J^T g for the clip p -> p * c / max(||p||, c), row by row: g where the row was not clipped (!(||p|| > c)), else
+  s*g - p*t with s = c / ||p||, t = s * (p . g) / ||p||^2 (the rule of det_apply_*_sparse_clip)"""
+  ss = (p * p).sum(-1, keepdim=True)
+  n = ss.sqrt()
+  s = c / n
+  t = (s * (p * g).sum(-1, keepdim=True)) / ss
+  return torch.where(n > c, g * s - p * t, g)
+
+
+def _check_trainable_sparse(params, sp_ids, sp_weights, combiner, who, composed, max_norm=None):
   """the refusals of the fused training lookups; `composed`: the function whose return_trainable=True path covers the
   rest"""
   if combiner not in ("mean", "sqrtn", "sum"):
@@ -280,9 +307,16 @@ def _check_trainable_sparse(params, sp_ids, sp_weights, combiner, who, composed)
     raise ValueError("%s: bp_v2 is not supported; use %s(return_trainable=True)" % (who, composed))
   if params.dim % 4 != 0 or params.dim > 128:
     raise ValueError("%s: dim must be a multiple of 4 and at most 128, got %d" % (who, params.dim))
+  if max_norm is not None:
+    if not float(max_norm) > 0:
+      raise ValueError("%s: max_norm must be > 0 (or None), got %r; use %s(max_norm=..., return_trainable=True)" %
+                       (who, max_norm, composed))
+    if params.value_dtype != torch.float32:
+      raise ValueError("%s: max_norm is fused for float32 variables only (the reference clips %s rows in their own "
+                       "dtype); use %s(max_norm=..., return_trainable=True)" % (who, params.value_dtype, composed))
 
 
-def trainable_embedding_lookup_sparse(params, sp_ids, sp_weights=None, combiner="mean"):
+def trainable_embedding_lookup_sparse(params, sp_ids, sp_weights=None, combiner="mean", max_norm=None):
   """embedding_lookup_sparse for training through the fused kernels: returns (out, SparseLookupTrainable).
 
   `out` [batch, dim] float32 is the fused forward (det_lookup_sparse).  In TRAIN mode on a trainable variable it is a
@@ -291,20 +325,24 @@ def trainable_embedding_lookup_sparse(params, sp_ids, sp_weights=None, combiner=
   synchronisation).  Per id i of segment b the gradient row is dL/dout[b] * w_i / den_b (den_b: the forward's
   normaliser), summed per unique id in increasing position -- the composed path's rule, deterministic.
 
+  `max_norm` (float32 variables): every looked-up row is clipped to that L2 norm before it is weighted
+  (det_lookup_sparse_clip), and the step takes each unique id's summed gradient through the clip's backward at the
+  row it steps (det_apply_*_sparse_clip; at ||row|| == max_norm the row counts as unclipped and its gradient is kept).
+
   Single-shard float32 / float16 / bfloat16 variables with a constant or keyed initializer, dim % 4 == 0 and
-  dim <= 128; no max_norm.  Everything else takes `embedding_lookup_sparse(..., return_trainable=True)`."""
+  dim <= 128.  Everything else takes `embedding_lookup_sparse(..., return_trainable=True)`."""
   _check_trainable_sparse(params, sp_ids, sp_weights, combiner, "trainable_embedding_lookup_sparse",
-                          "embedding_lookup_sparse")
+                          "embedding_lookup_sparse", max_norm)
   dev = params.tables[0].device
   ids = sp_ids.values.reshape(-1).to(dev).contiguous()
   seg = sp_ids.indices[:, 0].to(device=dev, dtype=torch.int32).contiguous()
   w = None if sp_weights is None else sp_weights.values.reshape(-1).to(device=dev, dtype=torch.float32).contiguous()
   batch = sp_ids.dense_shape[0]
-  out = lookup_sparse_fused(params, ids, seg, w, batch, combiner)
+  out = lookup_sparse_fused(params, ids, seg, w, batch, combiner, max_norm=max_norm)
   from .variable import ModelMode
   if params.trainable and ModelMode.CURRENT_SETTING == ModelMode.TRAIN:
     out.requires_grad_(True)
-  return out, SparseLookupTrainable(params, ids, seg, w, batch, combiner, out)
+  return out, SparseLookupTrainable(params, ids, seg, w, batch, combiner, out, max_norm=max_norm)
 
 
 def verify_embedding_param_weights(embedding_weights, sparse_ids, sparse_weights=None):
@@ -415,7 +453,8 @@ def safe_embedding_lookup_sparse(embedding_weights, sparse_ids, sparse_weights=N
   return (final, tw) if return_trainable else final
 
 
-def trainable_safe_embedding_lookup_sparse(params, sp_ids, sp_weights=None, combiner="mean", default_id=None):
+def trainable_safe_embedding_lookup_sparse(params, sp_ids, sp_weights=None, combiner="mean", default_id=None,
+                                           max_norm=None):
   """safe_embedding_lookup_sparse for training through the fused kernels: returns (out, SparseLookupTrainable).
 
   `out` [*dense_shape[:-1], dim] float32 is det_lookup_sparse_safe's forward, allocated in that shape, so in TRAIN mode
@@ -423,12 +462,14 @@ def trainable_safe_embedding_lookup_sparse(params, sp_ids, sp_weights=None, comb
   `optimizer.apply_gradients([(out.grad, handle)])` steps the table in one det_apply_*_sparse_safe call (no host
   synchronisation): the ids of the cleaned list (pruned entries take no part; an empty row's fill id does) get the
   gradients of trainable_embedding_lookup_sparse.  With default_id None, id 0 is stepped whenever a row is empty, with
-  a gradient of +0.0 from each such row, as the reference's composed path does.
+  a gradient of +0.0 from each such row, as the reference's composed path does.  `max_norm`: as in
+  trainable_embedding_lookup_sparse, for every row of the cleaned list (det_lookup_sparse_safe_clip and
+  det_apply_*_sparse_safe_clip).
 
   Same restrictions as trainable_embedding_lookup_sparse; everything else takes
   `safe_embedding_lookup_sparse(..., return_trainable=True)`."""
   _check_trainable_sparse(params, sp_ids, sp_weights, combiner, "trainable_safe_embedding_lookup_sparse",
-                          "safe_embedding_lookup_sparse")
+                          "safe_embedding_lookup_sparse", max_norm)
   verify_embedding_param_weights(params, sp_ids, sp_weights)
   dev = params.tables[0].device
   rows, lead, shape = _flat_rows(sp_ids)
@@ -436,8 +477,9 @@ def trainable_safe_embedding_lookup_sparse(params, sp_ids, sp_weights=None, comb
   seg = rows.to(dev).contiguous()
   w = None if sp_weights is None else sp_weights.values.reshape(-1).to(device=dev, dtype=torch.float32).contiguous()
   out = torch.empty(tuple(shape[:-1]) + (params.dim,), dtype=torch.float32, device=dev)
-  lookup_sparse_safe_fused(params, ids, seg, w, lead, combiner, default_id, out=out)
+  lookup_sparse_safe_fused(params, ids, seg, w, lead, combiner, default_id, out=out, max_norm=max_norm)
   from .variable import ModelMode
   if params.trainable and ModelMode.CURRENT_SETTING == ModelMode.TRAIN:
     out.requires_grad_(True)
-  return out, SparseLookupTrainable(params, ids, seg, w, lead, combiner, out, safe=True, default_id=default_id)
+  return out, SparseLookupTrainable(params, ids, seg, w, lead, combiner, out, safe=True, default_id=default_id,
+                                    max_norm=max_norm)

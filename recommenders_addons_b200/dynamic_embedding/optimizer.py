@@ -241,14 +241,20 @@ class _FusedBase(object):
 
   def _sparse_call(self, name, table, h, gout, *rest):
     """det_apply_<name>_sparse(table, ids, segment_ids, weights, nnz, batch, combiner, gout, *rest), or its _safe form
-    (has_default_id and default_id after the combiner) for a safe lookup"""
+    (has_default_id and default_id after the combiner) for a safe lookup; for a clipped lookup the _clip form of either
+    (max_norm right after the combiner)"""
     lib = _lib.lib()
     head = (table.handle, _ptr(h.ids), _ptr(h.segment_ids), _ptr(h.weights), h.ids.numel(), h.batch,
             _lib.COMBINERS[h.combiner])
+    fn = "det_apply_%s_sparse" % name
+    if h.max_norm is not None:
+      head += (h.max_norm,)
     if h.safe:
-      _lib.check(getattr(lib, "det_apply_%s_sparse_safe" % name)(*(head + h.safe_args()), _ptr(gout), *rest))
-    else:
-      _lib.check(getattr(lib, "det_apply_%s_sparse" % name)(*head, _ptr(gout), *rest))
+      head += h.safe_args()
+      fn += "_safe"
+    if h.max_norm is not None:
+      fn += "_clip"
+    _lib.check(getattr(lib, fn)(*head, _ptr(gout), *rest))
 
 
 class FusedAdagrad(_FusedBase):

@@ -17,12 +17,20 @@ about 10 % of the weights <= 0 (pruned), default_id None:
        trainable_safe_embedding_lookup_sparse with det_apply_adagrad_sparse_safe, rows checked bit for bit after one
        unweighted step of each from the same state;
   (s3) one id per row, no weights: de.safe_embedding_lookup_sparse with default_id None and 0 against det_lookup_sparse.
+With --max-norm C, training through a lookup that clips every row to norm C, at shape (1) (rows drawn as N(0, 0.05^2)
+per element, norm about 0.4, so that with the default C = 0.4 about half of them are clipped):
+  (c1) det_apply_adagrad_sparse_clip against det_apply_adagrad_sparse on the same inputs (the clip's backward inside
+       the fused step against no clip);
+  (c2) the public training step: trainable_embedding_lookup_sparse(max_norm=C) + FusedAdagrad against
+       embedding_lookup_sparse(max_norm=C, return_trainable=True) + FusedAdagrad (the composed path).
+  One step of each of the four arms is checked on the sampled ids like the arms above, the clipped gradients taken
+  through tests/clip_grad_oracle.py at the rows before the step (the fused arms bit for bit, the composed one to 1e-4).
 CUDA events, median of --rounds rounds that alternate the order of the arms.  A sample of every arm's result is checked
 against the oracle: the sampled ids' rows after one step of each arm (the fused arms bit for bit against
 tests/sparse_grad_oracle.py + oracle.sparse_adagrad_step; the composed arm, whose weighted denominators are summed by
 atomics, to 1e-4 relative).  The card name, power limit and max SM clock are read in the same run.  Prints one JSON line.
 
-  python scripts/sparse_train_microbench.py [--resident 40000000] [--rounds 5] [--calls 5] [--safe]
+  python scripts/sparse_train_microbench.py [--resident 40000000] [--rounds 5] [--calls 5] [--safe | --max-norm C]
 """
 import argparse
 import json
@@ -79,11 +87,16 @@ def main():
   ap.add_argument("--calls", type=int, default=5)
   ap.add_argument("--sample", type=int, default=2000)
   ap.add_argument("--safe", action="store_true", help="measure safe_embedding_lookup_sparse instead")
+  ap.add_argument("--max-norm", type=float, default=None, help="measure training through a max_norm-clipped lookup")
   args = ap.parse_args()
+  if args.safe and args.max_norm is not None:
+    ap.error("--safe and --max-norm measure different paths: give one of them")
   if not torch.cuda.is_available():
     raise SystemExit("sparse_train_microbench.py needs a GPU")
   if args.safe:
     return safe_main(args)
+  if args.max_norm is not None:
+    return clip_main(args)
   from oracle import oracle as O
   from recommenders_addons_b200 import _lib
   from recommenders_addons_b200 import dynamic_embedding as de
@@ -337,6 +350,116 @@ def safe_main(args):
     one_safe_default()
   result["one_per_row"] = dict(zip(("det_lookup_sparse", "safe_default_none", "safe_default_0"),
                                    medians(args.rounds, args.calls, [one_plain, one_safe_none, one_safe_default])))
+  result["checks"] = checks
+  result["ok"] = all(checks.values())
+  print(json.dumps(result))
+
+
+def clip_main(args):
+  from oracle import oracle as O
+  from recommenders_addons_b200 import _lib
+  from recommenders_addons_b200 import dynamic_embedding as de
+  from recommenders_addons_b200.dynamic_embedding.table import _ptr, _stream_ptr
+  from tests import clip_grad_oracle as CG
+  from tests import sparse_grad_oracle as SG
+  lib = _lib.lib()
+  dev = torch.device("cuda", torch.cuda.current_device())
+  rng = np.random.default_rng(2)
+  c = float(args.max_norm)
+  result = {"metric": "max_norm-clipped sparse training microbenchmark", "dim": DIM, "resident": args.resident,
+            "max_norm": c, "card": card(), "unit": "ms"}
+  v = de.Variable(dim=DIM, initializer=0.0, num_slot_planes=1, devices=[str(dev)], name="clip_bench",
+                  init_size=2 * args.resident)
+  step = 1 << 22
+  for b in range(0, args.resident, step):
+    k = torch.arange(b, min(b + step, args.resident), dtype=torch.int64, device=dev)
+    v.upsert(k, torch.randn(k.numel(), DIM, device=dev) * 0.05)
+  t = v.tables[0]
+  nnz = BAGS * PER_BAG
+  seg = torch.arange(BAGS, device=dev).repeat_interleave(PER_BAG)
+  ind = torch.stack([seg, torch.arange(PER_BAG, device=dev).repeat(BAGS)], 1)
+  per = args.resident // PER_BAG
+  r = np.empty(0, np.int64)
+  while r.shape[0] < nnz:                                   # Zipf(1.05) ranks per field, as in (1)
+    d = rng.zipf(1.05, 2 * nnz)
+    r = np.concatenate([r, d[d <= per] - 1])
+  ids = torch.as_tensor(r[:nnz] * PER_BAG + np.arange(nnz) % PER_BAG, device=dev)
+  wv = torch.as_tensor(rng.uniform(0.5, 2.0, nnz).astype(np.float32), device=dev)
+  sp, sw = de.SparseIds(ind, ids, (BAGS, PER_BAG)), de.SparseIds(ind, wv, (BAGS, PER_BAG))
+  seg32 = seg.to(torch.int32)
+  gout = torch.randn(BAGS, DIM, device=dev) * 1e-3
+  uniq = torch.unique(ids)
+  norms = v.lookup(uniq).norm(dim=1)
+  result["unique_ids"] = int(uniq.numel())
+  result["clipped_share_of_unique_rows"] = round(float((norms > c).float().mean()), 4)
+
+  ids_np, seg_np, w_np, g_np = ids.cpu().numpy(), seg.cpu().numpy().astype(np.int32), wv.cpu().numpy(), gout.cpu().numpy()
+  un = uniq.cpu().numpy()
+  pick = np.unique(np.concatenate([un[:50], rng.choice(un, min(args.sample, un.shape[0]), replace=False)]))
+  g_pick = SG.lookup_sparse_grad_of(ids_np, seg_np, w_np, BAGS, "mean", g_np, pick)
+  checks = {}
+
+  def check(name, fn, clip, exact):
+    """one step of `fn` on the sampled ids against oracle.sparse_adagrad_step of their (clipped) oracle gradients"""
+    p0 = v.lookup(torch.as_tensor(pick, device=dev)).cpu().numpy()
+    k_all, a_all = t.export(plane=1)
+    sel = torch.isin(k_all, torch.as_tensor(pick, device=dev))
+    ka, va = k_all[sel].cpu().numpy(), a_all[sel].cpu().numpy()
+    stepped = (va != 0).any(1)               # plane 1 exports 0 for a key the table has not stepped yet
+    pt, pa = O.PortTable(DIM), O.PortTable(DIM)
+    pt.insert(pick, p0)
+    pa.insert(ka[stepped], va[stepped])
+    fn()
+    torch.cuda.synchronize()
+    g = CG.clip_grad(p0, g_pick, c) if clip else g_pick
+    exp_p, _ = O.sparse_adagrad_step(pt, pa, pick, g, LR, np.zeros(DIM, np.float32), np.full(DIM, INIT_ACCUM, np.float32))
+    got = v.lookup(torch.as_tensor(pick, device=dev)).cpu().numpy()
+    checks[name] = bool(np.array_equal(got.view(np.uint32), exp_p.view(np.uint32))) if exact else \
+        bool(np.allclose(got, exp_p, rtol=1e-4, atol=1e-6))
+
+  # (c1) the C calls on the same inputs
+  init = t._default_value.to(device=dev, dtype=torch.float32).contiguous()
+  ws_n = int(lib.det_apply_sparse_workspace_bytes(nnz, BAGS, DIM))
+  raw = torch.empty(ws_n + 256, dtype=torch.uint8, device=dev)
+  off = (-raw.data_ptr()) % 256
+  ws = raw[off:off + ws_n]
+  head = (t.handle, _ptr(ids), _ptr(seg32), _ptr(wv), nnz, BAGS, _lib.COMBINERS["mean"])
+  tail = (_ptr(gout), LR, 0.0, _ptr(init), INIT_ACCUM, _ptr(ws), ws_n, None, _stream_ptr(dev))
+
+  def plain():
+    _lib.check(lib.det_apply_adagrad_sparse(*head, *tail))
+
+  def clipped():
+    _lib.check(lib.det_apply_adagrad_sparse_clip(*head, c, *tail))
+
+  check("det_apply_adagrad_sparse", plain, False, True)
+  check("det_apply_adagrad_sparse_clip", clipped, True, True)
+  for _ in range(2):
+    plain()
+    clipped()
+  result["apply"] = dict(zip(("det_apply_adagrad_sparse", "det_apply_adagrad_sparse_clip"),
+                             medians(args.rounds, args.calls, [plain, clipped])))
+
+  # (c2) the public step
+  opt = de.FusedAdagrad(LR, INIT_ACCUM)
+
+  def composed():
+    out, tw = de.embedding_lookup_sparse(v, sp, sw, combiner="mean", max_norm=c, return_trainable=True)
+    out.backward(gout)
+    opt.apply_gradients([(tw.values.grad, tw)])
+
+  def fused():
+    out, h = de.trainable_embedding_lookup_sparse(v, sp, sw, combiner="mean", max_norm=c)
+    out.backward(gout)
+    opt.apply_gradients([(out.grad, h)])
+
+  check("composed_public", composed, True, False)
+  check("fused_clip_public", fused, True, True)
+  for _ in range(2):
+    composed()
+    fused()
+  result["train_step"] = dict(zip(("composed_public", "fused_clip_public"),
+                                  medians(args.rounds, args.calls, [composed, fused])))
   result["checks"] = checks
   result["ok"] = all(checks.values())
   print(json.dumps(result))
